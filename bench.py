@@ -7,9 +7,8 @@
 
 One "step" = one whole `PointFusion(odom='gt')(frames)` call over a (B, L) batch of synthetic RGB-D
 sequences = B*L frame updates (per frame: K1r frame records, K2/K3 project+select, K3c per-tile append counts,
-K4 merge+append).  The timed region is EXACTLY --steps steps; because 20 steps are only ~0.1 s, the region is
-measured `--repeats` times back to back (default: enough repeats for >= 100 timed steps) and the MEDIAN region
-is reported (all of them are listed under "timed_regions_ms").
+K4 merge+append).  The timed region is EXACTLY --steps steps.  `--repeats R` measures R such regions back to back
+and reports the MEDIAN one (all of them are listed under "timed_regions_ms"); the default is one region.
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for what each key means.
 """
 import argparse
@@ -31,7 +30,7 @@ UNIT = "frames/s"
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="gsx", choices=["gsx", "reference"])
     ap.add_argument("--batch", type=int, default=8, help="sequences per GPU")
@@ -39,12 +38,14 @@ def parse():
     ap.add_argument("--height", type=int, default=480)
     ap.add_argument("--width", type=int, default=640)
     ap.add_argument("--cpu-sample-frames", type=int, default=12, help="frames of the CPU-baseline sample (B=1)")
-    ap.add_argument("--repeats", type=int, default=0, help="timed regions of --steps steps each (0: ceil(100/steps))")
+    ap.add_argument("--repeats", type=int, default=1, help="timed regions of --steps steps each (median reported)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra-configs", action="store_true", help="skip the B=1 / L=32 (config 2) line")
     ap.add_argument("--no-icp", action="store_true", help="skip the secondary ICP-odometry measurement")
     ap.add_argument("--no-raw", action="store_true", help="skip the dataset-native (uint8/uint16) ingest measurement")
     ap.add_argument("--no-e2e", action="store_true", help="diagnostic runs only: skip the end-to-end leg (e2e = null)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's poses and (sampled) maps as DIR/*.npy (rank 0's share)")
     return ap.parse_args()
 
 
@@ -193,9 +194,37 @@ def workload_config(args, world):
             {2: "peer pulls over CUDA IPC, job-wide store"}.get(world, "NCCL all-gather of the packed row arrays")
             if os.environ.get("GSX_MAP_EXCHANGE", "auto") == "auto" else os.environ["GSX_MAP_EXCHANGE"],
             EXCHANGE_SCHEDULE),
-        "l2_policy": "inputs (%.0f MB depth+rgb per GPU per step) exceed the 126 MB L2" % (
+        "l2_policy": "inputs (%.0f MB depth+rgb per GPU per step) exceed the 50 MB L2" % (
             args.batch * args.seqlen * args.height * args.width * 16 / 1e6),
     }
+
+
+DUMP_MAP_ROWS = 1 << 20  # 56 B per row: 56 MiB in all
+
+
+def dump_outputs(out_dir, pc, poses):
+    """The last timed step's poses, map sizes and map rows (rank 0's own sequences).  A map larger than its share of
+    DUMP_MAP_ROWS is represented by a fixed, seeded sample of its rows; `map_rows.npy` lists (sequence, row)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    counts = [int(c) for c in pc.num_points_per_pointcloud.tolist()]
+    per_seq = max(1, DUMP_MAP_ROWS // max(1, len(counts)))
+    rows = []
+    for b, n in enumerate(counts):
+        idx = torch.arange(n) if n <= per_seq else \
+            torch.randperm(n, generator=torch.Generator().manual_seed(b))[:per_seq].sort().values
+        rows.append(torch.stack([torch.full_like(idx, b), idx], 1))
+    rows = torch.cat(rows).to(torch.float64)
+    seq, row = rows[:, 0].long().to(pc.device), rows[:, 1].long().to(pc.device)
+    arrays = {"poses": poses, "num_points_per_pointcloud": torch.tensor(counts, dtype=torch.float64),
+              "map_rows": rows}
+    for key, padded in (("points", pc.points_padded), ("normals", pc.normals_padded), ("colors", pc.colors_padded),
+                        ("features", pc.features_padded)):
+        arrays[key] = padded[seq, row]
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -276,6 +305,8 @@ def main():
     if world > 1 and os.environ.get("GSX_BENCH_STORE", "shared" if exchange == "peer" else "fresh") == "shared":
         stores = [parallel.GatheredMaps(B, L * H * W, dev) for _ in range(2)]
 
+    last_out = []  # (map, poses) of the most recent step
+
     def run_steps(frames, steps, d2h):
         """`steps` whole-batch PointFusion calls.  N>1: the final-map exchange of step k (communication stream) overlaps
         the fusion of step k+1; the last one is awaited before returning.  d2h: the result (poses + the fused map of this
@@ -291,6 +322,7 @@ def main():
                 pc, poses = slam(frames, out=store.reset())
             else:
                 pc, poses = slam(frames)
+            last_out[:] = [pc, poses]
             fused = torch.cuda.Event()
             fused.record()
             if pending is not None:  # step k-1's maps travel while step k (just enqueued) computes
@@ -332,7 +364,7 @@ def main():
             all_ms.append(ms)
         return sorted(all_ms)[len(all_ms) // 2], all_ms, res
 
-    repeats = args.repeats if args.repeats > 0 else max(1, -(-100 // max(1, args.steps)))
+    repeats = max(1, args.repeats)
     if world > 1:  # setup, not warm-up: let the caching allocator reach its steady state (two map stores and two sets
         run_steps(frames_dev, 3, d2h=False)  # of gather buffers are alive at once in the pipelined loop)
     run_steps(frames_dev, max(args.warmup, 3), d2h=False)  # same (pipelined) code path as the timed region
@@ -341,6 +373,9 @@ def main():
         sampler.start()
     ms_dev, all_dev, _ = timed_median(frames_dev, args.steps, False, repeats)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last_out)
+    last_out.clear()
     if args.no_e2e:
         ms_e2e, all_e2e = float("nan"), []
     else:
@@ -380,7 +415,7 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = json.load(open(peaks_path))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
         else:
-            peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3), not measured"
         prof, frames_info = profiling.profile_pointfusion_gt(depth_d, rgb_d, K_d, poses_d, slam.dist_th, slam.dot_th,
                                                              slam.sigma)
         prof, frames_info = profiling.profile_pointfusion_gt(depth_d, rgb_d, K_d, poses_d, slam.dist_th, slam.dot_th,
@@ -398,9 +433,6 @@ def main():
                     "traffic": None, "peak_source": peak_src,
                     "bytes_per_launch": kernels[dom]["algorithmic_MB_per_launch"] * 1e6,
                     "avg_launch_us": kernels[dom]["avg_us"]}
-        tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tpath):  # dram bytes per launch from the committed ncu --set full capture
-            roofline["traffic"] = json.load(open(tpath)).get(dom)
 
     # secondary measurement: the same PointFusion with its default ICP odometry (gradLM, 20 iterations, dsratio 4),
     # on a corner-facing variant of the scene (yaw0=0.6) where point-to-plane ICP is well conditioned; plus the

@@ -1,4 +1,4 @@
-"""gradslam_b200 — a Blackwell (sm_100a) engine for gradslam's PointFusion / ICPSLAM inner loop.
+"""gradslam_b200 — a Hopper (sm_90a) engine for gradslam's PointFusion / ICPSLAM inner loop.
 
 Drop-in for the hot path of gradslam/gradslam: `RGBDImages`, `Pointclouds`, `PointFusion`, `ICPSLAM`, the
 odometry providers and the `fusionutils` / `icputils` functions keep the reference's names, arguments and

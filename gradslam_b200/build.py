@@ -1,4 +1,4 @@
-"""Builds gradslam_b200/_lib/libgsx.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds gradslam_b200/_lib/libgsx.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import glob
 import os
 import subprocess
@@ -10,7 +10,7 @@ OUT = os.path.join(_HERE, "_lib", "libgsx.so")
 
 # -fmad=false: the kernels' decisions must be bit-identical to the CPU oracle (no FMA contraction).
 # Where an FMA is wanted (the float64 polynomial of gsx_exp.cuh, the dual-number refinements) it is written as fma().
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC"]
 
 

@@ -1,4 +1,4 @@
-// Shared device helpers for libgsx (sm_100a).  Compiled with -fmad=false: every product and sum below
+// Shared device helpers for libgsx (sm_90a).  Compiled with -fmad=false: every product and sum below
 // is rounded separately to fp32, in the association order written, so results are bit-identical to the
 // CPU oracle's canonical arithmetic (oracle/gsx_oracle.py).
 #pragma once
@@ -28,7 +28,7 @@ void set_error(const char *fmt, ...);
     }                                                                             \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 struct Rigid {  // row-major rotation + translation of a 4x4 rigid transform
   float r[9];

@@ -1,4 +1,4 @@
-// Fused PointFusion map update for sm_100a.
+// Fused PointFusion map update for sm_90a.
 //   k_frame_records   (K1r)    one thread per live pixel: world-frame vertex / normal, confidence weight and depth of the
 //                              pixel as ONE 32-byte record (the whole op chain of rgbdimages.py:643-762 and
 //                              fusionutils.py:16-73, evaluated once per pixel); also re-arms the per-frame workspace.
@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
   }
   if (pend_pix >= 0) atomic_max_rec128_finish(best + pend_pix, mine, old);
   // bookkeeping for the roofline's algorithmic-byte count: ONE atomic per CTA (every warp of the grid adding to the same
-  // address serialises in the L2: 9472 same-address atomics cost ~20 us when the whole grid works on one map)
+  // address would serialise thousands of same-address atomics in the L2 when the whole grid works on one map)
   n_active = __reduce_add_sync(0xffffffffu, n_active);
   if ((threadIdx.x & 31) == 0) s_act[threadIdx.x >> 5] = n_active;
   __syncthreads();
@@ -386,8 +386,9 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
   }
 }
 
+// H100, bench workload: 24 beat 12 by 1.2 % and 9 by 2.3 % (spread 0.2 %, DESIGN.md section 4)
 #ifndef GSX_K2_CTAS_PER_SM
-#define GSX_K2_CTAS_PER_SM 8
+#define GSX_K2_CTAS_PER_SM 24
 #endif
 
 int launch_project_select(const ProjectArgs &a, int64_t max_count, cudaStream_t stream) {

@@ -1,4 +1,4 @@
-// Point-to-plane ICP / gradICP odometry for sm_100a, batched over B elements, no host synchronisation.
+// Point-to-plane ICP / gradICP odometry for sm_90a, batched over B elements, no host synchronisation.
 //
 //   k_icp_gather_src     live frame -> source cloud: lattice pixels (every ds-th row/column) with valid depth,
 //                        world-frame vertex at the PREVIOUS pose, stable row-major compaction

@@ -1,4 +1,4 @@
-// Differentiable small ops of the ICP / gradICP loop for sm_100a (K7 forward + backward, and the rigid transform of
+// Differentiable small ops of the ICP / gradICP loop for sm_90a (K7 forward + backward, and the rigid transform of
 // the source cloud).  They replace the ~80 tiny ATen kernels per iteration that PyTorch's tape records for
 //   solve_linear_system      gradslam/odometry/icputils.py:22-90
 //   se3_exp                  gradslam/geometry/se3utils.py:77-115

@@ -6,7 +6,7 @@ while the L frames are fused.  The only exchange is at the end: an all-gather of
 followed by a variable-length all-gather of the fused maps, after which every rank holds all B_total maps.  The maps
 travel as they are stored - packed geometry rows (8 floats) and colour rows (4 floats) - and are received in place in the
 output store, no zero fill on either side.  Three transports; GSX_MAP_EXCHANGE=auto (default) takes `peer` between two
-GPUs and `all_gather` beyond, as measured (see _exchange_mode, DESIGN.md section 7):
+GPUs and `all_gather` beyond (see _exchange_mode):
 
   peer        each rank PULLS its peers' rows out of their stores (CUDA IPC mappings) with one pitched copy per peer and
               row array, executed by the copy engines over NVLink: no communication kernel on any SM, no staging copy
@@ -82,9 +82,9 @@ def _control_group(group, device):
     """The process group the exchange's two tiny collectives (sizes + store descriptors before the pulls, the one-word
     release after them) run on: the same ranks as `group`, but a communicator whose kernels are launched on a
     HIGH-PRIORITY stream.  On an ordinary stream a NCCL kernel queues behind the thousands of thread blocks the two
-    fusion streams keep pending and only gets onto an SM when a step drains - measured at 2 GPUs: the size all-gather of
-    step k completed at the END of step k+1, the host (waiting for the sizes) enqueued step k+2 late, and the GPU idled
-    0.8 ms per step.  Created once per group (a collective call: every rank reaches gather_maps_begin)."""
+    fusion streams keep pending and only gets onto an SM when a step drains: the size all-gather of step k then completes
+    at the END of step k+1, the host (waiting for the sizes) enqueues step k+2 late, and the GPU idles before each step.
+    Created once per group (a collective call: every rank reaches gather_maps_begin)."""
     if device.type != "cuda" or os.environ.get("GSX_EXCHANGE_PRIORITY", "high") != "high":
         return group
     key = (id(group) if group is not None else None, str(device))
@@ -271,10 +271,8 @@ def gather_maps_end(h: "_GatherHandle", wait: bool = True) -> Pointclouds:
 
 def _exchange_mode(device=None, world=None):
     """GSX_MAP_EXCHANGE = auto | peer | all_gather | p2p.  CPU tensors (the gloo tests) always use all_gather.  `auto`
-    (default) follows the measurements of DESIGN.md section 7: copy-engine pulls between TWO GPUs (7.16 ms per step against
-    8.02 for the collective), NCCL all-gather beyond (4 GPUs: 7.73 ms against 8.26 for the pulls - NCCL's ring keeps one
-    sender per receiver and, on NVSwitch, can multicast; the serial pulls of one rank cost the concurrent fusion kernels
-    more than they cost NCCL's throttled copy kernels)."""
+    (default): copy-engine pulls between TWO GPUs, NCCL all-gather beyond (timed on an earlier GPU generation, not on
+    H100; DESIGN.md section 7)."""
     if device is not None and torch.device(device).type != "cuda":
         return "all_gather"
     mode = os.environ.get("GSX_MAP_EXCHANGE", "auto")
@@ -307,8 +305,7 @@ def _exchange_peer(pc, out, counts, meta, rank, world, B, group, stream, skip_ow
     pitch_rows = out.capacity  # row stride of the receiving store's elements
     with torch.cuda.device(dev):
         # rank r pulls from r+1, r+2, ... (mod world): at any moment every owner serves ONE reader.  With the same order
-        # on every rank all of them read owner 0 first, then owner 1, ... and share that one GPU's NVLink egress - measured
-        # at 8 GPUs: 20.3 ms per step instead of ~7.
+        # on every rank all of them read owner 0 first, then owner 1, ... and share that one GPU's NVLink egress.
         for q in [(rank + 1 + i) % world for i in range(world)]:
             nq = max(counts[q * B:(q + 1) * B])
             if nq == 0 or (skip_own and q == rank):

@@ -1,7 +1,7 @@
 """PointFusion map update: projective data association + confidence-weighted surfel fusion.
 
 Host-side mirror of gradslam/slam/fusionutils.py (same function names, arguments, return types, errors and
-warnings).  `update_map_fusion` runs as two hand-written sm_100a kernels over an in-place, capacity-backed
+warnings).  `update_map_fusion` runs as two hand-written sm_90a kernels over an in-place, capacity-backed
 map (csrc/gsx_fusion.cu): no table is materialised, no whole-map clone / cat per frame, no host sync.  The
 table-returning helpers (`find_active_map_points`, `find_similar_map_points`,
 `find_best_unique_correspondences`, `fuse_with_map`) are kept for API parity and run the same arithmetic

@@ -2,7 +2,7 @@
 
 Host-side mirror of gradslam.slam.ICPSLAM (gradslam/slam/icpslam.py:16-264): same constructor keywords and
 defaults, `forward(frames) -> (Pointclouds, poses[B,L,4,4])`, `step(pointclouds, live_frame, prev_frame,
-inplace)`.  The per-frame work runs in the sm_100a kernels of libgsx; with `odom='gt'` a whole sequence is
+inplace)`.  The per-frame work runs in the sm_90a kernels of libgsx; with `odom='gt'` a whole sequence is
 one C call (gsx_pointfusion_sequence_gt) with no host synchronisation between frames.
 """
 import warnings

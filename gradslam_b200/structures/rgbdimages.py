@@ -1,7 +1,7 @@
 """RGBDImages: batched RGB-D sequence container with lazily computed vertex / normal maps.
 
 Host-side mirror of gradslam.RGBDImages (gradslam/structures/rgbdimages.py:13-915): same constructor,
-properties, indexing and error behaviour.  The four cached maps are produced by ONE hand-written sm_100a
+properties, indexing and error behaviour.  The four cached maps are produced by ONE hand-written sm_90a
 kernel (gsx_backproject_normals_fwd) instead of the reference's einsum / slice / cross / norm chain
 (rgbdimages.py:643-762).  Containers may hold tensors on any device, but computing a map requires CUDA
 tensors: there is no CPU compute path.

@@ -1,4 +1,4 @@
-/* gsx.h — C ABI of libgsx.so, the B200 (sm_100a) engine behind gradslam's PointFusion / ICPSLAM hot path.
+/* gsx.h — C ABI of libgsx.so, the H100 (sm_90a) engine behind gradslam's PointFusion / ICPSLAM hot path.
  *
  * gradslam (reference @44470ee) is pure Python on PyTorch tensor ops: it has no FFI/plugin layer of its
  * own.  The boundary a maintainer would bind is therefore the set of tensor-op chains listed below; each

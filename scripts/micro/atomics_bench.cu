@@ -1,5 +1,5 @@
-// Calibration micro-benchmark (B200): cost of N scattered 32-bit reductions / CAS / 128-bit CAS / 32-byte gathers with the
-// access pattern of the association kernel (mostly consecutive targets with gaps).   nvcc -arch=sm_100a -O3 -o ab atomics_bench.cu
+// Calibration micro-benchmark: cost of N scattered 32-bit reductions / CAS / 128-bit CAS / 32-byte gathers with the
+// access pattern of the association kernel (mostly consecutive targets with gaps).   nvcc -arch=sm_90a -O3 -o ab atomics_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -13,7 +13,7 @@ def pytest_configure(config):
     import torch
 
     torch.set_num_threads(min(8, os.cpu_count() or 1))  # the oracle's small CPU ops crawl with 100+ threads
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session", autouse=True)
