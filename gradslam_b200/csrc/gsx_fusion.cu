@@ -391,10 +391,15 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
 #define GSX_K2_CTAS_PER_SM 24
 #endif
 
+// Test hook (tests/test_gpu_coverage.py): caps K2's total CTA count so that small maps take several grid-stride
+// passes.  0 = the shipped cap below.
+static int g_k2_grid_cap = 0;
+
 int launch_project_select(const ProjectArgs &a, int64_t max_count, cudaStream_t stream) {
   if (a.B == 0 || max_count <= 0) return 0;
   int64_t bx = (max_count + kBlock - 1) / kBlock;
-  const int64_t cap_blocks = (int64_t)kNumSMs * GSX_K2_CTAS_PER_SM;  // grid-stride beyond this many CTAs per SM
+  // grid-stride beyond this many CTAs per SM
+  const int64_t cap_blocks = g_k2_grid_cap > 0 ? (int64_t)g_k2_grid_cap : (int64_t)kNumSMs * GSX_K2_CTAS_PER_SM;
   if (bx * a.B > cap_blocks) bx = (cap_blocks + a.B - 1) / a.B;
   if (bx < 1) bx = 1;
   k_project_select<<<dim3((unsigned)bx, (unsigned)a.B), kBlock, 0, stream>>>(a);
@@ -852,6 +857,8 @@ extern "C" int gsx_fusion_project_select(const float *map_geometry, const int32_
                 (float)(W - 0.999), (float)(H - 0.999), sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
   return launch_project_select(a, max_count, (cudaStream_t)stream);
 }
+
+extern "C" void gsx_debug_set_k2_grid_cap(int ctas) { g_k2_grid_cap = ctas > 0 ? ctas : 0; }
 
 extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_ccounts,
                                        const int32_t *counts_in, int32_t *counts_out, int64_t capacity,

@@ -325,13 +325,14 @@ __global__ void __launch_bounds__(256) k_grid_clear(TargetGrid g, int B) {
 __global__ void __launch_bounds__(256) k_grid_count(const float *tgt_p, const int32_t *tgt_count, int nt_stride,
                                                     TargetGrid g) {
   const int b = blockIdx.y;
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  if (i >= tgt_count[b]) return;
+  const int nt = tgt_count[b];
   const GridParams gp = g.params[b];
-  const float *p = tgt_p + ((int64_t)b * nt_stride + i) * 3;
-  const int cx = cell_coord(__ldg(p), gp.ox, gp.inv_c, gp.nx), cy = cell_coord(__ldg(p + 1), gp.oy, gp.inv_c, gp.ny),
-            cz = cell_coord(__ldg(p + 2), gp.oz, gp.inv_c, gp.nz);
-  atomicAdd(g.cursor + (int64_t)b * kGridMaxCells + (cz * gp.ny + cy) * gp.nx + cx, 1);
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < nt; i += gridDim.x * 256) {
+    const float *p = tgt_p + ((int64_t)b * nt_stride + i) * 3;
+    const int cx = cell_coord(__ldg(p), gp.ox, gp.inv_c, gp.nx), cy = cell_coord(__ldg(p + 1), gp.oy, gp.inv_c, gp.ny),
+              cz = cell_coord(__ldg(p + 2), gp.oz, gp.inv_c, gp.nz);
+    atomicAdd(g.cursor + (int64_t)b * kGridMaxCells + (cz * gp.ny + cy) * gp.nx + cx, 1);
+  }
 }
 
 __global__ void __launch_bounds__(1024) k_grid_scan(TargetGrid g) {
@@ -372,15 +373,16 @@ __global__ void __launch_bounds__(1024) k_grid_scan(TargetGrid g) {
 __global__ void __launch_bounds__(256) k_grid_scatter(const float *tgt_p, const int32_t *tgt_count, int nt_stride,
                                                       TargetGrid g) {
   const int b = blockIdx.y;
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  if (i >= tgt_count[b]) return;
+  const int nt = tgt_count[b];
   const GridParams gp = g.params[b];
-  const float *p = tgt_p + ((int64_t)b * nt_stride + i) * 3;
-  const float x = __ldg(p), y = __ldg(p + 1), z = __ldg(p + 2);
-  const int cx = cell_coord(x, gp.ox, gp.inv_c, gp.nx), cy = cell_coord(y, gp.oy, gp.inv_c, gp.ny),
-            cz = cell_coord(z, gp.oz, gp.inv_c, gp.nz);
-  const int pos = atomicAdd(g.cursor + (int64_t)b * kGridMaxCells + (cz * gp.ny + cy) * gp.nx + cx, 1);
-  g.sorted[(int64_t)b * nt_stride + pos] = make_float4(x, y, z, __int_as_float(i));
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < nt; i += gridDim.x * 256) {
+    const float *p = tgt_p + ((int64_t)b * nt_stride + i) * 3;
+    const float x = __ldg(p), y = __ldg(p + 1), z = __ldg(p + 2);
+    const int cx = cell_coord(x, gp.ox, gp.inv_c, gp.nx), cy = cell_coord(y, gp.oy, gp.inv_c, gp.ny),
+              cz = cell_coord(z, gp.oz, gp.inv_c, gp.nz);
+    const int pos = atomicAdd(g.cursor + (int64_t)b * kGridMaxCells + (cz * gp.ny + cy) * gp.nx + cx, 1);
+    g.sorted[(int64_t)b * nt_stride + pos] = make_float4(x, y, z, __int_as_float(i));
+  }
 }
 
 // Exact nearest neighbour of (sx,sy,sz) through the grid.  Candidates are compared on (squared distance, original
@@ -582,7 +584,8 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_knn_linearize(KnnArgs a) {
   if (use && a.use_thresh) use = best < a.dist_thresh;
   if (a.nn_idx && valid) {
     a.nn_idx[(int64_t)b * a.ns_stride + i] = use ? (int64_t)bi : -1;
-    if (a.nn_d2) a.nn_d2[(int64_t)b * a.ns_stride + i] = best;
+    // an empty target has no neighbour: idx -1 and distance +inf, like the padding rows
+    if (a.nn_d2) a.nn_d2[(int64_t)b * a.ns_stride + i] = bi >= 0 ? best : __int_as_float(0x7f800000);
   }
   float acc[kNumSums];
 #pragma unroll
@@ -928,6 +931,13 @@ inline IcpWorkspace icp_carve(void *ws, int B, int H, int W, int ds, int64_t map
 // runs the LM / gradLM loop on clouds that are already in place
 constexpr int kGridThreshold = 4096;  // target clouds up to this size use the shared-memory brute force
 
+// CTAs per element of the grid count / scatter kernels (grid-stride loops over the target's actual size: the stride
+// of the target buffer is a loose upper bound, e.g. the whole map for the ICP target)
+inline unsigned grid_fill_blocks(int nt_stride) {
+  const int nb = (nt_stride + 255) / 256;
+  return (unsigned)(nb < 128 ? nb : 128);
+}
+
 inline int64_t grid_bytes(int B, int nt_stride) {
   if (nt_stride <= kGridThreshold) return 0;
   return up256((int64_t)B * sizeof(GridParams)) + up256((int64_t)B * (kGridMaxCells + 1) * 4) +
@@ -960,7 +970,7 @@ int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const floa
   const bool use_grid = grid_mem != nullptr && nt_stride > kGridThreshold;
   if (use_grid) {  // the target is fixed for the whole loop: bin it once
     ka.grid = grid_carve(grid_mem, B, nt_stride);
-    const unsigned nb = (unsigned)((nt_stride + 255) / 256);
+    const unsigned nb = grid_fill_blocks(nt_stride);
     k_grid_bbox<<<B, 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, ka.grid);
     k_grid_clear<<<(unsigned)(((int64_t)B * kGridMaxCells + 255) / 256), 256, 0, stream>>>(ka.grid, B);
     k_grid_count<<<dim3(nb, (unsigned)B), 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, ka.grid);
@@ -1114,7 +1124,7 @@ extern "C" int gsx_knn1(const float *src_points, const int32_t *src_count, int n
   if (nt_stride > kGridThreshold) {
     ka.grid = grid_carve((char *)scratch + part, B, nt_stride);
     if (build_grid) {  // (0: `scratch` still holds the grid a previous call built for this very target)
-      const unsigned nb = (unsigned)((nt_stride + 255) / 256);
+      const unsigned nb = grid_fill_blocks(nt_stride);
       k_grid_bbox<<<B, 256, 0, s>>>(tgt_points, tgt_count, nt_stride, ka.grid);
       k_grid_clear<<<(unsigned)(((int64_t)B * kGridMaxCells + 255) / 256), 256, 0, s>>>(ka.grid, B);
       k_grid_count<<<dim3(nb, (unsigned)B), 256, 0, s>>>(tgt_points, tgt_count, nt_stride, ka.grid);

@@ -636,6 +636,23 @@ class _IcpWorkspace:
         return self.epoch
 
 
+class _IcpTargetScratch:
+    """Target clouds (points, normals, search grid) of localize_against_map, cached per (device, B) and grown by
+    doubling: calls are stream-ordered, so one buffer serves every call on the device."""
+    _cache = {}
+
+    @classmethod
+    def get(cls, device, B, tgt_capacity):
+        key = (str(device), B)
+        buf = cls._cache.get(key)
+        need = _C.lib().gsx_icp_tgt_scratch_bytes(B, tgt_capacity)
+        if buf is None or buf.numel() < need:
+            grown = _C.lib().gsx_icp_tgt_scratch_bytes(B, min(2 * tgt_capacity, 1 << 29))
+            buf = torch.empty(max(need, grown), dtype=torch.uint8, device=device)
+            cls._cache[key] = buf
+        return buf
+
+
 def localize_against_map(pointclouds, live_frame, prev_frame, dsratio, odomprov):
     """ICPSLAM._localize for odom in {icp, gradicp} (slam/icpslam.py:238-247) as ONE C call: gathers the source
     (live frame on the ds lattice at the previous pose) and target (lattice-active map points) clouds, runs the
@@ -650,11 +667,11 @@ def localize_against_map(pointclouds, live_frame, prev_frame, dsratio, odomprov)
     _C.require_cuda(pointclouds._geo, "pointclouds (geometry rows)")
     geo = pointclouds._geo.contiguous()
     ws = _IcpWorkspace.get(dev, B, H, W, dsratio, pointclouds.capacity)
-    # target capacity: lattice-active map points.  32 map points per lattice pixel on average is far beyond
-    # anything a surfel map produces; if it is ever exceeded the kernel raises the map's overflow flag.
-    ns_cap = ((H + dsratio - 1) // dsratio) * ((W + dsratio - 1) // dsratio)
-    bound = max(1, min(pointclouds._bound, 32 * ns_cap))
-    tgt = torch.empty(_C.lib().gsx_icp_tgt_scratch_bytes(B, bound), dtype=torch.uint8, device=dev)
+    # target capacity: the lattice-active map points are a subset of the map, so the map's host-side size bound holds
+    # every target.  No per-pixel bound would do: ICPSLAM's aggregate map gains a point on every lattice pixel of every
+    # frame, so a camera that dwells piles up one more point per lattice pixel per frame.
+    bound = max(1, pointclouds._bound)
+    tgt = _IcpTargetScratch.get(dev, B, bound)
     out = torch.empty((B, 1, 4, 4), dtype=torch.float32, device=dev)
     mode = 1 if hasattr(odomprov, "lambda_max") else 0
     dth = odomprov.dist_thresh

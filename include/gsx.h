@@ -155,6 +155,9 @@ int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t 
                                 float dot_th, double sigma, void *workspace, int32_t *overflow_flag, void *stream);
 /* test hook: the next gsx_pointfusion_sequence_gt call reports a launch failure at frame s (once); -1 = off */
 void gsx_debug_fail_at_frame(int s);
+/* test hook: caps the total CTA count of the map projection kernel (K2), so that small maps take several grid-stride
+ * passes; 0 = the default cap.  Results do not depend on it. */
+void gsx_debug_set_k2_grid_cap(int ctas);
 
 /* ------------------------------------------------------------------------------------------------
  * Map exchange between the GPUs of a node through peer memory (SURVEY.md section 8e "Collective": the variable-length
@@ -247,7 +250,7 @@ int gsx_records_from_table(const int64_t *table, int64_t rows, int64_t capacity,
  * reference does (icputils.py:206).  Exact 1-NN ties resolve to the lowest target index.            */
 
 /* exact nearest neighbour of every source point: idx_out int64 (B, ns_stride) (-1 for rows >= size or an
- * empty target), d2_out squared distance (may be NULL).  scratch: gsx_knn1_scratch_bytes bytes.
+ * empty target), d2_out squared distance (may be NULL; +inf for an empty target).  scratch: gsx_knn1_scratch_bytes bytes.
  * Target clouds with nt_stride > 4096 are binned into a uniform grid and searched ring by ring with an exact
  * termination bound (full scan as the fallback); smaller ones are scanned from shared memory.  Both return
  * the same (distance, index): candidates are ordered by (squared distance, index).

@@ -125,6 +125,67 @@ def test_fullsize_properties():
     assert a.points_padded[~a.nonpad_mask].abs().sum() == 0
 
 
+def test_bench_configuration_matches_oracle(tmp_path):
+    """Exactly the inputs rank 0 of bench.py fuses (B=8, L=32, 640x480, seed 0), device-resident, one whole-sequence
+    call.  Elements 0 and 7 (the first of batch group 0, the last of group 1) equal the oracle bit for bit
+    (GSX_FULLSIZE_ALL=1: all eight, ~4 min of oracle).  The maps outgrow three K2 grid-stride passes.  The host-fed call,
+    the read-back on a side stream and bench.dump_outputs give the same rows."""
+    import os
+
+    import numpy as np
+
+    import bench
+    import gradslam_b200 as gs
+
+    B, L = 8, 32
+    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=0)
+    slam = gs.PointFusion(odom="gt", device=DEV)
+    pc, out_poses = slam(_frames(gs, rgb, depth, K, poses))
+    counts = [int(c) for c in pc.num_points_per_pointcloud.tolist()]
+    # K2's shipped cap: 132 SMs x 24 CTAs shared by the B elements, 256 threads each
+    rows_per_pass = 256 * -(-132 * 24 // B)
+    assert max(counts) > 2 * rows_per_pass
+
+    checked = list(range(B)) if os.environ.get("GSX_FULLSIZE_ALL") == "1" else [0, B - 1]
+    ref = oracle.run_slam(rgb[checked], depth[checked], K[checked], poses[checked], odom="gt").map
+    for i, b in enumerate(checked):
+        assert counts[b] == ref.counts()[i], b
+        assert torch.equal(pc.points_list[b].cpu(), ref.points[i]), b
+        assert torch.equal(pc.normals_list[b].cpu(), ref.normals[i]), b
+        assert torch.equal(pc.colors_list[b].cpu(), ref.colors[i]), b
+        assert torch.equal(pc.features_list[b].cpu(), ref.ccounts[i]), b
+
+    # --dump-outputs: the sampled rows of the checked sequences are the oracle's rows at the listed indices
+    bench.dump_outputs(str(tmp_path), pc, out_poses)
+    rows = np.load(tmp_path / "map_rows.npy")
+    dumped = {k: torch.from_numpy(np.load(tmp_path / (k + ".npy"))) for k in ("points", "normals", "colors", "features")}
+    assert torch.equal(torch.from_numpy(np.load(tmp_path / "poses.npy")), out_poses.cpu())
+    for i, b in enumerate(checked):
+        sel = torch.from_numpy(rows[:, 0] == b)
+        idx = torch.from_numpy(rows[:, 1]).long()[sel]
+        assert idx.numel() > 0
+        assert torch.equal(dumped["points"][sel], ref.points[i][idx]), b
+        assert torch.equal(dumped["normals"][sel], ref.normals[i][idx]), b
+        assert torch.equal(dumped["colors"][sel], ref.colors[i][idx]), b
+        assert torch.equal(dumped["features"][sel], ref.ccounts[i][idx]), b
+
+    # host-fed frames (pinned, uploaded in chunks on a side stream) and the read-back on a side stream
+    host = gs.RGBDImages(rgb.pin_memory(), depth.pin_memory(), K.pin_memory(), poses.pin_memory())
+    pc_host, _ = slam(host)
+    assert [int(c) for c in pc_host.num_points_per_pointcloud.tolist()] == counts
+    side = torch.cuda.Stream(device=DEV)
+    side.wait_stream(torch.cuda.current_stream(DEV))
+    down = pc.download(stream=side)
+    side.synchronize()
+    assert down._host_counts() == counts
+    for b in range(B):
+        n = counts[b]
+        assert torch.equal(pc_host._geo[b, :n], pc._geo[b, :n]), b
+        assert torch.equal(pc_host._col[b, :n], pc._col[b, :n]), b
+        assert torch.equal(down._geo[b, :n], pc._geo[b, :n].cpu()), b
+        assert torch.equal(down._col[b, :n], pc._col[b, :n].cpu()), b
+
+
 def test_fullsize_icp_localisation_matches_oracle():
     """One ICP-localised step at 640x480 (dsratio 4 => 19 200 source points, grid 1-NN): pose within 1e-4."""
     import gradslam_b200 as gs
