@@ -30,6 +30,25 @@ void set_error(const char *fmt, ...);
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
+// floats per packed map row / frame record (DESIGN.md section 2): geometry (px,py,pz,nx,ny,nz,ccount,0), colour
+// (r,g,b,0), frame record (gvx,gvy,gvz,gnx,gny,gnz,alpha,depth)
+constexpr int kGeoW = 8, kColW = 4, kRecW = 8;
+
+// Scratch and workspace layouts are each written once, as a function that walks a Carver over the allocation:
+// take<T>(n) hands out the next 256-byte aligned slot of n T's.  Given the allocation's base the function returns
+// pointers; given nullptr the pointers are the slots' byte offsets, and `bytes` is the size the allocation needs.
+struct Carver {
+  uintptr_t base;
+  int64_t bytes = 0;
+  explicit Carver(void *p) : base(reinterpret_cast<uintptr_t>(p)) {}
+  template <class T>
+  T *take(int64_t n) {
+    T *p = reinterpret_cast<T *>(base + bytes);
+    bytes += (n * (int64_t)sizeof(T) + 255) / 256 * 256;
+    return p;
+  }
+};
+
 struct Rigid {  // row-major rotation + translation of a 4x4 rigid transform
   float r[9];
   float t[3];
@@ -237,43 +256,6 @@ __device__ __forceinline__ U128 cas128(U128 *addr, U128 expected, U128 desired) 
   return old;
 }
 
-// ---- L2 residency hints (createpolicy + .L2::cache_hint) -----------------------------------------------------------
-// The per-frame arg-min records are hit by scattered read-modify-writes; if their sectors have left the L2 every one of
-// them becomes a DRAM read + write-back.  Streaming data (map rows, colours) is therefore loaded evict-first and the
-// records are touched evict-last, so the records of the frame in flight stay resident.
-__device__ __forceinline__ unsigned long long l2_policy_evict_last() {
-  unsigned long long p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ unsigned long long l2_policy_evict_first() {
-  unsigned long long p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ float4 ldg128_hint(const float *addr, unsigned long long pol) {
-  float4 v;
-  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-               : "l"(addr), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ float2 ldg64_hint(const float *addr, unsigned long long pol) {
-  float2 v;
-  asm volatile("ld.global.nc.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(v.x), "=f"(v.y) : "l"(addr), "l"(pol));
-  return v;
-}
-__device__ __forceinline__ void stg128_hint(float *addr, const float4 &v, unsigned long long pol) {
-  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z),
-               "f"(v.w), "l"(pol)
-               : "memory");
-}
-__device__ __forceinline__ U128 load128_relaxed(const U128 *addr) {
-  U128 v;
-  asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(v.lo), "=l"(v.hi) : "l"(addr) : "memory");
-  return v;
-}
-
 __device__ __forceinline__ bool rec_greater(const U128 &a, const U128 &b) {
   return a.hi > b.hi || (a.hi == b.hi && a.lo > b.lo);
 }
@@ -297,6 +279,142 @@ __device__ __forceinline__ void atomic_min_key128(U128 *addr, unsigned long long
     if (old.hi == cur.hi && old.lo == cur.lo) break;
     cur = old;
   }
+}
+
+// High word of the arg-min key of find_best_unique_correspondences (fusionutils.py:491-517): 1/(cc+1e-20), then the
+// squared distance d2 >= 0.  Positive floats order like their bit patterns; negatives are flipped so the order stays total.
+__device__ __forceinline__ unsigned long long argmin_key_hi(float cc, float d2) {
+  const float inv_cc = 1.0f / (cc + 1e-20f);
+  unsigned int kb = __float_as_uint(inv_cc);
+  kb = (kb & 0x80000000u) ? ~kb : (kb | 0x80000000u);
+  const unsigned int rb = __float_as_uint(d2) | 0x80000000u;
+  return ((unsigned long long)kb << 32) | rb;
+}
+
+// ---- projection of a map point into the live camera (fusionutils.py:249-274) ----------------------------------------
+struct ImageBounds {  // frustum limits of an H x W image (kernel argument)
+  float u_hi, v_hi;   // float(W - 0.999), float(H - 0.999)
+  int H, W;
+};
+inline ImageBounds image_bounds(int H, int W) { return ImageBounds{(float)(W - 0.999), (float)(H - 0.999), H, W}; }
+
+struct LiveCamera {  // per CTA, in shared memory: world -> camera (T^-1) and the first three rows of the 4x4 K
+  Rigid tinv;
+  float k[12];
+};
+// Camera of batch element b.  Called by every thread (thread 0 loads T^-1, threads 32..43 the K entries); the caller
+// synchronises.
+__device__ __forceinline__ void load_live_camera(LiveCamera &c, const float *poses, int64_t pose_bstride,
+                                                 const float *K, int64_t K_bstride, int b) {
+  if (threadIdx.x == 0) c.tinv = rigid_inverse(load_rigid(poses + b * pose_bstride));
+  if (threadIdx.x >= 32 && threadIdx.x < 44) c.k[threadIdx.x - 32] = __ldg(K + b * K_bstride + (threadIdx.x - 32));
+}
+
+struct PixelHit {
+  bool in_frustum;
+  int h, w;  // pixel under the projection, clamped to the image
+};
+// world -> camera (pointclouds.py:526-573), pinhole projection with the 4x4 K on the homogeneous point
+// (projutils.py:92-238; z == 0 divides by 1), frustum test, round-half-even like torch.round, then clamp
+__device__ __forceinline__ PixelHit project(const LiveCamera &c, const ImageBounds &ib, float x, float y, float z) {
+  const float3 q = rigid_apply(c.tinv, x, y, z);
+  const float hx = ((c.k[0] * q.x + c.k[1] * q.y) + c.k[2] * q.z) + c.k[3];
+  const float hy = ((c.k[4] * q.x + c.k[5] * q.y) + c.k[6] * q.z) + c.k[7];
+  const float hz = ((c.k[8] * q.x + c.k[9] * q.y) + c.k[10] * q.z) + c.k[11];
+  const float den = (hz != 0.0f) ? hz : 1.0f;
+  const float u = hx / den, v = hy / den;
+  PixelHit r;
+  r.in_frustum = (u > -1e-3f) && (u < ib.u_hi) && (v > -1e-3f) && (v < ib.v_hi) && (q.z > 0.0f);
+  r.w = min(max((int)rintf(u), 0), ib.W - 1);
+  r.h = min(max((int)rintf(v), 0), ib.H - 1);
+  return r;
+}
+
+// ---- stable compaction by single-pass decoupled look-back --------------------------------------------------------
+// A scan runs one CTA per tile.  Each tile owns a 64-bit state word  epoch<<34 | flag<<32 | value : flag kTileAggregate
+// = `value` counts the tile's own items, kTilePrefix = `value` counts the items of every tile up to and including it.
+// A word of another epoch reads as "not yet published": a scan passes a fresh epoch per launch, or zeroes its words
+// before each launch and passes epoch 1.  The last tile publishes nothing (no tile waits for it).
+constexpr unsigned long long kTileAggregate = 1ull, kTilePrefix = 2ull;
+
+__device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long long *p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_u64(unsigned long long *p, unsigned long long v) {
+  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+__device__ __forceinline__ void publish_tile(unsigned long long *state, int tile, int tiles, unsigned int epoch,
+                                             unsigned long long flag, unsigned int value) {
+  if (tile + 1 < tiles) st_release_u64(state + tile, ((unsigned long long)epoch << 34) | (flag << 32) | value);
+}
+
+// Called by one whole warp once the tile's aggregate `total` is published: returns the tile's exclusive prefix (32
+// predecessors per step, back to the nearest one that knows its inclusive prefix); lane 0 then publishes the tile's
+// inclusive prefix.
+__device__ __forceinline__ unsigned int lookback_warp(unsigned long long *state, int tile, int tiles,
+                                                      unsigned int epoch, unsigned int total) {
+  const int lane = threadIdx.x & 31;
+  unsigned int excl = 0;
+  for (int base = tile - 1; base >= 0; base -= 32) {
+    const int j = base - lane;
+    unsigned long long s = 0ull;
+    if (j >= 0) {
+      do {
+        s = ld_acquire_u64(state + j);
+      } while ((unsigned int)(s >> 34) != epoch);
+    }
+    const bool is_prefix = (j >= 0) && (((s >> 32) & 3ull) == kTilePrefix);
+    const unsigned int pm = __ballot_sync(0xffffffffu, is_prefix);
+    const int first = pm ? (__ffs(pm) - 1) : 32;  // nearest predecessor that already knows its inclusive prefix
+    const unsigned int v = (j >= 0 && lane <= first) ? (unsigned int)s : 0u;
+    excl += __reduce_add_sync(0xffffffffu, v);
+    if (pm) break;
+  }
+  if (lane == 0) publish_tile(state, tile, tiles, epoch, kTilePrefix, excl + total);
+  return excl;
+}
+
+// Dynamic tile id (tiles start in ticket order).  The CTA that draws the last ticket re-arms the counter for the next
+// launch (nobody else touches it any more in this one), so the number of tiles may differ from launch to launch.
+__device__ __forceinline__ int draw_tile_ticket(unsigned int *ticket, int tiles) {
+  const unsigned int t = atomicAdd(ticket, 1u);
+  if (t == (unsigned int)tiles - 1u) *ticket = 0u;
+  return (int)t;
+}
+
+// Stable positions of kPer flags per thread of a kThreads-thread CTA, in row-major order: chunk j, then warp, then lane.
+// flag(j) yields this thread's flag j; it is evaluated right before that flag's warp vote, so the work deciding each flag
+// is interleaved with the votes.  Every thread calls this: it synchronises the CTA once, and runs at_barrier() right
+// after that barrier (CTA-wide work of the caller that needs one).  On return off[j] = the number of set flags before
+// this thread's flag j; returns the CTA's total.  s_count is kPer x (kThreads / 32) ints of shared memory.
+template <int kThreads, int kPer, class Flag, class AtBarrier>
+__device__ __forceinline__ int block_offsets(Flag flag, int (&off)[kPer], int (*s_count)[kThreads / 32],
+                                             AtBarrier at_barrier) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int j = 0; j < kPer; ++j) {
+    const unsigned int ballot = __ballot_sync(0xffffffffu, flag(j));
+    off[j] = __popc(ballot & ((1u << lane) - 1u));
+    if (lane == 0) s_count[j][warp] = __popc(ballot);
+  }
+  __syncthreads();
+  at_barrier();
+  int total = 0;
+#pragma unroll
+  for (int j = 0; j < kPer; ++j) {
+    int excl = total;
+#pragma unroll
+    for (int i = 0; i < kThreads / 32; ++i) {
+      const int c = s_count[j][i];
+      if (i < warp) excl += c;
+      total += c;
+    }
+    off[j] += excl;
+  }
+  return total;
 }
 
 }  // namespace gsx

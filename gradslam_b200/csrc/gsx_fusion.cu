@@ -15,64 +15,13 @@
 
 #include "gsx_common.cuh"
 #include "gsx_exp.cuh"
+#include "gsx_fusion_ws.cuh"
 #include "gsx_thresholds.h"
 #include "../../include/gsx.h"
 
 namespace gsx {
 
 constexpr int kBlock = 256;
-#ifndef GSX_KPIX
-#define GSX_KPIX 2
-#endif
-constexpr int kMB = 256;                  // threads per CTA of the merge/append kernel
-constexpr int kPix = GSX_KPIX;            // pixels per thread
-constexpr int kTilePix = kMB * kPix;      // pixels per merge tile
-constexpr int kGeoW = 8, kColW = 4, kRecW = 8;  // floats per geometry row / colour row / frame record
-
-// ---- workspace layout -----------------------------------------------------------------------------------
-//   float  frec[B][P][8]       frame records (gvx,gvy,gvz,gnx,gny,gnz,alpha,depth)             written by K1r
-//   U128   best[B][P]          complemented arg-min records (0 = empty)                         cleared by K1r
-//   uint64 tile_state[B][T]    (flag<<32 | value) of the look-back scan, T = ceil(P / kTilePix) cleared by K1r
-//   uint32 ticket[B]           dynamic tile ids of K4                                           cleared by K1r
-//   uint64 stats[B][2]         running totals: {active map rows (in frustum), merged rows}      caller zeroes once
-// Nothing in here has to survive from one frame to the next (the stats are bookkeeping only): every frame's K1r
-// re-arms what K2 / K4 of that frame consume, so a failed or abandoned call cannot poison a later one.
-struct Workspace {
-  float *frec;
-  U128 *best;
-  unsigned long long *tile_state;
-  unsigned int *ticket;
-  unsigned long long *stats;
-  int tiles;
-};
-
-__host__ __device__ inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
-
-inline Workspace carve(void *ws, int B, int H, int W) {
-  const int64_t P = (int64_t)H * W;
-  Workspace w;
-  w.tiles = (int)((P + kTilePix - 1) / kTilePix);
-  char *p = (char *)ws;
-  w.frec = (float *)p;
-  p += align_up(B * P * 32, 256);
-  w.best = (U128 *)p;
-  p += align_up(B * P * 16, 256);
-  w.tile_state = (unsigned long long *)p;
-  p += align_up((int64_t)B * w.tiles * 8, 256);
-  w.ticket = (unsigned int *)p;
-  p += align_up((int64_t)B * 4, 256);
-  w.stats = (unsigned long long *)p;
-  return w;
-}
-
-inline int64_t stats_offset(int B, int H, int W) {
-  const int64_t P = (int64_t)H * W;
-  const int64_t tiles = (P + kTilePix - 1) / kTilePix;
-  return align_up(B * P * 32, 256) + align_up(B * P * 16, 256) + align_up(B * tiles * 8, 256) +
-         align_up((int64_t)B * 4, 256);
-}
-
-inline int64_t workspace_bytes(int B, int H, int W) { return stats_offset(B, H, W) + align_up((int64_t)B * 16, 256); }
 
 // alpha = clamp(exp(-|v|^2 / 2 sigma^2), 1e-7, 1.01) (fusionutils.py:69-72).  The exponential is evaluated in double and
 // rounded once: that is the correctly rounded float32 exp (up to 2^-29 odds), so the CUDA path and the CPU oracle agree
@@ -275,9 +224,10 @@ struct ProjectArgs {
   int64_t pose_bstride;
   const float *K;
   int64_t K_bstride;
-  int B, H, W;
-  float dot_th, u_hi, v_hi;  // u_hi = float(W - 0.999), v_hi = float(H - 0.999)
-  float d2_max;              // largest float x with sqrtf(x) < dist_th (-1 if none): sqrtf(d2) < dist_th <=> d2 <= d2_max
+  int B;
+  ImageBounds ib;
+  float dot_th;
+  float d2_max;  // largest float x with sqrtf(x) < dist_th (-1 if none): sqrtf(d2) < dist_th <=> d2 <= d2_max
   const float *frec;
   U128 *best;
   unsigned long long *stats;
@@ -305,16 +255,14 @@ __device__ __forceinline__ MapRow load_map_row(const float *geo, int64_t n) {
 //     threshold is found on the host, gsx_thresholds.h);
 //   * the result of the 128-bit CAS is only looked at one iteration later.
 __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectArgs a) {
-  __shared__ Rigid s_tinv;
-  __shared__ float s_k[12];
+  __shared__ LiveCamera s_cam;
   __shared__ unsigned int s_act[kBlock / 32];
   const int b = blockIdx.y;
   const int count = a.counts[b];
   if ((int64_t)blockIdx.x * kBlock >= count) return;
-  if (threadIdx.x == 0) s_tinv = rigid_inverse(load_rigid(a.poses + b * a.pose_bstride));
-  if (threadIdx.x >= 32 && threadIdx.x < 44) s_k[threadIdx.x - 32] = __ldg(a.K + b * a.K_bstride + (threadIdx.x - 32));
+  load_live_camera(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b);
   __syncthreads();
-  const int P = a.H * a.W;
+  const int P = a.ib.H * a.ib.W;
   const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   const float *frec = a.frec + (int64_t)b * P * kRecW;
   U128 *best = a.best + (int64_t)b * P;
@@ -328,23 +276,10 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
     const MapRow m = cur;
     const int64_t nn = n + stride;
     if (nn < count) cur = load_map_row(geo, nn);  // in flight while this row is processed
-    // world -> camera (pointclouds.py:526-573), then pinhole projection with the 4x4 K on the homogeneous
-    // point (projutils.py:92-238): z == 0 divides by 1.
-    const float3 q = rigid_apply(s_tinv, m.a.x, m.a.y, m.a.z);
-    const float hx = ((s_k[0] * q.x + s_k[1] * q.y) + s_k[2] * q.z) + s_k[3];
-    const float hy = ((s_k[4] * q.x + s_k[5] * q.y) + s_k[6] * q.z) + s_k[7];
-    const float hz = ((s_k[8] * q.x + s_k[9] * q.y) + s_k[10] * q.z) + s_k[11];
-    const float den = (hz != 0.0f) ? hz : 1.0f;
-    const float u = hx / den, v = hy / den;
-    // fusionutils.py:259-266
-    bool live = (u > -1e-3f) && (u < a.u_hi) && (v > -1e-3f) && (v < a.v_hi) && (q.z > 0.0f);
-    if (live) {
+    const PixelHit hit = project(s_cam, a.ib, m.a.x, m.a.y, m.a.z);
+    if (hit.in_frustum) {
       ++n_active;
-      // round-half-even like torch.round, then clamp (fusionutils.py:267-274)
-      int w = (int)rintf(u), h = (int)rintf(v);
-      w = min(max(w, 0), a.W - 1);
-      h = min(max(h, 0), a.H - 1);
-      const int pix = h * a.W + w;
+      const int pix = hit.h * a.ib.W + hit.w;
       const float4 f0 = __ldg(reinterpret_cast<const float4 *>(frec + (int64_t)pix * kRecW));
       const float2 f1 = __ldg(reinterpret_cast<const float2 *>(frec + (int64_t)pix * kRecW + 4));
       // are_points_close (fusionutils.py:130): ||frame - map|| < dist_th
@@ -352,21 +287,14 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
       const float d2 = (dx * dx + dy * dy) + dz * dz;
       // are_normals_similar (fusionutils.py:187-195): n_frame . n_map > dot_th
       const float dot = (f0.w * m.a.w + f1.x * m.b.x) + f1.y * m.b.y;
-      live = (d2 <= a.d2_max) && (dot > a.dot_th);
+      const bool live = (d2 <= a.d2_max) && (dot > a.dot_th);
       if (pend_pix >= 0) {  // settle the previous candidate's CAS before re-using the slot
         atomic_max_rec128_finish(best + pend_pix, mine, old);
         pend_pix = -1;
       }
       if (live) {
-        // sort key of find_best_unique_correspondences (fusionutils.py:491-517): 1/(cc+1e-20), then the squared
-        // distance (map - frame)^2 (== d2: squares are sign-independent), then n.
-        const float inv_cc = 1.0f / (m.b.z + 1e-20f);
-        // positive floats order like their bit patterns; flip negatives so the order stays total.
-        unsigned int kb = __float_as_uint(inv_cc);
-        kb = (kb & 0x80000000u) ? ~kb : (kb | 0x80000000u);
-        const unsigned int rb = __float_as_uint(d2) | 0x80000000u;  // d2 >= 0
-        const unsigned long long hi = ((unsigned long long)kb << 32) | rb;
-        mine = U128{~(unsigned long long)n, ~hi};
+        // key (1/(cc+1e-20), (map - frame)^2 == d2: squares are sign-independent, n)
+        mine = U128{~(unsigned long long)n, ~argmin_key_hi(m.b.z, d2)};
         old = cas128(best + pix, U128{0ull, 0ull}, mine);  // optimistic: most pixels see a single candidate
         pend_pix = pix;
       }
@@ -422,41 +350,8 @@ struct MergeArgs {
   int32_t *assoc;  // optional (B,P): +row+1 appended at `row`, -(row+1) merged into `row`, 0 untouched
 };
 
-constexpr unsigned long long kFlagAgg = 1ull, kFlagPrefix = 2ull;
-
-__device__ __forceinline__ unsigned long long pack_state(unsigned long long flag, unsigned int value) {
-  return (flag << 32) | value;
-}
-__device__ __forceinline__ unsigned long long ld_acquire_u64(const unsigned long long *p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_u64(unsigned long long *p, unsigned long long v) {
-  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
-// exclusive prefix of the new-point counts of all preceding tiles (decoupled look-back, one warp, 32
-// predecessors per step)
-__device__ __forceinline__ unsigned int lookback_warp(const unsigned long long *state, int tile, int lane) {
-  unsigned int excl = 0;
-  for (int base = tile - 1; base >= 0; base -= 32) {
-    const int j = base - lane;
-    unsigned long long s = 0ull;
-    if (j >= 0) {
-      do {
-        s = ld_acquire_u64(state + j);
-      } while ((s >> 32) == 0ull);
-    }
-    const bool is_prefix = (j >= 0) && ((s >> 32) == kFlagPrefix);
-    const unsigned int pm = __ballot_sync(0xffffffffu, is_prefix);
-    const int first = pm ? (__ffs(pm) - 1) : 32;  // nearest predecessor that already knows its inclusive prefix
-    const unsigned int v = (j >= 0 && lane <= first) ? (unsigned int)s : 0u;
-    excl += __reduce_add_sync(0xffffffffu, v);
-    if (pm) break;
-  }
-  return excl;
-}
+// K1r zeroes K4's tile states before every frame, so K4's scan always runs in epoch 1
+constexpr unsigned int kMergeEpoch = 1u;
 
 #ifndef GSX_K4_MINB
 #define GSX_K4_MINB 4
@@ -499,7 +394,6 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   unsigned long long rec_lo[kPix];
   float4 f0[kPix], f1[kPix];
   bool matched[kPix], is_new[kPix];
-  int warp_excl[kPix];
 #pragma unroll
   for (int j = 0; j < kPix; ++j) {
     pix[j] = pix0 + j * kMB + threadIdx.x;
@@ -515,37 +409,26 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   }
   int n_matched = 0;
 #pragma unroll
-  for (int j = 0; j < kPix; ++j) {
-    is_new[j] = (pix[j] < P) && (f1[j].w > 0.0f) && !matched[j];
-    n_matched += matched[j] ? 1 : 0;
-    // row-major order inside the tile: chunk j (256 consecutive pixels), then warp, then lane
-    const unsigned int ballot = __ballot_sync(0xffffffffu, is_new[j]);
-    warp_excl[j] = __popc(ballot & ((1u << lane) - 1u));
-    if (lane == 0) s_warp_sums[j][warp] = __popc(ballot);
-  }
+  for (int j = 0; j < kPix; ++j) n_matched += matched[j] ? 1 : 0;
   n_matched = __reduce_add_sync(0xffffffffu, n_matched);
   if (lane == 0) s_matched[warp] = n_matched;
-  __syncthreads();
-  if (threadIdx.x == 0) {  // bookkeeping (merged rows of this element): one atomic per CTA
-    int t = 0;
+  int new_off[kPix];  // position of each new pixel among the tile's new pixels (row-major)
+  const int block_total = block_offsets<kMB, kPix>(
+      [&](int j) {
+        is_new[j] = (pix[j] < P) && (f1[j].w > 0.0f) && !matched[j];
+        return is_new[j];
+      },
+      new_off, s_warp_sums,
+      [&] {
+        if (threadIdx.x == 0) {  // bookkeeping (merged rows of this element): one atomic per CTA
+          int t = 0;
 #pragma unroll
-    for (int i = 0; i < kMB / 32; ++i) t += s_matched[i];
-    if (t) atomicAdd(a.ws.stats + 2 * b + 1, (unsigned long long)t);
-  }
-  int block_total = 0;
-  int block_excl[kPix];
-#pragma unroll
-  for (int j = 0; j < kPix; ++j) {
-    block_excl[j] = block_total;
-#pragma unroll
-    for (int i = 0; i < kMB / 32; ++i) {
-      const int c = s_warp_sums[j][i];
-      if (i < warp) block_excl[j] += c;
-      block_total += c;
-    }
-  }
+          for (int i = 0; i < kMB / 32; ++i) t += s_matched[i];
+          if (t) atomicAdd(a.ws.stats + 2 * b + 1, (unsigned long long)t);
+        }
+      });
   unsigned long long *state = a.ws.tile_state + (int64_t)b * T;
-  if (threadIdx.x == 0 && tile + 1 < T) st_release_u64(state + tile, pack_state(kFlagAgg, (unsigned)block_total));
+  if (threadIdx.x == 0) publish_tile(state, tile, T, kMergeEpoch, kTileAggregate, (unsigned)block_total);
 
   float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   float *col = a.col + (int64_t)b * a.cap * kColW;
@@ -593,11 +476,8 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
 
   // decoupled look-back (warp 0): exclusive prefix of new-point counts over preceding tiles of this element
   if (warp == 0) {
-    const unsigned int excl = lookback_warp(state, tile, lane);
-    if (lane == 0) {
-      if (tile + 1 < T) st_release_u64(state + tile, pack_state(kFlagPrefix, excl + (unsigned)block_total));
-      s_excl = (int)excl;
-    }
+    const unsigned int excl = lookback_warp(state, tile, T, kMergeEpoch, (unsigned)block_total);
+    if (lane == 0) s_excl = (int)excl;
   }
   __syncthreads();
   const int64_t base = (int64_t)count_in + s_excl;
@@ -605,7 +485,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   for (int j = 0; j < kPix; ++j) {
     if (is_new[j]) {
       // append in row-major pixel order (fusionutils.py:702-720; pointclouds.py:1203-1235)
-      const int64_t n = base + block_excl[j] + warp_excl[j];
+      const int64_t n = base + new_off[j];
       if (n < a.cap) {
         const float *fc = s_rgb + (j * kMB + (int)threadIdx.x) * 3;
         *reinterpret_cast<float4 *>(geo + n * kGeoW) = f0[j];
@@ -773,7 +653,7 @@ __global__ void __launch_bounds__(256) k_merge_bwd_pixels(MergeBwdArgs a) {
 // frame may be computed (into another workspace) while this frame's update runs (gsx_pointfusion_sequence_gt).
 static Workspace group_workspace(void *workspace, int B_total, int b0, int H, int W) {
   const int64_t P = (int64_t)H * W;
-  Workspace ws = carve(workspace, B_total, H, W);
+  Workspace ws = fusion_workspace(workspace, B_total, H, W);
   ws.frec += (int64_t)b0 * P * kRecW;
   ws.best += (int64_t)b0 * P;
   ws.tile_state += (int64_t)b0 * ws.tiles;
@@ -798,8 +678,8 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   const Workspace ws = group_workspace(workspace, B_total, b0, H, W);
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
   if (max_count > 0) {
-    ProjectArgs pa{ggeo, cin + b0, cap, poses + (int64_t)b0 * pose_bs, pose_bs, K + (int64_t)b0 * K_bs, K_bs, nb, H, W,
-                   dot_th, (float)(W - 0.999), (float)(H - 0.999), sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
+    ProjectArgs pa{ggeo, cin + b0, cap, poses + (int64_t)b0 * pose_bs, pose_bs, K + (int64_t)b0 * K_bs, K_bs, nb,
+                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
     const int rc = launch_project_select(pa, max_count, st);
     if (rc) return rc;
   }
@@ -807,7 +687,11 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   return launch_merge_append(ma, st);
 }
 
-int64_t fusion_workspace_bytes(int B, int H, int W) { return workspace_bytes(B, H, W); }
+int64_t fusion_workspace_bytes(int B, int H, int W) {
+  int64_t bytes;
+  fusion_workspace(nullptr, B, H, W, &bytes);
+  return bytes;
+}
 
 }  // namespace gsx
 
@@ -815,12 +699,12 @@ using namespace gsx;
 
 extern "C" int64_t gsx_fusion_workspace_bytes(int B, int H, int W) {
   if (B < 0 || H < 0 || W < 0) return -1;
-  return workspace_bytes(B, H, W);
+  return fusion_workspace_bytes(B, H, W);
 }
 
 extern "C" int64_t gsx_fusion_workspace_stats_offset(int B, int H, int W) {
   if (B < 0 || H < 0 || W < 0) return -1;
-  return stats_offset(B, H, W);
+  return (int64_t)reinterpret_cast<uintptr_t>(fusion_workspace(nullptr, B, H, W).stats);
 }
 
 static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -836,7 +720,7 @@ extern "C" int gsx_fusion_frame_records(const float *depth, int64_t depth_bstrid
                 "gsx_fusion_frame_records: pass the three frame maps, or none of them together with the intrinsics");
   GSX_CHECK_ARG(aligned16(workspace), "gsx_fusion_frame_records: the workspace must be 16-byte aligned");
   FrameRecArgs a{depth, depth_bstride, intrinsics, K_bstride, poses, pose_bstride, gvertex, gnormal, vertex, B, H, W,
-                 (float)(2.0 * (sigma * sigma)), carve(workspace, B, H, W)};
+                 (float)(2.0 * (sigma * sigma)), fusion_workspace(workspace, B, H, W)};
   return launch_frame_records(a, (cudaStream_t)stream);
 }
 
@@ -852,9 +736,9 @@ extern "C" int gsx_fusion_project_select(const float *map_geometry, const int32_
                 "gsx_fusion_project_select: geometry rows and workspace must be 16-byte aligned");
   GSX_CHECK_ARG(max_count <= capacity, "gsx_fusion_project_select: max_count %lld > capacity %lld",
                 (long long)max_count, (long long)capacity);
-  const Workspace ws = carve(workspace, B, H, W);
-  ProjectArgs a{map_geometry, counts, capacity, poses, pose_bstride, intrinsics, K_bstride, B, H, W, dot_th,
-                (float)(W - 0.999), (float)(H - 0.999), sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
+  const Workspace ws = fusion_workspace(workspace, B, H, W);
+  ProjectArgs a{map_geometry, counts, capacity, poses, pose_bstride, intrinsics, K_bstride, B, image_bounds(H, W),
+                dot_th, sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
   return launch_project_select(a, max_count, (cudaStream_t)stream);
 }
 
@@ -873,7 +757,7 @@ extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, i
                 "gsx_fusion_merge_append: map rows and workspace must be 16-byte aligned");
   GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_merge_append: capacity must fit int32 (counts are int32)");
   MergeArgs a{map_geometry, map_colors, with_ccounts ? 1 : 0, counts_in, counts_out, capacity, rgb, rgb_bstride, B, H,
-              W, carve(workspace, B, H, W), overflow_flag, assoc_out};
+              W, fusion_workspace(workspace, B, H, W), overflow_flag, assoc_out};
   return launch_merge_append(a, (cudaStream_t)stream);
 }
 

@@ -1,0 +1,45 @@
+// Workspace of the fused PointFusion map update (gsx_fusion.cu), shared with the table variants (gsx_tables.cu).
+#pragma once
+#include "gsx_common.cuh"
+
+namespace gsx {
+
+#ifndef GSX_KPIX
+#define GSX_KPIX 2
+#endif
+constexpr int kMB = 256;              // threads per CTA of the merge/append kernel
+constexpr int kPix = GSX_KPIX;        // pixels per thread
+constexpr int kTilePix = kMB * kPix;  // pixels per merge tile
+
+//   float  frec[B][P][8]       frame records (gvx,gvy,gvz,gnx,gny,gnz,alpha,depth)             written by K1r
+//   U128   best[B][P]          complemented arg-min records (0 = empty)                         cleared by K1r
+//   uint64 tile_state[B][T]    look-back state of K4's scan (epoch 1), T = ceil(P / kTilePix)  cleared by K1r
+//   uint32 ticket[B]           dynamic tile ids of K4                                           cleared by K1r
+//   uint64 stats[B][2]         running totals: {active map rows (in frustum), merged rows}      caller zeroes once
+// Nothing in here has to survive from one frame to the next (the stats are bookkeeping only): every frame's K1r
+// re-arms what K2 / K4 of that frame consume, so a failed or abandoned call cannot poison a later one.
+struct Workspace {
+  float *frec;
+  U128 *best;
+  unsigned long long *tile_state;
+  unsigned int *ticket;
+  unsigned long long *stats;
+  int tiles;
+};
+
+// the workspace at `base` (nullptr: byte offsets); `bytes`, if given, receives its size
+inline Workspace fusion_workspace(void *base, int B, int H, int W, int64_t *bytes = nullptr) {
+  const int64_t P = (int64_t)H * W;
+  Carver c(base);
+  Workspace w;
+  w.tiles = (int)((P + kTilePix - 1) / kTilePix);
+  w.frec = c.take<float>(B * P * kRecW);
+  w.best = c.take<U128>(B * P);
+  w.tile_state = c.take<unsigned long long>((int64_t)B * w.tiles);
+  w.ticket = c.take<unsigned int>(B);
+  w.stats = c.take<unsigned long long>(2 * (int64_t)B);
+  if (bytes) *bytes = c.bytes;
+  return w;
+}
+
+}  // namespace gsx

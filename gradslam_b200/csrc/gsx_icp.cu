@@ -93,7 +93,6 @@ __global__ void __launch_bounds__(1024) k_icp_gather_src(GatherSrcArgs a) {
 // ---------------------------------------------------------------------------------------------------------
 // gather: target cloud (stable compaction of lattice-active map points; decoupled look-back over tiles)
 // ---------------------------------------------------------------------------------------------------------
-constexpr int kGeoW = 8;  // floats per packed geometry row (px,py,pz,nx,ny,nz,ccount,0), see gsx_fusion.cu
 struct GatherTgtArgs {
   const float *geo;  // (B,cap,8)
   const int32_t *counts;
@@ -102,8 +101,8 @@ struct GatherTgtArgs {
   int64_t pose_bstride;
   const float *K;
   int64_t K_bstride;
-  int B, H, W, ds;
-  float u_hi, v_hi;
+  int B, ds;
+  ImageBounds ib;
   float *tgt_p, *tgt_n;  // (B, nt_cap, 3)
   int32_t *tgt_count;    // (B)
   int nt_cap;
@@ -114,40 +113,18 @@ struct GatherTgtArgs {
   int32_t *overflow;  // set to 1 if the target cloud did not fit nt_cap (may be null)
 };
 
-constexpr unsigned long long kAgg = 1ull, kPrefix = 2ull;
-__device__ __forceinline__ unsigned long long icp_pack(unsigned int epoch, unsigned long long flag, unsigned int v) {
-  return ((unsigned long long)epoch << 34) | (flag << 32) | v;
-}
-__device__ __forceinline__ unsigned long long icp_ld_acquire(const unsigned long long *p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void icp_st_release(unsigned long long *p, unsigned long long v) {
-  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
 __global__ void __launch_bounds__(kIcpBlock) k_icp_gather_tgt(GatherTgtArgs a) {
-  __shared__ Rigid s_tinv;
-  __shared__ float s_k[12];
+  __shared__ LiveCamera s_cam;
   __shared__ int s_tile, s_excl;
   __shared__ int s_warp[4][kIcpBlock / 32];
   const int b = blockIdx.x % a.B;  // elements interleaved in the grid (short look-back chains)
-  if (threadIdx.x == 0) {
-    // dynamic tile id.  The block that draws the last ticket re-arms the counter for the next launch (nobody
-    // else will touch it any more in this one), so the number of tiles may differ from launch to launch.
-    const unsigned int t = atomicAdd(a.ticket + b, 1u);
-    if (t == (unsigned int)a.tiles - 1u) a.ticket[b] = 0u;
-    s_tile = (int)t;
-    s_tinv = rigid_inverse(load_rigid(a.poses + b * a.pose_bstride));
-  }
-  if (threadIdx.x >= 32 && threadIdx.x < 44) s_k[threadIdx.x - 32] = __ldg(a.K + b * a.K_bstride + (threadIdx.x - 32));
+  if (threadIdx.x == 0) s_tile = draw_tile_ticket(a.ticket + b, a.tiles);
+  load_live_camera(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b);
   __syncthreads();
   const int tile = s_tile;
   const int count = a.counts[b];
   const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int n[4], wexcl[4];
+  int n[4], off[4];
   bool keep[4];
   float px[4], py[4], pz[4], nx[4];
 #pragma unroll
@@ -161,59 +138,18 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_gather_tgt(GatherTgtArgs a) {
     pz[j] = g.z;
     nx[j] = g.w;
   }
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    // identical to the projection of k_project_select (fusionutils.py:249-274)
-    const float3 q = rigid_apply(s_tinv, px[j], py[j], pz[j]);
-    const float hx = ((s_k[0] * q.x + s_k[1] * q.y) + s_k[2] * q.z) + s_k[3];
-    const float hy = ((s_k[4] * q.x + s_k[5] * q.y) + s_k[6] * q.z) + s_k[7];
-    const float hz = ((s_k[8] * q.x + s_k[9] * q.y) + s_k[10] * q.z) + s_k[11];
-    const float den = (hz != 0.0f) ? hz : 1.0f;
-    const float u = hx / den, v = hy / den;
-    keep[j] = keep[j] && (u > -1e-3f) && (u < a.u_hi) && (v > -1e-3f) && (v < a.v_hi) && (q.z > 0.0f);
-    int w = (int)rintf(u), h = (int)rintf(v);
-    w = min(max(w, 0), a.W - 1);
-    h = min(max(h, 0), a.H - 1);
-    keep[j] = keep[j] && (h % a.ds == 0) && (w % a.ds == 0);  // icputils.py:596-597
-    const unsigned int ballot = __ballot_sync(0xffffffffu, keep[j]);
-    wexcl[j] = __popc(ballot & ((1u << lane) - 1u));
-    if (lane == 0) s_warp[j][warp] = __popc(ballot);
-  }
-  __syncthreads();
-  int total = 0, bexcl[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    bexcl[j] = total;
-#pragma unroll
-    for (int i = 0; i < kIcpBlock / 32; ++i) {
-      const int c = s_warp[j][i];
-      if (i < warp) bexcl[j] += c;
-      total += c;
-    }
-  }
+  const int total = block_offsets<kIcpBlock, 4>(
+      [&](int j) {  // the projection of k_project_select, then the lattice test (icputils.py:596-597)
+        const PixelHit hit = project(s_cam, a.ib, px[j], py[j], pz[j]);
+        keep[j] = keep[j] && hit.in_frustum && (hit.h % a.ds == 0) && (hit.w % a.ds == 0);
+        return keep[j];
+      },
+      off, s_warp, [] {});
   unsigned long long *state = a.tile_state + (int64_t)b * a.tiles;
-  if (threadIdx.x == 0 && tile + 1 < a.tiles) icp_st_release(state + tile, icp_pack(a.epoch, kAgg, (unsigned)total));
-  if (warp == 0) {
-    unsigned int excl = 0;
-    for (int base = tile - 1; base >= 0; base -= 32) {
-      const int j = base - lane;
-      unsigned long long s = 0ull;
-      if (j >= 0) {
-        do {
-          s = icp_ld_acquire(state + j);
-        } while ((unsigned int)(s >> 34) != a.epoch);
-      }
-      const bool is_prefix = (j >= 0) && (((s >> 32) & 3ull) == kPrefix);
-      const unsigned int pm = __ballot_sync(0xffffffffu, is_prefix);
-      const int first = pm ? (__ffs(pm) - 1) : 32;
-      const unsigned int v = (j >= 0 && lane <= first) ? (unsigned int)s : 0u;
-      excl += __reduce_add_sync(0xffffffffu, v);
-      if (pm) break;
-    }
-    if (lane == 0) {
-      if (tile + 1 < a.tiles) icp_st_release(state + tile, icp_pack(a.epoch, kPrefix, excl + (unsigned)total));
-      s_excl = (int)excl;
-    }
+  if (threadIdx.x == 0) publish_tile(state, tile, a.tiles, a.epoch, kTileAggregate, (unsigned)total);
+  if (threadIdx.x < 32) {
+    const unsigned int excl = lookback_warp(state, tile, a.tiles, a.epoch, (unsigned)total);
+    if (threadIdx.x == 0) s_excl = (int)excl;
   }
   __syncthreads();
   float *op = a.tgt_p + (int64_t)b * a.nt_cap * 3;
@@ -221,7 +157,7 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_gather_tgt(GatherTgtArgs a) {
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     if (keep[j]) {
-      const int pos = s_excl + bexcl[j] + wexcl[j];
+      const int pos = s_excl + off[j];
       if (pos < a.nt_cap) {
         op[(int64_t)pos * 3 + 0] = px[j];
         op[(int64_t)pos * 3 + 1] = py[j];
@@ -884,80 +820,121 @@ __global__ void k_pose_compose(const float *T, const float *prev, int64_t prev_b
 // ---------------------------------------------------------------------------------------------------------
 // workspace
 // ---------------------------------------------------------------------------------------------------------
-struct IcpWorkspace {
+// Scratch and workspace layouts (Carver, gsx_common.cuh).  The search grid is laid out only for targets larger than
+// kGridThreshold (smaller ones use the shared-memory brute force); `params` is null otherwise.
+constexpr int kGridThreshold = 4096;
+
+inline TargetGrid grid_layout(Carver &c, int B, int nt_stride) {
+  TargetGrid g{};
+  if (nt_stride <= kGridThreshold) return g;
+  g.params = c.take<GridParams>(B);
+  g.cell_start = c.take<int>((int64_t)B * (kGridMaxCells + 1));
+  g.cursor = c.take<int>((int64_t)B * kGridMaxCells);
+  g.sorted = c.take<float4>((int64_t)B * nt_stride);
+  return g;
+}
+
+inline float *partials_layout(Carver &c, int B, int ns_stride) {
+  return c.take<float>((int64_t)B * ((ns_stride + kIcpBlock - 1) / kIcpBlock) * kNumSums);
+}
+
+// T_total, T_pend, dT: 16 floats per element; xi, err, damp: 6 floats per element each
+inline IcpState icp_state_layout(Carver &c, int B) {
+  IcpState st;
+  st.T_total = c.take<float>(16 * B);
+  st.T_pend = c.take<float>(16 * B);
+  st.dT = c.take<float>(16 * B);
+  st.xi = c.take<float>(6 * B);
+  st.err = c.take<float>(6 * B);
+  st.damp = c.take<float>(6 * B);
+  return st;
+}
+
+struct IcpWorkspace {  // of gsx_icp_localize
   float *src;  // (B, ns_cap, 3)
   int32_t *src_count, *tgt_count;
   float *partials;  // (B, nblk, 28)
   IcpState st;
-  unsigned long long *tile_state;
-  unsigned int *ticket;
+  unsigned long long *tile_state;  // (B, tiles_cap) look-back tile states of k_icp_gather_tgt
+  unsigned int *ticket;            // (B)
   int ns_cap, nblk, tiles_cap;
 };
 
-inline int64_t up256(int64_t x) { return (x + 255) / 256 * 256; }
-
-inline int icp_ns_cap(int H, int W, int ds) { return ((H + ds - 1) / ds) * ((W + ds - 1) / ds); }
-
-inline int64_t icp_workspace_bytes(int B, int H, int W, int ds, int64_t map_capacity) {
-  const int ns = icp_ns_cap(H, W, ds);
-  const int nblk = (ns + kIcpBlock - 1) / kIcpBlock;
-  const int64_t tiles = (map_capacity + 1023) / 1024;
-  return up256((int64_t)B * ns * 12) + 2 * up256((int64_t)B * 4) + up256((int64_t)B * nblk * kNumSums * 4) +
-         4 * up256((int64_t)B * 64) + 3 * up256((int64_t)B * 24) + up256(B * tiles * 8) + up256((int64_t)B * 4);
-}
-
-inline IcpWorkspace icp_carve(void *ws, int B, int H, int W, int ds, int64_t map_capacity) {
+inline IcpWorkspace icp_workspace_layout(Carver &c, int B, int H, int W, int ds, int64_t map_capacity) {
   IcpWorkspace w;
-  w.ns_cap = icp_ns_cap(H, W, ds);
+  w.ns_cap = ((H + ds - 1) / ds) * ((W + ds - 1) / ds);
   w.nblk = (w.ns_cap + kIcpBlock - 1) / kIcpBlock;
   w.tiles_cap = (int)((map_capacity + 1023) / 1024);
-  char *p = (char *)ws;
-  w.src = (float *)p;            p += up256((int64_t)B * w.ns_cap * 12);
-  w.src_count = (int32_t *)p;    p += up256((int64_t)B * 4);
-  w.tgt_count = (int32_t *)p;    p += up256((int64_t)B * 4);
-  w.partials = (float *)p;       p += up256((int64_t)B * w.nblk * kNumSums * 4);
-  w.st.T_total = (float *)p;     p += up256((int64_t)B * 64);
-  w.st.T_pend = (float *)p;      p += up256((int64_t)B * 64);
-  w.st.dT = (float *)p;          p += up256((int64_t)B * 64);
-  p += up256((int64_t)B * 64);   // spare
-  w.st.xi = (float *)p;          p += up256((int64_t)B * 24);
-  w.st.err = (float *)p;         p += up256((int64_t)B * 24);
-  w.st.damp = (float *)p;        p += up256((int64_t)B * 24);
-  w.tile_state = (unsigned long long *)p;  p += up256((int64_t)B * w.tiles_cap * 8);
-  w.ticket = (unsigned int *)p;
+  w.src = c.take<float>((int64_t)B * w.ns_cap * 3);
+  w.src_count = c.take<int32_t>(B);
+  w.tgt_count = c.take<int32_t>(B);
+  w.partials = partials_layout(c, B, w.ns_cap);
+  w.st = icp_state_layout(c, B);
+  w.tile_state = c.take<unsigned long long>((int64_t)B * w.tiles_cap);
+  w.ticket = c.take<unsigned int>(B);
   return w;
 }
 
-// runs the LM / gradLM loop on clouds that are already in place
-constexpr int kGridThreshold = 4096;  // target clouds up to this size use the shared-memory brute force
+struct AlignScratch {  // of gsx_icp_align
+  float *src;  // (B, ns_stride, 3) working copy of the source
+  float *partials;
+  IcpState st;
+  TargetGrid grid;
+};
 
-// CTAs per element of the grid count / scatter kernels (grid-stride loops over the target's actual size: the stride
-// of the target buffer is a loose upper bound, e.g. the whole map for the ICP target)
-inline unsigned grid_fill_blocks(int nt_stride) {
-  const int nb = (nt_stride + 255) / 256;
-  return (unsigned)(nb < 128 ? nb : 128);
+inline AlignScratch align_scratch_layout(Carver &c, int B, int ns_stride, int nt_stride) {
+  AlignScratch s;
+  s.src = c.take<float>((int64_t)B * ns_stride * 3);
+  s.partials = partials_layout(c, B, ns_stride);
+  s.st = icp_state_layout(c, B);
+  s.grid = grid_layout(c, B, nt_stride);
+  return s;
 }
 
-inline int64_t grid_bytes(int B, int nt_stride) {
-  if (nt_stride <= kGridThreshold) return 0;
-  return up256((int64_t)B * sizeof(GridParams)) + up256((int64_t)B * (kGridMaxCells + 1) * 4) +
-         up256((int64_t)B * kGridMaxCells * 4) + up256((int64_t)B * nt_stride * 16);
+struct TargetScratch {  // of gsx_icp_localize: the target cloud and its search grid
+  float *p, *n;  // (B, tgt_capacity, 3)
+  TargetGrid grid;
+};
+
+inline TargetScratch target_scratch_layout(Carver &c, int B, int64_t tgt_capacity) {
+  TargetScratch s;
+  s.p = c.take<float>((int64_t)B * tgt_capacity * 3);
+  s.n = c.take<float>((int64_t)B * tgt_capacity * 3);
+  s.grid = grid_layout(c, B, (int)tgt_capacity);
+  return s;
 }
 
-inline TargetGrid grid_carve(void *mem, int B, int nt_stride) {
-  TargetGrid g;
-  char *p = (char *)mem;
-  g.params = (GridParams *)p;  p += up256((int64_t)B * sizeof(GridParams));
-  g.cell_start = (int *)p;     p += up256((int64_t)B * (kGridMaxCells + 1) * 4);
-  g.cursor = (int *)p;         p += up256((int64_t)B * kGridMaxCells * 4);
-  g.sorted = (float4 *)p;
-  return g;
+struct Knn1Scratch {  // of gsx_knn1
+  float *partials;  // block partials of the normal equations (not used by the caller)
+  TargetGrid grid;
+};
+
+inline Knn1Scratch knn1_scratch_layout(Carver &c, int B, int ns_stride, int nt_stride) {
+  Knn1Scratch s;
+  s.partials = partials_layout(c, B, ns_stride);
+  s.grid = grid_layout(c, B, nt_stride);
+  return s;
 }
 
+// bbox -> clear -> count -> scan -> scatter: bins the target cloud into `g` (laid out by grid_layout)
+void build_search_grid(const float *tgt_p, const int32_t *tgt_count, int nt_stride, int B, const TargetGrid &g,
+                       cudaStream_t stream) {
+  // CTAs per element of the count / scatter kernels (grid-stride loops over the target's actual size: the stride of
+  // the target buffer is a loose upper bound, e.g. the whole map for the ICP target)
+  const unsigned nb = (unsigned)((nt_stride + 255) / 256 < 128 ? (nt_stride + 255) / 256 : 128);
+  k_grid_bbox<<<B, 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, g);
+  k_grid_clear<<<(unsigned)(((int64_t)B * kGridMaxCells + 255) / 256), 256, 0, stream>>>(g, B);
+  k_grid_count<<<dim3(nb, (unsigned)B), 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, g);
+  k_grid_scan<<<B, 1024, 0, stream>>>(g);
+  k_grid_scatter<<<dim3(nb, (unsigned)B), 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, g);
+}
+
+// runs the LM / gradLM loop on clouds that are already in place; the target's search grid, if `tgt_grid` is laid out,
+// is built once here (the target does not move during the loop)
 int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const float *tgt_p, const float *tgt_n,
                  const int32_t *tgt_count, int nt_stride, int B, const float *T0, int mode, int numiters, float damp,
                  int use_thresh, float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *partials,
-                 int nblk_cap, IcpState st, int64_t *nn_idx, void *grid_mem, cudaStream_t stream) {
+                 int nblk_cap, IcpState st, int64_t *nn_idx, const TargetGrid &tgt_grid, cudaStream_t stream) {
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   if (nblk > nblk_cap) {
     set_error("icp: source cloud larger than workspace");
@@ -966,17 +943,9 @@ int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const floa
   k_icp_init<<<(B + 63) / 64, 64, 0, stream>>>(st, T0, damp, B);
   UpdateArgs u{mode, 1.0f / lambda_max, lambda_max, Bp, B2p, 1.0f / nu};
   KnnArgs ka{src, src_count, ns_stride, tgt_p, tgt_n, tgt_count, nt_stride, nullptr, 0, dist_thresh, use_thresh,
-             partials, nullptr, nullptr, TargetGrid{}};
-  const bool use_grid = grid_mem != nullptr && nt_stride > kGridThreshold;
-  if (use_grid) {  // the target is fixed for the whole loop: bin it once
-    ka.grid = grid_carve(grid_mem, B, nt_stride);
-    const unsigned nb = grid_fill_blocks(nt_stride);
-    k_grid_bbox<<<B, 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, ka.grid);
-    k_grid_clear<<<(unsigned)(((int64_t)B * kGridMaxCells + 255) / 256), 256, 0, stream>>>(ka.grid, B);
-    k_grid_count<<<dim3(nb, (unsigned)B), 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, ka.grid);
-    k_grid_scan<<<B, 1024, 0, stream>>>(ka.grid);
-    k_grid_scatter<<<dim3(nb, (unsigned)B), 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, ka.grid);
-  }
+             partials, nullptr, nullptr, tgt_grid};
+  const bool use_grid = tgt_grid.params != nullptr;
+  if (use_grid) build_search_grid(tgt_p, tgt_count, nt_stride, B, tgt_grid, stream);
   const dim3 grid((unsigned)nblk, (unsigned)B);
   for (int it = 0; it < numiters; ++it) {
     ka.pre = st.T_pend;
@@ -1002,7 +971,9 @@ using namespace gsx;
 
 extern "C" int64_t gsx_icp_workspace_bytes(int B, int H, int W, int ds, int64_t map_capacity) {
   if (B < 0 || H < 1 || W < 1 || ds < 1 || map_capacity < 0) return -1;
-  return icp_workspace_bytes(B, H, W, ds, map_capacity);
+  Carver c(nullptr);
+  icp_workspace_layout(c, B, H, W, ds, map_capacity);
+  return c.bytes;
 }
 
 extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
@@ -1014,43 +985,33 @@ extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, 
                 "gsx_icp_align: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1 && numiters >= 0, "gsx_icp_align: bad extents");
   GSX_CHECK_ARG(mode == 0 || mode == 1, "gsx_icp_align: mode must be 0 (ICP) or 1 (gradICP)");
-  // scratch: working copy of src (B,ns,3) + partials + state
+  Carver c(scratch);
+  const AlignScratch sc = align_scratch_layout(c, B, ns_stride, nt_stride);
+  GSX_CHECK_ARG(scratch_bytes >= c.bytes, "gsx_icp_align: scratch too small (%lld < %lld)", (long long)scratch_bytes,
+                (long long)c.bytes);
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
-  const int64_t need = up256((int64_t)B * ns_stride * 12) + up256((int64_t)B * nblk * kNumSums * 4) +
-                       3 * up256((int64_t)B * 64) + 3 * up256((int64_t)B * 24) + grid_bytes(B, nt_stride);
-  GSX_CHECK_ARG(scratch_bytes >= need, "gsx_icp_align: scratch too small (%lld < %lld)", (long long)scratch_bytes,
-                (long long)need);
-  char *p = (char *)scratch;
-  float *src = (float *)p;       p += up256((int64_t)B * ns_stride * 12);
-  float *partials = (float *)p;  p += up256((int64_t)B * nblk * kNumSums * 4);
-  IcpState st;
-  st.T_total = (float *)p;       p += up256((int64_t)B * 64);
-  st.T_pend = (float *)p;        p += up256((int64_t)B * 64);
-  st.dT = (float *)p;            p += up256((int64_t)B * 64);
-  st.xi = (float *)p;            p += up256((int64_t)B * 24);
-  st.err = (float *)p;           p += up256((int64_t)B * 24);
-  st.damp = (float *)p;        p += up256((int64_t)B * 24);
-  void *grid_mem = grid_bytes(B, nt_stride) ? (void *)p : nullptr;
   cudaStream_t s = (cudaStream_t)stream;
-  cudaMemcpyAsync(src, src_points, (size_t)B * ns_stride * 12, cudaMemcpyDeviceToDevice, s);
-  const int rc = run_icp_loop(src, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
+  cudaMemcpyAsync(sc.src, src_points, (size_t)B * ns_stride * 12, cudaMemcpyDeviceToDevice, s);
+  const int rc = run_icp_loop(sc.src, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
                               initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp,
-                              B2p, nu, partials, nblk, st, nn_idx_out, grid_mem, s);
+                              B2p, nu, sc.partials, nblk, sc.st, nn_idx_out, sc.grid, s);
   if (rc) return rc;
-  cudaMemcpyAsync(transform_out, st.T_total, (size_t)B * 64, cudaMemcpyDeviceToDevice, s);
+  cudaMemcpyAsync(transform_out, sc.st.T_total, (size_t)B * 64, cudaMemcpyDeviceToDevice, s);
   return 0;
 }
 
 extern "C" int64_t gsx_icp_align_scratch_bytes(int B, int ns_stride, int nt_stride) {
   if (B < 1 || ns_stride < 1 || nt_stride < 1) return -1;
-  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
-  return up256((int64_t)B * ns_stride * 12) + up256((int64_t)B * nblk * kNumSums * 4) + 3 * up256((int64_t)B * 64) +
-         3 * up256((int64_t)B * 24) + grid_bytes(B, nt_stride);
+  Carver c(nullptr);
+  align_scratch_layout(c, B, ns_stride, nt_stride);
+  return c.bytes;
 }
 
 extern "C" int64_t gsx_icp_tgt_scratch_bytes(int B, int64_t tgt_capacity) {
   if (B < 1 || tgt_capacity < 1 || tgt_capacity > (1ll << 30)) return -1;
-  return 2 * up256((int64_t)B * tgt_capacity * 12) + grid_bytes(B, (int)tgt_capacity);
+  Carver c(nullptr);
+  target_scratch_layout(c, B, tgt_capacity);
+  return c.bytes;
 }
 
 extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts,
@@ -1072,13 +1033,11 @@ extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts
   cudaStream_t s = (cudaStream_t)stream;
   GSX_CHECK_ARG(workspace_map_capacity >= max_count, "gsx_icp_localize: workspace sized for a smaller map");
   // the layout of the workspace is fixed by the capacity it was created for, not by today's map capacity
-  IcpWorkspace w = icp_carve(workspace, B, H, W, ds, workspace_map_capacity);
+  Carver cw(workspace);
+  const IcpWorkspace w = icp_workspace_layout(cw, B, H, W, ds, workspace_map_capacity);
   GSX_CHECK_ARG(tgt_capacity < (1ll << 30), "gsx_icp_localize: tgt_capacity too large");
-  float *tgt_p = (float *)tgt_scratch;
-  float *tgt_n = (float *)((char *)tgt_scratch + up256((int64_t)B * tgt_capacity * 12));
-  void *grid_mem = grid_bytes(B, (int)tgt_capacity)
-                       ? (void *)((char *)tgt_scratch + 2 * up256((int64_t)B * tgt_capacity * 12))
-                       : nullptr;
+  Carver ct(tgt_scratch);
+  const TargetScratch tgt = target_scratch_layout(ct, B, tgt_capacity);
   GatherSrcArgs gs{depth, depth_bstride, intrinsics, K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds,
                    w.src, w.src_count, w.ns_cap};
   k_icp_gather_src<<<B, 1024, 0, s>>>(gs);
@@ -1086,15 +1045,15 @@ extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts
   if (tiles > w.tiles_cap) tiles = w.tiles_cap;
   if (tiles == 0) cudaMemsetAsync(w.tgt_count, 0, (size_t)B * 4, s);
   if (tiles > 0) {
-    GatherTgtArgs gt{map_geometry, counts, capacity, prev_poses, prev_pose_bstride, intrinsics, K_bstride,
-                     B, H, W, ds, (float)(W - 0.999), (float)(H - 0.999), tgt_p, tgt_n, w.tgt_count,
-                     (int)tgt_capacity, w.tile_state, w.ticket, tiles, epoch, overflow_flag};
+    GatherTgtArgs gt{map_geometry, counts, capacity, prev_poses, prev_pose_bstride, intrinsics, K_bstride, B, ds,
+                     image_bounds(H, W), tgt.p, tgt.n, w.tgt_count, (int)tgt_capacity, w.tile_state, w.ticket, tiles,
+                     epoch, overflow_flag};
     k_icp_gather_tgt<<<dim3((unsigned)(tiles * B)), kIcpBlock, 0, s>>>(gt);
   }
   GSX_CHECK_LAUNCH("gsx_icp_localize(gather)");
-  const int rc = run_icp_loop(w.src, w.src_count, w.ns_cap, tgt_p, tgt_n, w.tgt_count, (int)tgt_capacity, B, nullptr,
+  const int rc = run_icp_loop(w.src, w.src_count, w.ns_cap, tgt.p, tgt.n, w.tgt_count, (int)tgt_capacity, B, nullptr,
                               mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu, w.partials,
-                              w.nblk, w.st, nullptr, grid_mem, s);
+                              w.nblk, w.st, nullptr, tgt.grid, s);
   if (rc) return rc;
   k_pose_compose<<<(B + 63) / 64, 64, 0, s>>>(w.st.T_total, prev_poses, prev_pose_bstride, poses_out,
                                               poses_out_bstride, B);
@@ -1104,8 +1063,9 @@ extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts
 
 extern "C" int64_t gsx_knn1_scratch_bytes(int B, int ns_stride, int nt_stride) {
   if (B < 1 || ns_stride < 1 || nt_stride < 1) return -1;
-  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
-  return up256((int64_t)B * nblk * kNumSums * 4) + grid_bytes(B, nt_stride);
+  Carver c(nullptr);
+  knn1_scratch_layout(c, B, ns_stride, nt_stride);
+  return c.bytes;
 }
 
 extern "C" int gsx_knn1(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
@@ -1113,24 +1073,17 @@ extern "C" int gsx_knn1(const float *src_points, const int32_t *src_count, int n
                         void *scratch, int64_t scratch_bytes, int build_grid, void *stream) {
   GSX_CHECK_ARG(src_points && src_count && tgt_points && tgt_count && idx_out && scratch, "gsx_knn1: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1, "gsx_knn1: bad extents");
-  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
-  const int64_t part = up256((int64_t)B * nblk * kNumSums * 4);
-  GSX_CHECK_ARG(scratch_bytes >= part + grid_bytes(B, nt_stride), "gsx_knn1: scratch too small");
+  Carver c(scratch);
+  const Knn1Scratch sc = knn1_scratch_layout(c, B, ns_stride, nt_stride);
+  GSX_CHECK_ARG(scratch_bytes >= c.bytes, "gsx_knn1: scratch too small");
   // the target normals are not needed for the association itself: reuse the points as a placeholder
   KnnArgs ka{const_cast<float *>(src_points), src_count, ns_stride, tgt_points, tgt_points, tgt_count, nt_stride,
-             nullptr, 0, 0.0f, 0, (float *)scratch, idx_out, d2_out, TargetGrid{}};
+             nullptr, 0, 0.0f, 0, sc.partials, idx_out, d2_out, sc.grid};
   cudaStream_t s = (cudaStream_t)stream;
-  const dim3 grid((unsigned)nblk, (unsigned)B);
-  if (nt_stride > kGridThreshold) {
-    ka.grid = grid_carve((char *)scratch + part, B, nt_stride);
-    if (build_grid) {  // (0: `scratch` still holds the grid a previous call built for this very target)
-      const unsigned nb = grid_fill_blocks(nt_stride);
-      k_grid_bbox<<<B, 256, 0, s>>>(tgt_points, tgt_count, nt_stride, ka.grid);
-      k_grid_clear<<<(unsigned)(((int64_t)B * kGridMaxCells + 255) / 256), 256, 0, s>>>(ka.grid, B);
-      k_grid_count<<<dim3(nb, (unsigned)B), 256, 0, s>>>(tgt_points, tgt_count, nt_stride, ka.grid);
-      k_grid_scan<<<B, 1024, 0, s>>>(ka.grid);
-      k_grid_scatter<<<dim3(nb, (unsigned)B), 256, 0, s>>>(tgt_points, tgt_count, nt_stride, ka.grid);
-    }
+  const dim3 grid((unsigned)((ns_stride + kIcpBlock - 1) / kIcpBlock), (unsigned)B);
+  if (sc.grid.params) {
+    // (build_grid == 0: `scratch` still holds the grid a previous call built for this very target)
+    if (build_grid) build_search_grid(tgt_points, tgt_count, nt_stride, B, sc.grid, s);
     k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, s>>>(ka);
   } else {
     k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, s>>>(ka);

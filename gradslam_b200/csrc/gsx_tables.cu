@@ -9,6 +9,7 @@
 //   k_records_from_table per table row: store the row as the pixel's winner (input of K4 for fuse_with_map)
 //   k_compact            generic stable compaction flag[] -> ascending indices (single-pass decoupled look-back)
 #include "gsx_common.cuh"
+#include "gsx_fusion_ws.cuh"
 #include "gsx_thresholds.h"
 #include "../../include/gsx.h"
 
@@ -22,90 +23,41 @@ struct CompactArgs {
   int64_t n;
   int64_t *out_idx;
   int64_t *out_count;
-  unsigned long long *state;  // (tiles)  epoch<<34 | flag<<32 | value
+  unsigned long long *state;  // (tiles) look-back tile states
   unsigned int *ticket;       // (1)
   int tiles;
   unsigned int epoch;
 };
 
-__device__ __forceinline__ unsigned long long t_ld_acquire(const unsigned long long *p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void t_st_release(unsigned long long *p, unsigned long long v) {
-  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
 __global__ void __launch_bounds__(kTB) k_compact(CompactArgs a) {
   __shared__ int s_tile, s_excl;
   __shared__ int s_warp[4][kTB / 32];
-  if (threadIdx.x == 0) {
-    const unsigned int t = atomicAdd(a.ticket, 1u);
-    if (t == (unsigned int)a.tiles - 1u) *a.ticket = 0u;  // last ticket drawn: re-arm for the next launch
-    s_tile = (int)t;
-  }
+  if (threadIdx.x == 0) s_tile = draw_tile_ticket(a.ticket, a.tiles);
   __syncthreads();
   const int tile = s_tile;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int64_t i[4];
   bool f[4];
-  int wex[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    i[j] = (int64_t)tile * (kTB * 4) + j * kTB + threadIdx.x;
-    f[j] = (i[j] < a.n) && (a.flags[i[j]] != 0);
-    const unsigned int ballot = __ballot_sync(0xffffffffu, f[j]);
-    wex[j] = __popc(ballot & ((1u << lane) - 1u));
-    if (lane == 0) s_warp[j][warp] = __popc(ballot);
-  }
-  __syncthreads();
-  int total = 0, bex[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    bex[j] = total;
-#pragma unroll
-    for (int w = 0; w < kTB / 32; ++w) {
-      const int c = s_warp[j][w];
-      if (w < warp) bex[j] += c;
-      total += c;
-    }
-  }
-  if (threadIdx.x == 0 && tile + 1 < a.tiles)
-    t_st_release(a.state + tile, ((unsigned long long)a.epoch << 34) | (1ull << 32) | (unsigned)total);
-  if (warp == 0) {
-    unsigned int excl = 0;
-    for (int base = tile - 1; base >= 0; base -= 32) {
-      const int j = base - lane;
-      unsigned long long s = 0ull;
-      if (j >= 0) {
-        do {
-          s = t_ld_acquire(a.state + j);
-        } while ((unsigned int)(s >> 34) != a.epoch);
-      }
-      const bool is_prefix = (j >= 0) && (((s >> 32) & 3ull) == 2ull);
-      const unsigned int pm = __ballot_sync(0xffffffffu, is_prefix);
-      const int first = pm ? (__ffs(pm) - 1) : 32;
-      const unsigned int v = (j >= 0 && lane <= first) ? (unsigned int)s : 0u;
-      excl += __reduce_add_sync(0xffffffffu, v);
-      if (pm) break;
-    }
-    if (lane == 0) {
-      if (tile + 1 < a.tiles)
-        t_st_release(a.state + tile, ((unsigned long long)a.epoch << 34) | (2ull << 32) | (excl + (unsigned)total));
-      s_excl = (int)excl;
-    }
+  int off[4];
+  const int total = block_offsets<kTB, 4>(
+      [&](int j) {
+        i[j] = (int64_t)tile * (kTB * 4) + j * kTB + threadIdx.x;
+        f[j] = (i[j] < a.n) && (a.flags[i[j]] != 0);
+        return f[j];
+      },
+      off, s_warp, [] {});
+  if (threadIdx.x == 0) publish_tile(a.state, tile, a.tiles, a.epoch, kTileAggregate, (unsigned)total);
+  if (threadIdx.x < 32) {
+    const unsigned int excl = lookback_warp(a.state, tile, a.tiles, a.epoch, (unsigned)total);
+    if (threadIdx.x == 0) s_excl = (int)excl;
   }
   __syncthreads();
 #pragma unroll
   for (int j = 0; j < 4; ++j)
-    if (f[j]) a.out_idx[(int64_t)s_excl + bex[j] + wex[j]] = i[j];
+    if (f[j]) a.out_idx[(int64_t)s_excl + off[j]] = i[j];
   if (tile == a.tiles - 1 && threadIdx.x == 0) *a.out_count = (int64_t)s_excl + total;
 }
 
 // ---- find_active_map_points ---------------------------------------------------------------------------------
-constexpr int kGeoW = 8;  // floats per packed geometry row (px,py,pz,nx,ny,nz,ccount,0), see gsx_fusion.cu
-
 struct ActiveArgs {
   const float *geo;
   const int32_t *counts;
@@ -115,18 +67,15 @@ struct ActiveArgs {
   int64_t pose_bstride;
   const float *K;
   int64_t K_bstride;
-  int B, H, W;
-  float u_hi, v_hi;
+  ImageBounds ib;
   uint8_t *flags;  // (B, width)
   int32_t *hw;     // (B, width)  h * W + w
 };
 
 __global__ void __launch_bounds__(kTB) k_active_eval(ActiveArgs a) {
-  __shared__ Rigid s_tinv;
-  __shared__ float s_k[12];
+  __shared__ LiveCamera s_cam;
   const int b = blockIdx.y;
-  if (threadIdx.x == 0) s_tinv = rigid_inverse(load_rigid(a.poses + b * a.pose_bstride));
-  if (threadIdx.x >= 32 && threadIdx.x < 44) s_k[threadIdx.x - 32] = __ldg(a.K + b * a.K_bstride + (threadIdx.x - 32));
+  load_live_camera(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b);
   __syncthreads();
   const int64_t n = (int64_t)blockIdx.x * kTB + threadIdx.x;
   if (n >= a.width) return;
@@ -134,17 +83,9 @@ __global__ void __launch_bounds__(kTB) k_active_eval(ActiveArgs a) {
   int pix = 0;
   if (live) {
     const float4 p = __ldg(reinterpret_cast<const float4 *>(a.geo + ((int64_t)b * a.cap + n) * kGeoW));
-    const float3 q = rigid_apply(s_tinv, p.x, p.y, p.z);
-    const float hx = ((s_k[0] * q.x + s_k[1] * q.y) + s_k[2] * q.z) + s_k[3];
-    const float hy = ((s_k[4] * q.x + s_k[5] * q.y) + s_k[6] * q.z) + s_k[7];
-    const float hz = ((s_k[8] * q.x + s_k[9] * q.y) + s_k[10] * q.z) + s_k[11];
-    const float den = (hz != 0.0f) ? hz : 1.0f;
-    const float u = hx / den, v = hy / den;
-    live = (u > -1e-3f) && (u < a.u_hi) && (v > -1e-3f) && (v < a.v_hi) && (q.z > 0.0f);
-    int w = (int)rintf(u), h = (int)rintf(v);
-    w = min(max(w, 0), a.W - 1);
-    h = min(max(h, 0), a.H - 1);
-    pix = h * a.W + w;
+    const PixelHit hit = project(s_cam, a.ib, p.x, p.y, p.z);
+    live = hit.in_frustum;
+    pix = hit.h * a.ib.W + hit.w;
   }
   a.flags[(int64_t)b * a.width + n] = live ? 1 : 0;
   a.hw[(int64_t)b * a.width + n] = pix;
@@ -192,14 +133,10 @@ __global__ void __launch_bounds__(kTB) k_unique_select(RowArgs a) {
   if (!row_ok(a, b, n, h, w)) return;
   const float *p = a.geo + (b * a.cap + n) * kGeoW;
   const float *g = a.gv + ((b * a.H + h) * a.W + w) * 3;
-  // key of fusionutils.py:491-517: 1/(cc+1e-20), then (map - frame)^2 summed left to right, then n
+  // key (1/(cc+1e-20), (map - frame)^2 summed left to right, n)
   const float dx = __ldg(p) - __ldg(g), dy = __ldg(p + 1) - __ldg(g + 1), dz = __ldg(p + 2) - __ldg(g + 2);
   const float d2 = (dx * dx + dy * dy) + dz * dz;
-  const float inv_cc = 1.0f / (__ldg(p + 6) + 1e-20f);
-  unsigned int kb = __float_as_uint(inv_cc);
-  kb = (kb & 0x80000000u) ? ~kb : (kb | 0x80000000u);
-  const unsigned int rb = __float_as_uint(d2) | 0x80000000u;
-  atomic_min_key128(a.best + (b * a.H + h) * a.W + w, ((unsigned long long)kb << 32) | rb, (unsigned long long)n);
+  atomic_min_key128(a.best + (b * a.H + h) * a.W + w, argmin_key_hi(__ldg(p + 6), d2), (unsigned long long)n);
 }
 
 __global__ void __launch_bounds__(kTB) k_records_from_table(RowArgs a) {
@@ -258,8 +195,8 @@ extern "C" int gsx_active_eval(const float *map_geometry, const int32_t *counts,
   GSX_CHECK_ARG(B >= 1 && H >= 1 && W >= 1 && width >= 0 && width <= capacity, "gsx_active_eval: bad extents");
   GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_geometry) & 15) == 0, "gsx_active_eval: geometry rows must be 16-byte aligned");
   if (width == 0) return 0;
-  ActiveArgs a{map_geometry, counts, capacity, width, poses, pose_bstride, intrinsics, K_bstride, B, H, W,
-               (float)(W - 0.999), (float)(H - 0.999), flags, hw};
+  ActiveArgs a{map_geometry, counts, capacity, width, poses, pose_bstride, intrinsics, K_bstride, image_bounds(H, W),
+               flags, hw};
   k_active_eval<<<dim3((unsigned)tb_blocks(width), (unsigned)B), kTB, 0, (cudaStream_t)stream>>>(a);
   GSX_CHECK_LAUNCH("gsx_active_eval");
   return 0;
@@ -302,9 +239,8 @@ extern "C" int gsx_records_from_table(const int64_t *table, int64_t rows, int64_
                                       void *workspace, void *stream) {
   if (rows == 0) return 0;
   GSX_CHECK_ARG(table && workspace, "gsx_records_from_table: null pointer");
-  const int64_t best_offset = ((int64_t)B * H * W * 32 + 255) / 256 * 256;  // frame records come first (gsx_fusion.cu)
   RowArgs a{table, rows, nullptr, capacity, nullptr, nullptr, B, H, W, 0.f, 0.f, nullptr,
-            (U128 *)((char *)workspace + best_offset)};
+            fusion_workspace(workspace, B, H, W).best};
   k_records_from_table<<<(unsigned)tb_blocks(rows), kTB, 0, (cudaStream_t)stream>>>(a);
   GSX_CHECK_LAUNCH("gsx_records_from_table");
   return 0;
