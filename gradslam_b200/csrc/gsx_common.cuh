@@ -30,9 +30,8 @@ void set_error(const char *fmt, ...);
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
-// floats per packed map row / frame record (DESIGN.md section 2): geometry (px,py,pz,nx,ny,nz,ccount,0), colour
-// (r,g,b,0), frame record (gvx,gvy,gvz,gnx,gny,gnz,alpha,depth)
-constexpr int kGeoW = 8, kColW = 4, kRecW = 8;
+// floats per packed map row (DESIGN.md section 2): geometry (px,py,pz,nx,ny,nz,ccount,0), colour (r,g,b,0)
+constexpr int kGeoW = 8, kColW = 4;
 
 // Scratch and workspace layouts are each written once, as a function that walks a Carver over the allocation:
 // take<T>(n) hands out the next 256-byte aligned slot of n T's.  Given the allocation's base the function returns
@@ -116,6 +115,30 @@ __device__ __forceinline__ float3 backproject(const KInv &k, float u, float v, f
   p.y = ((k.k11 * v + k.k12) * d) * vf;
   p.z = d * vf;
   return p;
+}
+
+// world-frame vertex of a pixel with depth d and local vertex v: (R v + t) * valid, or v itself when pose == nullptr
+// (world frame == camera frame).  K1r's gv, and what the fusion consumers recompute from the depth in the frame record.
+__device__ __forceinline__ float3 world_vertex(const Rigid *pose, const float3 &v, float d) {
+  if (!pose) return v;
+  const float vf = d > 0.0f ? 1.0f : 0.0f;
+  float3 g = rigid_apply(*pose, v.x, v.y, v.z);
+  g.x *= vf; g.y *= vf; g.z *= vf;
+  return g;
+}
+
+// The camera a frame was back-projected with (K1r's K^-1 and camera-to-world pose), kept per element in the fusion
+// workspace so that K2 and K4 recompute a pixel's vertex from its depth with exactly K1r's operands.
+struct FrameCamera {
+  Rigid pose;
+  KInv k;
+  int posed;  // 0: no pose, world frame == camera frame
+};
+__device__ __forceinline__ float3 frame_local_vertex(const FrameCamera &c, int h, int w, float d) {
+  return backproject(c.k, (float)w, (float)h, d);
+}
+__device__ __forceinline__ float3 frame_world_vertex(const FrameCamera &c, const float3 &v, float d) {
+  return world_vertex(c.posed ? &c.pose : nullptr, v, d);
 }
 
 // Vertex and normal of pixel (h,w) of depth image `dimg`, in the camera frame and (if pose != nullptr) in the
@@ -204,14 +227,8 @@ __device__ __forceinline__ FrameSample frame_sample_from(const DepthStencil &t, 
   const float dhx = a1.x - a0.x, dhy = a1.y - a0.y, dhz = a1.z - a0.z;
   const float dvx = b1.x - b0.x, dvy = b1.y - b0.y, dvz = b1.z - b0.z;
   s.n = normalize_masked(cross_ref(dhx, dhy, dhz, dvx, dvy, dvz), vf);
-  if (pose) {
-    s.gv = rigid_apply(*pose, s.v.x, s.v.y, s.v.z);
-    s.gv.x *= vf; s.gv.y *= vf; s.gv.z *= vf;
-    s.gn = rotate(*pose, s.n.x, s.n.y, s.n.z);
-  } else {
-    s.gv = s.v;
-    s.gn = s.n;
-  }
+  s.gv = world_vertex(pose, s.v, s.d);
+  s.gn = pose ? rotate(*pose, s.n.x, s.n.y, s.n.z) : s.n;
   return s;
 }
 
@@ -224,14 +241,8 @@ __device__ __forceinline__ FrameSample frame_sample(const float *__restrict__ di
   const float vf = dc > 0.0f ? 1.0f : 0.0f;
   s.v = backproject(k, (float)w, (float)h, dc);
   s.n = kWantNormal ? frame_normal(dimg, k, h, w, H, W, s.v, vf) : make_float3(0.f, 0.f, 0.f);
-  if (pose) {
-    s.gv = rigid_apply(*pose, s.v.x, s.v.y, s.v.z);
-    s.gv.x *= vf; s.gv.y *= vf; s.gv.z *= vf;
-    s.gn = kWantNormal ? rotate(*pose, s.n.x, s.n.y, s.n.z) : s.n;
-  } else {
-    s.gv = s.v;
-    s.gn = s.n;
-  }
+  s.gv = world_vertex(pose, s.v, dc);
+  s.gn = (pose && kWantNormal) ? rotate(*pose, s.n.x, s.n.y, s.n.z) : s.n;
   return s;
 }
 

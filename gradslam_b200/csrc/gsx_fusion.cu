@@ -1,8 +1,9 @@
 // Fused PointFusion map update for sm_90a.
-//   k_frame_records   (K1r)    one thread per live pixel: world-frame vertex / normal, confidence weight and depth of the
-//                              pixel as ONE 32-byte record (the whole op chain of rgbdimages.py:643-762 and
-//                              fusionutils.py:16-73, evaluated once per pixel); also re-arms the per-frame workspace.
-//   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, ONE 32-byte gather of
+//   k_frame_records   (K1r)    one thread per live pixel: world-frame normal and depth of the pixel as ONE 16-byte record
+//                              (the normal's op chain of rgbdimages.py:643-762, evaluated once per pixel), plus the
+//                              element's camera; also re-arms the per-frame workspace.  Consumers re-evaluate the world
+//                              vertex and the confidence weight (fusionutils.py:16-73) from the depth, bit for bit.
+//   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, ONE 16-byte gather of
 //                              the frame record under the projection, distance / normal tests, then a 128-bit atomic
 //                              arg-min per pixel on the key (1/ccount, ray distance, row index).
 //   k_merge_append    (K4)     one thread per pixel: confidence-weighted merge of the selected map row, or stable append of
@@ -51,6 +52,39 @@ struct FrameRecArgs {
 
 constexpr int kRecTW = 32, kRecTH = 8;  // pixel tile of one K1r CTA
 
+// element b's FrameHeader, by one thread of the element's first K1r CTA once s_k / s_pose are loaded.  k == nullptr:
+// the records are packed from caller-supplied maps (no camera); pose == nullptr: world frame == camera frame.  Fields a
+// record kind does not use stay zero.
+__device__ __forceinline__ void store_frame_header(const FrameRecArgs &a, int b, const KInv *k, const Rigid *pose) {
+  FrameHeader hd = {};
+  if (k) hd.cam.k = *k;
+  if (pose) hd.cam.pose = *pose;
+  hd.cam.posed = pose != nullptr;
+  hd.two_sigma_sq = a.two_sigma_sq;
+  hd.from_maps = k == nullptr;
+  a.ws.hdr[b] = hd;
+}
+
+// What the 16-byte frame record of pixel (h,w) with depth d leaves out: K1r's world vertex (x,y,z) and, if kAlpha, its
+// confidence weight (w) - re-evaluated with K1r's device functions and operands, so bit for bit the values K1r had.
+template <bool kAlpha>
+__device__ __forceinline__ float4 record_vertex(const FrameHeader &hd, const float4 *vrec, int h, int w, int W,
+                                                float d) {
+  if (hd.from_maps) return __ldg(vrec + h * W + w);
+  const float3 v = frame_local_vertex(hd.cam, h, w, d);
+  const float3 g = frame_world_vertex(hd.cam, v, d);
+  // alpha from the LOCAL vertex (fusionutils.py:657, 69-72)
+  return make_float4(g.x, g.y, g.z,
+                     kAlpha ? confidence_alpha((v.x * v.x + v.y * v.y) + v.z * v.z, hd.two_sigma_sq) : 0.0f);
+}
+
+// element b's header into shared memory, one word per thread of threads 64..; the caller synchronises
+__device__ __forceinline__ void load_frame_header(FrameHeader &s, const FrameHeader *g) {
+  constexpr int kWords = (int)(sizeof(FrameHeader) / 4);
+  const int i = (int)threadIdx.x - 64;
+  if (i >= 0 && i < kWords) reinterpret_cast<int *>(&s)[i] = __ldg(reinterpret_cast<const int *>(g) + i);
+}
+
 template <bool kFromMaps>
 __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records(FrameRecArgs a) {
   __shared__ Rigid s_pose;
@@ -66,29 +100,24 @@ __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records(FrameRecArgs a
   if (lin < a.ws.tiles) a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
   if (lin == 0) a.ws.ticket[b] = 0u;
   if (!kFromMaps) __syncthreads();
+  if (lin == 0) store_frame_header(a, b, kFromMaps ? nullptr : &s_k, (!kFromMaps && a.poses) ? &s_pose : nullptr);
   const int w = blockIdx.x * kRecTW + threadIdx.x, h = blockIdx.y * kRecTH + threadIdx.y;
   if (w >= a.W || h >= a.H) return;
   const int P = a.H * a.W;
   const int pix = h * a.W + w;
+  const int64_t i = (int64_t)b * P + pix;
   const float *dimg = a.depth + b * a.depth_bstride;
-  float4 r0, r1;
   if (kFromMaps) {
-    const int64_t o = ((int64_t)b * P + pix) * 3;
+    const int64_t o = i * 3;
     const float vx = __ldg(a.vloc + o), vy = __ldg(a.vloc + o + 1), vz = __ldg(a.vloc + o + 2);
-    r0 = make_float4(__ldg(a.gv + o), __ldg(a.gv + o + 1), __ldg(a.gv + o + 2), __ldg(a.gn + o));
-    r1 = make_float4(__ldg(a.gn + o + 1), __ldg(a.gn + o + 2),
-                     confidence_alpha((vx * vx + vy * vy) + vz * vz, a.two_sigma_sq), __ldg(dimg + pix));
+    a.ws.nrec[i] = make_float4(__ldg(a.gn + o), __ldg(a.gn + o + 1), __ldg(a.gn + o + 2), __ldg(dimg + pix));
+    a.ws.vrec[i] = make_float4(__ldg(a.gv + o), __ldg(a.gv + o + 1), __ldg(a.gv + o + 2),
+                               confidence_alpha((vx * vx + vy * vy) + vz * vz, a.two_sigma_sq));
   } else {
     const FrameSample f = frame_sample<true>(dimg, s_k, a.poses ? &s_pose : nullptr, h, w, a.H, a.W);
-    // alpha from the LOCAL vertex (fusionutils.py:657, 69-72)
-    const float s = (f.v.x * f.v.x + f.v.y * f.v.y) + f.v.z * f.v.z;
-    r0 = make_float4(f.gv.x, f.gv.y, f.gv.z, f.gn.x);
-    r1 = make_float4(f.gn.y, f.gn.z, confidence_alpha(s, a.two_sigma_sq), f.d);
+    a.ws.nrec[i] = make_float4(f.gn.x, f.gn.y, f.gn.z, f.d);
   }
-  float4 *rec = reinterpret_cast<float4 *>(a.ws.frec + ((int64_t)b * P + pix) * kRecW);
-  rec[0] = r0;
-  rec[1] = r1;
-  a.ws.best[(int64_t)b * P + pix] = U128{0ull, 0ull};
+  a.ws.best[i] = U128{0ull, 0ull};
 }
 
 // The same kernel with the depth tile staged by the TMA unit: the frame is a regular grid, so the (32 + halo) x (8 + halo)
@@ -132,6 +161,7 @@ __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records_tma(const __gr
   if (lin < a.ws.tiles) a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
   if (lin == 0) a.ws.ticket[b] = 0u;
   __syncthreads();
+  if (lin == 0) store_frame_header(a, b, &s_k, a.poses ? &s_pose : nullptr);
   {  // wait for the tile (phase 0 of the barrier)
     unsigned int done = 0;
     while (!done)
@@ -153,11 +183,7 @@ __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records_tma(const __gr
   t.u = s_d[ha - h0][threadIdx.x];
   t.d = s_d[ha - h0 + 1][threadIdx.x];
   const FrameSample f = frame_sample_from(t, s_k, a.poses ? &s_pose : nullptr, h, w, a.H, a.W);
-  // alpha from the LOCAL vertex (fusionutils.py:657, 69-72)
-  const float s = (f.v.x * f.v.x + f.v.y * f.v.y) + f.v.z * f.v.z;
-  float4 *rec = reinterpret_cast<float4 *>(a.ws.frec + ((int64_t)b * P + pix) * kRecW);
-  rec[0] = make_float4(f.gv.x, f.gv.y, f.gv.z, f.gn.x);
-  rec[1] = make_float4(f.gn.y, f.gn.z, confidence_alpha(s, a.two_sigma_sq), f.d);
+  a.ws.nrec[(int64_t)b * P + pix] = make_float4(f.gn.x, f.gn.y, f.gn.z, f.d);
   a.ws.best[(int64_t)b * P + pix] = U128{0ull, 0ull};
 }
 
@@ -228,7 +254,8 @@ struct ProjectArgs {
   ImageBounds ib;
   float dot_th;
   float d2_max;  // largest float x with sqrtf(x) < dist_th (-1 if none): sqrtf(d2) < dist_th <=> d2 <= d2_max
-  const float *frec;
+  const float4 *nrec, *vrec;
+  const FrameHeader *hdr;
   U128 *best;
   unsigned long long *stats;
 };
@@ -250,23 +277,26 @@ __device__ __forceinline__ MapRow load_map_row(const float *geo, int64_t n) {
 // The kernel is bound by (threads in flight) / (length of the dependent memory chain) and by instruction issue, not by
 // bytes, so the chain is kept short and the per-row work small:
 //   * the map row of the NEXT grid-stride iteration is fetched while the current row is processed (software pipelining);
-//   * everything the tests need from the frame sits in ONE 32-byte record under the projection (K1r): one gather;
+//   * the tests need ONE 16-byte gather of the frame record under the projection (K1r's normal and depth; the vertex is
+//     re-evaluated from the depth, ~20 flops): two records share a 32-byte sector, so neighbouring rows share sectors;
 //   * sqrtf(d2) < dist_th is decided as d2 <= d2_max (exact: the correctly rounded square root is monotonic; the
 //     threshold is found on the host, gsx_thresholds.h);
 //   * the result of the 128-bit CAS is only looked at one iteration later.
 __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectArgs a) {
   __shared__ LiveCamera s_cam;
+  __shared__ FrameHeader s_hdr;
   __shared__ unsigned int s_act[kBlock / 32];
   const int b = blockIdx.y;
   const int count = a.counts[b];
   if ((int64_t)blockIdx.x * kBlock >= count) return;
   load_live_camera(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b);
+  load_frame_header(s_hdr, a.hdr + b);
+  if (threadIdx.x < kBlock / 32) s_act[threadIdx.x] = 0u;
   __syncthreads();
   const int P = a.ib.H * a.ib.W;
   const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
-  const float *frec = a.frec + (int64_t)b * P * kRecW;
+  const float4 *nrec = a.nrec + (int64_t)b * P, *vrec = a.vrec + (int64_t)b * P;
   U128 *best = a.best + (int64_t)b * P;
-  unsigned int n_active = 0;
   const int64_t stride = (int64_t)gridDim.x * kBlock;
   int64_t n = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   U128 mine{0ull, 0ull}, old{0ull, 0ull};
@@ -278,15 +308,18 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
     if (nn < count) cur = load_map_row(geo, nn);  // in flight while this row is processed
     const PixelHit hit = project(s_cam, a.ib, m.a.x, m.a.y, m.a.z);
     if (hit.in_frustum) {
-      ++n_active;
+      {  // count the row (bookkeeping): one shared-memory add per converged group of lanes, no register kept for it
+        const unsigned int am = __activemask();
+        if ((int)(threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(s_act + (threadIdx.x >> 5), (unsigned int)__popc(am));
+      }
       const int pix = hit.h * a.ib.W + hit.w;
-      const float4 f0 = __ldg(reinterpret_cast<const float4 *>(frec + (int64_t)pix * kRecW));
-      const float2 f1 = __ldg(reinterpret_cast<const float2 *>(frec + (int64_t)pix * kRecW + 4));
-      // are_points_close (fusionutils.py:130): ||frame - map|| < dist_th
-      const float dx = f0.x - m.a.x, dy = f0.y - m.a.y, dz = f0.z - m.a.z;
-      const float d2 = (dx * dx + dy * dy) + dz * dz;
+      const float4 fn = __ldg(nrec + pix);
       // are_normals_similar (fusionutils.py:187-195): n_frame . n_map > dot_th
-      const float dot = (f0.w * m.a.w + f1.x * m.b.x) + f1.y * m.b.y;
+      const float dot = (fn.x * m.a.w + fn.y * m.b.x) + fn.z * m.b.y;
+      const float4 fv = record_vertex<false>(s_hdr, vrec, hit.h, hit.w, a.ib.W, fn.w);
+      // are_points_close (fusionutils.py:130): ||frame - map|| < dist_th
+      const float dx = fv.x - m.a.x, dy = fv.y - m.a.y, dz = fv.z - m.a.z;
+      const float d2 = (dx * dx + dy * dy) + dz * dz;
       const bool live = (d2 <= a.d2_max) && (dot > a.dot_th);
       if (pend_pix >= 0) {  // settle the previous candidate's CAS before re-using the slot
         atomic_max_rec128_finish(best + pend_pix, mine, old);
@@ -303,8 +336,6 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
   if (pend_pix >= 0) atomic_max_rec128_finish(best + pend_pix, mine, old);
   // bookkeeping for the roofline's algorithmic-byte count: ONE atomic per CTA (every warp of the grid adding to the same
   // address would serialise thousands of same-address atomics in the L2 when the whole grid works on one map)
-  n_active = __reduce_add_sync(0xffffffffu, n_active);
-  if ((threadIdx.x & 31) == 0) s_act[threadIdx.x >> 5] = n_active;
   __syncthreads();
   if (threadIdx.x == 0) {
     unsigned int t = 0;
@@ -364,11 +395,13 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   __shared__ int s_matched[kMB / 32];
   __shared__ int s_excl;
   __shared__ __align__(16) float s_rgb[kTilePix * 3];
+  __shared__ FrameHeader s_hdr;
   // batch element varies fastest in the grid: CTAs resident at the same time belong to different elements, so
   // each element's look-back chain only sees ~1/B of the in-flight tiles
   const int b = blockIdx.x % a.B;
   const int T = a.ws.tiles;
   if (threadIdx.x == 0) s_tile = (int)atomicAdd(a.ws.ticket + b, 1u);  // tiles start in ticket order
+  load_frame_header(s_hdr, a.ws.hdr + b);
   const int count_in = a.counts_in[b];  // loaded early: its latency hides behind everything below
   __syncthreads();
   const int tile = s_tile;
@@ -376,7 +409,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int pix0 = tile * kTilePix;
   const U128 *best = a.ws.best + (int64_t)b * P;
-  const float *frec = a.ws.frec + (int64_t)b * P * kRecW;
+  const float4 *nrec = a.ws.nrec + (int64_t)b * P, *vrec = a.ws.vrec + (int64_t)b * P;
   const float *rgb = a.rgb + b * a.rgb_bstride + (int64_t)pix0 * 3;
 
   // live colours of the tile: coalesced 128-bit loads into shared memory (stride-3 reads are conflict free)
@@ -392,17 +425,16 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
 
   int pix[kPix];
   unsigned long long rec_lo[kPix];
-  float4 f0[kPix], f1[kPix];
+  float4 fn[kPix];
   bool matched[kPix], is_new[kPix];
 #pragma unroll
   for (int j = 0; j < kPix; ++j) {
     pix[j] = pix0 + j * kMB + threadIdx.x;
     U128 rec{0ull, 0ull};
-    f0[j] = f1[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    fn[j] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (pix[j] < P) {
       rec = best[pix[j]];
-      f0[j] = __ldg(reinterpret_cast<const float4 *>(frec + (int64_t)pix[j] * kRecW));
-      f1[j] = __ldg(reinterpret_cast<const float4 *>(frec + (int64_t)pix[j] * kRecW + 4));
+      fn[j] = __ldg(nrec + pix[j]);
     }
     matched[j] = a.with_cc && ((rec.lo | rec.hi) != 0ull);
     rec_lo[j] = rec.lo;
@@ -415,7 +447,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   int new_off[kPix];  // position of each new pixel among the tile's new pixels (row-major)
   const int block_total = block_offsets<kMB, kPix>(
       [&](int j) {
-        is_new[j] = (pix[j] < P) && (f1[j].w > 0.0f) && !matched[j];
+        is_new[j] = (pix[j] < P) && (fn[j].w > 0.0f) && !matched[j];
         return is_new[j];
       },
       new_off, s_warp_sums,
@@ -433,6 +465,16 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   float *col = a.col + (int64_t)b * a.cap * kColW;
 
+  // what the frame record leaves out, for every pixel that is merged or appended
+  float4 fv[kPix];
+#pragma unroll
+  for (int j = 0; j < kPix; ++j) {
+    if (matched[j] || is_new[j]) {
+      const int ph = pix[j] / a.W;
+      fv[j] = record_vertex<true>(s_hdr, vrec, ph, pix[j] - ph * a.W, a.W, fn[j].w);
+    }
+  }
+
   // matched map rows: issue all loads first, then the arithmetic and the stores
   float4 g0[kPix], g1[kPix], c4[kPix];
 #pragma unroll
@@ -449,18 +491,18 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
     if (matched[j]) {
       // confidence-weighted running mean (fusionutils.py:678-699); exactly one pixel owns this map row
       const int64_t n = (int64_t)(~rec_lo[j]);
-      const float alpha = f1[j].z;
+      const float alpha = fv[j].w;
       const float c0 = g1[j].z;
       const float tot = c0 + alpha;
       const float inv = 1.0f / ((tot == 0.0f) ? 1.0f : tot);
       const float *fc = s_rgb + (j * kMB + (int)threadIdx.x) * 3;
       float4 o0, o1, oc;
-      o0.x = ((c0 * g0[j].x) + (alpha * f0[j].x)) * inv;
-      o0.y = ((c0 * g0[j].y) + (alpha * f0[j].y)) * inv;
-      o0.z = ((c0 * g0[j].z) + (alpha * f0[j].z)) * inv;
-      o0.w = ((c0 * g0[j].w) + (alpha * f0[j].w)) * inv;
-      o1.x = ((c0 * g1[j].x) + (alpha * f1[j].x)) * inv;
-      o1.y = ((c0 * g1[j].y) + (alpha * f1[j].y)) * inv;
+      o0.x = ((c0 * g0[j].x) + (alpha * fv[j].x)) * inv;
+      o0.y = ((c0 * g0[j].y) + (alpha * fv[j].y)) * inv;
+      o0.z = ((c0 * g0[j].z) + (alpha * fv[j].z)) * inv;
+      o0.w = ((c0 * g0[j].w) + (alpha * fn[j].x)) * inv;
+      o1.x = ((c0 * g1[j].x) + (alpha * fn[j].y)) * inv;
+      o1.y = ((c0 * g1[j].y) + (alpha * fn[j].z)) * inv;
       o1.z = tot;
       o1.w = 0.0f;
       oc.x = ((c0 * c4[j].x) + (alpha * fc[0])) * inv;
@@ -488,9 +530,9 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
       const int64_t n = base + new_off[j];
       if (n < a.cap) {
         const float *fc = s_rgb + (j * kMB + (int)threadIdx.x) * 3;
-        *reinterpret_cast<float4 *>(geo + n * kGeoW) = f0[j];
+        *reinterpret_cast<float4 *>(geo + n * kGeoW) = make_float4(fv[j].x, fv[j].y, fv[j].z, fn[j].x);
         *reinterpret_cast<float4 *>(geo + n * kGeoW + 4) =
-            make_float4(f1[j].x, f1[j].y, a.with_cc ? f1[j].z : 0.0f, 0.0f);
+            make_float4(fn[j].y, fn[j].z, a.with_cc ? fv[j].w : 0.0f, 0.0f);
         *reinterpret_cast<float4 *>(col + n * kColW) = make_float4(fc[0], fc[1], fc[2], 0.0f);
         if (kAssoc) a.assoc[(int64_t)b * P + pix[j]] = (int32_t)(n + 1);
       } else {
@@ -654,7 +696,9 @@ __global__ void __launch_bounds__(256) k_merge_bwd_pixels(MergeBwdArgs a) {
 static Workspace group_workspace(void *workspace, int B_total, int b0, int H, int W) {
   const int64_t P = (int64_t)H * W;
   Workspace ws = fusion_workspace(workspace, B_total, H, W);
-  ws.frec += (int64_t)b0 * P * kRecW;
+  ws.nrec += (int64_t)b0 * P;
+  ws.vrec += (int64_t)b0 * P;
+  ws.hdr += b0;
   ws.best += (int64_t)b0 * P;
   ws.tile_state += (int64_t)b0 * ws.tiles;
   ws.ticket += b0;
@@ -679,7 +723,7 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
   if (max_count > 0) {
     ProjectArgs pa{ggeo, cin + b0, cap, poses + (int64_t)b0 * pose_bs, pose_bs, K + (int64_t)b0 * K_bs, K_bs, nb,
-                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
+                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.best, ws.stats};
     const int rc = launch_project_select(pa, max_count, st);
     if (rc) return rc;
   }
@@ -738,7 +782,7 @@ extern "C" int gsx_fusion_project_select(const float *map_geometry, const int32_
                 (long long)max_count, (long long)capacity);
   const Workspace ws = fusion_workspace(workspace, B, H, W);
   ProjectArgs a{map_geometry, counts, capacity, poses, pose_bstride, intrinsics, K_bstride, B, image_bounds(H, W),
-                dot_th, sqrt_lt_threshold(dist_th), ws.frec, ws.best, ws.stats};
+                dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.best, ws.stats};
   return launch_project_select(a, max_count, (cudaStream_t)stream);
 }
 

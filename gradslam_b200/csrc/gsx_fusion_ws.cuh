@@ -11,7 +11,19 @@ constexpr int kMB = 256;              // threads per CTA of the merge/append ker
 constexpr int kPix = GSX_KPIX;        // pixels per thread
 constexpr int kTilePix = kMB * kPix;  // pixels per merge tile
 
-//   float  frec[B][P][8]       frame records (gvx,gvy,gvz,gnx,gny,gnz,alpha,depth)             written by K1r
+// How K2 / K4 get a pixel's world vertex and confidence weight, per batch element (written by K1r).  From depth, the
+// frame record keeps only (normal, depth): the vertex is ~20 flops from the depth and the camera (no division, no square
+// root), the weight one exp, so re-evaluating them beats moving them through DRAM.  Caller-supplied maps (differentiable
+// mode) need not equal that re-evaluation, so their vertex and weight are stored in vrec.
+struct FrameHeader {
+  FrameCamera cam;     // K1r's K^-1 and pose
+  float two_sigma_sq;  // of the confidence weight
+  int from_maps;       // 1: vertex and weight are in vrec
+};
+
+//   float4 nrec[B][P]          frame records (gnx,gny,gnz,depth)                                written by K1r
+//   float4 vrec[B][P]          (gvx,gvy,gvz,alpha), only for caller-supplied maps               written by K1r
+//   FrameHeader hdr[B]         how to re-evaluate vertex / weight from depth                    written by K1r
 //   U128   best[B][P]          complemented arg-min records (0 = empty)                         cleared by K1r
 //   uint64 tile_state[B][T]    look-back state of K4's scan (epoch 1), T = ceil(P / kTilePix)  cleared by K1r
 //   uint32 ticket[B]           dynamic tile ids of K4                                           cleared by K1r
@@ -19,7 +31,8 @@ constexpr int kTilePix = kMB * kPix;  // pixels per merge tile
 // Nothing in here has to survive from one frame to the next (the stats are bookkeeping only): every frame's K1r
 // re-arms what K2 / K4 of that frame consume, so a failed or abandoned call cannot poison a later one.
 struct Workspace {
-  float *frec;
+  float4 *nrec, *vrec;
+  FrameHeader *hdr;
   U128 *best;
   unsigned long long *tile_state;
   unsigned int *ticket;
@@ -33,7 +46,9 @@ inline Workspace fusion_workspace(void *base, int B, int H, int W, int64_t *byte
   Carver c(base);
   Workspace w;
   w.tiles = (int)((P + kTilePix - 1) / kTilePix);
-  w.frec = c.take<float>(B * P * kRecW);
+  w.nrec = c.take<float4>(B * P);
+  w.vrec = c.take<float4>(B * P);
+  w.hdr = c.take<FrameHeader>(B);
   w.best = c.take<U128>(B * P);
   w.tile_state = c.take<unsigned long long>((int64_t)B * w.tiles);
   w.ticket = c.take<unsigned int>(B);

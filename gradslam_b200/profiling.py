@@ -5,7 +5,7 @@ from Python with a CUDA event between launches, and reads the device-side counte
 algorithmic byte count of every launch comes from the run itself (SURVEY.md §8d).  The step's algorithmic bytes are
 SURVEY's fusion-step formula  16*P + 12*M + 16*A + 12*U + 40*U + 40*New;  they are attributed to the kernels as
 
-    K1r frame records                            4*P                (the depth image; its 32-byte records are an
+    K1r frame records                            4*P                (the depth image; its 16-byte records are an
                                                                      internal intermediate, not algorithmic traffic)
     K2  project+select                           12*M + 16*A        (map positions; normal+ccount of active)
     K4  merge+append                             12*P + 52*U + 40*New  (rgb; read colour 12 + write 40 per merged

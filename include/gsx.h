@@ -68,8 +68,9 @@ int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const
 
 /* ------------------------------------------------------------------------------------------------
  * Fused PointFusion map update, one live frame for all B elements: three kernels
- *   K1r  gsx_fusion_frame_records    per pixel: world vertex, world normal, confidence weight, depth -> one
- *                                    32-byte record; re-arms the workspace for this frame
+ *   K1r  gsx_fusion_frame_records    per pixel: world normal, depth -> one 16-byte record (the world vertex and
+ *                                    confidence weight are re-evaluated from the depth where they are needed);
+ *                                    re-arms the workspace for this frame
  *   K2   gsx_fusion_project_select   per map row: projection, tests, per-pixel 128-bit arg-min
  *   K4   gsx_fusion_merge_append     per pixel: merge the selected row or append a new surfel
  * replaces update_map_fusion = find_active_map_points + find_similar_map_points +
