@@ -449,7 +449,11 @@ def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numite
     int32 sizes (Bn,).  One chain of batched ops for all elements; returns (T (Bn,4,4), last nn idx (Bn,Ns), -1 = none).
     Per element the values are bit-identical to the per-element chain and to the fused no-grad loop."""
     dev = src.device
-    Bn = src.shape[0]
+    Bn, Ns = src.shape[0], src.shape[1]
+    # No valid source (or target) point in any element gives a padded width of 0, which the kernels reject.  One zero
+    # padding row (the sizes stay 0) makes every element an empty element of a ragged batch, as the fused loop sees it.
+    pad = lambda t: torch.cat([t, t.new_zeros(Bn, 1, 3)], 1) if t.shape[1] == 0 else t
+    src, tgt, tgt_n = pad(src), pad(tgt), pad(tgt_n)
     dampt = torch.full((Bn,), float(damp), dtype=torch.float32, device=dev)
     T = (torch.eye(4, dtype=torch.float32, device=dev).repeat(Bn, 1, 1) if T0 is None
          else T0.to(torch.float32).expand(Bn, 4, 4).contiguous())
@@ -465,7 +469,7 @@ def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numite
         dampt, dT_applied, T = _UpdateBatchedFn.apply(xi, sums[:, 27], sums_next[:, 27], dampt, T, mode, lambda_max, B,
                                                       B2, nu)
         cur = _RigidTransformBatchedFn.apply(cur, dT_applied, src_counts)
-    return T, idx
+    return T, (None if idx is None else idx[:, :Ns])
 
 
 def _normal_equations(src, tgt, tgt_n, dist_thresh):

@@ -18,6 +18,18 @@ from .fusionutils import update_map_aggregate
 __all__ = ["ICPSLAM"]
 
 
+def _compose_canonical(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """a · b for rigid (..., 4, 4) transforms in the canonical order of the fused step's k_pose_compose: every entry is
+    (a_i0 b_0j + a_i1 b_1j) + a_i2 b_2j (+ a_i3 in the last column), each product and sum rounded on its own.  A
+    matmul may fuse or reorder these (cuBLAS does, at some batch sizes), so the differentiable step composes with
+    separate elementwise ops and returns the fused step's poses bit for bit.  The bottom row is [0, 0, 0, 1]."""
+    p = [a[..., :3, k:k + 1] * b[..., k:k + 1, :] for k in range(3)]
+    top = (p[0] + p[1]) + p[2]
+    top = torch.cat([top[..., :3], top[..., 3:] + a[..., :3, 3:]], -1)
+    bottom = torch.tensor([0.0, 0.0, 0.0, 1.0], dtype=a.dtype, device=a.device).expand(*a.shape[:-2], 1, 4)
+    return torch.cat([top, bottom], -2)
+
+
 def _normalize_device(device):
     """torch.device with an explicit index for CUDA (the engine's default device is CUDA, not CPU)."""
     device = torch.device(device)
@@ -127,14 +139,13 @@ class ICPSLAM(nn.Module):
         if _wants_grad(live_frame.depth_image, prev_frame.poses, *pointclouds._grad_tensors()):
             # differentiable mode (reference op order, slam/icpslam.py:238-247): the K1 maps carry their hand-written
             # backward, the association kernels are index-only, the ICP algebra is taped.
-            from ..geometry.geometryutils import compose_transformations
             from .fusionutils import find_active_map_points
 
             frames_pc = downsample_rgbdimages(live_frame, self.dsratio)
             pc2im_bnhw = find_active_map_points(pointclouds, prev_frame)
             maps_pc = downsample_pointclouds(pointclouds, pc2im_bnhw, self.dsratio)
             transform = self.odomprov.provide(maps_pc, frames_pc)
-            return compose_transformations(transform.squeeze(1), prev_frame.poses.squeeze(1)).unsqueeze(1)
+            return _compose_canonical(transform.squeeze(1), prev_frame.poses.squeeze(1)).unsqueeze(1)
         # source / target gathering, the ICP loop and the final T_icp · prev_pose all happen in one C call
         return localize_against_map(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov)
 

@@ -415,3 +415,409 @@ def test_batched_differentiable_icp_equals_per_element_chain():
     for b in range(Bn):
         scale = leaves[0].grad[b].abs().max().item()
         torch.testing.assert_close(s_req[b].grad, leaves[0].grad[b, : sizes_s[b]], rtol=1e-4, atol=1e-5 * scale)
+
+
+# ------------------------------------------------------------------------------------------ large shapes and edges
+U32 = 2.0 ** -24  # unit roundoff of float32
+
+
+def _k1_reference_grads(depth, K, poses, ups, which):
+    """float64 autograd of _torch_maps: d(sum(ups[i] * map i for i in which))/d(depth, poses)."""
+    d = depth.detach().double().requires_grad_(True)
+    p = None if poses is None else poses.detach().double().requires_grad_(True)
+    refs = _torch_maps(d, K.double(), p if p is not None else torch.eye(4, dtype=torch.float64, device=d.device)
+                       .expand(depth.shape[0], depth.shape[1], 4, 4))
+    sum((refs[i] * ups[i].double()).sum() for i in which).backward()
+    return d.grad, (None if p is None else p.grad)
+
+
+@pytest.mark.parametrize("B,L,H,W,holes", [(2, 2, 480, 640, "zero"), (1, 3, 37, 45, "negative"),
+                                           (2, 1, 2, 9, "zero"), (1, 2, 11, 2, "negative"), (1, 1, 2, 2, "zero")])
+def test_k1_backward_large_and_minimal_shapes(B, L, H, W, holes):
+    """K1 backward against float64 autograd: 480x640 with B*L = 4 (1200 tiles of pose partials per image reduced by
+    k_pose_grad_reduce), H*W not a multiple of the 256-pixel tile, and H or W = 2 (the border stencil terms coincide:
+    the first row / column is also the one before the last).  Holes are zeros or negative depths (both invalid)."""
+    from gradslam_b200.structures.rgbdimages import backproject
+
+    rgb, depth, K, poses = make_sequence(B, L, max(H, 8), max(W, 8), seed=51 + H)
+    depth = depth[:, :, :H, :W].clone()
+    depth[:, :, 0, 0] = 0.0  # (no pixel has this one as its right or lower neighbour: no degenerate normal)
+    if holes == "negative":
+        depth = torch.where(depth > 0, depth, -0.5 - depth)
+        assert (depth < 0).any()
+    g = torch.Generator().manual_seed(H * W)
+    ups = [torch.randn(B, L, H, W, 3, generator=g).to(DEV) for _ in range(4)]
+    d1 = depth.to(DEV).requires_grad_(True)
+    p1 = poses.to(DEV).requires_grad_(True)
+    outs = backproject(d1, K.to(DEV), p1)
+    sum((o * u).sum() for o, u in zip(outs, ups)).backward()
+    gd, gp = _k1_reference_grads(depth.to(DEV), K.to(DEV), poses.to(DEV), ups, range(4))
+    torch.testing.assert_close(d1.grad.double(), gd, rtol=1e-3, atol=1e-4 * gd.abs().max().item())
+    torch.testing.assert_close(p1.grad[..., :3, :].double(), gp[..., :3, :], rtol=1e-3,
+                               atol=1e-4 * gp.abs().max().item())
+    assert p1.grad[..., 3, :].abs().max() == 0
+    assert d1.grad[depth.to(DEV) <= 0].abs().max() == 0
+
+
+@pytest.mark.parametrize("which", [0, 1, 2, 3])
+def test_k1_backward_single_upstream_map(which):
+    """Only one of the four maps reaches the loss: the other three upstream pointers are null in the kernel."""
+    from gradslam_b200.structures.rgbdimages import backproject
+
+    B, L, H, W = 1, 2, 29, 35
+    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=61)
+    ups = [torch.randn(B, L, H, W, 3, generator=torch.Generator().manual_seed(i)).to(DEV) for i in range(4)]
+    d1 = depth.to(DEV).requires_grad_(True)
+    p1 = poses.to(DEV).requires_grad_(True)
+    outs = backproject(d1, K.to(DEV), p1)
+    (outs[which] * ups[which]).sum().backward()
+    gd, gp = _k1_reference_grads(depth.to(DEV), K.to(DEV), poses.to(DEV), ups, [which])
+    torch.testing.assert_close(d1.grad.double(), gd, rtol=1e-3, atol=1e-4 * gd.abs().max().item())
+    if which < 2:  # the local maps do not depend on the pose
+        assert p1.grad is None or p1.grad.abs().max() == 0
+    else:
+        torch.testing.assert_close(p1.grad[..., :3, :].double(), gp[..., :3, :], rtol=1e-3,
+                                   atol=1e-4 * gp.abs().max().item())
+
+
+def test_k1_backward_without_poses_and_strided_depth_view():
+    """poses=None with a global-vertex upstream (world frame == camera frame), and the depth of frame s passed as the
+    view frames[:, s] of a (B, L) tensor: its element stride is L*H*W, not the dense H*W."""
+    import gradslam_b200 as gs
+
+    B, L, H, W = 2, 3, 23, 31
+    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=62)
+    ups = [torch.randn(B, 1, H, W, 3, generator=torch.Generator().manual_seed(i)).to(DEV) for i in range(4)]
+    d_all = depth.to(DEV).requires_grad_(True)
+    fr = gs.RGBDImages(rgb.to(DEV), d_all, K.to(DEV))[:, 1]
+    assert fr.depth_image.stride(0) == L * H * W
+    (fr.global_vertex_map * ups[2]).sum().backward()
+    gd, _ = _k1_reference_grads(depth[:, 1:2].to(DEV), K.to(DEV), None, ups, [2])
+    torch.testing.assert_close(d_all.grad[:, 1:2].double(), gd, rtol=1e-3, atol=1e-4 * gd.abs().max().item())
+    assert d_all.grad[:, 0].abs().max() == 0 and d_all.grad[:, 2].abs().max() == 0
+    # and with poses, through the same view: pose gradient of that frame only
+    d_all.grad = None
+    p_all = poses.to(DEV).requires_grad_(True)
+    fr = gs.RGBDImages(rgb.to(DEV), d_all, K.to(DEV), p_all)[:, 1]
+    (fr.global_normal_map * ups[3]).sum().backward()
+    gd, gp = _k1_reference_grads(depth[:, 1:2].to(DEV), K.to(DEV), poses[:, 1:2].to(DEV), ups, [3])
+    torch.testing.assert_close(d_all.grad[:, 1:2].double(), gd, rtol=1e-3, atol=1e-4 * gd.abs().max().item())
+    torch.testing.assert_close(p_all.grad[:, 1:2, :3].double(), gp[..., :3, :], rtol=1e-3,
+                               atol=1e-4 * gp.abs().max().item())
+    assert p_all.grad[:, 0].abs().max() == 0 and p_all.grad[:, 2].abs().max() == 0
+
+
+def test_k1_backward_zero_cross_product_pixel():
+    """A valid pixel whose right AND lower neighbours are missing: dh = dv = -v.  At pixel (0,0) with the principal
+    point at (0,0), v = (0, 0, d) exactly, so every product of the cross product has a zero factor and c = 0 in any
+    rounding (checked with the FMA-contracted arithmetic of cross_ref).  The kernel takes its nrm == 0 branch (the
+    normal is c itself, d n / d c = I); float64 autograd of the reference formula does the same."""
+    from gradslam_b200.structures.rgbdimages import backproject
+
+    B, L, H, W = 1, 1, 6, 8
+    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=63)
+    K = K.clone()
+    K[..., 0, 2] = 0.0
+    K[..., 1, 2] = 0.0
+    depth = depth.clone()
+    depth[0, 0, 0, 0] = 1.25
+    depth[0, 0, 0, 1] = 0.0
+    depth[0, 0, 1, 0] = 0.0
+    ups = [torch.randn(B, L, H, W, 3, generator=torch.Generator().manual_seed(i)).to(DEV) for i in range(4)]
+    d1 = depth.to(DEV).requires_grad_(True)
+    p1 = poses.to(DEV).requires_grad_(True)
+    outs = backproject(d1, K.to(DEV), p1)
+    v = outs[0].detach()[0, 0].cpu()
+    c, nrm = oracle_cross(v[0, 1] - v[0, 0], v[1, 0] - v[0, 0])
+    assert torch.equal(c, torch.zeros(3)) and nrm.item() == 0.0
+    assert torch.equal(outs[1].detach()[0, 0, 0, 0].cpu(), torch.zeros(3))
+    sum((o * u).sum() for o, u in zip(outs, ups)).backward()
+    gd, gp = _k1_reference_grads(depth.to(DEV), K.to(DEV), poses.to(DEV), ups, range(4))
+    assert d1.grad[0, 0, 0, 0].abs().item() > 0
+    torch.testing.assert_close(d1.grad.double(), gd, rtol=1e-3, atol=1e-4 * gd.abs().max().item())
+    torch.testing.assert_close(p1.grad[..., :3, :].double(), gp[..., :3, :], rtol=1e-3,
+                               atol=1e-4 * gp.abs().max().item())
+
+
+def oracle_cross(a, b):
+    import gsx_oracle as oracle
+    c, n = oracle.cross_norm_fma(a.view(1, 3).float(), b.view(1, 3).float())
+    return c.view(3), n.view(-1)
+
+
+def _normal_eq_reference(s, p, n, idx):
+    """The 28 sums in float64 and, for the error bound, the same sums of absolute values."""
+    keep = idx >= 0
+    s, pp, nn = s[keep], p[idx[keep]], n[idx[keep]]
+    sx, sy, sz = s[:, 0:1], s[:, 1:2], s[:, 2:3]
+    nx, ny, nz = nn[:, 0:1], nn[:, 1:2], nn[:, 2:3]
+    A = torch.cat([nx, ny, nz, nz * sy - ny * sz, nx * sz - nz * sx, ny * sx - nx * sy], 1)
+    b = nx * (pp[:, 0:1] - sx) + ny * (pp[:, 1:2] - sy) + nz * (pp[:, 2:3] - sz)
+    iu = torch.triu_indices(6, 6)
+    sums = torch.cat([(A.t() @ A)[iu[0], iu[1]], (A.t() @ b)[:, 0], (b * b).sum().view(1)])
+    Aa, ba = A.abs(), b.abs()
+    mags = torch.cat([(Aa.t() @ Aa)[iu[0], iu[1]], (Aa.t() @ ba)[:, 0], (ba * ba).sum().view(1)])
+    return sums, mags
+
+
+def _sum_bound(mags, n_terms):
+    """Error bound of a float32 sum of n_terms products whose factors carry a few roundings each: every term passes
+    through at most n_terms additions (any order), plus 8 roundings for the factors; |error| <= (n + 8) u sum|term|."""
+    return (n_terms + 8) * U32 * mags + 1e-30
+
+
+def test_normal_equation_op_large_sizes_and_batched_ragged():
+    """K6 as an op at ns = 2^17 + 37 (513 reduction blocks, a partial last block): the 28 sums within the float32
+    summation bound of float64, the backward against float64 autograd; then the batched op on ragged elements (a
+    zero-size element, an element whose rows are all filtered) equal per element, bit for bit, to the unbatched op."""
+    from gradslam_b200.odometry.icputils import _NormalEqBatchedFn, _NormalEqFn
+
+    g = torch.Generator().manual_seed(71)
+    ns, nt = (1 << 17) + 37, 5000
+    src = torch.randn(ns, 3, generator=g)
+    tgt = torch.randn(nt, 3, generator=g)
+    tn = torch.nn.functional.normalize(torch.randn(nt, 3, generator=g), dim=1)
+    idx = torch.randint(0, nt, (ns,), generator=g)
+    idx[::5] = -1
+    w = torch.randn(28, generator=g)
+    a = [t.clone().double().requires_grad_(True) for t in (src, tgt, tn)]
+    want, mags = _normal_eq_reference(*a, idx)
+    (want * w.double()).sum().backward()
+    b_ = [t.clone().to(DEV).requires_grad_(True) for t in (src, tgt, tn)]
+    got = _NormalEqFn.apply(b_[0], b_[1], b_[2], idx.to(DEV))
+    err = (got.detach().cpu().double() - want.detach()).abs()
+    assert (err <= _sum_bound(mags.detach(), ns)).all(), (err / mags.detach()).max()
+    # a sum that dropped blocks would miss ~(1 - kept/513) of every entry: far outside the bound
+    assert (want.detach().abs() > 10 * _sum_bound(mags.detach(), ns))[:21].any()
+    (got * w.to(DEV)).sum().backward()
+    for x, y in zip(b_, a):
+        torch.testing.assert_close(x.grad.cpu().double(), y.grad, rtol=1e-3, atol=1e-4 * y.grad.abs().max().item())
+
+    # batched, ragged: sizes 3000, 0, 2^15 + 5 (all filtered), 70001
+    sizes = [3000, 0, (1 << 15) + 5, 70001]
+    Bn, Ns = len(sizes), max(sizes)
+    srcb = torch.zeros(Bn, Ns, 3)
+    idxb = torch.full((Bn, Ns), -1, dtype=torch.int64)
+    tgtb = torch.randn(Bn, nt, 3, generator=g)
+    tnb = torch.nn.functional.normalize(torch.randn(Bn, nt, 3, generator=g), dim=2)
+    for e, n in enumerate(sizes):
+        srcb[e, :n] = torch.randn(n, 3, generator=g)
+        if e != 2:
+            idxb[e, :n] = torch.randint(0, nt, (n,), generator=g)
+    counts = torch.tensor(sizes, dtype=torch.int32, device=DEV)
+    wb = torch.randn(Bn, 28, generator=g).to(DEV)
+    lb = [t.to(DEV).requires_grad_(True) for t in (srcb, tgtb, tnb)]
+    sums_b = _NormalEqBatchedFn.apply(lb[0], lb[1], lb[2], idxb.to(DEV), counts)
+    (sums_b * wb).sum().backward()
+    assert torch.equal(sums_b[1].detach(), torch.zeros(28, device=DEV))
+    assert torch.equal(sums_b[2].detach(), torch.zeros(28, device=DEV))
+    for e, n in enumerate(sizes):
+        if n == 0:
+            assert lb[0].grad[e].abs().max() == 0 and lb[1].grad[e].abs().max() == 0
+            continue
+        l1 = [lb[0].detach()[e, :n].clone().requires_grad_(True), lb[1].detach()[e].clone().requires_grad_(True),
+              lb[2].detach()[e].clone().requires_grad_(True)]
+        s1 = _NormalEqFn.apply(l1[0], l1[1], l1[2], idxb[e, :n].to(DEV))
+        assert torch.equal(s1.detach(), sums_b[e].detach()), e
+        (s1 * wb[e]).sum().backward()
+        assert torch.equal(l1[0].grad, lb[0].grad[e, :n]), e
+        assert lb[0].grad[e, n:].numel() == 0 or lb[0].grad[e, n:].abs().max() == 0
+        torch.testing.assert_close(l1[1].grad, lb[1].grad[e], rtol=1e-5, atol=1e-6 * l1[1].grad.abs().max().item() + 1e-30)
+        torch.testing.assert_close(l1[2].grad, lb[2].grad[e], rtol=1e-5, atol=1e-6 * l1[2].grad.abs().max().item() + 1e-30)
+        if e == 2:
+            assert lb[0].grad[e].abs().max() == 0 and lb[1].grad[e].abs().max() == 0
+        else:
+            ref, mg = _normal_eq_reference(srcb[e, :n].double(), tgtb[e].double(), tnb[e].double(), idxb[e, :n])
+            assert ((sums_b[e].detach().cpu().double() - ref).abs() <= _sum_bound(mg, n)).all(), e
+
+
+def test_rigid_transform_backward_large_empty_and_batched():
+    """d/dT of the rigid transform (k_rigid_bwd partials + k_rigid_bwd_reduce) at n = 2^20 + 3 (4097 blocks) within the
+    float32 summation bound of float64; n = 0 gives an exactly zero g_T; in a batched call a zero-count element gets a
+    zero g_T and its padding rows zero gradient."""
+    from gradslam_b200.odometry import icputils as iu
+    refm = _lm_reference_functions()
+
+    g = torch.Generator().manual_seed(81)
+    n = (1 << 20) + 3
+    P64 = torch.randn(n, 3, dtype=torch.float64, generator=g)
+    T64 = refm._se3_exp(torch.randn(6, dtype=torch.float64, generator=g) * 0.5)
+    G64 = torch.randn(n, 3, dtype=torch.float64, generator=g)
+    P32, G32 = P64.float(), G64.float()
+    p_gpu, t_gpu = P32.to(DEV).requires_grad_(True), T64.float().to(DEV).requires_grad_(True)
+    out = iu._RigidTransformFn.apply(p_gpu, t_gpu)
+    (out * G32.to(DEV)).sum().backward()
+    Pd, Gd = P32.double(), G32.double()  # the float32 inputs, summed exactly in float64
+    ph = torch.cat([Pd, torch.ones(n, 1, dtype=torch.float64)], 1)
+    want = Gd.t() @ ph
+    mags = Gd.abs().t() @ ph.abs()
+    got = t_gpu.grad.cpu().double()
+    nblk = -(-n // 256)
+    bound = (5 + 8 + nblk + 1) * U32 * mags  # shuffle tree, 8 warps, the blocks in order, the product
+    assert ((got[:3] - want).abs() <= bound).all(), ((got[:3] - want).abs() / mags).max()
+    assert got[3].abs().max() == 0
+    torch.testing.assert_close(p_gpu.grad.cpu().double(), Gd @ T64[:3, :3].float().double(), rtol=0, atol=1e-5)
+
+    # n = 0
+    p0 = torch.zeros(0, 3, device=DEV, requires_grad=True)
+    t0 = T64.float().to(DEV).requires_grad_(True)
+    iu._RigidTransformFn.apply(p0, t0).sum().backward()
+    assert torch.equal(t0.grad, torch.zeros(4, 4, device=DEV))
+
+    # batched with a zero-count element
+    sizes = [700, 0, 1500]
+    Bn, N = len(sizes), max(sizes)
+    Pb = torch.randn(Bn, N, 3, generator=g)
+    Tb = torch.stack([refm._se3_exp(torch.randn(6, dtype=torch.float64, generator=g) * 0.5).float() for _ in sizes])
+    Gb = torch.randn(Bn, N, 3, generator=g)
+    pb, tb = Pb.to(DEV).requires_grad_(True), Tb.to(DEV).requires_grad_(True)
+    counts = torch.tensor(sizes, dtype=torch.int32, device=DEV)
+    ob = iu._RigidTransformBatchedFn.apply(pb, tb, counts)
+    (ob * Gb.to(DEV)).sum().backward()
+    for e, m in enumerate(sizes):
+        assert ob[e, m:].abs().max() == 0 if m < N else True
+        assert pb.grad[e, m:].numel() == 0 or pb.grad[e, m:].abs().max() == 0
+        ph = torch.cat([Pb[e, :m].double(), torch.ones(m, 1, dtype=torch.float64)], 1)
+        want = Gb[e, :m].double().t() @ ph
+        bound = (5 + 8 + -(-m // 256) + 1) * U32 * (Gb[e, :m].double().abs().t() @ ph.abs())
+        assert ((tb.grad[e, :3].cpu().double() - want).abs() <= bound).all(), e
+        assert tb.grad[e, 3].abs().max() == 0
+    assert torch.equal(tb.grad[1], torch.zeros(4, 4, device=DEV))
+
+
+def test_batched_differentiable_icp_on_the_grid_path():
+    """B = 3 ragged targets of 20 k - 60 k points (the grid 1-NN, kGridThreshold = 4096), the grid built by the first
+    association and reused by the other 2 * numiters - 1 through target_cache: _taped_icp_batched equals the per-element
+    chain AND the fused icp_align bit for bit, its gradients equal the per-element chain's, and for one element they
+    match the oracle's autograd (the tolerance of test_gradicp_function_gradients_match_oracle_autograd)."""
+    import gsx_oracle as oracle
+    import gradslam_b200 as gs
+    from gradslam_b200.odometry import icputils as iu
+
+    g = torch.Generator().manual_seed(91)
+    rgb, depth, K, poses = make_sequence(1, 1, 240, 320, seed=92, yaw0=0.6)
+    fr = gs.RGBDImages(rgb.to(DEV), depth.to(DEV), K.to(DEV), poses.to(DEV))
+    valid = (depth[0, 0, ..., 0] > 0).reshape(-1).to(DEV)
+    base_p = fr.global_vertex_map[0, 0].reshape(-1, 3)[valid]
+    base_n = fr.global_normal_map[0, 0].reshape(-1, 3)[valid]
+    sizes_t, sizes_s = [20000, 60000, 41234], [5000, 3000, 7001]
+    Bn, Nt, Ns, numiters = 3, max(sizes_t), max(sizes_s), 4
+    src = torch.zeros(Bn, Ns, 3, device=DEV)
+    tgt = torch.zeros(Bn, Nt, 3, device=DEV)
+    tgt_n = torch.zeros(Bn, Nt, 3, device=DEV)
+    for b in range(Bn):
+        T = oracle.se3_exp(torch.tensor([0.01 * (b + 1), -0.005, 0.004 * b, 0.01, -0.008 * b, 0.005])).to(DEV)
+        pick_t = torch.randperm(base_p.shape[0], generator=g)[: sizes_t[b]].to(DEV)
+        pick_s = torch.randperm(base_p.shape[0], generator=g)[: sizes_s[b]].to(DEV)
+        tgt[b, : sizes_t[b]] = base_p[pick_t]
+        tgt_n[b, : sizes_t[b]] = base_n[pick_t]
+        src[b, : sizes_s[b]] = base_p[pick_s] @ T[:3, :3].t() + T[:3, 3]
+    cs = torch.tensor(sizes_s, dtype=torch.int32, device=DEV)
+    ct = torch.tensor(sizes_t, dtype=torch.int32, device=DEV)
+    w = torch.randn(Bn, 4, 4, generator=g).to(DEV)
+    leaves = [t.clone().requires_grad_(True) for t in (src, tgt, tgt_n)]
+    T_b, idx_b = iu._taped_icp_batched(leaves[0], cs, leaves[1], leaves[2], ct, None, 1, numiters, 1e-8, None)
+    (T_b * w).sum().backward()
+    T_f, _ = iu.icp_align(src, cs, tgt, tgt_n, ct, None, 1, numiters, 1e-8, None)
+    assert torch.equal(T_f, T_b.detach())
+    for b in range(Bn):
+        ns, nt = sizes_s[b], sizes_t[b]
+        l1 = [src[b:b + 1, :ns].clone().requires_grad_(True), tgt[b:b + 1, :nt].clone().requires_grad_(True),
+              tgt_n[b:b + 1, :nt].clone().requires_grad_(True)]
+        T_1, idx_1 = iu._taped_icp(l1[0], l1[1], l1[2], None, 1, numiters, 1e-8, None)
+        (T_1 * w[b]).sum().backward()
+        assert torch.equal(T_1, T_b[b])
+        assert torch.equal(idx_1, idx_b[b, :ns][idx_b[b, :ns] >= 0])
+        for got, want, n in ((leaves[0].grad[b], l1[0].grad[0], ns), (leaves[1].grad[b], l1[1].grad[0], nt),
+                             (leaves[2].grad[b], l1[2].grad[0], nt)):
+            torch.testing.assert_close(got[:n], want, rtol=1e-4, atol=1e-5 * want.abs().max().item())
+            assert got[n:].numel() == 0 or got[n:].abs().max() == 0
+    # element 0 against the oracle's tape
+    s_ref = src[0, : sizes_s[0]].cpu().clone().requires_grad_(True)
+    T_ref, _ = oracle.point_to_plane_gradicp(s_ref, tgt[0, : sizes_t[0]].cpu(), tgt_n[0, : sizes_t[0]].cpu(),
+                                             torch.eye(4), numiters=numiters)
+    (T_ref * w[0].cpu()).sum().backward()
+    torch.testing.assert_close(T_b[0].detach().cpu(), T_ref.detach(), rtol=0, atol=1e-4)
+    scale = s_ref.grad.abs().max().item()
+    torch.testing.assert_close(leaves[0].grad[0, : sizes_s[0]].cpu(), s_ref.grad, rtol=2e-2, atol=2e-3 * scale)
+
+
+def test_aggregate_backward_full_size():
+    """update_map_aggregate with gradients (K4 backward with with_ccounts = 0, as in ICPSLAM) at 480x640, B = 2: the
+    previous map's rows pass their gradient through, every appended row carries its pixel's gradient back to K1; against
+    float64 autograd of the same formulas (rows appended in row-major pixel order)."""
+    import gradslam_b200 as gs
+    from gradslam_b200.slam import fusionutils as fu
+
+    B, H, W = 2, 480, 640
+    rgb, depth, K, poses = make_sequence(B, 2, H, W, seed=101, yaw0=0.6)
+    with torch.no_grad():
+        base = fu.update_map_aggregate(gs.Pointclouds(device=DEV),
+                                       gs.RGBDImages(rgb[:, :1].to(DEV), depth[:, :1].to(DEV), K.to(DEV),
+                                                     poses[:, :1].to(DEV)))
+    n0 = base.num_points_per_pointcloud.tolist()
+    leaves = {k: getattr(base, k + "_padded").clone().requires_grad_(True) for k in ("points", "normals", "colors")}
+    pc = gs.Pointclouds(leaves["points"], leaves["normals"], leaves["colors"])
+    pc._set_counts(n0)
+    d1 = depth[:, 1:2].to(DEV).requires_grad_(True)
+    c1 = rgb[:, 1:2].to(DEV).requires_grad_(True)
+    out = fu.update_map_aggregate(pc, gs.RGBDImages(c1, d1, K.to(DEV), poses[:, 1:2].to(DEV)))
+    n1 = out.num_points_per_pointcloud.tolist()
+    valid = depth[:, 1, ..., 0] > 0
+    assert [n1[b] - n0[b] for b in range(B)] == valid.flatten(1).sum(1).tolist()
+    g = torch.Generator().manual_seed(102)
+    wts = {k: torch.randn(B, max(n1), 3, generator=g).to(DEV) for k in ("points", "normals", "colors")}
+    mask = out.nonpad_mask.unsqueeze(-1)
+    sum((getattr(out, k + "_padded") * wts[k] * mask).sum() for k in wts).backward()
+
+    d64 = depth[:, 1:2].to(DEV).double().requires_grad_(True)
+    _, _, gv, gn = _torch_maps(d64, K.to(DEV).double(), poses[:, 1:2].to(DEV).double())
+    c64 = rgb[:, 1:2].to(DEV).double().requires_grad_(True)
+    loss = 0
+    for b in range(B):
+        m = valid[b].to(DEV)
+        for k, t in (("points", gv), ("normals", gn), ("colors", c64)):
+            loss = loss + (t[b, 0][m] * wts[k][b, n0[b]:n1[b]].double()).sum()
+    loss.backward()
+    torch.testing.assert_close(d1.grad.double(), d64.grad, rtol=1e-3, atol=1e-4 * d64.grad.abs().max().item())
+    torch.testing.assert_close(c1.grad.double(), c64.grad, rtol=0, atol=0)
+    for k in leaves:
+        for b in range(B):
+            assert torch.equal(leaves[k].grad[b, : n0[b]], wts[k][b, : n0[b]])
+
+
+def test_confidence_clamp_backward():
+    """alpha = clamp(exp(-|v|^2 / 2 sigma^2), 1e-7, 1.01): with a small sigma a known set of pixels has exp below 1e-7.
+    Fusing one frame into an empty map appends every valid pixel with confidence alpha, so d(sum w * confidence)/d depth
+    is w * d alpha / d depth per pixel: exactly zero where the clamp is active (as torch.clamp's autograd gives), and the
+    float64 derivative of the formula elsewhere."""
+    import math
+
+    import gradslam_b200 as gs
+    from gradslam_b200.slam import fusionutils as fu
+
+    B, H, W = 1, 40, 56
+    rgb, depth, K, poses = make_sequence(B, 1, H, W, seed=111, yaw0=0.6)
+    d64 = depth.to(DEV).double().requires_grad_(True)
+    v = _torch_maps(d64, K.to(DEV).double(), poses.to(DEV).double())[0][0, 0]
+    sq = (v * v).sum(-1)
+    valid = depth[0, 0, ..., 0].to(DEV) > 0
+    sigma = (sq[valid].median().sqrt() / math.sqrt(2 * 16.5)).item()  # about half of the pixels clamp
+    e = torch.exp(-sq / (2 * sigma * sigma))
+    clamped = valid & (e < 0.5e-7)
+    free = valid & (e > 2e-7)
+    assert clamped.sum() > 100 and free.sum() > 100
+    wts = torch.randn(H * W, generator=torch.Generator().manual_seed(112)).to(DEV)
+    (torch.clamp(e, 1e-7, 1.01)[valid] * wts[: int(valid.sum())].double()).sum().backward()
+
+    d1 = depth.to(DEV).requires_grad_(True)
+    pc = fu.update_map_fusion(gs.Pointclouds(device=DEV), gs.RGBDImages(rgb.to(DEV), d1, K.to(DEV), poses.to(DEV)),
+                              0.05, 0.94, sigma)
+    n = int(valid.sum())
+    assert pc.num_points_per_pointcloud.tolist() == [n]
+    (pc.features_list[0][:, 0] * wts[:n]).sum().backward()
+    g = d1.grad[0, 0, ..., 0]
+    assert g[clamped].abs().max() == 0
+    assert (g[free] != 0).all()
+    want = d64.grad[0, 0, ..., 0]
+    torch.testing.assert_close(g[free].double(), want[free], rtol=1e-4, atol=1e-6 * want.abs().max().item())

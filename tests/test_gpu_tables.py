@@ -145,3 +145,66 @@ def test_downsample_helpers_match_oracle():
         assert torch.equal(got.points_list[b].cpu(), r_pts[b]) and torch.equal(got.normals_list[b].cpu(), r_nrm[b])
         torch.testing.assert_close(got_m.points_list[b].cpu(), rm_pts[b], rtol=1e-6, atol=1e-6)
         assert got_m.points_list[b].shape == rm_pts[b].shape
+
+
+@pytest.mark.parametrize("n,density", [(2_000_003, 0.0), (3_000_017, 1e-4), (4_194_303, 0.5), (10_000_001, 1.0),
+                                       (5_000_011, "edges")])
+def test_compact_matches_nonzero(n, density):
+    """The look-back compaction (k_compact, ~1000-10000 tiles of 1024 flags, n % 1024 != 0) against torch.nonzero:
+    densities 0, 1e-4, 1/2 and 1, and a pattern whose first and last tiles are empty."""
+    from gradslam_b200.slam import fusionutils as fu
+
+    g = torch.Generator(device=DEV).manual_seed(n)
+    if density == "edges":
+        flags = (torch.rand(n, generator=g, device=DEV) < 0.5).to(torch.uint8)
+        flags[:3 * 1024] = 0
+        flags[-(n % 1024) - 2 * 1024:] = 0
+        assert flags.sum() > 0
+    else:
+        flags = (torch.rand(n, generator=g, device=DEV) < density).to(torch.uint8)
+    flags[flags.bool()] = torch.randint(1, 256, (int(flags.sum()),), generator=g, device=DEV,
+                                        dtype=torch.int64).to(torch.uint8)  # any non-zero byte is a flag
+    got = fu._compact(flags)
+    want = torch.nonzero(flags).view(-1)
+    assert got.dtype == torch.int64 and torch.equal(got, want)
+
+
+def test_tables_full_size_match_oracle():
+    """The three correspondence tables at the benchmark's frame size and batch (640x480, B=8, seed 0), after two fused
+    frames: B x map bound ~ 4.9 M active-point flags.  Rows of elements 0 and 7 equal the oracle's tables exactly."""
+    import gradslam_b200 as gs
+    from gradslam_b200.slam import fusionutils as fu
+
+    B, L, H, W = 8, 3, 480, 640
+    checked = [0, B - 1]
+    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=0)
+    frames = gs.RGBDImages(rgb.to(DEV), depth.to(DEV), K.to(DEV), poses.to(DEV))
+    pc = gs.Pointclouds(device=DEV)
+    smap = oracle.SurfelMap()
+    r_rgb, r_depth, r_K, r_poses = rgb[checked], depth[checked], K[checked], poses[checked]
+    for s in range(2):
+        pc = fu.update_map_fusion(pc, frames[:, s], 0.05, DOT_TH, 0.6, inplace=True)
+        m = oracle.frame_maps(r_depth[:, s:s + 1], r_K, r_poses[:, s:s + 1])
+        smap = oracle.update_map_fusion(smap, m, r_rgb[:, s:s + 1], r_poses[:, s], r_K[:, 0], 0.05, DOT_TH, 0.6)
+    assert [pc.num_points_per_pointcloud.tolist()[b] for b in checked] == smap.counts()
+    live = frames[:, 2]
+    maps = oracle.frame_maps(r_depth[:, 2:3], r_K, r_poses[:, 2:3])
+    gv, gn = maps["gvertex"][:, 0], maps["gnormal"][:, 0]
+
+    def rows(table, b, i):
+        t = table[table[:, 0] == b].cpu().clone()
+        t[:, 0] = i
+        return t
+
+    active = fu.find_active_map_points(pc, live)
+    r_active = oracle.find_active_map_points(smap, r_poses[:, 2], r_K[:, 0], H, W)
+    similar, mask = fu.find_similar_map_points(pc, live, active, 0.05, DOT_TH)
+    r_similar, r_mask = oracle.find_similar_map_points(smap, gv, gn, r_active, 0.05, DOT_TH)
+    unique = fu.find_best_unique_correspondences(pc, live, similar)
+    r_unique = oracle.find_best_unique_correspondences(smap, gv, r_similar)
+    assert r_unique.shape[0] > 100_000
+    for i, b in enumerate(checked):
+        assert torch.equal(rows(active, b, i), r_active[r_active[:, 0] == i]), b
+        assert torch.equal(rows(similar, b, i), r_similar[r_similar[:, 0] == i]), b
+        assert torch.equal(mask[active[:, 0] == b].cpu(), r_mask[r_active[:, 0] == i]), b
+        assert torch.equal(rows(unique, b, i), r_unique[r_unique[:, 0] == i]), b

@@ -112,3 +112,72 @@ def test_edge_cases(frozen, name):
             if n:
                 torch.testing.assert_close(pc.points_list[b].cpu(), torch.from_numpy(frozen["%s/points/%d" % (name, b)]),
                                            rtol=0, atol=2e-5)
+
+
+@pytest.mark.parametrize("name", EDGE_CASES)
+def test_edge_cases_differentiable_pointfusion(name):
+    """The same inputs with depth and colours requiring grad (K1 -> association -> K4 as differentiable ops): maps
+    bit-identical to the oracle and to the no-grad call, d/d depth and d/d colours against the oracle's autograd (loss
+    of test_pointfusion_map_gradients_match_oracle_autograd: points, colours and confidence counts), and an element whose
+    map stays empty gets exactly zero gradient."""
+    import gradslam_b200 as gs
+
+    rgb, depth, K, poses = edge_inputs(name)
+    d_ref, c_ref = depth.clone().requires_grad_(True), rgb.clone().requires_grad_(True)
+    ref = oracle.run_slam(c_ref, d_ref, K, poses, odom="gt")
+    counts = ref.map.counts()
+    g = torch.Generator().manual_seed(7)
+    ws = [[torch.randn(n, c, generator=g) for c in (3, 3, 1)] for n in counts]
+    loss = 0
+    for b in range(len(counts)):
+        for t, w in zip((ref.map.points[b], ref.map.colors[b], ref.map.ccounts[b]), ws[b]):
+            loss = loss + (t * w).sum()
+    loss.backward()
+
+    d_gpu, c_gpu = depth.clone().to(DEV).requires_grad_(True), rgb.clone().to(DEV).requires_grad_(True)
+    slam = gs.PointFusion(odom="gt", device=DEV)
+    pc, _ = slam(gs.RGBDImages(c_gpu, d_gpu, K.to(DEV), poses.to(DEV)))
+    with torch.no_grad():
+        pc_ng, _ = slam(gs.RGBDImages(rgb.to(DEV), depth.to(DEV), K.to(DEV), poses.to(DEV)))
+    assert [int(c) for c in pc.num_points_per_pointcloud.tolist()] == counts
+    assert [int(c) for c in pc_ng.num_points_per_pointcloud.tolist()] == counts
+    loss = 0
+    for b in range(len(counts)):
+        for attr, want in (("points_list", ref.map.points[b]), ("normals_list", ref.map.normals[b]),
+                           ("colors_list", ref.map.colors[b]), ("features_list", ref.map.ccounts[b])):
+            got = getattr(pc, attr)[b].detach()
+            assert torch.equal(got.cpu(), want.detach()), (attr, b)
+            assert torch.equal(got, getattr(pc_ng, attr)[b]), (attr, b)
+        for t, w in zip((pc.points_list[b], pc.colors_list[b], pc.features_list[b]), ws[b]):
+            loss = loss + (t * w.to(DEV)).sum()
+    loss.backward()
+    for got, want in ((d_gpu.grad.cpu(), d_ref.grad), (c_gpu.grad.cpu(), c_ref.grad)):
+        assert torch.isfinite(got).all()
+        torch.testing.assert_close(got, want, rtol=1e-3, atol=1e-4 * want.abs().max().item())
+    for b, n in enumerate(counts):
+        if n == 0:
+            assert d_gpu.grad[b].abs().max() == 0 and c_gpu.grad[b].abs().max() == 0
+
+
+@pytest.mark.parametrize("name", ["edge_empty_mid_frame", "edge_empty_first_frame", "edge_empty_element",
+                                  "edge_no_overlap"])
+def test_edge_cases_differentiable_icpslam(name):
+    """ICPSLAM(odom='gradicp') with depth, colours and poses requiring grad on the edge-case inputs.  An all-invalid
+    live frame leaves every source cloud empty (padded width 0), an empty first frame or element an empty ICP target:
+    the taped chain runs, its poses equal the fused no-grad call's bit for bit, and the gradients are finite."""
+    import gradslam_b200 as gs
+
+    rgb, depth, K, poses = edge_inputs(name)
+    slam = gs.ICPSLAM(odom="gradicp", numiters=3, dsratio=2, device=DEV)
+    d = depth.clone().to(DEV).requires_grad_(True)
+    c = rgb.clone().to(DEV).requires_grad_(True)
+    p = poses.clone().to(DEV).requires_grad_(True)
+    pc, rec = slam(gs.RGBDImages(c, d, K.to(DEV), p))
+    w = torch.randn(rec.shape, generator=torch.Generator().manual_seed(3)).to(DEV)
+    (rec * w).sum().backward()
+    assert torch.isfinite(d.grad).all() and torch.isfinite(p.grad).all()
+    assert c.grad is None or torch.isfinite(c.grad).all()
+    with torch.no_grad():
+        pc_f, rec_f = slam(gs.RGBDImages(rgb.to(DEV), depth.to(DEV), K.to(DEV), poses.to(DEV)))
+    assert pc.num_points_per_pointcloud.tolist() == pc_f.num_points_per_pointcloud.tolist()
+    assert torch.equal(rec.detach(), rec_f), (rec.detach() - rec_f).abs().max()

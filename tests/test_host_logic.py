@@ -420,3 +420,23 @@ def test_bind_host_to_gpu_is_harmless_without_a_gpu():
     before = os.sched_getaffinity(0)
     assert parallel.bind_host_to_gpu("cuda:0") is None or os.sched_getaffinity(0) <= before
     os.sched_setaffinity(0, before)
+
+
+def test_differentiable_pose_composition_uses_canonical_order():
+    """ICPSLAM's differentiable step composes T_icp · prev pose with separately rounded products and sums in the
+    order of the fused step's k_pose_compose (the oracle's rigid_compose), so both steps return the same bits."""
+    import gsx_oracle as oracle
+    from gradslam_b200.slam.icpslam import _compose_canonical
+
+    g = torch.Generator().manual_seed(0)
+    A = torch.stack([oracle.se3_exp(torch.randn(6, generator=g)) for _ in range(64)]).requires_grad_(True)
+    P = torch.stack([oracle.se3_exp(torch.randn(6, generator=g)) for _ in range(64)]).requires_grad_(True)
+    out = _compose_canonical(A, P)
+    assert torch.equal(out.detach(), oracle.rigid_compose(A.detach(), P.detach()))
+    w = torch.randn(64, 4, 4, generator=g)
+    (out * w).sum().backward()
+    A2, P2 = A.detach().double().requires_grad_(True), P.detach().double().requires_grad_(True)
+    ((A2[:, :3, :3] @ P2[:, :3, :] + torch.cat([torch.zeros(64, 3, 3, dtype=torch.float64), A2[:, :3, 3:]], -1))
+     * w[:, :3].double()).sum().backward()
+    torch.testing.assert_close(A.grad.double(), A2.grad, rtol=1e-6, atol=1e-6)
+    torch.testing.assert_close(P.grad.double(), P2.grad, rtol=1e-6, atol=1e-6)
