@@ -94,6 +94,13 @@ SIGNATURES = {
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int,
                 c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64,
                 c_vp, c_i64, c_u32, c_vp, c_vp]),
+    "gsx_render_views": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                c_vp, c_vp, c_vp]),
+    "gsx_render_views_bwd_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
+    "gsx_render_views_bwd": (
+        c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
 }
 
 _lib = None

@@ -349,6 +349,36 @@ int gsx_icp_localize(const float *map_geometry, const int32_t *counts, int64_t c
                      float *poses_out, int64_t poses_out_bstride, void *workspace,
                      int64_t workspace_map_capacity, uint32_t epoch, int32_t *overflow_flag, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Rendering of the surfel map into L views per element: depth, colour, camera-frame normal, confidence and index images.
+ * The reference has no counterpart; the pixel assignment is find_active_map_points'
+ * (gradslam/slam/fusionutils.py:249-274): a row n < counts[b] covers the pixel it projects to (T^-1 with the
+ * camera-to-world pose, the 4x4 K, frustum (-1e-3, W - 0.999) x (-1e-3, H - 0.999), z > 0, round half to even, clamp),
+ * and each pixel keeps the covering row with the smallest camera-frame z (the z of T^-1 p), ties to the smallest n.
+ * intrinsics: B matrices 4x4, stride K_bstride; poses (B,L,4,4) with element stride pose_bstride and 16 between views.
+ * Outputs (B,L,H,W[,C]) dense: index int64 (n, or -1 where no row covers the pixel), depth (,1), rgb (,3) = the row's
+ * colour, normals (,3) = R^T n, confidence (,1) = the row's ccount; zeros where uncovered.  index is required and is
+ * the z-buffer while the call runs (the call fills it); every other output may be NULL (not computed: a depth-only
+ * render reads no colour row).  max_count = host upper bound on counts[b] (sizes the grid); the map pointers may be
+ * NULL when it is 0. */
+int gsx_render_views(const float *map_geometry, const float *map_colors, const int32_t *counts, int64_t capacity,
+                     int64_t max_count, const float *intrinsics, int64_t K_bstride, const float *poses,
+                     int64_t pose_bstride, int B, int L, int H, int W, int64_t *index, float *depth, float *rgb,
+                     float *normals, float *confidence, void *stream);
+
+/* Backward of gsx_render_views at a fixed index image: from the upstream gradients of the outputs (NULL = zero),
+ * d_geometry (B,cap,8) / d_colors (B,cap,4): every row written (padding rows and slots zero), a row summing, in view
+ * order, the gradients of the pixels it won; d_poses (B*L,4,4): d/d(camera-to-world pose) of depth and normals (top
+ * 3x4 block; bottom row zero), reduced per pixel tile then summed in tile order.  Any of the three may be NULL.
+ * Deterministic, no atomics; no gradient w.r.t. the intrinsics.  scratch: gsx_render_views_bwd_scratch_bytes(B,L,H,W)
+ * bytes (only needed for d_poses). */
+int64_t gsx_render_views_bwd_scratch_bytes(int B, int L, int H, int W);
+int gsx_render_views_bwd(const float *map_geometry, const int32_t *counts, int64_t capacity, const float *intrinsics,
+                         int64_t K_bstride, const float *poses, int64_t pose_bstride, const int64_t *index, int B,
+                         int L, int H, int W, const float *g_depth, const float *g_rgb, const float *g_normals,
+                         const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses, void *scratch,
+                         int64_t scratch_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
