@@ -3,6 +3,7 @@ implementation of the same op chain (gradslam/structures/rgbdimages.py:643-762).
 import pytest
 import torch
 
+from cameras import CameraShape, camera_inputs
 from gradslam_b200.synthetic import make_sequence as _make_sequence, punch_lattice_holes
 
 pytestmark = pytest.mark.gpu
@@ -45,12 +46,17 @@ def _torch_maps(depth, K, poses):
     return vert, n, gv, gn
 
 
-@pytest.mark.parametrize("shape", [(2, 2, 24, 40), (1, 1, 17, 23)])
+@pytest.mark.parametrize("shape", [(2, 2, 24, 40), (1, 1, 17, 23),
+                                   pytest.param(CameraShape((3, 2, 24, 40)), id="cameras")])
 def test_backproject_backward_matches_autograd(shape):
+    """With a camera per element, d/d pose of each element is checked against its own camera's chain."""
     import gradslam_b200 as gs
 
     B, L, H, W = shape
-    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=21)
+    if isinstance(shape, CameraShape):
+        rgb, depth, K, poses = camera_inputs(B, L, H, W, 21, skew=0.75, lattice_holes=True)
+    else:
+        rgb, depth, K, poses = make_sequence(B, L, H, W, seed=21)
     g = torch.Generator().manual_seed(3)
     ups = [torch.randn(B, L, H, W, 3, generator=g).to(DEV) for _ in range(4)]
     # engine
@@ -144,16 +150,20 @@ def test_icpslam_pose_gradient_wrt_live_depth():
         torch.testing.assert_close(g_gpu, g_ref, rtol=5e-2, atol=5e-3 * scale)
 
 
-@pytest.mark.parametrize("B,L", [(1, 2), (2, 3)])
-def test_pointfusion_map_gradients_match_oracle_autograd(B, L):
+@pytest.mark.parametrize("B,L,cameras", [(1, 2, False), (2, 3, False), (3, 3, True)], ids=["1-2", "2-3", "cameras"])
+def test_pointfusion_map_gradients_match_oracle_autograd(B, L, cameras):
     """PointFusion(odom='gt') in differentiable mode: d(fused map)/d(depth, colours) through the K1 backward kernel and
     the K4 backward kernel (gsx_fusion_merge_append_bwd), against PyTorch autograd of the oracle restatement
-    (fusionutils.py:580-722).  L=3 chains a merge into rows that were themselves merged one frame earlier."""
+    (fusionutils.py:580-722).  L=3 chains a merge into rows that were themselves merged one frame earlier.  cameras:
+    a camera per element (tests/golden/cameras.py) with skew and 4th intrinsics column."""
     import gradslam_b200 as gs
     import gsx_oracle as oracle
 
     H, W = 24, 32
-    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=41, yaw0=0.6)
+    if cameras:
+        rgb, depth, K, poses = camera_inputs(B, L, H, W, 41, skew=0.75, lattice_holes=True)
+    else:
+        rgb, depth, K, poses = make_sequence(B, L, H, W, seed=41, yaw0=0.6)
     d_ref, c_ref = depth.clone().requires_grad_(True), rgb.clone().requires_grad_(True)
     ref = oracle.run_slam(c_ref, d_ref, K, poses, odom="gt")
     g = torch.Generator().manual_seed(5)

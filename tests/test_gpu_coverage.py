@@ -6,6 +6,7 @@ import pytest
 import torch
 
 import gsx_oracle as oracle
+from cameras import CameraShape, camera_inputs
 from gradslam_b200.synthetic import make_sequence
 
 pytestmark = pytest.mark.gpu
@@ -16,11 +17,15 @@ SENTINEL = 0x7FC0DEAD  # a NaN bit pattern no kernel writes
 _ref_cache = {}
 
 
-def _inputs_and_ref(B, L, H, W, seed=0):
-    """Seeded inputs and the oracle's PointFusion(odom='gt') run on them (cached: several tests share a shape)."""
-    key = (B, L, H, W, seed)
+def _inputs_and_ref(B, L, H, W, seed=0, cameras=False):
+    """Seeded inputs and the oracle's PointFusion(odom='gt') run on them (cached: several tests share a shape).
+    cameras=True: a camera per element (tests/golden/cameras.py), skew and 4th intrinsics column set."""
+    key = (B, L, H, W, seed, cameras)
     if key not in _ref_cache:
-        rgb, depth, K, poses = make_sequence(B, L, H, W, seed=seed)
+        if cameras:
+            rgb, depth, K, poses = camera_inputs(B, L, H, W, seed, skew=0.75)
+        else:
+            rgb, depth, K, poses = make_sequence(B, L, H, W, seed=seed)
         _ref_cache[key] = (rgb, depth, K, poses, oracle.run_slam(rgb, depth, K, poses, odom="gt").map)
     return _ref_cache[key]
 
@@ -56,14 +61,15 @@ def k2_grid_cap():
     _C.lib().gsx_debug_set_k2_grid_cap(0)
 
 
-@pytest.mark.parametrize("shape", [(2, 4, 48, 64), (3, 3, 64, 64), (1, 5, 120, 160)])
+@pytest.mark.parametrize("shape", [(2, 4, 48, 64), (3, 3, 64, 64), (1, 5, 120, 160),
+                                   pytest.param(CameraShape((3, 4, 48, 64)), id="cameras")])
 def test_k2_multi_pass_grid_stride_matches_oracle(shape, k2_grid_cap):
     """K2 capped to 1, 3 or 7 CTAs in all (3 and 7 do not divide B): every thread walks several map rows, prefetching
     the next row and settling each 128-bit CAS one iteration late across passes.  Whole-sequence call and step loop."""
     import gradslam_b200 as gs
 
     B, L, H, W = shape
-    rgb, depth, K, poses, ref = _inputs_and_ref(B, L, H, W)
+    rgb, depth, K, poses, ref = _inputs_and_ref(B, L, H, W, cameras=isinstance(shape, CameraShape))
     frames = _frames(gs, rgb, depth, K, poses)
     # every frame after the first projects at least the first frame's valid pixels
     min_rows = int((depth[:, 0, ..., 0] > 0).flatten(1).sum(1).min())
@@ -89,7 +95,8 @@ def _k1r_uses_tma(H, W):
 
 @pytest.mark.parametrize("shape,branch", [((2, 3, 41, 64), "plain: (H-1) % 8 == 0"),
                                           ((2, 3, 33, 47), "plain: W % 4 != 0, misaligned K4 colours"),
-                                          ((2, 3, 42, 100), "tma: partial tiles in both dimensions")])
+                                          ((2, 3, 42, 100), "tma: partial tiles in both dimensions"),
+                                          ((3, 3, 42, 100), "tma: partial tiles, a camera per element")])
 def test_frame_record_layouts_match_oracle(shape, branch, monkeypatch):
     import gradslam_b200 as gs
 
@@ -101,7 +108,7 @@ def test_frame_record_layouts_match_oracle(shape, branch, monkeypatch):
     if "misaligned" in branch:
         # frame (b, s) starts (b*L + s) * H*W * 3 floats into the colour tensor: odd H*W puts odd frames off 16 bytes
         assert (H * W) % 2 == 1 and B * L > 1
-    rgb, depth, K, poses, ref = _inputs_and_ref(B, L, H, W)
+    rgb, depth, K, poses, ref = _inputs_and_ref(B, L, H, W, cameras="camera per element" in branch)
     pc, _ = gs.PointFusion(odom="gt", device=DEV)(_frames(gs, rgb, depth, K, poses))
     _assert_matches_oracle(pc, ref)
     if tma:  # the plain kernel on the same shape gives the same bits
@@ -114,31 +121,34 @@ def test_frame_record_layouts_match_oracle(shape, branch, monkeypatch):
 @pytest.mark.parametrize("groups", [1, 2, 3, 4])
 def test_batch_groups_match_oracle(groups, monkeypatch):
     """B=5 split into 1..4 groups (G=3: sizes 1, 2, 2; G=4: 1, 1, 1, 2); L=5 alternates the two workspace halves
-    more than once."""
+    more than once.  With a camera per element, a group that read its first element's camera (or element 0's) fails."""
     import gradslam_b200 as gs
     from gradslam_b200 import _C
 
     monkeypatch.setenv("GSX_SEQ_GROUPS", str(groups))
     assert _C.lib().gsx_pointfusion_sequence_groups(5) == groups
-    rgb, depth, K, poses, ref = _inputs_and_ref(5, 5, 48, 64)
-    pc, out_poses = gs.PointFusion(odom="gt", device=DEV)(_frames(gs, rgb, depth, K, poses))
-    _assert_matches_oracle(pc, ref)
-    assert torch.equal(out_poses.cpu(), poses)
+    for cameras in (False, True):
+        rgb, depth, K, poses, ref = _inputs_and_ref(5, 5, 48, 64, cameras=cameras)
+        pc, out_poses = gs.PointFusion(odom="gt", device=DEV)(_frames(gs, rgb, depth, K, poses))
+        _assert_matches_oracle(pc, ref)
+        assert torch.equal(out_poses.cpu(), poses)
 
 
 def test_host_fed_frames_equal_device_resident():
-    """Pinned host frames are uploaded 4 frames at a time, so L=5 makes a second sequence call with s_begin = 4."""
+    """Pinned host frames are uploaded 4 frames at a time, so L=5 makes a second sequence call with s_begin = 4.  On
+    the synthetic inputs and with a camera per element."""
     import gradslam_b200 as gs
 
-    rgb, depth, K, poses, ref = _inputs_and_ref(5, 5, 48, 64)
     slam = gs.PointFusion(odom="gt", device=DEV)
-    dev_pc, _ = slam(_frames(gs, rgb, depth, K, poses))
-    host = gs.RGBDImages(rgb.pin_memory(), depth.pin_memory(), K.pin_memory(), poses.pin_memory())
-    assert not host.depth_image.is_cuda
-    host_pc, host_poses = slam(host)
-    _assert_same_rows(host_pc, dev_pc)
-    _assert_matches_oracle(host_pc, ref)
-    assert torch.equal(host_poses.cpu(), poses)
+    for cameras in (False, True):
+        rgb, depth, K, poses, ref = _inputs_and_ref(5, 5, 48, 64, cameras=cameras)
+        dev_pc, _ = slam(_frames(gs, rgb, depth, K, poses))
+        host = gs.RGBDImages(rgb.pin_memory(), depth.pin_memory(), K.pin_memory(), poses.pin_memory())
+        assert not host.depth_image.is_cuda
+        host_pc, host_poses = slam(host)
+        _assert_same_rows(host_pc, dev_pc)
+        _assert_matches_oracle(host_pc, ref)
+        assert torch.equal(host_poses.cpu(), poses)
 
 
 def test_merge_capacity_overflow_clamps_only_the_overflowing_element():

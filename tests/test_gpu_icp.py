@@ -6,6 +6,7 @@ import pytest
 import torch
 
 import gsx_oracle as oracle
+from cameras import camera_inputs
 from gradslam_b200.synthetic import make_sequence
 
 pytestmark = pytest.mark.gpu
@@ -112,12 +113,22 @@ def _nn_dist(a, b):
     return oracle.knn1(a, b)[0].sqrt()
 
 
-@pytest.mark.parametrize("cls,odom", [("PointFusion", "gradicp"), ("PointFusion", "icp"), ("ICPSLAM", "gradicp")])
-def test_slam_with_icp_odometry_matches_oracle(cls, odom):
+ICP_CASES = [("PointFusion", "gradicp", False), ("PointFusion", "icp", False), ("ICPSLAM", "gradicp", False),
+             ("PointFusion", "gradicp", True), ("PointFusion", "icp", True), ("ICPSLAM", "icp", True)]
+
+
+@pytest.mark.parametrize("cls,odom,cameras", ICP_CASES,
+                         ids=["%s-%s%s" % (c, o, "-cameras" if cam else "") for c, o, cam in ICP_CASES])
+def test_slam_with_icp_odometry_matches_oracle(cls, odom, cameras):
+    """cameras: B=3, a camera per element (tests/golden/cameras.py) with skew and 4th intrinsics column."""
     import gradslam_b200 as gs
 
-    B, L, H, W = 2, 3, 64, 64
-    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=2)
+    if cameras:
+        B, L, H, W = 3, 3, 48, 64
+        rgb, depth, K, poses = camera_inputs(B, L, H, W, 2, skew=0.75)
+    else:
+        B, L, H, W = 2, 3, 64, 64
+        rgb, depth, K, poses = make_sequence(B, L, H, W, seed=2)
     slam = getattr(gs, cls)(odom=odom, numiters=10, device=DEV)
     frames = gs.RGBDImages(rgb.to(DEV), depth.to(DEV), K.to(DEV), poses.to(DEV))
     pc, rec = slam(frames)

@@ -3,6 +3,7 @@ import pytest
 import torch
 
 import gsx_oracle as oracle
+from cameras import CameraShape, camera_inputs
 from gradslam_b200.synthetic import make_sequence
 
 pytestmark = pytest.mark.gpu
@@ -16,13 +17,18 @@ def _frames(gs, rgb, depth, K, poses, dev):
     return gs.RGBDImages(rgb.to(dev), depth.to(dev), K.to(dev), None if poses is None else poses.to(dev))
 
 
-@pytest.mark.parametrize("shape", [(2, 3, 48, 64), (1, 2, 120, 160), (3, 1, 33, 47)])
+@pytest.mark.parametrize("shape", [(2, 3, 48, 64), (1, 2, 120, 160), (3, 1, 33, 47),
+                                   pytest.param(CameraShape((3, 4, 48, 64)), id="cameras")])
 def test_frame_maps_bit_exact(shape):
-    """K1 against oracle.frame_maps: all four maps identical to the last bit (canonical arithmetic)."""
+    """K1 against oracle.frame_maps: all four maps identical to the last bit (canonical arithmetic).  With a camera per
+    element (skew and 4th column set, which back-projection ignores)."""
     import gradslam_b200 as gs
 
     B, L, H, W = shape
-    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=3)
+    if isinstance(shape, CameraShape):
+        rgb, depth, K, poses = camera_inputs(B, L, H, W, seed=3, skew=0.75)
+    else:
+        rgb, depth, K, poses = make_sequence(B, L, H, W, seed=3)
     fr = _frames(gs, rgb, depth, K, poses, _dev())
     ref = oracle.frame_maps(depth, K, poses)
     for name, got in (("vertex", fr.vertex_map), ("normal", fr.normal_map), ("gvertex", fr.global_vertex_map),
@@ -46,12 +52,16 @@ def _compare_maps(pc, ref_map, exact_structure=True):
         assert torch.equal(pc.features_list[b].cpu(), ref_map.ccounts[b])
 
 
-@pytest.mark.parametrize("shape", [(2, 4, 48, 64), (1, 5, 120, 160), (3, 3, 64, 64)])
+@pytest.mark.parametrize("shape", [(2, 4, 48, 64), (1, 5, 120, 160), (3, 3, 64, 64),
+                                   pytest.param(CameraShape((3, 4, 48, 64)), id="cameras")])
 def test_pointfusion_gt_sequence_matches_oracle(shape):
     import gradslam_b200 as gs
 
     B, L, H, W = shape
-    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=0)
+    if isinstance(shape, CameraShape):
+        rgb, depth, K, poses = camera_inputs(B, L, H, W, seed=0, skew=0.75)
+    else:
+        rgb, depth, K, poses = make_sequence(B, L, H, W, seed=0)
     slam = gs.PointFusion(odom="gt", device=_dev())
     pc, out_poses = slam(_frames(gs, rgb, depth, K, poses, _dev()))
     ref = oracle.run_slam(rgb, depth, K, poses, odom="gt")
@@ -60,23 +70,25 @@ def test_pointfusion_gt_sequence_matches_oracle(shape):
 
 
 def test_step_api_equals_sequence_call():
-    """slam.step() frame by frame (per-frame C calls) == slam(frames) (single C call)."""
+    """slam.step() frame by frame (per-frame C calls) == slam(frames) (single C call), on the synthetic inputs and with
+    a camera per element."""
     import gradslam_b200 as gs
 
     B, L, H, W = 2, 4, 48, 64
-    rgb, depth, K, poses = make_sequence(B, L, H, W, seed=5)
     dev = _dev()
     slam = gs.PointFusion(odom="gt", device=dev)
-    frames = _frames(gs, rgb, depth, K, poses, dev)
-    pc_seq, _ = slam(frames)
-    pc = gs.Pointclouds(device=dev)
-    for s in range(L):
-        pc, _ = slam.step(pc, frames[:, s], None, inplace=True)
-    assert pc.num_points_per_pointcloud.tolist() == pc_seq.num_points_per_pointcloud.tolist()
-    for b in range(B):
-        assert torch.equal(pc.points_list[b], pc_seq.points_list[b])
-        assert torch.equal(pc.features_list[b], pc_seq.features_list[b])
-        assert torch.equal(pc.colors_list[b], pc_seq.colors_list[b])
+    for rgb, depth, K, poses in (make_sequence(B, L, H, W, seed=5), camera_inputs(3, L, H, W, seed=5, skew=0.75)):
+        B = rgb.shape[0]
+        frames = _frames(gs, rgb, depth, K, poses, dev)
+        pc_seq, _ = slam(frames)
+        pc = gs.Pointclouds(device=dev)
+        for s in range(L):
+            pc, _ = slam.step(pc, frames[:, s], None, inplace=True)
+        assert pc.num_points_per_pointcloud.tolist() == pc_seq.num_points_per_pointcloud.tolist()
+        for b in range(B):
+            assert torch.equal(pc.points_list[b], pc_seq.points_list[b])
+            assert torch.equal(pc.features_list[b], pc_seq.features_list[b])
+            assert torch.equal(pc.colors_list[b], pc_seq.colors_list[b])
     # not-inplace step leaves the input map untouched
     before = [p.clone() for p in pc.points_list]
     pc2, _ = slam.step(pc, frames[:, 0], None, inplace=False)

@@ -445,3 +445,66 @@ def test_edge_cases_match_frozen_reference(ref_params, name):
                                    rtol=0, atol=2e-5)
         torch.testing.assert_close(res.map.ccounts[b], torch.from_numpy(ref_params["%s/ccounts/%d" % (name, b)]),
                                    rtol=1e-6, atol=1e-7)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# a camera of its own per batch element (tests/golden/cameras.py, frozen by tests/golden/make_golden_cameras.py):
+# fx != fy, off-centre principal points, skew and a 4th intrinsics column, a trajectory per element
+# ---------------------------------------------------------------------------------------------------------------
+from cameras import CAMERA_CASES, SAMPLE_STRIDE, TABLES_CASE, camera_inputs, frozen_table  # noqa: E402
+
+
+@pytest.fixture(scope="module")
+def ref_cameras():
+    return dict(np.load(os.path.join(GOLD, "ref_cameras.npz")))
+
+
+def _check_map_summary(ref, prefix, smap, attrs):
+    """smap against the summary make_golden_cameras.py froze: equal sizes; every SAMPLE_STRIDE-th row within the per-row
+    bound (rtol, atol) of attrs; float64 column sums and absolute sums within the sum of those bounds over the rows."""
+    counts = smap.counts()
+    assert counts == ref[prefix + "/counts"].tolist()
+    for attr, rtol, atol in attrs:
+        rows = [getattr(smap, attr)[b].double() for b in range(len(counts))]
+        sample = torch.from_numpy(ref["%s/%s/sample" % (prefix, attr)]).double()
+        got = torch.cat([r[::SAMPLE_STRIDE] for r in rows])
+        torch.testing.assert_close(got, sample, rtol=rtol, atol=atol)
+        for b, r in enumerate(rows):
+            for stat, val in (("sum", r.sum(0)), ("abs_sum", r.abs().sum(0))):
+                want = torch.from_numpy(ref["%s/%s/%s" % (prefix, attr, stat)][b])
+                bound = counts[b] * atol + rtol * torch.from_numpy(ref["%s/%s/abs_sum" % (prefix, attr)][b])
+                assert ((val - want).abs() <= bound).all(), (attr, stat, b, val, want)
+
+
+@pytest.mark.parametrize("case", CAMERA_CASES, ids=[c[0] for c in CAMERA_CASES])
+def test_slam_runs_with_per_element_cameras_match_frozen_reference(ref_cameras, case):
+    name, cls, B, L, H, W, seed, cam_kw, kw = case
+    rgb, depth, K, poses = camera_inputs(B, L, H, W, seed, **cam_kw)
+    res = oracle.run_slam(rgb, depth, K, poses, mode="pointfusion" if cls == "PointFusion" else "aggregate", **kw)
+    torch.testing.assert_close(res.poses, torch.from_numpy(ref_cameras[name + "/poses"]), rtol=0, atol=1e-5)
+    attrs = [("points", 0, 2e-5), ("normals", 0, 2e-5), ("colors", 0, 2e-6)]
+    _check_map_summary(ref_cameras, name, res.map, attrs + ([("ccounts", 1e-6, 1e-7)] if cls == "PointFusion" else []))
+
+
+def test_correspondence_tables_with_per_element_cameras_match_frozen_reference(ref_cameras):
+    """The three tables of one fusion step, projected with each element's skewed K and 4th column, row for row."""
+    c = TABLES_CASE
+    B, H, W = c["B"], c["H"], c["W"]
+    rgb, depth, K, poses = camera_inputs(B, c["L"], H, W, c["seed"], skew=c["skew"])
+    assert (K[:, 0, 0, 1] != 0).all() and (K[:, 0, :2, 3] != 0).all()
+    dot_th = math.cos(20 * math.pi / 180)
+    smap = oracle.SurfelMap()
+    for s in range(2):
+        maps = oracle.frame_maps(depth[:, s:s + 1], K, poses[:, s:s + 1])
+        smap = oracle.update_map_fusion(smap, maps, rgb[:, s:s + 1], poses[:, s], K[:, 0], 0.05, dot_th, 0.6)
+    _check_map_summary(ref_cameras, "tables/map_before", smap,
+                       [("points", 0, 2e-6), ("normals", 0, 2e-5), ("colors", 0, 2e-6), ("ccounts", 1e-6, 1e-7)])
+    maps = oracle.frame_maps(depth[:, 2:3], K, poses[:, 2:3])
+    gv, gn = maps["gvertex"][:, 0], maps["gnormal"][:, 0]
+    active = oracle.find_active_map_points(smap, poses[:, 2], K[:, 0], H, W)
+    assert torch.equal(active, frozen_table(ref_cameras, "active"))
+    similar, mask = oracle.find_similar_map_points(smap, gv, gn, active, 0.05, dot_th)
+    assert torch.equal(mask, torch.from_numpy(ref_cameras["tables/similar_mask"]))
+    assert torch.equal(similar, frozen_table(ref_cameras, "similar"))
+    unique = oracle.find_best_unique_correspondences(smap, gv, similar)
+    assert torch.equal(unique, frozen_table(ref_cameras, "unique"))
