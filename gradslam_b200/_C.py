@@ -129,6 +129,40 @@ def check(rc, what):
         raise RuntimeError("%s failed (status %d): %s" % (what, rc, lib().gsx_last_error().decode()))
 
 
+# (library handle, name) -> function object.  Keyed by the handle as well: scripts/tune.py swaps `_lib` for a variant.
+_entries = {}
+
+
+def launch(name, *args, device=None, stream=None):
+    """Calls the entry point `name` of libgsx, whose last parameter is the stream, and raises on a non-zero status.
+
+    A tensor argument passes as its data pointer and None as NULL; anything else goes to the ctypes argtypes as is.
+    `args` holds every tensor until the call returns, so a temporary such as `t.contiguous()` may be passed directly.
+    The tensors must be CUDA tensors on one device; the call runs on that device (`device`, when no tensor is passed)
+    and enqueues its work on `stream`, by default the device's current stream."""
+    handle = lib()
+    fn = _entries.get((handle, name))
+    if fn is None:
+        fn = _entries[handle, name] = getattr(handle, name)
+    if device is not None and not isinstance(device, int):
+        device = torch.device(device).index
+    conv = []
+    for i, a in enumerate(args):
+        if isinstance(a, torch.Tensor):
+            d = a.get_device()  # -1 unless a CUDA tensor
+            if device is None and d >= 0:
+                device = d
+            if d < 0 or d != device:
+                raise RuntimeError("gradslam_b200: %s takes CUDA tensors on one device; argument %d is on %s%s" % (
+                    name, i, a.device, "" if device is None else ", not cuda:%d" % device))
+            a = ctypes.c_void_p(a.data_ptr())
+        conv.append(a)
+    with torch.cuda.device(device):
+        s = torch.cuda.current_stream(device) if stream is None else stream
+        rc = fn(*conv, ctypes.c_void_p(s.cuda_stream))
+    check(rc, name)
+
+
 def require_cuda(t, name):
     if not t.is_cuda:
         raise RuntimeError(

@@ -27,10 +27,8 @@ def scale_intrinsics(intrinsics: torch.Tensor, h_ratio: Union[float, int], w_rat
         K = intrinsics.to(torch.float).contiguous()
         out = torch.empty_like(K)
         n = K.numel() // (K.shape[-1] * K.shape[-1])
-        with torch.cuda.device(K.device):
-            rc = _C.lib().gsx_ingest_calibration(_C.ptr(K), n, K.shape[-1], float(h_ratio), float(w_ratio), _C.ptr(out),
-                                                 None, 0, 0, None, None, _C.stream_ptr(K.device))
-        _C.check(rc, "gsx_ingest_calibration")
+        _C.launch("gsx_ingest_calibration", K, n, K.shape[-1], float(h_ratio), float(w_ratio), out, None, 0, 0, None,
+                  None)
         return out
     out = intrinsics.to(torch.float).clone()
     out[..., 0, 0] *= w_ratio
@@ -53,10 +51,7 @@ def relative_poses(poses: torch.Tensor) -> torch.Tensor:
     B, L = (1, p.shape[0]) if p.dim() == 3 else p.shape[:2]
     out = torch.empty_like(p)
     flag = torch.zeros(1, dtype=torch.int32, device=p.device)
-    with torch.cuda.device(p.device):
-        rc = _C.lib().gsx_ingest_calibration(None, 0, 4, 1.0, 1.0, None, _C.ptr(p), B, L, _C.ptr(out), _C.ptr(flag),
-                                             _C.stream_ptr(p.device))
-    _C.check(rc, "gsx_ingest_calibration")
+    _C.launch("gsx_ingest_calibration", None, 0, 4, 1.0, 1.0, None, p, B, L, out, flag)
     return out
 
 
@@ -83,10 +78,8 @@ def raw_to_float(colors_u8: torch.Tensor, depths_u16: torch.Tensor, scaling_fact
     dev = colors_u8.device
     rgb = out_rgb if out_rgb is not None else torch.empty(colors_u8.shape, dtype=torch.float32, device=dev)
     depth = out_depth if out_depth is not None else torch.empty((*depths_u16.shape, 1), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _C.lib().gsx_ingest_raw(_C.ptr(colors_u8), _C.ptr(depths_u16), depths_u16.numel(), float(scaling_factor),
-                                     1 if normalize_color else 0, _C.ptr(rgb), _C.ptr(depth), _C.stream_ptr(dev))
-    _C.check(rc, "gsx_ingest_raw")
+    _C.launch("gsx_ingest_raw", colors_u8, depths_u16, depths_u16.numel(), float(scaling_factor),
+              1 if normalize_color else 0, rgb, depth)
     return rgb, depth
 
 

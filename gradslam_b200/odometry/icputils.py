@@ -91,12 +91,8 @@ def knn1(src: torch.Tensor, tgt: torch.Tensor, src_counts=None, tgt_counts=None,
     # (the kernel writes the rows below each source size; the padding rows keep -1 / inf)
     idx = torch.full((B, Ns), -1, dtype=torch.int64, device=src.device)
     d2 = torch.full((B, Ns), float("inf"), dtype=torch.float32, device=src.device)
-    ns_t = _counts(Ns, B, src.device) if src_counts is None else src_counts  # (kept alive across the call)
-    with torch.cuda.device(src.device):
-        rc = _C.lib().gsx_knn1(_C.ptr(src), _C.ptr(ns_t), Ns, _C.ptr(tgt_c), _C.ptr(nt_t), Nt, B, _C.ptr(idx),
-                               _C.ptr(d2), _C.ptr(scratch), scratch.numel(), 0 if hit else 1,
-                               _C.stream_ptr(src.device))
-    _C.check(rc, "gsx_knn1")
+    ns_t = _counts(Ns, B, src.device) if src_counts is None else src_counts
+    _C.launch("gsx_knn1", src, ns_t, Ns, tgt_c, nt_t, Nt, B, idx, d2, scratch, scratch.numel(), 0 if hit else 1)
     return d2, idx
 
 
@@ -145,18 +141,13 @@ def icp_align(src, src_counts, tgt, tgt_normals, tgt_counts, T0, mode, numiters,
     dev = src.device
     out = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
     idx = torch.empty((Bn, Ns), dtype=torch.int64, device=dev) if want_idx else None
-    lib = _C.lib()
-    nbytes = lib.gsx_icp_align_scratch_bytes(Bn, Ns, Nt)
+    nbytes = _C.lib().gsx_icp_align_scratch_bytes(Bn, Ns, Nt)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     T0c = None if T0 is None else T0.to(dev).float().contiguous()
-    with torch.cuda.device(dev):
-        rc = lib.gsx_icp_align(
-            _C.ptr(src.contiguous()), _C.ptr(src_counts), Ns, _C.ptr(tgt.contiguous()),
-            _C.ptr(tgt_normals.contiguous()), _C.ptr(tgt_counts), Nt, Bn, _C.ptr(T0c), int(mode), int(numiters),
-            float(damp), 0 if dist_thresh is None else 1, 0.0 if dist_thresh is None else float(dist_thresh),
-            float(lambda_max), float(B), float(B2), float(nu), _C.ptr(out), _C.ptr(idx), _C.ptr(scratch), nbytes,
-            _C.stream_ptr(dev))
-    _C.check(rc, "gsx_icp_align")
+    _C.launch("gsx_icp_align", src.contiguous(), src_counts, Ns, tgt.contiguous(), tgt_normals.contiguous(), tgt_counts,
+              Nt, Bn, T0c, int(mode), int(numiters), float(damp), 0 if dist_thresh is None else 1,
+              0.0 if dist_thresh is None else float(dist_thresh), float(lambda_max), float(B), float(B2), float(nu), out,
+              idx, scratch, nbytes)
     return out, idx
 
 
@@ -176,27 +167,20 @@ class _NormalEqFn(torch.autograd.Function):
             _C.require_cuda(t, name)
         ns, dev = src_c.shape[0], src_c.device
         sums = torch.empty(28, dtype=torch.float32, device=dev)
-        lib = _C.lib()
-        nbytes = lib.gsx_icp_normal_eq_scratch_bytes(ns)
+        nbytes = _C.lib().gsx_icp_normal_eq_scratch_bytes(ns)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.gsx_icp_normal_eq_fwd(_C.ptr(src_c), ns, _C.ptr(tgt_c), _C.ptr(tn_c), _C.ptr(idx_c), _C.ptr(sums),
-                                           _C.ptr(scratch), nbytes, _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_normal_eq_fwd")
+        _C.launch("gsx_icp_normal_eq_fwd", src_c, ns, tgt_c, tn_c, idx_c, sums, scratch, nbytes)
         ctx.saved = (src_c, tgt_c, tn_c, idx_c)
         return sums
 
     @staticmethod
     def backward(ctx, g):
         src_c, tgt_c, tn_c, idx_c = ctx.saved
-        ns, dev = src_c.shape[0], src_c.device
+        ns = src_c.shape[0]
         g = g.contiguous().float()
         g_src = torch.empty_like(src_c)
         rows_p, rows_n = torch.empty_like(src_c), torch.empty_like(src_c)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_normal_eq_bwd(_C.ptr(src_c), ns, _C.ptr(tgt_c), _C.ptr(tn_c), _C.ptr(idx_c), _C.ptr(g),
-                                                _C.ptr(g_src), _C.ptr(rows_p), _C.ptr(rows_n), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_normal_eq_bwd")
+        _C.launch("gsx_icp_normal_eq_bwd", src_c, ns, tgt_c, tn_c, idx_c, g, g_src, rows_p, rows_n)
         safe = idx_c.clamp(min=0)  # rows with idx < 0 carry zero gradients
         g_tgt = torch.zeros_like(tgt_c).index_add_(0, safe, rows_p)
         g_tn = torch.zeros_like(tn_c).index_add_(0, safe, rows_n)
@@ -214,23 +198,17 @@ class _SolveFn(torch.autograd.Function):
         dev = s.device
         xi = torch.empty(6, dtype=torch.float32, device=dev)
         dT = torch.empty((4, 4), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_solve_fwd(_C.ptr(s), _C.ptr(d), 1, _C.ptr(xi), _C.ptr(dT), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_solve_fwd")
+        _C.launch("gsx_icp_solve_fwd", s, d, 1, xi, dT)
         ctx.saved = (s, d, damp.shape)
         return xi, dT
 
     @staticmethod
     def backward(ctx, g_xi, g_dT):
         s, d, damp_shape = ctx.saved
-        dev = s.device
         g_xi = None if g_xi is None else g_xi.contiguous().float()
         g_dT = None if g_dT is None else g_dT.contiguous().float()
         g_s, g_d = torch.empty_like(s), torch.empty_like(d)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_solve_bwd(_C.ptr(s), _C.ptr(d), 1, _C.ptr(g_xi), _C.ptr(g_dT), _C.ptr(g_s),
-                                            _C.ptr(g_d), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_solve_bwd")
+        _C.launch("gsx_icp_solve_bwd", s, d, 1, g_xi, g_dT, g_s, g_d)
         return g_s, g_d.view(damp_shape)
 
 
@@ -249,23 +227,16 @@ class _UpdateFn(torch.autograd.Function):
         dT = torch.empty((4, 4), dtype=torch.float32, device=dev)
         Tn = torch.empty((4, 4), dtype=torch.float32, device=dev)
         par = (int(mode), float(lambda_max), float(B), float(B2), float(nu))
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_update_fwd(*[_C.ptr(t) for t in ins], 1, *par, _C.ptr(damp_out), _C.ptr(dT),
-                                             _C.ptr(Tn), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_update_fwd")
+        _C.launch("gsx_icp_update_fwd", *ins, 1, *par, damp_out, dT, Tn)
         ctx.saved = (ins, par, (xi.shape, err.shape, new_err.shape, damp.shape, T.shape))
         return damp_out.view(damp.shape), dT, Tn
 
     @staticmethod
     def backward(ctx, g_damp, g_dT, g_T):
         ins, par, shapes = ctx.saved
-        dev = ins[0].device
         gs = [None if g is None else g.contiguous().float() for g in (g_damp, g_dT, g_T)]
         outs = [torch.empty_like(t) for t in ins]
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_update_bwd(*[_C.ptr(t) for t in ins], 1, *par, *[_C.ptr(g) for g in gs],
-                                             *[_C.ptr(o) for o in outs], _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_update_bwd")
+        _C.launch("gsx_icp_update_bwd", *ins, 1, *par, *gs, *outs)
         return tuple(o.view(sh) for o, sh in zip(outs, shapes)) + (None,) * 5
 
 
@@ -277,11 +248,8 @@ class _RigidTransformFn(torch.autograd.Function):
     def forward(ctx, points, T):
         p, Tc = points.detach().contiguous().float(), T.detach().contiguous().float()
         _C.require_cuda(p, "points")
-        dev = p.device
         out = torch.empty_like(p)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_rigid_transform_fwd(_C.ptr(p), p.shape[0], _C.ptr(Tc), _C.ptr(out), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_rigid_transform_fwd")
+        _C.launch("gsx_rigid_transform_fwd", p, p.shape[0], Tc, out)
         ctx.saved = (p, Tc)
         return out
 
@@ -291,13 +259,9 @@ class _RigidTransformFn(torch.autograd.Function):
         dev, n = p.device, p.shape[0]
         g = g.contiguous().float()
         g_p, g_T = torch.empty_like(p), torch.empty_like(Tc)
-        lib = _C.lib()
-        nbytes = lib.gsx_rigid_transform_bwd_scratch_bytes(n)
+        nbytes = _C.lib().gsx_rigid_transform_bwd_scratch_bytes(n)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.gsx_rigid_transform_bwd(_C.ptr(p), n, _C.ptr(Tc), _C.ptr(g), _C.ptr(g_p), _C.ptr(g_T),
-                                             _C.ptr(scratch), nbytes, _C.stream_ptr(dev))
-        _C.check(rc, "gsx_rigid_transform_bwd")
+        _C.launch("gsx_rigid_transform_bwd", p, n, Tc, g, g_p, g_T, scratch, nbytes)
         return g_p, g_T
 
 
@@ -315,14 +279,10 @@ class _NormalEqBatchedFn(torch.autograd.Function):
         Bn, Ns, _ = src_c.shape
         Nt, dev = tgt_c.shape[1], src_c.device
         sums = torch.empty((Bn, 28), dtype=torch.float32, device=dev)
-        lib = _C.lib()
-        nbytes = Bn * lib.gsx_icp_normal_eq_scratch_bytes(Ns)
+        nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.gsx_icp_normal_eq_batched_fwd(_C.ptr(src_c), _C.ptr(src_counts), Ns, _C.ptr(tgt_c), _C.ptr(tn_c), Nt,
-                                                   Bn, _C.ptr(idx_c), _C.ptr(sums), _C.ptr(scratch), nbytes,
-                                                   _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_normal_eq_batched_fwd")
+        _C.launch("gsx_icp_normal_eq_batched_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums, scratch,
+                  nbytes)
         ctx.saved = (src_c, tgt_c, tn_c, idx_c, src_counts)
         return sums
 
@@ -334,11 +294,8 @@ class _NormalEqBatchedFn(torch.autograd.Function):
         g = g.contiguous().float()
         g_src = torch.empty_like(src_c)
         rows_p, rows_n = torch.empty_like(src_c), torch.empty_like(src_c)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_normal_eq_batched_bwd(_C.ptr(src_c), _C.ptr(src_counts), Ns, _C.ptr(tgt_c),
-                                                        _C.ptr(tn_c), Nt, Bn, _C.ptr(idx_c), _C.ptr(g), _C.ptr(g_src),
-                                                        _C.ptr(rows_p), _C.ptr(rows_n), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_normal_eq_batched_bwd")
+        _C.launch("gsx_icp_normal_eq_batched_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src, rows_p,
+                  rows_n)
         # rows with idx < 0 carry zero gradients; scatter the per-source-row target gradients with the association
         flat = (idx_c.clamp(min=0) + torch.arange(Bn, device=dev).view(Bn, 1) * Nt).view(-1)
         g_tgt = torch.zeros((Bn * Nt, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_p.view(-1, 3))
@@ -354,23 +311,17 @@ class _SolveBatchedFn(torch.autograd.Function):
         Bn, dev = s.shape[0], s.device
         xi = torch.empty((Bn, 6), dtype=torch.float32, device=dev)
         dT = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_solve_fwd(_C.ptr(s), _C.ptr(d), Bn, _C.ptr(xi), _C.ptr(dT), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_solve_fwd")
+        _C.launch("gsx_icp_solve_fwd", s, d, Bn, xi, dT)
         ctx.saved = (s, d)
         return xi, dT
 
     @staticmethod
     def backward(ctx, g_xi, g_dT):
         s, d = ctx.saved
-        dev = s.device
         g_xi = None if g_xi is None else g_xi.contiguous().float()
         g_dT = None if g_dT is None else g_dT.contiguous().float()
         g_s, g_d = torch.empty_like(s), torch.empty_like(d)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_solve_bwd(_C.ptr(s), _C.ptr(d), s.shape[0], _C.ptr(g_xi), _C.ptr(g_dT), _C.ptr(g_s),
-                                            _C.ptr(g_d), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_solve_bwd")
+        _C.launch("gsx_icp_solve_bwd", s, d, s.shape[0], g_xi, g_dT, g_s, g_d)
         return g_s, g_d
 
 
@@ -385,23 +336,16 @@ class _UpdateBatchedFn(torch.autograd.Function):
         dT = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
         Tn = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
         par = (int(mode), float(lambda_max), float(B), float(B2), float(nu))
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_update_fwd(*[_C.ptr(t) for t in ins], Bn, *par, _C.ptr(damp_out), _C.ptr(dT),
-                                             _C.ptr(Tn), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_update_fwd")
+        _C.launch("gsx_icp_update_fwd", *ins, Bn, *par, damp_out, dT, Tn)
         ctx.saved = (ins, par)
         return damp_out, dT, Tn
 
     @staticmethod
     def backward(ctx, g_damp, g_dT, g_T):
         ins, par = ctx.saved
-        dev = ins[0].device
         gs = [None if g is None else g.contiguous().float() for g in (g_damp, g_dT, g_T)]
         outs = [torch.empty_like(t) for t in ins]
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_icp_update_bwd(*[_C.ptr(t) for t in ins], ins[0].shape[0], *par, *[_C.ptr(g) for g in gs],
-                                             *[_C.ptr(o) for o in outs], _C.stream_ptr(dev))
-        _C.check(rc, "gsx_icp_update_bwd")
+        _C.launch("gsx_icp_update_bwd", *ins, ins[0].shape[0], *par, *gs, *outs)
         return tuple(outs) + (None,) * 5
 
 
@@ -410,12 +354,8 @@ class _RigidTransformBatchedFn(torch.autograd.Function):
     def forward(ctx, points, T, counts):
         p, Tc = points.detach().contiguous().float(), T.detach().contiguous().float()
         _C.require_cuda(p, "points")
-        dev = p.device
         out = torch.empty_like(p)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_rigid_transform_batched_fwd(_C.ptr(p), _C.ptr(counts), p.shape[1], p.shape[0], _C.ptr(Tc),
-                                                          _C.ptr(out), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_rigid_transform_batched_fwd")
+        _C.launch("gsx_rigid_transform_batched_fwd", p, counts, p.shape[1], p.shape[0], Tc, out)
         ctx.saved = (p, Tc, counts)
         return out
 
@@ -426,13 +366,9 @@ class _RigidTransformBatchedFn(torch.autograd.Function):
         Bn, n = p.shape[0], p.shape[1]
         g = g.contiguous().float()
         g_p, g_T = torch.empty_like(p), torch.empty_like(Tc)
-        lib = _C.lib()
-        nbytes = Bn * lib.gsx_rigid_transform_bwd_scratch_bytes(n)
+        nbytes = Bn * _C.lib().gsx_rigid_transform_bwd_scratch_bytes(n)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.gsx_rigid_transform_batched_bwd(_C.ptr(p), _C.ptr(counts), n, Bn, _C.ptr(Tc), _C.ptr(g), _C.ptr(g_p),
-                                                     _C.ptr(g_T), _C.ptr(scratch), nbytes, _C.stream_ptr(dev))
-        _C.check(rc, "gsx_rigid_transform_batched_bwd")
+        _C.launch("gsx_rigid_transform_batched_bwd", p, counts, n, Bn, Tc, g, g_p, g_T, scratch, nbytes)
         return g_p, g_T, None
 
 
@@ -679,14 +615,10 @@ def localize_against_map(pointclouds, live_frame, prev_frame, dsratio, odomprov)
     out = torch.empty((B, 1, 4, 4), dtype=torch.float32, device=dev)
     mode = 1 if hasattr(odomprov, "lambda_max") else 0
     dth = odomprov.dist_thresh
-    with torch.cuda.device(dev):
-        rc = _C.lib().gsx_icp_localize(
-            _C.ptr(geo), _C.ptr(pointclouds._counts_dev[pointclouds._cur]),
-            pointclouds.capacity, pointclouds._bound, _C.ptr(depth), d_bs, _C.ptr(K), 16, _C.ptr(prev), 16, B, H, W,
-            int(dsratio), mode, int(odomprov.numiters), float(odomprov.damp), 0 if dth is None else 1,
-            0.0 if dth is None else float(dth), float(getattr(odomprov, "lambda_max", 2.0)),
-            float(getattr(odomprov, "B", 1.0)), float(getattr(odomprov, "B2", 1.0)),
-            float(getattr(odomprov, "nu", 200.0)), _C.ptr(tgt), bound, _C.ptr(out), 16, _C.ptr(ws.buf),
-            ws.capacity, ws.next_epoch(), _C.ptr(pointclouds._overflow_flag()), _C.stream_ptr(dev))
-    _C.check(rc, "gsx_icp_localize")
+    _C.launch("gsx_icp_localize", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
+              pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters),
+              float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth),
+              float(getattr(odomprov, "lambda_max", 2.0)), float(getattr(odomprov, "B", 1.0)),
+              float(getattr(odomprov, "B2", 1.0)), float(getattr(odomprov, "nu", 200.0)), tgt, bound, out, 16, ws.buf,
+              ws.capacity, ws.next_epoch(), pointclouds._overflow_flag())
     return out

@@ -144,11 +144,7 @@ def _launch_frame_records(ws, frames, sigma, device, maps=None, world=True):
         gv = gn = vl = None
         K = _dense(frames.intrinsics, "intrinsics", device)
         poses = _dense(frames.poses, "poses", device) if (world and frames.poses is not None) else None
-    with torch.cuda.device(device):
-        rc = _C.lib().gsx_fusion_frame_records(_C.ptr(depth), d_bs, _C.ptr(K), 16, _C.ptr(poses), 16, _C.ptr(gv),
-                                               _C.ptr(gn), _C.ptr(vl), B, H, W, sigma, _C.ptr(ws.buf),
-                                               _C.stream_ptr(device))
-    _C.check(rc, "gsx_fusion_frame_records")
+    _C.launch("gsx_fusion_frame_records", depth, d_bs, K, 16, poses, 16, gv, gn, vl, B, H, W, sigma, ws.buf)
 
 
 def _dense_frame(t, name, device):
@@ -169,12 +165,8 @@ def _launch_merge_append(pointclouds, frames, ws, assoc=None):
     geo, col = _map_ptrs(pointclouds, dev)
     cin = pointclouds._counts_dev[pointclouds._cur]
     cout = pointclouds._counts_dev[pointclouds._cur ^ 1]
-    with torch.cuda.device(dev):
-        rc = _C.lib().gsx_fusion_merge_append(
-            _C.ptr(geo), _C.ptr(col), 1 if pointclouds._has_cc else 0, _C.ptr(cin), _C.ptr(cout),
-            pointclouds.capacity, _C.ptr(rgb), c_bs, B, H, W, _C.ptr(ws.buf), _C.ptr(pointclouds._overflow_flag()),
-            _C.ptr(assoc), _C.stream_ptr(dev))
-    _C.check(rc, "gsx_fusion_merge_append")
+    _C.launch("gsx_fusion_merge_append", geo, col, 1 if pointclouds._has_cc else 0, cin, cout, pointclouds.capacity, rgb,
+              c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc)
     pointclouds._mark_device_updated(pointclouds._bound + P)
 
 
@@ -233,12 +225,8 @@ def _fused_update(pointclouds, frames, dist_th, dot_th, sigma):
         geo, _ = _map_ptrs(pointclouds, dev)
         poses = _dense(frames.poses, "poses", dev)
         K = _dense(frames.intrinsics, "intrinsics", dev)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_fusion_project_select(
-                _C.ptr(geo), _C.ptr(pointclouds._counts_dev[pointclouds._cur]), pointclouds.capacity,
-                pointclouds._bound, _C.ptr(poses), 16, _C.ptr(K), 16, B, H, W, float(dist_th), float(dot_th),
-                _C.ptr(ws.buf), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_fusion_project_select")
+        _C.launch("gsx_fusion_project_select", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
+                  pointclouds._bound, poses, 16, K, 16, B, H, W, float(dist_th), float(dot_th), ws.buf)
     _launch_merge_append(pointclouds, frames, ws)
     return pointclouds
 
@@ -248,14 +236,10 @@ def _compact(flags: torch.Tensor) -> torch.Tensor:
     """Ascending indices of the non-zero entries of a flat uint8 CUDA tensor (stable compaction kernel)."""
     n = flags.numel()
     dev = flags.device
-    lib = _C.lib()
-    scratch = torch.zeros(lib.gsx_compact_scratch_bytes(n), dtype=torch.uint8, device=dev)
+    scratch = torch.zeros(_C.lib().gsx_compact_scratch_bytes(n), dtype=torch.uint8, device=dev)
     idx = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
     cnt = torch.zeros(1, dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        rc = lib.gsx_compact_indices(_C.ptr(flags), n, _C.ptr(idx), _C.ptr(cnt), _C.ptr(scratch), 1,
-                                     _C.stream_ptr(dev))
-    _C.check(rc, "gsx_compact_indices")
+    _C.launch("gsx_compact_indices", flags, n, idx, cnt, scratch, 1)
     return idx[: int(cnt.item())]  # the table's length is data dependent: this is the API's one host sync
 
 
@@ -302,11 +286,8 @@ def find_active_map_points(pointclouds: Pointclouds, rgbdimages: RGBDImages) -> 
     flags = torch.empty((B, width), dtype=torch.uint8, device=device)
     hw = torch.empty((B, width), dtype=torch.int32, device=device)
     poses, K = _dense(frames.poses, "poses", device), _dense(frames.intrinsics, "intrinsics", device)
-    with torch.cuda.device(device):
-        rc = _C.lib().gsx_active_eval(_C.ptr(geo), _C.ptr(pointclouds._counts_dev[pointclouds._cur]),
-                                      pointclouds.capacity, width, _C.ptr(poses), 16, _C.ptr(K), 16, B, H, W,
-                                      _C.ptr(flags), _C.ptr(hw), _C.stream_ptr(device))
-    _C.check(rc, "gsx_active_eval")
+    _C.launch("gsx_active_eval", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, width, poses, 16,
+              K, 16, B, H, W, flags, hw)
     idx = _compact(flags.view(-1))
     pix = hw.view(-1)[idx].to(torch.int64)
     table = torch.stack([idx // width, idx % width, pix // W, pix % W], dim=1)
@@ -339,11 +320,8 @@ def find_similar_map_points(pointclouds: Pointclouds, rgbdimages: RGBDImages, pc
     gv, gn = frames.global_vertex_map.contiguous(), frames.global_normal_map.contiguous()
     geo = _dense(pointclouds._geo, "pointclouds (geometry rows)", device)
     flags = torch.empty(rows, dtype=torch.uint8, device=device)
-    with torch.cuda.device(device):
-        rc = _C.lib().gsx_similar_eval(_C.ptr(table), rows, _C.ptr(geo), pointclouds.capacity, _C.ptr(gv),
-                                       _C.ptr(gn), B, H, W, float(dist_th), float(dot_th), _C.ptr(flags),
-                                       _C.stream_ptr(device))
-    _C.check(rc, "gsx_similar_eval")
+    _C.launch("gsx_similar_eval", table, rows, geo, pointclouds.capacity, gv, gn, B, H, W, float(dist_th), float(dot_th),
+              flags)
     keep = _compact(flags)
     similar = table[keep]
     if similar.shape[0] == 0:
@@ -378,10 +356,7 @@ def find_best_unique_correspondences(pointclouds: Pointclouds, rgbdimages: RGBDI
     records = torch.empty(B * H * W * 2, dtype=torch.int64, device=device)  # 16-byte arg-min records (scratch)
     pflags = torch.empty(B * H * W, dtype=torch.uint8, device=device)
     pn = torch.empty(B * H * W, dtype=torch.int64, device=device)
-    with torch.cuda.device(device):
-        rc = _C.lib().gsx_unique_select(_C.ptr(table), table.shape[0], _C.ptr(geo), pointclouds.capacity, _C.ptr(gv),
-                                        B, H, W, _C.ptr(records), _C.ptr(pflags), _C.ptr(pn), _C.stream_ptr(device))
-    _C.check(rc, "gsx_unique_select")
+    _C.launch("gsx_unique_select", table, table.shape[0], geo, pointclouds.capacity, gv, B, H, W, records, pflags, pn)
     pix = _compact(pflags)
     rem = pix % (H * W)
     return torch.stack([pix // (H * W), pn[pix], rem // W, rem % W], dim=1)
@@ -430,10 +405,7 @@ def fuse_with_map(pointclouds: Pointclouds, rgbdimages: RGBDImages, pc2im_bnhw: 
 
 def _records_from_table(ws, table, pointclouds, B, H, W, device):
     table = table.to(device).contiguous()
-    with torch.cuda.device(device):
-        rc = _C.lib().gsx_records_from_table(_C.ptr(table), table.shape[0], pointclouds.capacity, B, H, W,
-                                             _C.ptr(ws.buf), _C.stream_ptr(device))
-    _C.check(rc, "gsx_records_from_table")
+    _C.launch("gsx_records_from_table", table, table.shape[0], pointclouds.capacity, B, H, W, ws.buf)
 
 
 # --------------------------------------------------------------------------------------------- differentiable mode
@@ -471,12 +443,8 @@ class _MergeAppendFn(torch.autograd.Function):
         counts_out = pointclouds._counts_dev[pointclouds._cur ^ 1]
         assoc = torch.zeros((B, P), dtype=torch.int32, device=dev)
         with_cc = 1 if pointclouds._has_cc else 0
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_fusion_merge_append(
-                _C.ptr(outs[0]), _C.ptr(outs[1]), with_cc, _C.ptr(counts_in), _C.ptr(counts_out), cap_out,
-                _C.ptr(rgb_c), P * 3, B, H, W, _C.ptr(ws.buf), _C.ptr(pointclouds._overflow_flag()), _C.ptr(assoc),
-                _C.stream_ptr(dev))
-        _C.check(rc, "gsx_fusion_merge_append")
+        _C.launch("gsx_fusion_merge_append", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c, P * 3, B,
+                  H, W, ws.buf, pointclouds._overflow_flag(), assoc)
         ctx.saved = (assoc, counts_in, geo.detach(), col.detach(), gv_c, gn_c, rgb_c, vloc_c)
         ctx.dims = (B, H, W, cap_in, cap_out, float(sigma), with_cc)
         ctx.shapes = (gv.shape, rgb.shape)
@@ -491,13 +459,8 @@ class _MergeAppendFn(torch.autograd.Function):
         geo_c, col_c = geo.contiguous(), col.contiguous()
         d_map = [torch.empty_like(geo_c), torch.empty_like(col_c)]
         d_frame = [torch.empty((B, 1, H, W, 3), dtype=torch.float32, device=dev) for _ in range(4)]
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_fusion_merge_append_bwd(
-                _C.ptr(assoc), _C.ptr(counts_in), _C.ptr(geo_c), _C.ptr(col_c), with_cc, cap_in, _C.ptr(gs[0]),
-                _C.ptr(gs[1]), cap_out, _C.ptr(gv), _C.ptr(gn), _C.ptr(rgb), _C.ptr(vloc), B, H, W, sigma,
-                _C.ptr(d_map[0]), _C.ptr(d_map[1]), _C.ptr(d_frame[0]), _C.ptr(d_frame[1]), _C.ptr(d_frame[2]),
-                _C.ptr(d_frame[3]), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_fusion_merge_append_bwd")
+        _C.launch("gsx_fusion_merge_append_bwd", assoc, counts_in, geo_c, col_c, with_cc, cap_in, *gs, cap_out, gv, gn,
+                  rgb, vloc, B, H, W, sigma, *d_map, *d_frame)
         gv_shape, rgb_shape = ctx.shapes
         return (None, d_map[0], d_map[1], d_frame[0].view(gv_shape), d_frame[1].view(gv_shape),
                 d_frame[2].view(rgb_shape), d_frame[3].view(gv_shape))
@@ -528,12 +491,8 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
         geo = _dense(pointclouds._geo.detach(), "pointclouds (geometry rows)", dev)
         K = _dense(frames.intrinsics.detach(), "intrinsics", dev)
         poses = _dense(frames.poses.detach(), "poses", dev)
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_fusion_project_select(
-                _C.ptr(geo), _C.ptr(pointclouds._counts_dev[pointclouds._cur]), pointclouds.capacity,
-                pointclouds._bound, _C.ptr(poses), 16, _C.ptr(K), 16, B, H, W, float(dist_th), float(dot_th),
-                _C.ptr(ws.buf), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_fusion_project_select")
+        _C.launch("gsx_fusion_project_select", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
+                  pointclouds._bound, poses, 16, K, 16, B, H, W, float(dist_th), float(dot_th), ws.buf)
     geo_out, col_out = _MergeAppendFn.apply((pointclouds, frames, sig, ws), pointclouds._geo, pointclouds._col, gv, gn,
                                             frames.rgb_image, vloc)
     pointclouds._geo, pointclouds._col = geo_out, col_out

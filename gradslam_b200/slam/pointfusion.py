@@ -124,39 +124,33 @@ class PointFusion(ICPSLAM):
             pc._allocate(B, L * P, 1, zero=False)
         ws = _SequenceWorkspace.get(dev, B, H, W)
         main = torch.cuda.current_stream(dev)
-        with torch.cuda.device(dev):
-            ready = []
-            if not on_device:
-                copy_stream.wait_stream(main)  # the fresh buffers must exist before the copies start
-                with torch.cuda.stream(copy_stream):
-                    for s0 in range(0, L, chunk):
-                        s1 = min(L, s0 + chunk)
-                        dst_d, dst_c = (raw_depth, raw_rgb) if raw else (depth, rgb)
-                        for b in range(B):  # per-element slices are contiguous: true async DMA from pinned memory
-                            dst_d[b, s0:s1].copy_(src_depth[b, s0:s1], non_blocking=True)
-                            dst_c[b, s0:s1].copy_(src_rgb[b, s0:s1], non_blocking=True)
-                        ev = torch.cuda.Event()
-                        ev.record(copy_stream)
-                        ready.append(ev)
-            for i, s0 in enumerate(range(0, L, chunk)):
-                s1 = min(L, s0 + chunk)
-                if ready:
-                    main.wait_event(ready[i])
-                if raw:  # u8 / u16 -> float32 for this chunk (per element: the chunk is contiguous inside an element)
-                    for b in range(B):
-                        _C.check(_C.lib().gsx_ingest_raw(
-                            _C.ptr(raw_rgb[b, s0:s1]), _C.ptr(raw_depth[b, s0:s1]), (s1 - s0) * P,
-                            frames.scaling_factor, 1 if frames.normalize_color else 0, _C.ptr(rgb[b, s0:s1]),
-                            _C.ptr(depth[b, s0:s1]), _C.stream_ptr(dev)), "gsx_ingest_raw")
-                rc = _C.lib().gsx_pointfusion_sequence_gt(
-                    _C.ptr(pc._geo), _C.ptr(pc._col), _C.ptr(pc._counts_dev), pc.capacity, min(s0 * P, pc.capacity),
-                    _C.ptr(depth), _C.ptr(rgb), _C.ptr(K), _C.ptr(poses), B, L, s0, s1, H, W, float(self.dist_th),
-                    float(self.dot_th), float(self.sigma), _C.ptr(ws.buf), _C.ptr(pc._overflow_flag()),
-                    _C.stream_ptr(dev))
-                _C.check(rc, "gsx_pointfusion_sequence_gt")
-            if not on_device:
-                for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
-                    t.record_stream(copy_stream)
+        ready = []
+        if not on_device:
+            copy_stream.wait_stream(main)  # the fresh buffers must exist before the copies start
+            with torch.cuda.stream(copy_stream):
+                for s0 in range(0, L, chunk):
+                    s1 = min(L, s0 + chunk)
+                    dst_d, dst_c = (raw_depth, raw_rgb) if raw else (depth, rgb)
+                    for b in range(B):  # per-element slices are contiguous: true async DMA from pinned memory
+                        dst_d[b, s0:s1].copy_(src_depth[b, s0:s1], non_blocking=True)
+                        dst_c[b, s0:s1].copy_(src_rgb[b, s0:s1], non_blocking=True)
+                    ev = torch.cuda.Event()
+                    ev.record(copy_stream)
+                    ready.append(ev)
+        for i, s0 in enumerate(range(0, L, chunk)):
+            s1 = min(L, s0 + chunk)
+            if ready:
+                main.wait_event(ready[i])
+            if raw:  # u8 / u16 -> float32 for this chunk (per element: the chunk is contiguous inside an element)
+                for b in range(B):
+                    _C.launch("gsx_ingest_raw", raw_rgb[b, s0:s1], raw_depth[b, s0:s1], (s1 - s0) * P,
+                              frames.scaling_factor, 1 if frames.normalize_color else 0, rgb[b, s0:s1], depth[b, s0:s1])
+            _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                      min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                      float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag())
+        if not on_device:
+            for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
+                t.record_stream(copy_stream)
         pc._cur = L & 1
         pc._counts_host = None
         pc._bound = pc.capacity

@@ -48,11 +48,7 @@ class _BackprojectFn(torch.autograd.Function):
             _C.require_cuda(poses, "poses")
             P = poses.detach().contiguous()
         outs = [torch.empty((B, L, H, W, 3), dtype=torch.float32, device=depth.device) if w else None for w in want]
-        with torch.cuda.device(depth.device):
-            rc = _C.lib().gsx_backproject_normals_fwd(
-                _C.ptr(d), d_bs, _C.ptr(K), 16, _C.ptr(P), L * 16, B, L, H, W,
-                _C.ptr(outs[0]), _C.ptr(outs[1]), _C.ptr(outs[2]), _C.ptr(outs[3]), _C.stream_ptr(depth.device))
-        _C.check(rc, "gsx_backproject_normals_fwd")
+        _C.launch("gsx_backproject_normals_fwd", d, d_bs, K, 16, P, L * 16, B, L, H, W, *outs)
         ctx.saved = (d, d_bs, K, P, (B, L, H, W))
         ctx.need_pose = poses is not None and poses.requires_grad
         return tuple(outs)
@@ -64,15 +60,10 @@ class _BackprojectFn(torch.autograd.Function):
         gs = [None if g is None else g.contiguous() for g in (g_v, g_n, g_gv, g_gn)]
         g_depth = torch.empty((B, L, H, W, 1), dtype=torch.float32, device=dev)
         g_poses = torch.empty((B, L, 4, 4), dtype=torch.float32, device=dev) if ctx.need_pose else None
-        lib = _C.lib()
-        nbytes = lib.gsx_backproject_normals_bwd_scratch_bytes(B, L, H, W)
+        nbytes = _C.lib().gsx_backproject_normals_bwd_scratch_bytes(B, L, H, W)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if ctx.need_pose else None
-        with torch.cuda.device(dev):
-            rc = lib.gsx_backproject_normals_bwd(
-                _C.ptr(d), d_bs, _C.ptr(K), 16, _C.ptr(P), L * 16, B, L, H, W, _C.ptr(gs[0]), _C.ptr(gs[1]),
-                _C.ptr(gs[2]), _C.ptr(gs[3]), _C.ptr(g_depth), _C.ptr(g_poses), _C.ptr(scratch),
-                nbytes if ctx.need_pose else 0, _C.stream_ptr(dev))
-        _C.check(rc, "gsx_backproject_normals_bwd")
+        _C.launch("gsx_backproject_normals_bwd", d, d_bs, K, 16, P, L * 16, B, L, H, W, *gs, g_depth, g_poses, scratch,
+                  nbytes if ctx.need_pose else 0)
         return g_depth, None, g_poses, None
 
 

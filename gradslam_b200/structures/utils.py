@@ -50,11 +50,8 @@ def _render(geo, col, counts, bound, K, poses, H, W, want_normals, want_conf):
     index = torch.empty((B, L, H, W), dtype=torch.int64, device=dev)
     depth, rgb = img(1), None if col is None else img(3)
     normals, conf = img(3) if want_normals else None, img(1) if want_conf else None
-    with torch.cuda.device(dev):
-        rc = _C.lib().gsx_render_views(
-            _C.ptr(geo), _C.ptr(col), _C.ptr(counts), cap, bound, _C.ptr(K), 16, _C.ptr(poses), L * 16, B, L, H, W,
-            _C.ptr(index), _C.ptr(depth), _C.ptr(rgb), _C.ptr(normals), _C.ptr(conf), _C.stream_ptr(dev))
-    _C.check(rc, "gsx_render_views")
+    _C.launch("gsx_render_views", geo, col, counts, cap, bound, K, 16, poses, L * 16, B, L, H, W, index, depth, rgb,
+              normals, conf)
     return depth, rgb, normals, conf, index
 
 
@@ -88,12 +85,8 @@ class _RenderFn(torch.autograd.Function):
             scratch = torch.empty(_C.lib().gsx_render_views_bwd_scratch_bytes(B, L, H, W), dtype=torch.uint8,
                                   device=dev)
         gs = [None if g is None else g.contiguous() for g in (g_depth, g_rgb, g_normals, g_conf)]
-        with torch.cuda.device(dev):
-            rc = _C.lib().gsx_render_views_bwd(
-                _C.ptr(geo.detach()), _C.ptr(counts), cap, _C.ptr(K), 16, _C.ptr(poses.detach()), L * 16,
-                _C.ptr(index), B, L, H, W, *(_C.ptr(g) for g in gs), _C.ptr(d_geo), _C.ptr(d_col), _C.ptr(d_poses),
-                _C.ptr(scratch), 0 if scratch is None else scratch.numel(), _C.stream_ptr(dev))
-        _C.check(rc, "gsx_render_views_bwd")
+        _C.launch("gsx_render_views_bwd", geo.detach(), counts, cap, K, 16, poses.detach(), L * 16, index, B, L, H, W, *gs,
+                  d_geo, d_col, d_poses, scratch, 0 if scratch is None else scratch.numel())
         return None, d_geo, d_col, d_poses
 
 

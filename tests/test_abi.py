@@ -3,19 +3,57 @@ import ctypes
 import os
 import re
 
+import pytest
+import torch
+
 from gradslam_b200 import _C
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _declared():
+def _header():
     text = open(os.path.join(ROOT, "include", "gsx.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return set(re.findall(r"\b(gsx_[a-z0-9_]+)\s*\(", text))
+    return re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+
+
+def _declared():
+    return set(re.findall(r"\b(gsx_[a-z0-9_]+)\s*\(", _header()))
 
 
 def test_header_and_binding_list_the_same_symbols():
     assert _declared() == set(_C.SIGNATURES)
+
+
+def test_binding_matches_every_prototype_parameter_by_parameter():
+    """A scalar bound with the wrong width (int for int64_t) would silently truncate a size: every prototype's return
+    type and parameter kinds must be the ones SIGNATURES declares."""
+    text = "\n".join(l for l in _header().splitlines() if not l.lstrip().startswith("#"))
+    scalar = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "float": ctypes.c_float, "double": ctypes.c_double,
+              "uint32_t": ctypes.c_uint32}
+    result = {**scalar, "void": None, "const char *": ctypes.c_char_p}
+    protos = re.findall(r"((?:const\s+)?[A-Za-z_]\w*\s*\**)\s*\b(gsx_\w+)\s*\(([^)]*)\)\s*;", text)
+    assert {name for _, name, _ in protos} == set(_C.SIGNATURES)
+    for ret, name, params in protos:
+        want_args = []
+        for p in params.split(","):
+            p = p.strip()
+            if p == "void":
+                continue
+            want_args.append(ctypes.c_void_p if "*" in p else scalar[" ".join(p.split()[:-1])])
+        res, args = _C.SIGNATURES[name]
+        assert res is result[" ".join(ret.replace("*", " *").split())], name
+        assert args == want_args, name
+
+
+@pytest.mark.parametrize("position", [0, 3])
+def test_launch_refuses_a_cpu_tensor_before_calling_the_library(position, monkeypatch):
+    calls = []
+    monkeypatch.setitem(_C._entries, (_C.lib(), "gsx_icp_solve_fwd"), lambda *a: calls.append(a) or 0)
+    args = [None, None, 1, None, None]
+    args[position] = torch.zeros(28)
+    with pytest.raises(RuntimeError, match=r"gsx_icp_solve_fwd takes CUDA tensors.*argument %d is on cpu" % position):
+        _C.launch("gsx_icp_solve_fwd", *args)
+    assert calls == []
 
 
 def test_library_exports_every_declared_symbol():

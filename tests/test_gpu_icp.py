@@ -88,6 +88,30 @@ def test_long_gradicp_run_tracks_oracle():
     assert (T.cpu() @ T_true - torch.eye(4)).abs().max().item() <= err0 + 1e-5
 
 
+@pytest.mark.parametrize("mode", [0, 1])
+def test_icp_align_takes_non_dense_clouds(mode):
+    """Clouds that are every other row of larger tensors (each copied to a dense temporary for the call) give the
+    transform and association of the dense clouds, bit for bit."""
+    from gradslam_b200.odometry import icputils
+
+    tgt, tgt_n = _cloud(5)
+    src = oracle.rigid_apply(oracle.se3_exp(torch.tensor([0.02, -0.01, 0.015, 0.03, -0.02, 0.01])), tgt)
+    g = torch.Generator().manual_seed(3)
+    dense, strided = [], []
+    for t in (src, tgt, tgt_n):
+        big = torch.randn(1, 2 * t.shape[0], 3, generator=g)  # the rows in between are noise
+        big[0, ::2] = t
+        dense.append(t[None].to(DEV))
+        strided.append(big.to(DEV)[:, ::2])
+        assert not strided[-1].is_contiguous()
+    cs, ct = icputils._counts(src.shape[0], 1, DEV), icputils._counts(tgt.shape[0], 1, DEV)
+    T, idx = icputils.icp_align(dense[0], cs, dense[1], dense[2], ct, None, mode, 10, 1e-8, None, want_idx=True)
+    T_s, idx_s = icputils.icp_align(strided[0], cs, strided[1], strided[2], ct, None, mode, 10, 1e-8, None,
+                                    want_idx=True)
+    assert torch.equal(T_s, T)
+    assert torch.equal(idx_s, idx)
+
+
 def test_providers_ragged_batch_match_oracle():
     import gradslam_b200 as gs
 
