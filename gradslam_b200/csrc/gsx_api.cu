@@ -36,7 +36,7 @@ int64_t fusion_workspace_bytes(int B, int H, int W);
 // Batch elements own independent maps, so the sequence driver splits the batch into groups that walk the frame
 // sequence on their own streams: the kernels of one group overlap those of another instead of alternating on an otherwise
 // idle GPU (none of them saturates a unit on its own: they are bound by memory latency).  Inside a group the frame
-// records of frame s+1 (K1r: instruction-bound, independent of the map) are computed on a second stream while K2 / K4 of
+// records of frame s+1 (K1r: independent of the map) are computed on a second stream while K2 / K4 of
 // frame s (latency-bound) run: the workspace has two halves used alternately, events order
 //     K1r(s) -> K2(s), K4(s)      and      K4(s) -> K1r(s+2)  (same half).
 constexpr int kMaxGroups = 4, kMaxDevices = 16;

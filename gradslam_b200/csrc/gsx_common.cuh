@@ -196,20 +196,26 @@ __device__ __forceinline__ float3 frame_normal(const float *__restrict__ dimg, c
 }
 
 // The five depth values the sample of pixel (h,w) depends on: centre, the two ends of its horizontal difference
-// (w_a, w_a+1) and of its vertical difference (h_a, h_a+1), where w_a = min(w, W-2), h_a = min(h, H-2).
+// (w_a, w_a+1) and of its vertical difference (h_a, h_a+1), where w_a = min(w, W-2), h_a = min(h, H-2).  Away from the
+// last column / row l and u are the centre itself, so only the centre, its right and its lower neighbour are loaded.
 struct DepthStencil {
   float c, l, r, u, d;
 };
-__device__ __forceinline__ DepthStencil load_stencil(const float *__restrict__ dimg, int h, int w, int H, int W) {
+// the stencil of pixel (h,w) whose own depth c is already loaded
+__device__ __forceinline__ DepthStencil load_stencil_around(const float *__restrict__ dimg, float c, int h, int w, int H,
+                                                           int W) {
   const int wa = (w < W - 1) ? w : w - 1;
   const int ha = (h < H - 1) ? h : h - 1;
   DepthStencil s;
-  s.c = __ldg(dimg + h * W + w);
-  s.l = __ldg(dimg + h * W + wa);
+  s.c = c;
   s.r = __ldg(dimg + h * W + wa + 1);
-  s.u = __ldg(dimg + ha * W + w);
   s.d = __ldg(dimg + (ha + 1) * W + w);
+  s.l = (wa == w) ? s.c : __ldg(dimg + h * W + wa);
+  s.u = (ha == h) ? s.c : __ldg(dimg + ha * W + w);
   return s;
+}
+__device__ __forceinline__ DepthStencil load_stencil(const float *__restrict__ dimg, int h, int w, int H, int W) {
+  return load_stencil_around(dimg, __ldg(dimg + h * W + w), h, w, H, W);
 }
 // frame_sample<true> evaluated from an already loaded stencil (bit-identical arithmetic)
 __device__ __forceinline__ FrameSample frame_sample_from(const DepthStencil &t, const KInv &k, const Rigid *pose, int h,

@@ -1,10 +1,11 @@
 // Fused PointFusion map update for sm_90a.
-//   k_frame_records   (K1r)    one thread per live pixel: world-frame normal and depth of the pixel as ONE 16-byte record
-//                              (the normal's op chain of rgbdimages.py:643-762, evaluated once per pixel), plus the
-//                              element's camera; also re-arms the per-frame workspace.  Consumers re-evaluate the world
-//                              vertex and the confidence weight (fusionutils.py:16-73) from the depth, bit for bit.
-//   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, ONE 16-byte gather of
-//                              the frame record under the projection, distance / normal tests, then a 128-bit atomic
+//   k_frame_records   (K1r)    one thread per live pixel: re-arms the per-frame workspace and writes the element's header
+//                              (camera, depth image).  Nothing per pixel is stored from depth: the consumers re-evaluate
+//                              the world vertex, world normal (rgbdimages.py:643-762) and confidence weight
+//                              (fusionutils.py:16-73) from the pixel's depth stencil, bit for bit.  Caller-supplied maps
+//                              (differentiable mode) are packed into per-pixel records instead.
+//   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, gather of the depth
+//                              stencil under the projection, distance / normal tests, then a 128-bit atomic
 //                              arg-min per pixel on the key (1/ccount, ray distance, row index).
 //   k_merge_append    (K4)     one thread per pixel: confidence-weighted merge of the selected map row, or stable append of
 //                              unmatched valid pixels (single-pass decoupled look-back scan, row-major order per batch
@@ -12,8 +13,6 @@
 // Map rows are sector-packed (DESIGN.md section 2): geometry rows (px,py,pz,nx,ny,nz,ccount,0) of exactly one 32-byte
 // sector, colour rows (r,g,b,0) of 16 bytes; every row access is a 128-bit load / store.
 // Reference op chains: gradslam/slam/fusionutils.py:198-722 (see include/gsx.h).
-#include <cuda.h>  // CUtensorMap (the encoder is fetched with cudaGetDriverEntryPoint: no link against libcuda)
-
 #include "gsx_common.cuh"
 #include "gsx_exp.cuh"
 #include "gsx_fusion_ws.cuh"
@@ -52,30 +51,46 @@ struct FrameRecArgs {
 
 constexpr int kRecTW = 32, kRecTH = 8;  // pixel tile of one K1r CTA
 
-// element b's FrameHeader, by one thread of the element's first K1r CTA once s_k / s_pose are loaded.  k == nullptr:
-// the records are packed from caller-supplied maps (no camera); pose == nullptr: world frame == camera frame.  Fields a
-// record kind does not use stay zero.
-__device__ __forceinline__ void store_frame_header(const FrameRecArgs &a, int b, const KInv *k, const Rigid *pose) {
+// element b's FrameHeader, by one thread of the element's first K1r CTA.  From maps there is no camera; without poses
+// world frame == camera frame.  Fields a record kind does not use stay zero.
+__device__ __forceinline__ void store_frame_header(const FrameRecArgs &a, int b) {
   FrameHeader hd = {};
-  if (k) hd.cam.k = *k;
-  if (pose) hd.cam.pose = *pose;
-  hd.cam.posed = pose != nullptr;
+  hd.from_maps = a.gv != nullptr;
+  if (!hd.from_maps) {
+    hd.cam.k = load_kinv(a.K + b * a.K_bstride);
+    if (a.poses) hd.cam.pose = load_rigid(a.poses + b * a.pose_bstride);
+    hd.cam.posed = a.poses != nullptr;
+  }
   hd.two_sigma_sq = a.two_sigma_sq;
-  hd.from_maps = k == nullptr;
+  hd.depth = a.depth + b * a.depth_bstride;
   a.ws.hdr[b] = hd;
 }
 
-// What the 16-byte frame record of pixel (h,w) with depth d leaves out: K1r's world vertex (x,y,z) and, if kAlpha, its
-// confidence weight (w) - re-evaluated with K1r's device functions and operands, so bit for bit the values K1r had.
+// Pixel (h,w)'s world normal gn and world vertex fv.xyz (and, if kAlpha, its confidence weight fv.w): the values K1
+// computes for that pixel, bit for bit.  Packed maps are gathered from nrec / vrec; from depth, the stencil is gathered
+// (its centre dc already loaded) and re-evaluated with K1r's camera and the same device functions and operands.
+// from_maps is hd.from_maps and pose is hd.cam.posed ? &hd.cam.pose : nullptr, passed separately so that a caller may
+// make them compile-time constants.
 template <bool kAlpha>
-__device__ __forceinline__ float4 record_vertex(const FrameHeader &hd, const float4 *vrec, int h, int w, int W,
-                                                float d) {
-  if (hd.from_maps) return __ldg(vrec + h * W + w);
-  const float3 v = frame_local_vertex(hd.cam, h, w, d);
-  const float3 g = frame_world_vertex(hd.cam, v, d);
+__device__ __forceinline__ void frame_values(const FrameHeader &hd, bool from_maps, const Rigid *pose,
+                                             const float4 *nrec, const float4 *vrec, int h, int w, int H, int W, float dc,
+                                             float3 &gn, float4 &fv) {
+  if (from_maps) {
+    const float4 n = __ldg(nrec + h * W + w);
+    gn = make_float3(n.x, n.y, n.z);
+    fv = __ldg(vrec + h * W + w);
+    return;
+  }
+  const FrameSample f = frame_sample_from(load_stencil_around(hd.depth, dc, h, w, H, W), hd.cam.k, pose, h, w, H, W);
+  gn = f.gn;
   // alpha from the LOCAL vertex (fusionutils.py:657, 69-72)
-  return make_float4(g.x, g.y, g.z,
-                     kAlpha ? confidence_alpha((v.x * v.x + v.y * v.y) + v.z * v.z, hd.two_sigma_sq) : 0.0f);
+  fv = make_float4(f.gv.x, f.gv.y, f.gv.z,
+                   kAlpha ? confidence_alpha((f.v.x * f.v.x + f.v.y * f.v.y) + f.v.z * f.v.z, hd.two_sigma_sq) : 0.0f);
+}
+
+// pixel (h,w)'s depth: K1r's copy in nrec for packed maps, else the caller's depth image
+__device__ __forceinline__ float frame_depth(const FrameHeader &hd, bool from_maps, const float4 *nrec, int pix) {
+  return from_maps ? __ldg(nrec + pix).w : __ldg(hd.depth + pix);
 }
 
 // element b's header into shared memory, one word per thread of threads 64..; the caller synchronises
@@ -85,154 +100,39 @@ __device__ __forceinline__ void load_frame_header(FrameHeader &s, const FrameHea
   if (i >= 0 && i < kWords) reinterpret_cast<int *>(&s)[i] = __ldg(reinterpret_cast<const int *>(g) + i);
 }
 
+// From depth, K1r only re-arms the workspace for the frame and writes the header: K2 and K4 evaluate what they need
+// from the depth image itself.  From maps it packs them into nrec / vrec.
 template <bool kFromMaps>
 __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records(FrameRecArgs a) {
-  __shared__ Rigid s_pose;
-  __shared__ KInv s_k;
   const int b = blockIdx.z;
   const int tid = threadIdx.y * kRecTW + threadIdx.x;
-  if (!kFromMaps) {
-    if (tid == 0) s_k = load_kinv(a.K + b * a.K_bstride);
-    if (tid == 32 && a.poses) s_pose = load_rigid(a.poses + b * a.pose_bstride);
-  }
   // re-arm the scan state of this element for the frame's K4
   const int lin = (blockIdx.y * gridDim.x + blockIdx.x) * (kRecTW * kRecTH) + tid;
   if (lin < a.ws.tiles) a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
-  if (lin == 0) a.ws.ticket[b] = 0u;
-  if (!kFromMaps) __syncthreads();
-  if (lin == 0) store_frame_header(a, b, kFromMaps ? nullptr : &s_k, (!kFromMaps && a.poses) ? &s_pose : nullptr);
+  if (lin == 0) {
+    a.ws.ticket[b] = 0u;
+    store_frame_header(a, b);
+  }
   const int w = blockIdx.x * kRecTW + threadIdx.x, h = blockIdx.y * kRecTH + threadIdx.y;
   if (w >= a.W || h >= a.H) return;
   const int P = a.H * a.W;
   const int pix = h * a.W + w;
   const int64_t i = (int64_t)b * P + pix;
-  const float *dimg = a.depth + b * a.depth_bstride;
   if (kFromMaps) {
     const int64_t o = i * 3;
     const float vx = __ldg(a.vloc + o), vy = __ldg(a.vloc + o + 1), vz = __ldg(a.vloc + o + 2);
-    a.ws.nrec[i] = make_float4(__ldg(a.gn + o), __ldg(a.gn + o + 1), __ldg(a.gn + o + 2), __ldg(dimg + pix));
+    a.ws.nrec[i] = make_float4(__ldg(a.gn + o), __ldg(a.gn + o + 1), __ldg(a.gn + o + 2),
+                               __ldg(a.depth + b * a.depth_bstride + pix));
     a.ws.vrec[i] = make_float4(__ldg(a.gv + o), __ldg(a.gv + o + 1), __ldg(a.gv + o + 2),
                                confidence_alpha((vx * vx + vy * vy) + vz * vz, a.two_sigma_sq));
-  } else {
-    const FrameSample f = frame_sample<true>(dimg, s_k, a.poses ? &s_pose : nullptr, h, w, a.H, a.W);
-    a.ws.nrec[i] = make_float4(f.gn.x, f.gn.y, f.gn.z, f.d);
   }
   a.ws.best[i] = U128{0ull, 0ull};
-}
-
-// The same kernel with the depth tile staged by the TMA unit: the frame is a regular grid, so the (32 + halo) x (8 + halo)
-// depth tile a CTA needs (each pixel reads its right and lower neighbour) is ONE 3-D tensor-map box {36, 9, 1} of the
-// (W, H, element) depth tensor, copied into shared memory by cp.async.bulk.tensor (SASS: UTMALDG) and signalled on an
-// mbarrier, while the CTA fetches its constants.  Elements of the box beyond the image are zero-filled by the unit; they
-// are never used (edge pixels take the difference of the previous column / row, which lies inside the box).  The arithmetic
-// is frame_sample_from(): bit-identical to frame_sample<true>() of the plain kernel.
-constexpr int kRecBoxW = kRecTW + 4, kRecBoxH = kRecTH + 1;  // box width: 36 floats = 144 bytes (a multiple of 16)
-
-__device__ __forceinline__ unsigned int smem_u32(const void *p) { return (unsigned int)__cvta_generic_to_shared(p); }
-
-__global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records_tma(const __grid_constant__ CUtensorMap tmap,
-                                                                       FrameRecArgs a) {
-  __shared__ __align__(128) float s_d[kRecBoxH][kRecBoxW];
-  __shared__ __align__(8) unsigned long long s_bar;
-  __shared__ Rigid s_pose;
-  __shared__ KInv s_k;
-  const int b = blockIdx.z;
-  const int tid = threadIdx.y * kRecTW + threadIdx.x;
-  const int w0 = blockIdx.x * kRecTW, h0 = blockIdx.y * kRecTH;
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&s_bar)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid == 0) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&s_bar)),
-                 "r"((unsigned int)(kRecBoxH * kRecBoxW * 4))
-                 : "memory");
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-            smem_u32(&s_d[0][0])),
-        "l"(&tmap), "r"(smem_u32(&s_bar)), "r"(w0), "r"(h0), "r"(b)
-        : "memory");
-  }
-  // constants and the scan state of the frame's K4 while the tile is in flight
-  if (tid == 32) s_k = load_kinv(a.K + b * a.K_bstride);
-  if (tid == 64 && a.poses) s_pose = load_rigid(a.poses + b * a.pose_bstride);
-  const int lin = (blockIdx.y * gridDim.x + blockIdx.x) * (kRecTW * kRecTH) + tid;
-  if (lin < a.ws.tiles) a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
-  if (lin == 0) a.ws.ticket[b] = 0u;
-  __syncthreads();
-  if (lin == 0) store_frame_header(a, b, &s_k, a.poses ? &s_pose : nullptr);
-  {  // wait for the tile (phase 0 of the barrier)
-    unsigned int done = 0;
-    while (!done)
-      asm volatile(
-          "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-          : "=r"(done)
-          : "r"(smem_u32(&s_bar))
-          : "memory");
-  }
-  const int w = w0 + threadIdx.x, h = h0 + threadIdx.y;
-  if (w >= a.W || h >= a.H) return;
-  const int P = a.H * a.W;
-  const int pix = h * a.W + w;
-  const int wa = (w < a.W - 1) ? w : w - 1, ha = (h < a.H - 1) ? h : h - 1;
-  DepthStencil t;
-  t.c = s_d[threadIdx.y][threadIdx.x];
-  t.l = s_d[threadIdx.y][wa - w0];
-  t.r = s_d[threadIdx.y][wa - w0 + 1];
-  t.u = s_d[ha - h0][threadIdx.x];
-  t.d = s_d[ha - h0 + 1][threadIdx.x];
-  const FrameSample f = frame_sample_from(t, s_k, a.poses ? &s_pose : nullptr, h, w, a.H, a.W);
-  a.ws.nrec[(int64_t)b * P + pix] = make_float4(f.gn.x, f.gn.y, f.gn.z, f.d);
-  a.ws.best[(int64_t)b * P + pix] = U128{0ull, 0ull};
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn tensor_map_encoder() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-    cudaGetLastError();  // (a failed query must not poison the next launch check)
-  }
-  return fn;
-}
-
-// depth (nb, H, W) with element stride depth_bstride as a 3-D tensor map; false if the layout does not qualify
-static bool depth_tensor_map(const FrameRecArgs &a, CUtensorMap *tm) {
-  if (getenv("GSX_NO_TMA")) return false;
-  const EncodeTiledFn enc = tensor_map_encoder();
-  if (!enc) return false;
-  // strides must be multiples of 16 bytes, the base 16-byte aligned; a last column / row that starts a tile of its own
-  // would need a halo on the other side
-  if (a.W % 4 || a.depth_bstride % 4 || (reinterpret_cast<uintptr_t>(a.depth) & 15)) return false;
-  if ((a.W - 1) % kRecTW == 0 || (a.H - 1) % kRecTH == 0 || a.W < 2 || a.H < 2) return false;
-  const cuuint64_t dims[3] = {(cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.B};
-  const cuuint64_t strides[2] = {(cuuint64_t)a.W * 4, (cuuint64_t)a.depth_bstride * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)kRecBoxW, (cuuint32_t)kRecBoxH, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  return enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float *>(a.depth), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 int launch_frame_records(const FrameRecArgs &a, cudaStream_t stream) {
   if (a.B == 0) return 0;
   const dim3 grid((unsigned)((a.W + kRecTW - 1) / kRecTW), (unsigned)((a.H + kRecTH - 1) / kRecTH), (unsigned)a.B);
   const dim3 block(kRecTW, kRecTH);
-  CUtensorMap tm;
-  if (!a.gv && depth_tensor_map(a, &tm)) {
-    k_frame_records_tma<<<grid, block, 0, stream>>>(tm, a);
-    GSX_CHECK_LAUNCH("gsx_fusion_frame_records(tma)");
-    return 0;
-  }
   if (a.gv)
     k_frame_records<true><<<grid, block, 0, stream>>>(a);
   else
@@ -260,8 +160,10 @@ struct ProjectArgs {
   unsigned long long *stats;
 };
 
+// 4 CTAs/SM: the loop holds the normal's re-evaluation; at 5 CTAs/SM (48 registers) it spills 24 bytes
+// (DESIGN.md section 4)
 #ifndef GSX_K2_MINB
-#define GSX_K2_MINB 5
+#define GSX_K2_MINB 4
 #endif
 
 struct MapRow {  // one geometry row
@@ -277,22 +179,16 @@ __device__ __forceinline__ MapRow load_map_row(const float *geo, int64_t n) {
 // The kernel is bound by (threads in flight) / (length of the dependent memory chain) and by instruction issue, not by
 // bytes, so the chain is kept short and the per-row work small:
 //   * the map row of the NEXT grid-stride iteration is fetched while the current row is processed (software pipelining);
-//   * the tests need ONE 16-byte gather of the frame record under the projection (K1r's normal and depth; the vertex is
-//     re-evaluated from the depth, ~20 flops): two records share a 32-byte sector, so neighbouring rows share sectors;
+//   * the tests gather the depth stencil under the projection (centre, right and lower neighbour: the frame's depth
+//     image, 1.2 MB per element, stays in L2) and re-evaluate K1's world vertex and world normal from it;
 //   * sqrtf(d2) < dist_th is decided as d2 <= d2_max (exact: the correctly rounded square root is monotonic; the
 //     threshold is found on the host, gsx_thresholds.h);
 //   * the result of the 128-bit CAS is only looked at one iteration later.
-__global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectArgs a) {
-  __shared__ LiveCamera s_cam;
-  __shared__ FrameHeader s_hdr;
-  __shared__ unsigned int s_act[kBlock / 32];
-  const int b = blockIdx.y;
-  const int count = a.counts[b];
-  if ((int64_t)blockIdx.x * kBlock >= count) return;
-  load_live_camera(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b);
-  load_frame_header(s_hdr, a.hdr + b);
-  if (threadIdx.x < kBlock / 32) s_act[threadIdx.x] = 0u;
-  __syncthreads();
+// The grid-stride loop of one CTA over element b's rows; the record kind is a template argument so that each of the two
+// loops only holds the registers of its own kind.
+template <bool kFromMaps>
+__device__ __forceinline__ void select_rows(const ProjectArgs &a, const LiveCamera &s_cam, const FrameHeader &s_hdr,
+                                            unsigned int *s_act, int b, int count) {
   const int P = a.ib.H * a.ib.W;
   const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   const float4 *nrec = a.nrec + (int64_t)b * P, *vrec = a.vrec + (int64_t)b * P;
@@ -313,10 +209,12 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
         if ((int)(threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(s_act + (threadIdx.x >> 5), (unsigned int)__popc(am));
       }
       const int pix = hit.h * a.ib.W + hit.w;
-      const float4 fn = __ldg(nrec + pix);
+      float3 gn;
+      float4 fv;
+      frame_values<false>(s_hdr, kFromMaps, s_hdr.cam.posed ? &s_hdr.cam.pose : nullptr, nrec, vrec, hit.h, hit.w,
+                          a.ib.H, a.ib.W, frame_depth(s_hdr, kFromMaps, nrec, pix), gn, fv);
       // are_normals_similar (fusionutils.py:187-195): n_frame . n_map > dot_th
-      const float dot = (fn.x * m.a.w + fn.y * m.b.x) + fn.z * m.b.y;
-      const float4 fv = record_vertex<false>(s_hdr, vrec, hit.h, hit.w, a.ib.W, fn.w);
+      const float dot = (gn.x * m.a.w + gn.y * m.b.x) + gn.z * m.b.y;
       // are_points_close (fusionutils.py:130): ||frame - map|| < dist_th
       const float dx = fv.x - m.a.x, dy = fv.y - m.a.y, dz = fv.z - m.a.z;
       const float d2 = (dx * dx + dy * dy) + dz * dz;
@@ -334,6 +232,23 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
     }
   }
   if (pend_pix >= 0) atomic_max_rec128_finish(best + pend_pix, mine, old);
+}
+
+__global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectArgs a) {
+  __shared__ LiveCamera s_cam;
+  __shared__ FrameHeader s_hdr;
+  __shared__ unsigned int s_act[kBlock / 32];
+  const int b = blockIdx.y;
+  const int count = a.counts[b];
+  if ((int64_t)blockIdx.x * kBlock >= count) return;
+  load_live_camera(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b);
+  load_frame_header(s_hdr, a.hdr + b);
+  if (threadIdx.x < kBlock / 32) s_act[threadIdx.x] = 0u;
+  __syncthreads();
+  if (s_hdr.from_maps)
+    select_rows<true>(a, s_cam, s_hdr, s_act, b, count);
+  else
+    select_rows<false>(a, s_cam, s_hdr, s_act, b, count);
   // bookkeeping for the roofline's algorithmic-byte count: ONE atomic per CTA (every warp of the grid adding to the same
   // address would serialise thousands of same-address atomics in the L2 when the whole grid works on one map)
   __syncthreads();
@@ -431,16 +346,16 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
 
   int pix[kPix];
   unsigned long long rec_lo[kPix];
-  float4 fn[kPix];
+  float dep[kPix];
   bool matched[kPix], is_new[kPix];
 #pragma unroll
   for (int j = 0; j < kPix; ++j) {
     pix[j] = pix0 + j * kMB + threadIdx.x;
     U128 rec{0ull, 0ull};
-    fn[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    dep[j] = 0.0f;
     if (pix[j] < P) {
       rec = best[pix[j]];
-      fn[j] = __ldg(nrec + pix[j]);
+      dep[j] = frame_depth(s_hdr, s_hdr.from_maps, nrec, pix[j]);
     }
     matched[j] = a.with_cc && ((rec.lo | rec.hi) != 0ull);
     rec_lo[j] = rec.lo;
@@ -458,7 +373,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   int new_off[kPix];  // position of each new pixel among the tile's new pixels (row-major)
   const int block_total = block_offsets<kMB, kPix>(
       [&](int j) {
-        is_new[j] = (pix[j] < P) && (fn[j].w > 0.0f) && !matched[j];
+        is_new[j] = (pix[j] < P) && (dep[j] > 0.0f) && !matched[j];
         return is_new[j];
       },
       new_off, s_warp_sums,
@@ -476,13 +391,15 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   float *col = a.col + (int64_t)b * a.cap * kColW;
 
-  // what the frame record leaves out, for every pixel that is merged or appended
+  // K1's world vertex, confidence weight and world normal of every pixel that is merged or appended (the tile's depth
+  // and the row below it are in L1 / L2 by now)
   float4 fv[kPix];
+  float3 fn[kPix];
 #pragma unroll
   for (int j = 0; j < kPix; ++j) {
     if (matched[j] || is_new[j]) {
       const int ph = pix[j] / a.W;
-      fv[j] = record_vertex<true>(s_hdr, vrec, ph, pix[j] - ph * a.W, a.W, fn[j].w);
+      frame_values<true>(s_hdr, s_hdr.from_maps, s_hdr.cam.posed ? &s_hdr.cam.pose : nullptr, nrec, vrec, ph, pix[j] - ph * a.W, a.H, a.W, dep[j], fn[j], fv[j]);
     }
   }
 

@@ -11,19 +11,21 @@ constexpr int kMB = 256;              // threads per CTA of the merge/append ker
 constexpr int kPix = GSX_KPIX;        // pixels per thread
 constexpr int kTilePix = kMB * kPix;  // pixels per merge tile
 
-// How K2 / K4 get a pixel's world vertex and confidence weight, per batch element (written by K1r).  From depth, the
-// frame record keeps only (normal, depth): the vertex is ~20 flops from the depth and the camera (no division, no square
-// root), the weight one exp, so re-evaluating them beats moving them through DRAM.  Caller-supplied maps (differentiable
-// mode) need not equal that re-evaluation, so their vertex and weight are stored in vrec.
+// How K2 / K4 get a pixel's world vertex, world normal and confidence weight, per batch element (written by K1r).  From
+// depth, nothing per pixel is stored: K2 and K4 gather the pixel's depth stencil from the caller's depth image and
+// re-evaluate vertex, normal and weight with K1r's camera and device functions, bit for bit.  The 1.2 MB depth image of
+// an element stays in L2 where a 4.9 MB record array did not.  Caller-supplied maps (differentiable mode) need not equal
+// that re-evaluation, so K1r packs them into nrec / vrec.
 struct FrameHeader {
   FrameCamera cam;     // K1r's K^-1 and pose
   float two_sigma_sq;  // of the confidence weight
-  int from_maps;       // 1: vertex and weight are in vrec
+  int from_maps;       // 1: normal and depth are in nrec, vertex and weight in vrec
+  const float *depth;  // the element's (H,W) depth image; it must stay unchanged until the frame's K4 has run
 };
 
-//   float4 nrec[B][P]          frame records (gnx,gny,gnz,depth)                                written by K1r
+//   float4 nrec[B][P]          (gnx,gny,gnz,depth), only for caller-supplied maps               written by K1r
 //   float4 vrec[B][P]          (gvx,gvy,gvz,alpha), only for caller-supplied maps               written by K1r
-//   FrameHeader hdr[B]         how to re-evaluate vertex / weight from depth                    written by K1r
+//   FrameHeader hdr[B]         where the depth is, how to re-evaluate vertex / normal / weight  written by K1r
 //   U128   best[B][P]          complemented arg-min records (0 = empty)                         cleared by K1r
 //   uint64 tile_state[B][T]    look-back state of K4's scan (epoch 1), T = ceil(P / kTilePix)  cleared by K1r
 //   uint32 ticket[B]           dynamic tile ids of K4                                           cleared by K1r

@@ -5,11 +5,13 @@ from Python with a CUDA event between launches, and reads the device-side counte
 algorithmic byte count of every launch comes from the run itself (SURVEY.md §8d).  The step's algorithmic bytes are
 SURVEY's fusion-step formula  16*P + 12*M + 16*A + 12*U + 40*U + 40*New;  they are attributed to the kernels as
 
-    K1r frame records                            4*P                (the depth image; its 16-byte records are an
-                                                                     internal intermediate, not algorithmic traffic)
+    K1r frame records                            0                  (re-arms the workspace; reads no frame data)
     K2  project+select                           12*M + 16*A        (map positions; normal+ccount of active)
-    K4  merge+append                             12*P + 52*U + 40*New  (rgb; read colour 12 + write 40 per merged
-                                                                        point; write 40 per new point)
+    K4  merge+append                             16*P + 52*U + 40*New  (depth and rgb; read colour 12 + write 40 per
+                                                                        merged point; write 40 per new point)
+
+K2 and K4 read the depth image: every pixel's depth once in K4, the depth stencils under the projections in K2 (an
+intermediate re-read, not algorithmic traffic).
 """
 import torch
 
@@ -59,10 +61,10 @@ def profile_pointfusion_gt(depth, rgb, K, poses, dist_th, dot_th, sigma):
         New = sum(counts) - M
         A = cur_stats[0] - prev_stats[0]
         U = cur_stats[1] - prev_stats[1]
-        out["K1r_frame_records"].append((ev[0].elapsed_time(ev[1]), 4 * B * P))
+        out["K1r_frame_records"].append((ev[0].elapsed_time(ev[1]), 0))
         if s > 0:
             out["K2_project_select"].append((ev[1].elapsed_time(ev[2]), 12 * M + 16 * A))
-        out["K4_merge_append"].append((ev[2].elapsed_time(ev[3]), 12 * B * P + 52 * U + 40 * New))
+        out["K4_merge_append"].append((ev[2].elapsed_time(ev[3]), 16 * B * P + 52 * U + 40 * New))
         frames.append({"frame": s, "map_points": M, "active": A, "merged": U, "new": New})
         prev_counts, prev_stats = counts, cur_stats
     return out, frames

@@ -145,6 +145,9 @@ def _launch_frame_records(ws, frames, sigma, device, maps=None, world=True):
         K = _dense(frames.intrinsics, "intrinsics", device)
         poses = _dense(frames.poses, "poses", device) if (world and frames.poses is not None) else None
     _C.launch("gsx_fusion_frame_records", depth, d_bs, K, 16, poses, 16, gv, gn, vl, B, H, W, sigma, ws.buf)
+    # K2 and K4 read this depth (it may be a dense copy made just above): keep it alive until the next frame's records
+    # replace it, which is after this frame's merge in stream order
+    ws.depth = depth
 
 
 def _dense_frame(t, name, device):

@@ -68,9 +68,9 @@ int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const
 
 /* ------------------------------------------------------------------------------------------------
  * Fused PointFusion map update, one live frame for all B elements: three kernels
- *   K1r  gsx_fusion_frame_records    per pixel: world normal, depth -> one 16-byte record (the world vertex and
- *                                    confidence weight are re-evaluated from the depth where they are needed);
- *                                    re-arms the workspace for this frame
+ *   K1r  gsx_fusion_frame_records    re-arms the workspace for this frame and records where its depth image and camera
+ *                                    are (from depth nothing per pixel is stored: K2 and K4 re-evaluate the world
+ *                                    vertex, world normal and confidence weight from the depth where they need them)
  *   K2   gsx_fusion_project_select   per map row: projection, tests, per-pixel 128-bit arg-min
  *   K4   gsx_fusion_merge_append     per pixel: merge the selected row or append a new surfel
  * replaces update_map_fusion = find_active_map_points + find_similar_map_points +
@@ -93,7 +93,10 @@ int64_t gsx_fusion_workspace_stats_offset(int B, int H, int W);
  * Either evaluate everything from the depth image (gvertex = gnormal = vertex = NULL; intrinsics required; poses =
  * camera-to-world, or NULL for "world frame == camera frame"), or pack already materialised maps: gvertex / gnormal /
  * vertex (B,H,W,3) (outputs of gsx_backproject_normals_fwd, used by the differentiable mode; intrinsics / poses are
- * then ignored).  Same arithmetic either way, bit for bit. */
+ * then ignored).  Same arithmetic either way, bit for bit.
+ * Lifetime: the workspace keeps a pointer to `depth`, and gsx_fusion_project_select / gsx_fusion_merge_append of this
+ * frame read it.  `depth` must stay valid and unchanged until this frame's gsx_fusion_merge_append has run (in stream
+ * order: do not free, reuse or overwrite it before that launch). */
 int gsx_fusion_frame_records(const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
                              const float *poses, int64_t pose_bstride, const float *gvertex, const float *gnormal,
                              const float *vertex, int B, int H, int W, double sigma, void *workspace, void *stream);
@@ -102,7 +105,7 @@ int gsx_fusion_frame_records(const float *depth, int64_t depth_bstride, const fl
  * the frame vertex they land on and with a similar normal, and reduce per pixel to the best candidate
  * (largest confidence count, then smallest ray distance, then smallest index) with a 128-bit atomic
  * min.  max_count = host upper bound on counts[b] (sizes the grid).  The frame records of the live frame must be in
- * the workspace (gsx_fusion_frame_records). */
+ * the workspace (gsx_fusion_frame_records), and the depth it was given still valid. */
 int gsx_fusion_project_select(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                               const float *poses, int64_t pose_bstride, const float *intrinsics, int64_t K_bstride,
                               int B, int H, int W, float dist_th, float dot_th, void *workspace, void *stream);
