@@ -94,6 +94,13 @@ SIGNATURES = {
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int,
                 c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64,
                 c_vp, c_i64, c_u32, c_vp, c_vp]),
+    "gsx_icp_projective_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
+    "gsx_icp_localize_projective": (
+        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
+                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_vp]),
+    "gsx_icp_project_associate": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp,
+                c_vp]),
     "gsx_render_views": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                 c_vp, c_vp, c_vp]),

@@ -16,6 +16,13 @@
 //                        (solve_linear_system, icputils.py:22-90), se3_exp (geometry/se3utils.py:77-115)
 //   k_icp_update         one warp per element: look-ahead error, LM accept/reject (icputils.py:356-365) or gradLM
 //                        smooth gates (icputils.py:527-543), pose accumulation
+// Projective association (an extension, no reference counterpart; gsx_icp_localize_projective):
+//   render_icp_targets   (gsx_render.cu) the map seen from the previous pose through R1's z-buffer: index image and the
+//                        winning rows' world-frame points / normals at full resolution
+//   k_icp_proj_linearize a source point is associated with the pixel it projects to in the previous camera (the fusion
+//                        step's project()) if a row covers that pixel; the same rows, reduction and partials layout as
+//                        k_icp_knn_linearize, so k_icp_solve / k_icp_update run unchanged
+//   k_icp_project_associate  the association alone (index-only op of the differentiable mode)
 #include "gsx_common.cuh"
 #include "../../include/gsx.h"
 
@@ -531,6 +538,94 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_knn_linearize(KnnArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// projective association + point-to-plane linearisation + block reduction
+// ---------------------------------------------------------------------------------------------------------
+struct ProjTargets {  // the target images rendered from the previous pose, and that camera
+  const float *poses;  // camera-to-world of the previous frame, element stride pose_bstride
+  int64_t pose_bstride;
+  const float *K;
+  int64_t K_bstride;
+  ImageBounds ib;
+  const int64_t *idx;          // (B, H*W) map row covering the pixel, or -1
+  const float *tgt_p, *tgt_n;  // (B, H*W, 3) world-frame point / normal of that row, zeros where uncovered
+  float dist_thresh;           // compared with the SQUARED distance, as on the 1-NN path (icputils.py:206)
+  int use_thresh;
+};
+
+// Pixel j of element b's target images that the world-frame source point s is associated with, or -1: s lies in the
+// frustum of the previous camera (project(): canonical arithmetic, round half to even, clamp), a row covers pixel j, and
+// with use_thresh the squared distance d2 = |s - tgt_p[j]|^2 is below dist_thresh.  d2 is +inf unless a row covers the
+// pixel s projects to.  `cam` is element b's camera; idx / tp point at element b's images.
+__device__ __forceinline__ int project_associate(const LiveCamera &cam, const ProjTargets &t, const int64_t *idx,
+                                                 const float *tp, float sx, float sy, float sz, float &d2) {
+  d2 = __int_as_float(0x7f800000);
+  const PixelHit hit = project(cam, t.ib, sx, sy, sz);
+  if (!hit.in_frustum) return -1;
+  const int j = hit.h * t.ib.W + hit.w;
+  if (__ldg(idx + j) < 0) return -1;
+  const float dx = sx - __ldg(tp + (int64_t)j * 3), dy = sy - __ldg(tp + (int64_t)j * 3 + 1),
+              dz = sz - __ldg(tp + (int64_t)j * 3 + 2);
+  d2 = (dx * dx + dy * dy) + dz * dz;
+  return (t.use_thresh && !(d2 < t.dist_thresh)) ? -1 : j;
+}
+
+struct ProjLinArgs {
+  float *src;  // (B, ns_stride, 3); read, transformed by `pre` on load, optionally written back
+  const int32_t *src_count;
+  int ns_stride;
+  const float *pre;  // (B,16)
+  int write_back;
+  ProjTargets t;
+  float *partials;  // (B, gridDim.x, 28)
+};
+
+__global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a) {
+  __shared__ float s_red[kIcpBlock / 32][kNumSums];
+  __shared__ Rigid s_pre;
+  __shared__ LiveCamera s_cam;
+  const int b = blockIdx.y;
+  if (threadIdx.x == 64) s_pre = load_rigid(a.pre + b * 16);
+  load_live_camera(s_cam, a.t.poses, a.t.pose_bstride, a.t.K, a.t.K_bstride, b);
+  __syncthreads();
+  const int64_t P = (int64_t)a.t.ib.H * a.t.ib.W;
+  const int i = blockIdx.x * kIcpBlock + threadIdx.x;
+  float acc[kNumSums];
+#pragma unroll
+  for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0f;
+  if (i < a.src_count[b]) {
+    float *src = a.src + ((int64_t)b * a.ns_stride + i) * 3;
+    const float3 q = rigid_apply(s_pre, src[0], src[1], src[2]);
+    if (a.write_back) {
+      src[0] = q.x;
+      src[1] = q.y;
+      src[2] = q.z;
+    }
+    const float *tp = a.t.tgt_p + b * P * 3;
+    float d2;
+    const int j = project_associate(s_cam, a.t, a.t.idx + b * P, tp, q.x, q.y, q.z, d2);
+    if (j >= 0) row_products(q.x, q.y, q.z, tp, a.t.tgt_n + b * P * 3, (int64_t)j, acc);
+  }
+  block_reduce_sums(acc, s_red, a.partials + ((int64_t)b * gridDim.x + blockIdx.x) * kNumSums);
+}
+
+__global__ void __launch_bounds__(kIcpBlock) k_icp_project_associate(const float *src, const int32_t *src_count,
+                                                                    int ns_stride, ProjTargets t, int64_t *idx_out,
+                                                                    float *d2_out) {
+  __shared__ LiveCamera s_cam;
+  const int b = blockIdx.y;
+  load_live_camera(s_cam, t.poses, t.pose_bstride, t.K, t.K_bstride, b);
+  __syncthreads();
+  const int i = blockIdx.x * kIcpBlock + threadIdx.x;
+  if (i >= src_count[b]) return;
+  const int64_t P = (int64_t)t.ib.H * t.ib.W;
+  const float *s = src + ((int64_t)b * ns_stride + i) * 3;
+  float d2;
+  const int j = project_associate(s_cam, t, t.idx + b * P, t.tgt_p + b * P * 3, s[0], s[1], s[2], d2);
+  idx_out[(int64_t)b * ns_stride + i] = j;
+  if (d2_out) d2_out[(int64_t)b * ns_stride + i] = d2;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // normal equations for a GIVEN association (the differentiable op of the taped ICP): forward + backward
 // ---------------------------------------------------------------------------------------------------------
 // (batched: element b = blockIdx.y lives at b * ns_stride / b * nt_stride rows; counts may be null = ns_stride rows each)
@@ -929,12 +1024,14 @@ void build_search_grid(const float *tgt_p, const int32_t *tgt_count, int nt_stri
   k_grid_scatter<<<dim3(nb, (unsigned)B), 256, 0, stream>>>(tgt_p, tgt_count, nt_stride, g);
 }
 
-// runs the LM / gradLM loop on clouds that are already in place; the target's search grid, if `tgt_grid` is laid out,
-// is built once here (the target does not move during the loop)
-int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const float *tgt_p, const float *tgt_n,
-                 const int32_t *tgt_count, int nt_stride, int B, const float *T0, int mode, int numiters, float damp,
-                 int use_thresh, float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *partials,
-                 int nblk_cap, IcpState st, int64_t *nn_idx, const TargetGrid &tgt_grid, cudaStream_t stream) {
+// The LM / gradLM loop over an association `lin`: lin.prepare(stream) once after the state is initialised, then per
+// iteration lin(pre, write_back, last, grid, stream) launches the linearisation that writes the block partials of the
+// 28 sums, the source transformed by `pre` on load (and written back with write_back).  Both associations share this
+// order of launches: linearise at T_pend, solve, linearise the look-ahead at dT, update.
+template <class Linearize>
+int icp_iterations(Linearize &lin, int ns_stride, int B, const float *T0, int mode, int numiters, float damp,
+                   float lambda_max, float Bp, float B2p, float nu, float *partials, int nblk_cap, IcpState st,
+                   cudaStream_t stream) {
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   if (nblk > nblk_cap) {
     set_error("icp: source cloud larger than workspace");
@@ -942,28 +1039,87 @@ int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const floa
   }
   k_icp_init<<<(B + 63) / 64, 64, 0, stream>>>(st, T0, damp, B);
   UpdateArgs u{mode, 1.0f / lambda_max, lambda_max, Bp, B2p, 1.0f / nu};
-  KnnArgs ka{src, src_count, ns_stride, tgt_p, tgt_n, tgt_count, nt_stride, nullptr, 0, dist_thresh, use_thresh,
-             partials, nullptr, nullptr, tgt_grid};
-  const bool use_grid = tgt_grid.params != nullptr;
-  if (use_grid) build_search_grid(tgt_p, tgt_count, nt_stride, B, tgt_grid, stream);
+  lin.prepare(stream);
   const dim3 grid((unsigned)nblk, (unsigned)B);
   for (int it = 0; it < numiters; ++it) {
-    ka.pre = st.T_pend;
-    ka.write_back = 1;
-    ka.nn_idx = (it == numiters - 1) ? nn_idx : nullptr;
-    if (use_grid) k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, stream>>>(ka);
-    else k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, stream>>>(ka);
+    lin(st.T_pend, 1, it == numiters - 1, grid, stream);
     k_icp_solve<<<B, 32, 0, stream>>>(partials, nblk, st);
-    ka.pre = st.dT;
-    ka.write_back = 0;
-    ka.nn_idx = nullptr;
-    if (use_grid) k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, stream>>>(ka);
-    else k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, stream>>>(ka);
+    lin(st.dT, 0, false, grid, stream);
     k_icp_update<<<B, 32, 0, stream>>>(partials, nblk, st, u);
   }
   GSX_CHECK_LAUNCH("gsx_icp");
   return 0;
 }
+
+// exact 1-NN association; the target's search grid, if laid out, is built once (the target does not move in the loop)
+struct KnnLinearize {
+  KnnArgs ka;
+  int64_t *nn_idx;  // written by the last iteration's first association (may be null)
+  int B;
+  void prepare(cudaStream_t s) {
+    if (ka.grid.params) build_search_grid(ka.tgt_p, ka.tgt_count, ka.nt_stride, B, ka.grid, s);
+  }
+  void operator()(const float *pre, int write_back, bool last, dim3 grid, cudaStream_t s) {
+    ka.pre = pre;
+    ka.write_back = write_back;
+    ka.nn_idx = last ? nn_idx : nullptr;
+    if (ka.grid.params) k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, s>>>(ka);
+    else k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, s>>>(ka);
+  }
+};
+
+// projective association against target images rendered from the previous pose
+struct ProjLinearize {
+  ProjLinArgs pa;
+  void prepare(cudaStream_t) {}
+  void operator()(const float *pre, int write_back, bool, dim3 grid, cudaStream_t s) {
+    pa.pre = pre;
+    pa.write_back = write_back;
+    k_icp_proj_linearize<<<grid, kIcpBlock, 0, s>>>(pa);
+  }
+};
+
+// runs the LM / gradLM loop with the exact 1-NN association on clouds that are already in place
+int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const float *tgt_p, const float *tgt_n,
+                 const int32_t *tgt_count, int nt_stride, int B, const float *T0, int mode, int numiters, float damp,
+                 int use_thresh, float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *partials,
+                 int nblk_cap, IcpState st, int64_t *nn_idx, const TargetGrid &tgt_grid, cudaStream_t stream) {
+  KnnLinearize lin{KnnArgs{src, src_count, ns_stride, tgt_p, tgt_n, tgt_count, nt_stride, nullptr, 0, dist_thresh,
+                           use_thresh, partials, nullptr, nullptr, tgt_grid},
+                   nn_idx, B};
+  return icp_iterations(lin, ns_stride, B, T0, mode, numiters, damp, lambda_max, Bp, B2p, nu, partials, nblk_cap, st,
+                        stream);
+}
+
+struct ProjectiveWorkspace {  // of gsx_icp_localize_projective; nothing in it outlives a call
+  float *src;  // (B, ns_cap, 3)
+  int32_t *src_count;
+  float *partials;  // (B, nblk, 28)
+  IcpState st;
+  int64_t *index;        // (B, H*W) z-buffer, then the index image
+  float *tgt_p, *tgt_n;  // (B, H*W, 3)
+  int ns_cap, nblk;
+};
+
+inline ProjectiveWorkspace projective_workspace_layout(Carver &c, int B, int H, int W, int ds) {
+  ProjectiveWorkspace w;
+  const int64_t P = (int64_t)H * W;
+  w.ns_cap = ((H + ds - 1) / ds) * ((W + ds - 1) / ds);
+  w.nblk = (w.ns_cap + kIcpBlock - 1) / kIcpBlock;
+  w.src = c.take<float>((int64_t)B * w.ns_cap * 3);
+  w.src_count = c.take<int32_t>(B);
+  w.partials = partials_layout(c, B, w.ns_cap);
+  w.st = icp_state_layout(c, B);
+  w.index = c.take<int64_t>((int64_t)B * P);
+  w.tgt_p = c.take<float>((int64_t)B * P * 3);
+  w.tgt_n = c.take<float>((int64_t)B * P * 3);
+  return w;
+}
+
+// defined in gsx_render.cu
+int render_icp_targets(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                       const float *intrinsics, int64_t K_bstride, const float *poses, int64_t pose_bstride, int B,
+                       int H, int W, int64_t *index, float *tgt_p, float *tgt_n, cudaStream_t s);
 
 }  // namespace gsx
 
@@ -1160,5 +1316,66 @@ extern "C" int gsx_icp_normal_eq_bwd(const float *src_points, int ns, const floa
                                                                     nn_idx, g_sums, g_src, g_tgt_points_rows,
                                                                     g_tgt_normals_rows);
   GSX_CHECK_LAUNCH("gsx_icp_normal_eq_bwd");
+  return 0;
+}
+
+extern "C" int64_t gsx_icp_projective_workspace_bytes(int B, int H, int W, int ds) {
+  if (B < 1 || H < 1 || W < 1 || ds < 1) return -1;
+  Carver c(nullptr);
+  projective_workspace_layout(c, B, H, W, ds);
+  return c.bytes;
+}
+
+extern "C" int gsx_icp_localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                           int64_t max_count, const float *depth, int64_t depth_bstride,
+                                           const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                           int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
+                                           int numiters, float damp, int use_dist_thresh, float dist_thresh,
+                                           float lambda_max, float Bp, float B2p, float nu, float *poses_out,
+                                           int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
+                                           void *stream) {
+  GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace,
+                "gsx_icp_localize_projective: null pointer");
+  GSX_CHECK_ARG(B >= 1 && H >= 2 && W >= 2 && ds >= 1 && numiters >= 0, "gsx_icp_localize_projective: bad extents");
+  GSX_CHECK_ARG(mode == 0 || mode == 1, "gsx_icp_localize_projective: mode must be 0 (ICP) or 1 (gradICP)");
+  Carver c(workspace);
+  const ProjectiveWorkspace w = projective_workspace_layout(c, B, H, W, ds);
+  GSX_CHECK_ARG(workspace_bytes >= c.bytes, "gsx_icp_localize_projective: workspace too small (%lld < %lld)",
+                (long long)workspace_bytes, (long long)c.bytes);
+  cudaStream_t s = (cudaStream_t)stream;
+  GatherSrcArgs gs{depth, depth_bstride, intrinsics, K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds,
+                   w.src, w.src_count, w.ns_cap};
+  k_icp_gather_src<<<B, 1024, 0, s>>>(gs);
+  if (render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
+                         prev_pose_bstride, B, H, W, w.index, w.tgt_p, w.tgt_n, s))
+    return 1;
+  ProjLinearize lin{ProjLinArgs{w.src, w.src_count, w.ns_cap, nullptr, 0,
+                                ProjTargets{prev_poses, prev_pose_bstride, intrinsics, K_bstride, image_bounds(H, W),
+                                            w.index, w.tgt_p, w.tgt_n, dist_thresh, use_dist_thresh},
+                                w.partials}};
+  const int rc = icp_iterations(lin, w.ns_cap, B, nullptr, mode, numiters, damp, lambda_max, Bp, B2p, nu, w.partials,
+                                w.nblk, w.st, s);
+  if (rc) return rc;
+  k_pose_compose<<<(B + 63) / 64, 64, 0, s>>>(w.st.T_total, prev_poses, prev_pose_bstride, poses_out,
+                                              poses_out_bstride, B);
+  GSX_CHECK_LAUNCH("gsx_icp_localize_projective");
+  return 0;
+}
+
+extern "C" int gsx_icp_project_associate(const float *src_points, const int32_t *src_count, int ns_stride,
+                                         const float *tgt_points, const int64_t *tgt_index, const float *prev_poses,
+                                         int64_t pose_bstride, const float *intrinsics, int64_t K_bstride, int B, int H,
+                                         int W, int use_dist_thresh, float dist_thresh, int64_t *idx_out,
+                                         float *d2_out, void *stream) {
+  GSX_CHECK_ARG(src_points && src_count && tgt_points && tgt_index && prev_poses && intrinsics && idx_out,
+                "gsx_icp_project_associate: null pointer");
+  GSX_CHECK_ARG(B >= 1 && B <= 65535 && ns_stride >= 1 && H >= 1 && W >= 1 && (int64_t)H * W <= INT32_MAX,
+                "gsx_icp_project_associate: bad extents");
+  const ProjTargets t{prev_poses, pose_bstride, intrinsics, K_bstride, image_bounds(H, W), tgt_index, tgt_points,
+                      nullptr, dist_thresh, use_dist_thresh};
+  const dim3 grid((unsigned)((ns_stride + kIcpBlock - 1) / kIcpBlock), (unsigned)B);
+  k_icp_project_associate<<<grid, kIcpBlock, 0, (cudaStream_t)stream>>>(src_points, src_count, ns_stride, t, idx_out,
+                                                                        d2_out);
+  GSX_CHECK_LAUNCH("gsx_icp_project_associate");
   return 0;
 }

@@ -7,6 +7,9 @@
 //                              into the pixel's slot of the int64 index image, which the entry point filled with ones.
 //   k_render_resolve     (R2)  per pixel: key -> n or -1 in place; depth from the key, gathers of the winning row only for
 //                              the outputs requested.
+//   k_render_resolve_world (R2w) per pixel of one view per element: key -> n or -1 in place, the winning row's
+//                              world-frame point and normal (two 128-bit row loads), zeros where uncovered: the target
+//                              images of the projective ICP (gsx_icp.cu, render_icp_targets).
 //   k_render_bwd_rows    (R3)  per map row: re-projects the row into every view; where it won the pixel, accumulates the
 //                              pixel's upstream gradients in view order (a row wins at most one pixel per view: no atomics).
 //   k_render_bwd_pose    (R3)  per pixel tile: d/d(camera-to-world pose) of depth and normals, reduced per tile, then
@@ -110,6 +113,26 @@ __global__ void __launch_bounds__(kRB) k_render_resolve(RenderArgs a) {
     if (covered) c = __ldg(reinterpret_cast<const float4 *>(a.col + ((int64_t)b * a.cap + n) * kColW));
     st3(a.rgb + i * 3, c.x, c.y, c.z);
   }
+}
+
+__global__ void __launch_bounds__(kRB) k_render_resolve_world(unsigned long long *key, const float *geo, int64_t cap,
+                                                           int64_t P, float *tgt_p, float *tgt_n) {
+  const int b = blockIdx.y;
+  const int64_t pix = (int64_t)blockIdx.x * kRB + threadIdx.x;
+  if (pix >= P) return;
+  const int64_t i = b * P + pix;
+  const unsigned long long k = key[i];
+  const bool covered = k != kEmptyKey;
+  const int64_t n = covered ? (int64_t)(k & 0xffffffffull) : -1;
+  reinterpret_cast<int64_t *>(key)[i] = n;
+  float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
+  if (covered) {
+    const float *row = geo + ((int64_t)b * cap + n) * kGeoW;
+    g0 = __ldg(reinterpret_cast<const float4 *>(row));
+    g1 = __ldg(reinterpret_cast<const float4 *>(row + 4));
+  }
+  st3(tgt_p + i * 3, g0.x, g0.y, g0.z);
+  st3(tgt_n + i * 3, g0.w, g1.x, g1.y);
 }
 
 // ---- backward -----------------------------------------------------------------------------------------------
@@ -250,6 +273,19 @@ static int check_render_extents(const char *fn, int B, int L, int H, int W, int6
 
 static inline unsigned pixel_tiles(int H, int W) { return (unsigned)(((int64_t)H * W + kRB - 1) / kRB); }
 
+// Fills the index image with empty keys, then runs R1 over the rows of every element (max_count = host bound on the
+// element sizes; no row pass when it is 0).
+static void launch_zbuffer(const RenderArgs &a, int B, int64_t max_count, cudaStream_t s) {
+  cudaMemsetAsync(a.key, 0xFF, (size_t)B * a.L * a.ib.H * a.ib.W * sizeof(int64_t), s);
+  if (max_count > 0) {
+    const unsigned chunks = (unsigned)((a.L + kViews - 1) / kViews);
+    int64_t bx = (max_count + kRB - 1) / kRB;
+    const int64_t cap_blocks = (int64_t)kNumSMs * kRenderCtasPerSM;  // grid-stride beyond
+    if (bx * B * chunks > cap_blocks) bx = (cap_blocks + B * chunks - 1) / (B * chunks);
+    k_render_zbuffer<<<dim3((unsigned)bx, (unsigned)B, chunks), kRB, 0, s>>>(a);
+  }
+}
+
 extern "C" int gsx_render_views(const float *map_geometry, const float *map_colors, const int32_t *counts,
                                 int64_t capacity, int64_t max_count, const float *intrinsics, int64_t K_bstride,
                                 const float *poses, int64_t pose_bstride, int B, int L, int H, int W, int64_t *index,
@@ -265,18 +301,32 @@ extern "C" int gsx_render_views(const float *map_geometry, const float *map_colo
   cudaStream_t s = (cudaStream_t)stream;
   RenderArgs a{map_geometry, map_colors, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, L,
                image_bounds(H, W), reinterpret_cast<unsigned long long *>(index), depth, rgb, normals, confidence};
-  cudaMemsetAsync(index, 0xFF, (size_t)B * L * H * W * sizeof(int64_t), s);
-  if (max_count > 0) {
-    const unsigned chunks = (unsigned)((L + kViews - 1) / kViews);
-    int64_t bx = (max_count + kRB - 1) / kRB;
-    const int64_t cap_blocks = (int64_t)kNumSMs * kRenderCtasPerSM;  // grid-stride beyond
-    if (bx * B * chunks > cap_blocks) bx = (cap_blocks + B * chunks - 1) / (B * chunks);
-    k_render_zbuffer<<<dim3((unsigned)bx, (unsigned)B, chunks), kRB, 0, s>>>(a);
-  }
+  launch_zbuffer(a, B, max_count, s);
   k_render_resolve<<<dim3(pixel_tiles(H, W), (unsigned)(B * L)), kRB, 0, s>>>(a);
   GSX_CHECK_LAUNCH("gsx_render_views");
   return 0;
 }
+
+namespace gsx {
+// Target images of the projective ICP (declared in gsx_icp.cu): one view per element from `poses`, resolved to the
+// index image (B, H*W) and the winning rows' world-frame points and normals (B, H*W, 3).  Same checks as
+// gsx_render_views; returns non-zero (error set) if they fail.
+int render_icp_targets(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                       const float *intrinsics, int64_t K_bstride, const float *poses, int64_t pose_bstride, int B,
+                       int H, int W, int64_t *index, float *tgt_p, float *tgt_n, cudaStream_t s) {
+  if (check_render_extents("render_icp_targets", B, 1, H, W, capacity)) return 1;
+  GSX_CHECK_ARG(max_count >= 0 && max_count <= capacity, "render_icp_targets: max_count %lld outside [0, capacity %lld]",
+                (long long)max_count, (long long)capacity);
+  GSX_CHECK_ARG(aligned16(map_geometry), "render_icp_targets: map rows must be 16-byte aligned");
+  RenderArgs a{map_geometry, nullptr, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, 1,
+               image_bounds(H, W), reinterpret_cast<unsigned long long *>(index), nullptr, nullptr, nullptr, nullptr};
+  launch_zbuffer(a, B, max_count, s);
+  k_render_resolve_world<<<dim3(pixel_tiles(H, W), (unsigned)B), kRB, 0, s>>>(a.key, map_geometry, capacity,
+                                                                             (int64_t)H * W, tgt_p, tgt_n);
+  GSX_CHECK_LAUNCH("render_icp_targets");
+  return 0;
+}
+}  // namespace gsx
 
 extern "C" int64_t gsx_render_views_bwd_scratch_bytes(int B, int L, int H, int W) {
   if (B < 1 || L < 1 || H < 1 || W < 1) return -1;

@@ -372,18 +372,23 @@ class _RigidTransformBatchedFn(torch.autograd.Function):
         return g_p, g_T, None
 
 
-def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, target_cache=None):
-    d2, idx = knn1(src.detach(), tgt.detach(), src_counts, tgt_counts, target_cache)
-    if dist_thresh is not None:
-        idx = torch.where(d2 < dist_thresh, idx, torch.full_like(idx, -1))
+def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, target_cache=None, associate=None):
+    if associate is None:
+        d2, idx = knn1(src.detach(), tgt.detach(), src_counts, tgt_counts, target_cache)
+        if dist_thresh is not None:
+            idx = torch.where(d2 < dist_thresh, idx, torch.full_like(idx, -1))
+    else:
+        idx = associate(src.detach())
     return _NormalEqBatchedFn.apply(src, tgt, tgt_n, idx, src_counts), idx
 
 
 def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numiters, damp, dist_thresh, lambda_max=2.0,
-                       B=1.0, B2=1.0, nu=200.0):
+                       B=1.0, B2=1.0, nu=200.0, associate=None):
     """The differentiable ICP / gradICP loop of `_taped_icp` for a padded batch: src (Bn,Ns,3), tgt / tgt_n (Bn,Nt,3),
     int32 sizes (Bn,).  One chain of batched ops for all elements; returns (T (Bn,4,4), last nn idx (Bn,Ns), -1 = none).
-    Per element the values are bit-identical to the per-element chain and to the fused no-grad loop."""
+    Per element the values are bit-identical to the per-element chain and to the fused no-grad loop.
+    associate: None = exact 1-NN in tgt (thresholded by dist_thresh); otherwise a function of the current source
+    (Bn,Ns,3), detached, returning the int64 target row per source row (-1 = none) - the projective association."""
     dev = src.device
     Bn, Ns = src.shape[0], src.shape[1]
     # No valid source (or target) point in any element gives a padded width of 0, which the kernels reject.  One zero
@@ -398,10 +403,11 @@ def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numite
     idx = None
     grid = {}  # the target's search grid: built by the first of the 2 * numiters associations
     for _ in range(numiters):
-        sums, idx = _normal_equations_batched(cur, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid)
+        sums, idx = _normal_equations_batched(cur, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid, associate)
         xi, dT = _SolveBatchedFn.apply(sums, dampt)
         one_step = _RigidTransformBatchedFn.apply(cur, dT, src_counts)
-        sums_next, _ = _normal_equations_batched(one_step, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid)
+        sums_next, _ = _normal_equations_batched(one_step, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid,
+                                                 associate)
         dampt, dT_applied, T = _UpdateBatchedFn.apply(xi, sums[:, 27], sums_next[:, 27], dampt, T, mode, lambda_max, B,
                                                       B2, nu)
         cur = _RigidTransformBatchedFn.apply(cur, dT_applied, src_counts)
@@ -622,3 +628,99 @@ def localize_against_map(pointclouds, live_frame, prev_frame, dsratio, odomprov)
               float(getattr(odomprov, "B2", 1.0)), float(getattr(odomprov, "nu", 200.0)), tgt, bound, out, 16, ws.buf,
               ws.capacity, ws.next_epoch(), pointclouds._overflow_flag())
     return out
+
+
+# ------------------------------------------------------------------------------------ projective association
+def project_associate(src, src_counts, tgt_points, tgt_index, prev_poses, K, H, W, dist_thresh=None):
+    """Projective association of a padded source batch src (B,Ns,3) (world frame, int32 sizes (B,)) with target images
+    rendered from prev_poses (B,4,4) with intrinsics K (B,4,4): tgt_points (B,H*W,3), tgt_index (B,H*W) int64 (-1 =
+    uncovered).  Returns (squared distances (B,Ns), pixel index int64 (B,Ns), -1 = none); rows beyond a source size get
+    -1 / inf.  CUDA kernel k_icp_project_associate, the association of gsx_icp_localize_projective."""
+    _C.require_cuda(src, "src")
+    src = src.contiguous()
+    Bn, Ns, _ = src.shape
+    idx = torch.full((Bn, Ns), -1, dtype=torch.int64, device=src.device)
+    d2 = torch.full((Bn, Ns), float("inf"), dtype=torch.float32, device=src.device)
+    _C.launch("gsx_icp_project_associate", src, src_counts, Ns, tgt_points.contiguous(), tgt_index.contiguous(),
+              prev_poses.contiguous(), 16, K.contiguous(), 16, Bn, int(H), int(W), 0 if dist_thresh is None else 1,
+              0.0 if dist_thresh is None else float(dist_thresh), idx, d2)
+    return d2, idx
+
+
+class _ProjectiveWorkspace:
+    """Workspace of gsx_icp_localize_projective per (device, B, H, W, ds): nothing in it outlives a call, so one
+    buffer serves every stream-ordered call with that shape."""
+    _cache = {}
+
+    @classmethod
+    def get(cls, device, B, H, W, ds):
+        key = (str(device), B, H, W, ds)
+        buf = cls._cache.get(key)
+        if buf is None:
+            buf = torch.empty(_C.lib().gsx_icp_projective_workspace_bytes(B, H, W, ds), dtype=torch.uint8, device=device)
+            cls._cache[key] = buf
+        return buf
+
+
+def _solver_params(odomprov):
+    return (1 if hasattr(odomprov, "lambda_max") else 0, float(getattr(odomprov, "lambda_max", 2.0)),
+            float(getattr(odomprov, "B", 1.0)), float(getattr(odomprov, "B2", 1.0)), float(getattr(odomprov, "nu", 200.0)))
+
+
+def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov):
+    """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective): the source is the
+    live frame on the ds lattice at the previous pose, the target is the map rendered from the previous pose at full
+    resolution, each source point is associated with the pixel it projects to.  Returns the new poses (B,1,4,4) =
+    T_icp · prev pose.  No host synchronisation."""
+    live = live_frame.to_channels_last()
+    B, _, H, W = live.shape
+    dev = pointclouds.device
+    _C.require_cuda(live.depth_image, "depth_image")
+    _C.require_cuda(pointclouds._geo, "pointclouds (geometry rows)")
+    depth, d_bs = _frame_base(live.depth_image, H * W)
+    K = live.intrinsics.contiguous()
+    prev = prev_frame.poses.contiguous()
+    ws = _ProjectiveWorkspace.get(dev, B, H, W, int(dsratio))
+    out = torch.empty((B, 1, 4, 4), dtype=torch.float32, device=dev)
+    mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
+    dth = odomprov.dist_thresh
+    _C.launch("gsx_icp_localize_projective", pointclouds._geo.contiguous(), pointclouds._counts_dev[pointclouds._cur],
+              pointclouds.capacity, pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode,
+              int(odomprov.numiters), float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth),
+              lambda_max, Bp, B2p, nu, out, 16, ws, ws.numel())
+    return out
+
+
+def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov):
+    """The differentiable counterpart of `localize_projective`, bit-identical poses: the index image comes from
+    gsx_render_views, the target images are gathers of the map rows at that index (so the gradient reaches the rows that
+    won a pixel, each at most one), and the batched ICP chain runs with the projective association.  live_frame.poses
+    must be the previous poses.  Returns (B,1,4,4)."""
+    from ..slam.icpslam import _compose_canonical
+
+    frames_pc = downsample_rgbdimages(live_frame, dsratio)
+    live = live_frame.to_channels_last()
+    B, _, H, W = live.shape
+    dev = pointclouds.device
+    K = live.intrinsics.detach().contiguous()
+    prev = prev_frame.poses
+    prev_d = prev.detach().contiguous()
+    index = torch.empty((B, H * W), dtype=torch.int64, device=dev)
+    _C.launch("gsx_render_views", pointclouds._geo.detach().contiguous(), None, pointclouds._counts_dev[pointclouds._cur],
+              pointclouds.capacity, pointclouds._bound, K, 16, prev_d, 16, B, 1, H, W, index, None, None, None, None)
+    covered = (index >= 0).unsqueeze(-1)
+    rows = index.clamp(min=0).unsqueeze(-1).expand(B, H * W, 3)
+
+    def target(padded):  # (one zero row appended: an element, or a batch, of empty maps still gathers)
+        padded = torch.cat([padded, padded.new_zeros(B, 1, 3)], 1)
+        return torch.where(covered, torch.gather(padded, 1, rows), torch.zeros((), dtype=padded.dtype, device=dev))
+
+    tgt_p, tgt_n = target(pointclouds.points_padded), target(pointclouds.normals_padded)
+    src_counts = frames_pc._counts_dev[frames_pc._cur]
+    dth = odomprov.dist_thresh
+    tgt_p_d = tgt_p.detach().contiguous()
+    assoc = lambda cur: project_associate(cur, src_counts, tgt_p_d, index, prev_d.view(B, 4, 4), K, H, W, dth)[1]
+    mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
+    T, _ = _taped_icp_batched(frames_pc.points_padded, src_counts, tgt_p, tgt_n, None, None, mode, odomprov.numiters,
+                              odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc)
+    return _compose_canonical(T, prev.squeeze(1)).unsqueeze(1)

@@ -42,8 +42,16 @@ class ICPSLAM(nn.Module):
     def __init__(self, *, odom: str = "gradicp", dsratio: int = 4, numiters: int = 20, damp: float = 1e-8,
                  dist_thresh: Union[float, int, None] = None, lambda_max: Union[float, int] = 2.0,
                  B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0, nu: Union[float, int] = 200.0,
-                 device: Union[torch.device, str, None] = None):
+                 association: str = "nn", device: Union[torch.device, str, None] = None):
+        """association (extension): how the ICP odometry pairs live points with the map.  'nn' (default, the
+        reference's) = exact 1-NN between the lattice-thinned live cloud and the lattice-active map points; 'projective'
+        = each live point with the map row visible at the pixel it projects to in the map rendered from the previous
+        pose (Keller et al.'s PointFusion, KinectFusion).  The two give different poses.  No effect with odom='gt'."""
         super().__init__()
+        if not isinstance(association, str):
+            raise TypeError("Expected association to be of type str. Got {0}.".format(type(association)))
+        if association not in ("nn", "projective"):
+            raise ValueError("association must be 'nn' or 'projective'. Got {!r}.".format(association))
         if odom not in ["gt", "icp", "gradicp"]:
             msg = "odometry method ({}) not supported for PointFusion. ".format(odom)
             msg += "Currently supported odometry modules for PointFusion are: 'gt', 'icp', 'gradicp'"
@@ -60,6 +68,7 @@ class ICPSLAM(nn.Module):
         self.odom = odom
         self.odomprov = odomprov
         self.dsratio = dsratio
+        self.association = association
         self.device = _normalize_device(device if device is not None else "cuda")
 
     # ------------------------------------------------------------------ sequence driver
@@ -136,7 +145,15 @@ class ICPSLAM(nn.Module):
         from ..odometry.icputils import _wants_grad, downsample_pointclouds, downsample_rgbdimages, localize_against_map
 
         live_frame.poses = prev_frame.poses
-        if _wants_grad(live_frame.depth_image, prev_frame.poses, *pointclouds._grad_tensors()):
+        wants_grad = _wants_grad(live_frame.depth_image, prev_frame.poses, *pointclouds._grad_tensors())
+        if self.association == "projective":
+            from ..odometry.icputils import localize_projective, localize_projective_taped
+
+            if not pointclouds.has_normals:
+                raise ValueError("projective ICP association needs a map with normals")
+            fn = localize_projective_taped if wants_grad else localize_projective
+            return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov)
+        if wants_grad:
             # differentiable mode (reference op order, slam/icpslam.py:238-247): the K1 maps carry their hand-written
             # backward, the association kernels are index-only, the ICP algebra is taped.
             from .fusionutils import find_active_map_points

@@ -40,9 +40,10 @@ class PointFusion(ICPSLAM):
                  angle_th: Union[float, int] = 20, sigma: Union[float, int] = 0.6, dsratio: int = 4,
                  numiters: int = 20, damp: float = 1e-8, dist_thresh: Union[float, int, None] = None,
                  lambda_max: Union[float, int] = 2.0, B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0,
-                 nu: Union[float, int] = 200.0, device: Union[torch.device, str, None] = None):
+                 nu: Union[float, int] = 200.0, association: str = "nn",
+                 device: Union[torch.device, str, None] = None):
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
-                         lambda_max=lambda_max, B=B, B2=B2, nu=nu, device=device)
+                         lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device)
         if not isinstance(dist_th, (float, int)):
             raise TypeError("Distance threshold must be of type float or int; but was of type {}.".format(
                 type(dist_th)))

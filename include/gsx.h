@@ -352,6 +352,35 @@ int gsx_icp_localize(const float *map_geometry, const int32_t *counts, int64_t c
                      float *poses_out, int64_t poses_out_bstride, void *workspace,
                      int64_t workspace_map_capacity, uint32_t epoch, int32_t *overflow_flag, void *stream);
 
+/* Projective frame-to-model ICP / gradICP odometry (an extension: the reference associates by exact 1-NN).  One call
+ * per frame step: source cloud as in gsx_icp_localize (live depth on the ds-lattice at the previous pose, valid pixels
+ * in row-major order); target images = the map rendered from the previous pose at full resolution H x W through the
+ * z-buffer of gsx_render_views (index image, and the winning rows' world-frame points and normals); the ICP loop of
+ * gsx_icp_localize, except that a source point s is associated with the pixel j it projects to in the previous camera
+ * (the projection of gsx_render_views: frustum (-1e-3, W - 0.999) x (-1e-3, H - 0.999), z > 0, round half to even,
+ * clamp) iff a map row covers j and, with use_dist_thresh, |s - p_j|^2 < dist_thresh; poses_out[b] = T_icp[b] *
+ * prev_poses[b].  intrinsics / prev_poses: B 4x4 matrices (the previous frame's camera) with the given element strides.
+ * workspace: gsx_icp_projective_workspace_bytes(B,H,W,ds) bytes, any content (nothing in it outlives a call).
+ * max_count = host upper bound on counts[b] <= capacity <= INT32_MAX.  An element with an empty map, or with no valid
+ * live depth, keeps its previous pose exactly.  No host synchronisation. */
+int64_t gsx_icp_projective_workspace_bytes(int B, int H, int W, int ds);
+int gsx_icp_localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                                const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
+                                const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds,
+                                int mode, int numiters, float damp, int use_dist_thresh, float dist_thresh,
+                                float lambda_max, float Bp, float B2p, float nu, float *poses_out,
+                                int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes, void *stream);
+
+/* The association of gsx_icp_localize_projective alone (the index-only op of the differentiable mode): for the source
+ * rows i < src_count[b] of src_points (B, ns_stride, 3), world frame, idx_out int64 (B, ns_stride) = the pixel
+ * j = h*W + w of the target images they are associated with, or -1; d2_out (may be NULL) = |s - tgt_points[b, j]|^2
+ * where a row covers the pixel s projects to (even when dist_thresh rejects it), +inf otherwise.  Rows i >= src_count[b]
+ * are not written.  tgt_points (B, H*W, 3) and tgt_index (B, H*W) are the target images (index -1 = uncovered). */
+int gsx_icp_project_associate(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
+                              const int64_t *tgt_index, const float *prev_poses, int64_t pose_bstride,
+                              const float *intrinsics, int64_t K_bstride, int B, int H, int W, int use_dist_thresh,
+                              float dist_thresh, int64_t *idx_out, float *d2_out, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Rendering of the surfel map into L views per element: depth, colour, camera-frame normal, confidence and index images.
  * The reference has no counterpart; the pixel assignment is find_active_map_points'
