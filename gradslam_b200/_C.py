@@ -48,6 +48,13 @@ SIGNATURES = {
     "gsx_pointfusion_sequence_gt": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                 c_float, c_float, c_double, c_vp, c_vp, c_vp]),
+    "gsx_fusion_prune_scratch_bytes": (c_i64, [c_int, c_i64]),
+    "gsx_fusion_prune_unstable": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_float, c_int, c_vp, c_vp, c_i64, c_vp]),
+    "gsx_fusion_prune_unstable_bwd": (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp]),
+    "gsx_pointfusion_sequence_gt_prune": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_vp, c_vp]),
     "gsx_debug_fail_at_frame": (None, [c_int]),
     "gsx_debug_set_k2_grid_cap": (None, [c_int]),
     "gsx_peer_export": (c_int, [c_vp, c_vp, c_vp, c_vp]),

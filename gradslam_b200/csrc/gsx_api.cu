@@ -32,6 +32,18 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
                         int64_t rgb_bs, int B_total, int b0, int nb, int H, int W, float dist_th, float dot_th,
                         void *workspace, int32_t *overflow, cudaStream_t st);
 int64_t fusion_workspace_bytes(int B, int H, int W);
+// gsx_prune.cu: removal of unstable surfels for the elements [b0, b0 + nb)
+int prune_group(float *geo, float *col, int32_t *counts, int64_t cap, int32_t *ring, int ring_len, int step, int t_max,
+                float c_stable, int B_total, int b0, int nb, int32_t *keep_map, void *scratch, cudaStream_t st);
+int64_t prune_scratch_bytes(int B, int64_t capacity);
+
+// Pruning of the sequence driver (Keller et al. 2013): frame s of the call is pruned step s; null = pruning off
+struct SequencePrune {
+  int32_t *ring;  // (t_max + 2, B)
+  int t_max;
+  float c_stable;
+  void *scratch;
+};
 
 // Batch elements own independent maps, so the sequence driver splits the batch into groups that walk the frame
 // sequence on their own streams: the kernels of one group overlap those of another instead of alternating on an otherwise
@@ -88,11 +100,11 @@ extern "C" void gsx_debug_fail_at_frame(int s) { g_fail_at_frame = s; }
 
 extern "C" int gsx_pointfusion_sequence_groups(int B) { return B <= 0 ? 0 : gsx::sequence_groups(B); }
 
-extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                           int64_t max_count0, const float *depth, const float *rgb,
-                                           const float *intrinsics, const float *poses, int B, int L, int s_begin,
-                                           int s_end, int H, int W, float dist_th, float dot_th, double sigma,
-                                           void *workspace, int32_t *overflow_flag, void *stream) {
+// The one driver behind gsx_pointfusion_sequence_gt (prune == nullptr) and gsx_pointfusion_sequence_gt_prune.
+static int sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int64_t max_count0,
+                       const float *depth, const float *rgb, const float *intrinsics, const float *poses, int B, int L,
+                       int s_begin, int s_end, int H, int W, float dist_th, float dot_th, double sigma, void *workspace,
+                       int32_t *overflow_flag, const gsx::SequencePrune *prune, void *stream) {
   GSX_CHECK_ARG(B >= 0 && L >= 0 && H >= 2 && W >= 2, "gsx_pointfusion_sequence_gt: bad extents");
   GSX_CHECK_ARG(0 <= s_begin && s_begin <= s_end && s_end <= L, "gsx_pointfusion_sequence_gt: bad frame range");
   GSX_CHECK_ARG(counts && depth && rgb && intrinsics && poses, "gsx_pointfusion_sequence_gt: null pointer");
@@ -123,6 +135,9 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
                                       counts + (int64_t)((s + 1) & 1) * B, capacity, max_count, poses + (int64_t)s * 16,
                                       (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, 0, B,
                                       H, W, dist_th, dot_th, half[0], overflow_flag, user);
+      if (rc == 0 && prune)
+        rc = gsx::prune_group(map_geometry, map_colors, counts + (int64_t)((s + 1) & 1) * B, capacity, prune->ring,
+                              prune->t_max + 2, s, prune->t_max, prune->c_stable, B, 0, B, nullptr, prune->scratch, user);
     }
     return rc;
   }
@@ -155,6 +170,9 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
       rc = gsx::fusion_update_group(map_geometry, map_colors, cin, cout, capacity, max_count, poses + (int64_t)s * 16,
                                     (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, b0,
                                     b1 - b0, H, W, dist_th, dot_th, half[h], overflow_flag, gs->stream[g]);
+      if (rc == 0 && prune)
+        rc = gsx::prune_group(map_geometry, map_colors, cout, capacity, prune->ring, prune->t_max + 2, s, prune->t_max,
+                              prune->c_stable, B, b0, b1 - b0, nullptr, prune->scratch, gs->stream[g]);
       cudaEventRecord(gs->upd_done[g][h], gs->stream[g]);
     }
   }
@@ -167,6 +185,34 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
     cudaStreamWaitEvent(user, gs->rec_join[g], 0);
   }
   return rc;
+}
+
+extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                           int64_t max_count0, const float *depth, const float *rgb,
+                                           const float *intrinsics, const float *poses, int B, int L, int s_begin,
+                                           int s_end, int H, int W, float dist_th, float dot_th, double sigma,
+                                           void *workspace, int32_t *overflow_flag, void *stream) {
+  return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
+                     s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, nullptr, stream);
+}
+
+extern "C" int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map_colors, int32_t *counts,
+                                                 int64_t capacity, int64_t max_count0, const float *depth,
+                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
+                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
+                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
+                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                                 int32_t *overflow_flag, void *stream) {
+  GSX_CHECK_ARG(t_max >= 0 && c_stable >= 0.0f, "gsx_pointfusion_sequence_gt_prune: need t_max >= 0, c_stable >= 0");
+  if (B > 0 && s_begin < s_end) {
+    GSX_CHECK_ARG(ring && prune_scratch, "gsx_pointfusion_sequence_gt_prune: null ring / scratch pointer");
+    GSX_CHECK_ARG(prune_scratch_bytes >= gsx::prune_scratch_bytes(B, capacity),
+                  "gsx_pointfusion_sequence_gt_prune: prune scratch of %lld bytes < gsx_fusion_prune_scratch_bytes",
+                  (long long)prune_scratch_bytes);
+  }
+  const gsx::SequencePrune prune{ring, t_max, c_stable, prune_scratch};
+  return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
+                     s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, &prune, stream);
 }
 
 extern "C" int64_t gsx_pointfusion_sequence_workspace_bytes(int B, int H, int W) {

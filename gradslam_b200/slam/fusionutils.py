@@ -14,10 +14,10 @@ from typing import Union
 import torch
 
 from .. import _C
-from ..structures.pointclouds import Pointclouds
+from ..structures.pointclouds import Pointclouds, _PruneHistory
 from ..structures.rgbdimages import RGBDImages, _frame_base
 
-__all__ = ["update_map_fusion", "update_map_aggregate"]
+__all__ = ["update_map_fusion", "update_map_aggregate", "prune_unstable"]
 
 
 # --------------------------------------------------------------------------------------------- small helpers
@@ -501,6 +501,85 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
     pointclouds._geo, pointclouds._col = geo_out, col_out
     pointclouds._uninit = False
     pointclouds._mark_device_updated(pointclouds._bound + P)
+    return pointclouds
+
+
+# --------------------------------------------------------------------------------------------- unstable surfels
+def _prune_history(pointclouds, t_max):
+    """The map's pruning history, created at its first pruned step (rows already in the map count as created then)."""
+    h = pointclouds._prune
+    if h is None:
+        h = pointclouds._prune = _PruneHistory.fresh(len(pointclouds), t_max, pointclouds.device)
+    elif h.t_max != t_max:
+        raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
+            t_max, h.t_max))
+    return h
+
+
+def _prune_scratch(B, capacity, device):
+    return torch.empty(_C.lib().gsx_fusion_prune_scratch_bytes(B, capacity), dtype=torch.uint8, device=device)
+
+
+def _pruned(pointclouds, h):
+    """Bookkeeping after a prune launch: one more pruned step, sizes changed on the device (the host bound stays an upper
+    bound), and rows past the new sizes hold stale values until a padded view zeroes them."""
+    h.step += 1
+    pointclouds._counts_host = None
+    pointclouds._list_cache = {}
+    pointclouds._uninit = pointclouds._tail_dirty = True
+
+
+class _PruneFn(torch.autograd.Function):
+    """The prune as one differentiable op on the packed rows: forward = gsx_fusion_prune_unstable on a copy of the rows,
+    recording where every row went (keep_map); backward = gsx_fusion_prune_unstable_bwd, a gather.  The removal itself
+    is a decision on the confidence and carries no gradient, as an index_select would not."""
+
+    @staticmethod
+    def forward(ctx, pack, geo, col):
+        pointclouds, h, c_stable = pack
+        B, cap = geo.shape[0], geo.shape[1]
+        dev = geo.device
+        geo_o, col_o = geo.detach().clone(), col.detach().clone()
+        counts = pointclouds._counts_dev[pointclouds._cur]
+        counts_in = counts.clone()
+        keep_map = torch.arange(cap, dtype=torch.int32, device=dev).repeat(B, 1)  # rows before the window: identity
+        scratch = _prune_scratch(B, cap, dev)
+        _C.launch("gsx_fusion_prune_unstable", geo_o, col_o, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
+                  float(c_stable), B, keep_map, scratch, scratch.numel())
+        ctx.saved = (keep_map, counts_in)
+        return geo_o, col_o
+
+    @staticmethod
+    def backward(ctx, g_geo, g_col):
+        keep_map, counts_in = ctx.saved
+        B, cap = keep_map.shape
+        gs = [None if g is None else g.contiguous().float() for g in (g_geo, g_col)]
+        d_geo = torch.empty((B, cap, 8), dtype=torch.float32, device=keep_map.device)
+        d_col = torch.empty((B, cap, 4), dtype=torch.float32, device=keep_map.device)
+        _C.launch("gsx_fusion_prune_unstable_bwd", keep_map, counts_in, cap, gs[0], gs[1], cap, B, d_geo, d_col)
+        return None, d_geo, d_col
+
+
+def prune_unstable(pointclouds: Pointclouds, stable_confidence: float, max_unstable_age: int) -> Pointclouds:
+    """Removes unstable surfels, in place, as one pruned step of the map (Keller et al. 2013, section 4.3; an extension:
+    gradslam keeps every surfel).  The rows created `max_unstable_age` pruned steps ago whose confidence (the
+    `features_padded` value: gradslam's alpha summed over merges) is still below `stable_confidence` are removed; every
+    other row keeps its order.  Run it after each fused update (PointFusion does, when configured)."""
+    if not pointclouds.has_points:
+        return pointclouds
+    if not pointclouds._has_cc or pointclouds._col is None:
+        raise ValueError("pruning needs maps with colours and a confidence count per point")
+    h = _prune_history(pointclouds, int(max_unstable_age))
+    B, dev = len(pointclouds), pointclouds.device
+    if torch.is_grad_enabled() and any(t.requires_grad for t in pointclouds._grad_tensors()):
+        pointclouds._geo, pointclouds._col = _PruneFn.apply((pointclouds, h, stable_confidence), pointclouds._geo,
+                                                            pointclouds._col)
+    else:
+        geo, col = _map_ptrs(pointclouds, dev)
+        scratch = _prune_scratch(B, pointclouds.capacity, dev)
+        _C.launch("gsx_fusion_prune_unstable", geo, col, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
+                  h.ring, h.t_max + 2, h.step, h.t_max, float(stable_confidence), B, None, scratch, scratch.numel())
+    _pruned(pointclouds, h)
     return pointclouds
 
 

@@ -5,14 +5,15 @@ defaults (dist_th=0.05, angle_th=20, sigma=0.6), `dot_th = cos(angle_th)`.
 """
 import math
 import warnings
-from typing import Union
+from typing import Optional, Union
 
 import torch
 
 from .. import _C
 from ..structures.pointclouds import Pointclouds
 from ..structures.rgbdimages import RGBDImages
-from .fusionutils import update_map_fusion
+from ..structures.pointclouds import _PruneHistory
+from .fusionutils import _prune_scratch, prune_unstable, update_map_fusion
 from .icpslam import ICPSLAM
 
 __all__ = ["PointFusion"]
@@ -41,7 +42,25 @@ class PointFusion(ICPSLAM):
                  numiters: int = 20, damp: float = 1e-8, dist_thresh: Union[float, int, None] = None,
                  lambda_max: Union[float, int] = 2.0, B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0,
                  nu: Union[float, int] = 200.0, association: str = "nn",
-                 device: Union[torch.device, str, None] = None):
+                 device: Union[torch.device, str, None] = None, stable_confidence: Union[float, int, None] = None,
+                 max_unstable_age: Optional[int] = None):
+        """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
+        surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
+        (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
+        clamp(exp(-|v|^2 / 2 sigma^2), 1e-7, 1.01) of the camera-frame vertex, summed over merges - so a good threshold
+        depends on the scene's depth range and on sigma; there is no universal default.  max_unstable_age = 0 tests each
+        surfel in the frame that creates it.  Default: nothing is removed (gradslam's behaviour)."""
+        for name, val, kinds in (("stable_confidence", stable_confidence, (float, int)),
+                                 ("max_unstable_age", max_unstable_age, (int,))):
+            if val is not None and (isinstance(val, bool) or not isinstance(val, kinds)):
+                raise TypeError("{} must be of type {}; but was of type {}.".format(
+                    name, " or ".join(k.__name__ for k in kinds), type(val)))
+        if (stable_confidence is None) != (max_unstable_age is None):
+            raise ValueError("give both stable_confidence and max_unstable_age, or neither")
+        if stable_confidence is not None and not stable_confidence >= 0:
+            raise ValueError("stable_confidence ({}) must be >= 0".format(stable_confidence))
+        if max_unstable_age is not None and max_unstable_age < 0:
+            raise ValueError("max_unstable_age ({}) must be >= 0".format(max_unstable_age))
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
                          lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device)
         if not isinstance(dist_th, (float, int)):
@@ -57,9 +76,18 @@ class PointFusion(ICPSLAM):
         self.dist_th = dist_th
         self.dot_th = math.cos((angle_th * math.pi) / 180)
         self.sigma = sigma
+        self.stable_confidence = stable_confidence
+        self.max_unstable_age = max_unstable_age
 
     def _map(self, pointclouds: Pointclouds, live_frame: RGBDImages, inplace: bool = False):
-        return update_map_fusion(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, inplace)
+        if self.stable_confidence is not None and isinstance(pointclouds, Pointclouds):
+            if pointclouds._prune is not None and pointclouds._prune.t_max != self.max_unstable_age:
+                raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
+                    self.max_unstable_age, pointclouds._prune.t_max))
+        pointclouds = update_map_fusion(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, inplace)
+        if self.stable_confidence is not None:
+            prune_unstable(pointclouds, self.stable_confidence, self.max_unstable_age)
+        return pointclouds
 
     def forward(self, frames, out=None):
         """As ICPSLAM.forward; additionally accepts a `gradslam_b200.ingest.RawRGBD` batch (uint8 colour + uint16 depth)
@@ -124,6 +152,9 @@ class PointFusion(ICPSLAM):
             pc = Pointclouds(device=dev)
             pc._allocate(B, L * P, 1, zero=False)
         ws = _SequenceWorkspace.get(dev, B, H, W)
+        if self.stable_confidence is not None:  # a fresh map: frame s of the call is pruned step s
+            pc._prune = hist = _PruneHistory.fresh(B, self.max_unstable_age, dev)
+            prune_scratch = _prune_scratch(B, pc.capacity, dev)
         main = torch.cuda.current_stream(dev)
         ready = []
         if not on_device:
@@ -146,9 +177,15 @@ class PointFusion(ICPSLAM):
                 for b in range(B):
                     _C.launch("gsx_ingest_raw", raw_rgb[b, s0:s1], raw_depth[b, s0:s1], (s1 - s0) * P,
                               frames.scaling_factor, 1 if frames.normalize_color else 0, rgb[b, s0:s1], depth[b, s0:s1])
-            _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                      min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                      float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag())
+            if self.stable_confidence is None:
+                _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                          min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                          float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag())
+            else:
+                _C.launch("gsx_pointfusion_sequence_gt_prune", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                          min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                          float(self.dot_th), float(self.sigma), ws.buf, hist.ring, self.max_unstable_age,
+                          float(self.stable_confidence), prune_scratch, prune_scratch.numel(), pc._overflow_flag())
         if not on_device:
             for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
                 t.record_stream(copy_stream)
@@ -157,4 +194,7 @@ class PointFusion(ICPSLAM):
         pc._bound = pc.capacity
         pc._list_cache = {}
         pc._tail_dirty = pc._uninit
+        if self.stable_confidence is not None:  # rows past the pruned sizes hold stale values
+            hist.step = L
+            pc._uninit = pc._tail_dirty = True
         return pc, poses.clone()

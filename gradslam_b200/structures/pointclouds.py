@@ -33,6 +33,23 @@ def _f32(t, device):
     return t.to(device=device, dtype=torch.float32)
 
 
+class _PruneHistory:
+    """Pruning history of a batch of maps (the removal of unstable surfels, fusionutils.prune_unstable): `ring` int32
+    (t_max + 2, B) on the map's device, where ring[k % (t_max + 2), b] is element b's row count after pruned step k, and
+    `step`, the number of pruned steps so far (host).  Rows are appended in step order and removed by a stable
+    compaction, so the rows created at step k are [ring(k - 1), ring(k)) and no per-row timestamp is stored."""
+
+    def __init__(self, ring: torch.Tensor, step: int, t_max: int):
+        self.ring, self.step, self.t_max = ring, int(step), int(t_max)
+
+    @classmethod
+    def fresh(cls, B: int, t_max: int, device):
+        return cls(torch.zeros((t_max + 2, B), dtype=torch.int32, device=device), 0, t_max)
+
+    def to(self, device):
+        return _PruneHistory(self.ring.to(device, copy=True), self.step, self.t_max)
+
+
 class Pointclouds(object):
     def __init__(self, points=None, normals=None, colors=None, features=None,
                  device: Union[torch.device, str, None] = None):
@@ -59,6 +76,7 @@ class Pointclouds(object):
         self._list_cache = {}
         self._uninit = False  # store was allocated without zero-fill: rows >= counts[b] may hold garbage
         self._tail_dirty = False  # the ragged tail [counts[b], max(counts)) must be zeroed before a padded view
+        self._prune = None  # _PruneHistory once unstable surfels have been removed from this map (PointFusion)
 
         if isinstance(points, list):
             shapes = [p.shape for p in points]
@@ -573,6 +591,7 @@ class Pointclouds(object):
         other._bound = min(self._bound, keep)
         other._overflow = None if self._overflow is None else self._overflow.clone().to(other.device)
         other._uninit, other._tail_dirty = self._uninit, self._tail_dirty
+        other._prune = None if self._prune is None else self._prune.to(other.device)
         return other
 
     def clone(self):
@@ -646,6 +665,7 @@ class Pointclouds(object):
         self._counts_dev, self._cur = src._counts_dev, src._cur
         self._counts_host, self._bound, self._overflow = src._counts_host, src._bound, src._overflow
         self._uninit, self._tail_dirty = src._uninit, src._tail_dirty
+        self._prune = src._prune
         self._list_cache = {}
 
     def append_points(self, pointclouds: "Pointclouds"):

@@ -157,6 +157,42 @@ int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t 
                                 int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
                                 const float *poses, int B, int L, int s_begin, int s_end, int H, int W, float dist_th,
                                 float dot_th, double sigma, void *workspace, int32_t *overflow_flag, void *stream);
+/* ------------------------------------------------------------------------------------------------
+ * Removal of unstable surfels (opt-in extension; gradslam has no such step, so no reference line is replaced).
+ * Keller et al. 2013, "Real-time 3D reconstruction in dynamic scenes using point-based fusion", section 4.3: a surfel
+ * whose confidence is still below c_stable t_max frames after it was created is an outlier and is removed.  Confidence
+ * is the map's ccount slot (gradslam's alpha, summed over merges), so c_stable is in those units.
+ * Pruning history: ring int32 (t_max + 2, B), where ring[k mod (t_max + 2)][b] = element b's row count after pruned
+ * step k (ring(-1) = 0, implicit).  The creation step of a row is the first pruned step after which it is in the map.
+ * Pruned step `step`, run after that step's K4: when step >= t_max, the rows of element b with index in
+ * [ring(step - t_max - 1), ring(step - t_max)) and ccount < c_stable are removed by a stable compaction IN PLACE (every
+ * surviving row keeps its order); counts[b] and ring(k) for k in [step - t_max, step) lose the removed rows, and
+ * ring(step) = the new counts[b].  Rows >= the new counts[b] keep stale values (never read).
+ * scratch: gsx_fusion_prune_scratch_bytes(B, capacity) bytes; every call re-arms it (no initialisation needed).
+ * keep_map: NULL, or int32 (B, capacity) that receives, for every row from the window start on, its destination row
+ * or -1 if removed; entries before the window start are not written (the differentiable mode fills them with the
+ * identity). */
+int64_t gsx_fusion_prune_scratch_bytes(int B, int64_t capacity);
+int gsx_fusion_prune_unstable(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int32_t *ring,
+                              int ring_len, int step, int t_max, float c_stable, int B, int32_t *keep_map,
+                              void *scratch, int64_t scratch_bytes, void *stream);
+/* Backward of gsx_fusion_prune_unstable (Keller et al. 2013, as above): a gather.  d_map[b][n] = g[b][keep_map[b][n]]
+ * for n < counts_in[b] with keep_map >= 0, else zero (removed and padding rows; padding slots zero).  keep_map
+ * (B, capacity_in) as the forward left it over an identity fill; upstream gradients (B, capacity_out, 8 / 4), either
+ * may be NULL = zero; outputs (B, capacity_in, 8 / 4), every row written.  No atomics. */
+int gsx_fusion_prune_unstable_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
+                                  const float *g_geometry, const float *g_colors, int64_t capacity_out, int B,
+                                  float *d_map_geometry, float *d_map_colors, void *stream);
+/* gsx_pointfusion_sequence_gt followed, after every frame's K4, by gsx_fusion_prune_unstable (Keller et al. 2013, as
+ * above) on the group stream: frame s of the call is pruned step s, so a call with s_begin > 0 continues the same ring.
+ * ring int32 (t_max + 2, B); prune_scratch: gsx_fusion_prune_scratch_bytes(B, capacity) bytes.  Both entry points run
+ * one driver; gsx_pointfusion_sequence_gt is this one with pruning off. */
+int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                      int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
+                                      const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
+                                      float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring,
+                                      int t_max, float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                      int32_t *overflow_flag, void *stream);
 /* test hook: the next gsx_pointfusion_sequence_gt call reports a launch failure at frame s (once); -1 = off */
 void gsx_debug_fail_at_frame(int s);
 /* test hook: caps the total CTA count of the map projection kernel (K2), so that small maps take several grid-stride
