@@ -252,52 +252,6 @@ __device__ __forceinline__ FrameSample frame_sample(const float *__restrict__ di
   return s;
 }
 
-// 128-bit record used for the per-pixel arg-min.  The workspace is zero-initialised and zero means
-// "no candidate", so a key (hi:lo) is stored as its bitwise complement and the arg-min over keys
-// becomes an atomic MAX over the stored 128-bit unsigned integers.
-struct __align__(16) U128 {
-  unsigned long long lo, hi;
-};
-
-__device__ __forceinline__ U128 cas128(U128 *addr, U128 expected, U128 desired) {
-  U128 old;
-  asm volatile(
-      "{\n\t.reg .b128 e, d, o;\n\t"
-      "mov.b128 e, {%2, %3};\n\t"
-      "mov.b128 d, {%4, %5};\n\t"
-      "atom.global.relaxed.gpu.cas.b128 o, [%6], e, d;\n\t"
-      "mov.b128 {%0, %1}, o;\n\t}"
-      : "=l"(old.lo), "=l"(old.hi)
-      : "l"(expected.lo), "l"(expected.hi), "l"(desired.lo), "l"(desired.hi), "l"(addr)
-      : "memory");
-  return old;
-}
-
-__device__ __forceinline__ bool rec_greater(const U128 &a, const U128 &b) {
-  return a.hi > b.hi || (a.hi == b.hi && a.lo > b.lo);
-}
-
-// Finishes an arg-min update whose first (optimistic, expected = empty) CAS returned `old`.
-__device__ __forceinline__ void atomic_max_rec128_finish(U128 *addr, const U128 &mine, U128 old) {
-  U128 cur{0ull, 0ull};
-  while (!(old.hi == cur.hi && old.lo == cur.lo)) {  // the CAS did not take effect
-    cur = old;
-    if (!rec_greater(mine, cur)) return;  // somebody better is already there
-    old = cas128(addr, cur, mine);
-  }
-}
-
-// arg-min over keys == max over complemented records
-__device__ __forceinline__ void atomic_min_key128(U128 *addr, unsigned long long key_hi, unsigned long long key_lo) {
-  const U128 mine{~key_lo, ~key_hi};
-  U128 cur{0ull, 0ull};  // optimistic: most pixels see a single candidate, so expect "empty" first
-  while (mine.hi > cur.hi || (mine.hi == cur.hi && mine.lo > cur.lo)) {
-    const U128 old = cas128(addr, cur, mine);
-    if (old.hi == cur.hi && old.lo == cur.lo) break;
-    cur = old;
-  }
-}
-
 // High word of the arg-min key of find_best_unique_correspondences (fusionutils.py:491-517): 1/(cc+1e-20), then the
 // squared distance d2 >= 0.  Positive floats order like their bit patterns; negatives are flipped so the order stays total.
 __device__ __forceinline__ unsigned long long argmin_key_hi(float cc, float d2) {
@@ -306,6 +260,38 @@ __device__ __forceinline__ unsigned long long argmin_key_hi(float cc, float d2) 
   kb = (kb & 0x80000000u) ? ~kb : (kb | 0x80000000u);
   const unsigned int rb = __float_as_uint(d2) | 0x80000000u;
   return ((unsigned long long)kb << 32) | rb;
+}
+
+// Squared distance between a pixel's frame vertex fv and a map point: the ray distance of the arg-min key and the
+// quantity of the distance test.  Negating the difference does not change a square, so map - frame gives the same bits.
+__device__ __forceinline__ float ray_d2(const float3 &fv, float x, float y, float z) {
+  const float dx = fv.x - x, dy = fv.y - y, dz = fv.z - z;
+  return (dx * dx + dy * dy) + dz * dz;
+}
+
+// ---- per-pixel arg-min over map rows (find_best_unique_correspondences, fusionutils.py:414-546) ----------------------
+// A pixel's 4-byte slot holds n + 1 of the row that currently wins it, 0 for none.  The key of a candidate row n,
+// (argmin_key_hi(cc, ray_d2(fv, p)), n), is a fixed function of the row (read-only while the arg-min runs) and of the
+// pixel's frame vertex fv, which every candidate of the pixel computes bit for bit; so the slot holds no key, and a
+// candidate that finds the slot taken gathers the stored row and recomputes that row's key.
+// Claiming is optimistic (most pixels see a single candidate) and returns the slot's previous value; argmin_settle
+// finishes the update from it, so that a caller may look at the result of the CAS later.
+__device__ __forceinline__ unsigned int argmin_claim(unsigned int *slot, unsigned int n) {
+  return atomicCAS(slot, 0u, n + 1u);
+}
+
+// geo: the element's geometry rows.  Replaces the stored row while this candidate's key is the smaller one.
+__device__ __forceinline__ void argmin_settle(unsigned int *slot, unsigned int n, unsigned long long key_hi,
+                                              const float3 &fv, const float *geo, unsigned int old) {
+  unsigned int cur = 0u;
+  while (old != cur) {  // the last CAS did not take effect: row old - 1 holds the slot
+    cur = old;
+    const unsigned int m = cur - 1u;
+    const float4 p = __ldg(reinterpret_cast<const float4 *>(geo + (int64_t)m * kGeoW));
+    const unsigned long long k = argmin_key_hi(__ldg(geo + (int64_t)m * kGeoW + 6), ray_d2(fv, p.x, p.y, p.z));
+    if (k < key_hi || (k == key_hi && m <= n)) return;
+    old = atomicCAS(slot, cur, n + 1u);
+  }
 }
 
 // ---- projection of a map point into the live camera (fusionutils.py:249-274) ----------------------------------------

@@ -5,8 +5,9 @@
 //                              (fusionutils.py:16-73) from the pixel's depth stencil, bit for bit.  Caller-supplied maps
 //                              (differentiable mode) are packed into per-pixel records instead.
 //   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, gather of the depth
-//                              stencil under the projection, distance / normal tests, then a 128-bit atomic
-//                              arg-min per pixel on the key (1/ccount, ray distance, row index).
+//                              stencil under the projection, distance / normal tests, then an atomic arg-min per
+//                              pixel on the key (1/ccount, ray distance, row index) into a 4-byte slot holding the
+//                              winning row (argmin_claim / argmin_settle, gsx_common.cuh).
 //   k_merge_append    (K4)     one thread per pixel: confidence-weighted merge of the selected map row, or stable append of
 //                              unmatched valid pixels (single-pass decoupled look-back scan, row-major order per batch
 //                              element).  No float atomics anywhere.
@@ -126,7 +127,7 @@ __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records(FrameRecArgs a
     a.ws.vrec[i] = make_float4(__ldg(a.gv + o), __ldg(a.gv + o + 1), __ldg(a.gv + o + 2),
                                confidence_alpha((vx * vx + vy * vy) + vz * vz, a.two_sigma_sq));
   }
-  a.ws.best[i] = U128{0ull, 0ull};
+  a.ws.win[i] = 0u;
 }
 
 int launch_frame_records(const FrameRecArgs &a, cudaStream_t stream) {
@@ -156,7 +157,7 @@ struct ProjectArgs {
   float d2_max;  // largest float x with sqrtf(x) < dist_th (-1 if none): sqrtf(d2) < dist_th <=> d2 <= d2_max
   const float4 *nrec, *vrec;
   const FrameHeader *hdr;
-  U128 *best;
+  unsigned int *win;
   unsigned long long *stats;
 };
 
@@ -183,7 +184,7 @@ __device__ __forceinline__ MapRow load_map_row(const float *geo, int64_t n) {
 //     image, 1.2 MB per element, stays in L2) and re-evaluate K1's world vertex and world normal from it;
 //   * sqrtf(d2) < dist_th is decided as d2 <= d2_max (exact: the correctly rounded square root is monotonic; the
 //     threshold is found on the host, gsx_thresholds.h);
-//   * the result of the 128-bit CAS is only looked at one iteration later.
+//   * the result of the arg-min CAS is only looked at one iteration later.
 // The grid-stride loop of one CTA over element b's rows; the record kind is a template argument so that each of the two
 // loops only holds the registers of its own kind.
 template <bool kFromMaps>
@@ -192,11 +193,14 @@ __device__ __forceinline__ void select_rows(const ProjectArgs &a, const LiveCame
   const int P = a.ib.H * a.ib.W;
   const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   const float4 *nrec = a.nrec + (int64_t)b * P, *vrec = a.vrec + (int64_t)b * P;
-  U128 *best = a.best + (int64_t)b * P;
+  unsigned int *win = a.win + (int64_t)b * P;
   const int64_t stride = (int64_t)gridDim.x * kBlock;
   int64_t n = (int64_t)blockIdx.x * kBlock + threadIdx.x;
-  U128 mine{0ull, 0ull}, old{0ull, 0ull};
+  // the pending candidate: its pixel, row, key, the pixel's frame vertex and what its claim returned
   int pend_pix = -1;
+  unsigned int pend_n = 0u, pend_old = 0u;
+  unsigned long long pend_key = 0ull;
+  float3 pend_fv = make_float3(0.f, 0.f, 0.f);
   MapRow cur = load_map_row(geo, n < count ? n : 0);
   for (; n < count; n += stride) {
     const MapRow m = cur;
@@ -216,22 +220,23 @@ __device__ __forceinline__ void select_rows(const ProjectArgs &a, const LiveCame
       // are_normals_similar (fusionutils.py:187-195): n_frame . n_map > dot_th
       const float dot = (gn.x * m.a.w + gn.y * m.b.x) + gn.z * m.b.y;
       // are_points_close (fusionutils.py:130): ||frame - map|| < dist_th
-      const float dx = fv.x - m.a.x, dy = fv.y - m.a.y, dz = fv.z - m.a.z;
-      const float d2 = (dx * dx + dy * dy) + dz * dz;
+      const float3 fv3 = make_float3(fv.x, fv.y, fv.z);
+      const float d2 = ray_d2(fv3, m.a.x, m.a.y, m.a.z);
       const bool live = (d2 <= a.d2_max) && (dot > a.dot_th);
-      if (pend_pix >= 0) {  // settle the previous candidate's CAS before re-using the slot
-        atomic_max_rec128_finish(best + pend_pix, mine, old);
+      if (pend_pix >= 0) {  // settle the previous candidate's CAS before re-using the registers
+        argmin_settle(win + pend_pix, pend_n, pend_key, pend_fv, geo, pend_old);
         pend_pix = -1;
       }
       if (live) {
-        // key (1/(cc+1e-20), (map - frame)^2 == d2: squares are sign-independent, n)
-        mine = U128{~(unsigned long long)n, ~argmin_key_hi(m.b.z, d2)};
-        old = cas128(best + pix, U128{0ull, 0ull}, mine);  // optimistic: most pixels see a single candidate
+        pend_n = (unsigned int)n;
+        pend_key = argmin_key_hi(m.b.z, d2);
+        pend_fv = fv3;
+        pend_old = argmin_claim(win + pix, pend_n);
         pend_pix = pix;
       }
     }
   }
-  if (pend_pix >= 0) atomic_max_rec128_finish(best + pend_pix, mine, old);
+  if (pend_pix >= 0) argmin_settle(win + pend_pix, pend_n, pend_key, pend_fv, geo, pend_old);
 }
 
 __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectArgs a) {
@@ -304,7 +309,7 @@ constexpr unsigned int kMergeEpoch = 1u;
 #endif
 
 // Starts moving the sector at p from DRAM into L2 without waiting for it and without a register.  K4 knows the row a
-// pixel merges into as soon as its arg-min record arrives, but gathers the row only after the CTA's scan barrier and the
+// pixel merges into as soon as its arg-min slot arrives, but gathers the row only after the CTA's scan barrier and the
 // vertex re-evaluation: issued here, the DRAM round trip overlaps that work and the gather hits L2.  H100 80GB HBM3,
 // 400 W, bench workload: K4 185 -> 178 us per launch, 21.6-21.7 k -> 21.9-22.0 k frames/s (DESIGN.md section 4).
 __device__ __forceinline__ void prefetch_l2(const float *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
@@ -329,7 +334,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   const int P = a.H * a.W;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int pix0 = tile * kTilePix;
-  const U128 *best = a.ws.best + (int64_t)b * P;
+  const unsigned int *win = a.ws.win + (int64_t)b * P;
   const float4 *nrec = a.ws.nrec + (int64_t)b * P, *vrec = a.ws.vrec + (int64_t)b * P;
   const float *rgb = a.rgb + b * a.rgb_bstride + (int64_t)pix0 * 3;
 
@@ -345,22 +350,21 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   }
 
   int pix[kPix];
-  unsigned long long rec_lo[kPix];
+  unsigned int slot[kPix];  // arg-min slot: the matched map row + 1
   float dep[kPix];
   bool matched[kPix], is_new[kPix];
 #pragma unroll
   for (int j = 0; j < kPix; ++j) {
     pix[j] = pix0 + j * kMB + threadIdx.x;
-    U128 rec{0ull, 0ull};
+    slot[j] = 0u;
     dep[j] = 0.0f;
     if (pix[j] < P) {
-      rec = best[pix[j]];
+      slot[j] = win[pix[j]];
       dep[j] = frame_depth(s_hdr, s_hdr.from_maps, nrec, pix[j]);
     }
-    matched[j] = a.with_cc && ((rec.lo | rec.hi) != 0ull);
-    rec_lo[j] = rec.lo;
+    matched[j] = a.with_cc && slot[j] != 0u;
     if (matched[j]) {  // the matched row's geometry and colour sectors, gathered below
-      const int64_t n = (int64_t)(~rec.lo);
+      const int64_t n = (int64_t)slot[j] - 1;
       prefetch_l2(a.geo + ((int64_t)b * a.cap + n) * kGeoW);
       prefetch_l2(a.col + ((int64_t)b * a.cap + n) * kColW);
     }
@@ -408,7 +412,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
 #pragma unroll
   for (int j = 0; j < kPix; ++j) {
     if (matched[j]) {
-      const int64_t n = (int64_t)(~rec_lo[j]);
+      const int64_t n = (int64_t)slot[j] - 1;
       g0[j] = *reinterpret_cast<const float4 *>(geo + n * kGeoW);
       g1[j] = *reinterpret_cast<const float4 *>(geo + n * kGeoW + 4);
       c4[j] = *reinterpret_cast<const float4 *>(col + n * kColW);
@@ -418,7 +422,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   for (int j = 0; j < kPix; ++j) {
     if (matched[j]) {
       // confidence-weighted running mean (fusionutils.py:678-699); exactly one pixel owns this map row
-      const int64_t n = (int64_t)(~rec_lo[j]);
+      const int64_t n = (int64_t)slot[j] - 1;
       const float alpha = fv[j].w;
       const float c0 = g1[j].z;
       const float tot = c0 + alpha;
@@ -627,7 +631,7 @@ static Workspace group_workspace(void *workspace, int B_total, int b0, int H, in
   ws.nrec += (int64_t)b0 * P;
   ws.vrec += (int64_t)b0 * P;
   ws.hdr += b0;
-  ws.best += (int64_t)b0 * P;
+  ws.win += (int64_t)b0 * P;
   ws.tile_state += (int64_t)b0 * ws.tiles;
   ws.ticket += b0;
   ws.stats += 2 * b0;
@@ -651,7 +655,7 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
   if (max_count > 0) {
     ProjectArgs pa{ggeo, cin + b0, cap, poses + (int64_t)b0 * pose_bs, pose_bs, K + (int64_t)b0 * K_bs, K_bs, nb,
-                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.best, ws.stats};
+                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.win, ws.stats};
     const int rc = launch_project_select(pa, max_count, st);
     if (rc) return rc;
   }
@@ -710,7 +714,7 @@ extern "C" int gsx_fusion_project_select(const float *map_geometry, const int32_
                 (long long)max_count, (long long)capacity);
   const Workspace ws = fusion_workspace(workspace, B, H, W);
   ProjectArgs a{map_geometry, counts, capacity, poses, pose_bstride, intrinsics, K_bstride, B, image_bounds(H, W),
-                dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.best, ws.stats};
+                dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.win, ws.stats};
   return launch_project_select(a, max_count, (cudaStream_t)stream);
 }
 

@@ -26,7 +26,7 @@ struct FrameHeader {
 //   float4 nrec[B][P]          (gnx,gny,gnz,depth), only for caller-supplied maps               written by K1r
 //   float4 vrec[B][P]          (gvx,gvy,gvz,alpha), only for caller-supplied maps               written by K1r
 //   FrameHeader hdr[B]         where the depth is, how to re-evaluate vertex / normal / weight  written by K1r
-//   U128   best[B][P]          complemented arg-min records (0 = empty)                         cleared by K1r
+//   uint32 win[B][P]           arg-min slot: n + 1 of the winning row, 0 = none                  cleared by K1r
 //   uint64 tile_state[B][T]    look-back state of K4's scan (epoch 1), T = ceil(P / kTilePix)  cleared by K1r
 //   uint32 ticket[B]           dynamic tile ids of K4                                           cleared by K1r
 //   uint64 stats[B][2]         running totals: {active map rows (in frustum), merged rows}      caller zeroes once
@@ -35,7 +35,7 @@ struct FrameHeader {
 struct Workspace {
   float4 *nrec, *vrec;
   FrameHeader *hdr;
-  U128 *best;
+  unsigned int *win;
   unsigned long long *tile_state;
   unsigned int *ticket;
   unsigned long long *stats;
@@ -51,7 +51,7 @@ inline Workspace fusion_workspace(void *base, int B, int H, int W, int64_t *byte
   w.nrec = c.take<float4>(B * P);
   w.vrec = c.take<float4>(B * P);
   w.hdr = c.take<FrameHeader>(B);
-  w.best = c.take<U128>(B * P);
+  w.win = c.take<unsigned int>(B * P);
   w.tile_state = c.take<unsigned long long>((int64_t)B * w.tiles);
   w.ticket = c.take<unsigned int>(B);
   w.stats = c.take<unsigned long long>(2 * (int64_t)B);

@@ -4,7 +4,7 @@
 // (gsx_fusion.cu) but materialise flags / per-pixel winners so the host can hand out int64 (N,4) tables.
 //   k_active_eval        per map slot (b,n): frustum test + pixel                       -> flag, h, w
 //   k_similar_eval       per table row: distance + normal test against the frame maps  -> flag
-//   k_unique_select      per table row: 128-bit arg-min per pixel (same key as K2/K3)
+//   k_unique_select      per table row: arg-min per pixel (same key and device functions as K2/K3)
 //   k_unique_emit        per pixel: winner present? which n?                            -> flag, n   (and clears)
 //   k_records_from_table per table row: store the row as the pixel's winner (input of K4 for fuse_with_map)
 //   k_compact            generic stable compaction flag[] -> ascending indices (single-pass decoupled look-back)
@@ -101,7 +101,7 @@ struct RowArgs {
   int B, H, W;
   float d2_max, dot_th;  // sqrtf(d2) < dist_th  <=>  d2 <= d2_max (gsx_thresholds.h)
   uint8_t *flags;  // (rows)            k_similar_eval
-  U128 *best;      // (B,H,W)           k_unique_select / k_records_from_table
+  unsigned int *win;  // (B,H,W) arg-min slots: k_unique_select / k_records_from_table
 };
 
 __device__ __forceinline__ bool row_ok(const RowArgs &a, int64_t b, int64_t n, int64_t h, int64_t w) {
@@ -131,12 +131,12 @@ __global__ void __launch_bounds__(kTB) k_unique_select(RowArgs a) {
   if (r >= a.rows) return;
   const int64_t b = a.table[r * 4], n = a.table[r * 4 + 1], h = a.table[r * 4 + 2], w = a.table[r * 4 + 3];
   if (!row_ok(a, b, n, h, w)) return;
-  const float *p = a.geo + (b * a.cap + n) * kGeoW;
+  const float *geo = a.geo + b * a.cap * kGeoW, *p = geo + n * kGeoW;
   const float *g = a.gv + ((b * a.H + h) * a.W + w) * 3;
-  // key (1/(cc+1e-20), (map - frame)^2 summed left to right, n)
-  const float dx = __ldg(p) - __ldg(g), dy = __ldg(p + 1) - __ldg(g + 1), dz = __ldg(p + 2) - __ldg(g + 2);
-  const float d2 = (dx * dx + dy * dy) + dz * dz;
-  atomic_min_key128(a.best + (b * a.H + h) * a.W + w, argmin_key_hi(__ldg(p + 6), d2), (unsigned long long)n);
+  const float3 fv = make_float3(__ldg(g), __ldg(g + 1), __ldg(g + 2));
+  const unsigned long long key = argmin_key_hi(__ldg(p + 6), ray_d2(fv, __ldg(p), __ldg(p + 1), __ldg(p + 2)));
+  unsigned int *slot = a.win + (b * a.H + h) * a.W + w;
+  argmin_settle(slot, (unsigned int)n, key, fv, geo, argmin_claim(slot, (unsigned int)n));
 }
 
 __global__ void __launch_bounds__(kTB) k_records_from_table(RowArgs a) {
@@ -144,17 +144,17 @@ __global__ void __launch_bounds__(kTB) k_records_from_table(RowArgs a) {
   if (r >= a.rows) return;
   const int64_t b = a.table[r * 4], n = a.table[r * 4 + 1], h = a.table[r * 4 + 2], w = a.table[r * 4 + 3];
   if (!row_ok(a, b, n, h, w)) return;
-  a.best[(b * a.H + h) * a.W + w] = U128{~(unsigned long long)n, ~0ull >> 1};  // non-zero record holding n
+  a.win[(b * a.H + h) * a.W + w] = (unsigned int)n + 1u;
 }
 
 // per pixel: is there a winner?  which map row?
-__global__ void __launch_bounds__(kTB) k_unique_emit(const U128 *best, int64_t pixels, uint8_t *flags, int64_t *n_out) {
+__global__ void __launch_bounds__(kTB) k_unique_emit(const unsigned int *win, int64_t pixels, uint8_t *flags,
+                                                     int64_t *n_out) {
   const int64_t i = (int64_t)blockIdx.x * kTB + threadIdx.x;
   if (i >= pixels) return;
-  const U128 rec = best[i];
-  const bool has = (rec.lo | rec.hi) != 0ull;
-  flags[i] = has ? 1 : 0;
-  n_out[i] = has ? (int64_t)(~rec.lo) : -1;
+  const unsigned int v = win[i];
+  flags[i] = v != 0u ? 1 : 0;
+  n_out[i] = (int64_t)v - 1;
 }
 
 }  // namespace gsx
@@ -214,21 +214,23 @@ extern "C" int gsx_similar_eval(const int64_t *table, int64_t rows, const float 
   return 0;
 }
 
-// `records`: B*H*W 16-byte arg-min records (scratch; cleared here)
+// `records`: B*H*W 4-byte arg-min slots (scratch; cleared here)
 extern "C" int gsx_unique_select(const int64_t *table, int64_t rows, const float *map_geometry, int64_t capacity,
                                  const float *gvertex, int B, int H, int W, void *records, uint8_t *pixel_flags,
                                  int64_t *pixel_n, void *stream) {
   GSX_CHECK_ARG(records && pixel_flags && pixel_n, "gsx_unique_select: null pointer");
-  GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(records) & 15) == 0, "gsx_unique_select: records must be 16-byte aligned");
+  GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(records) & 3) == 0, "gsx_unique_select: records must be 4-byte aligned");
+  GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_unique_select: capacity must fit int32");
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t pixels = (int64_t)B * H * W;
-  cudaMemsetAsync(records, 0, (size_t)pixels * 16, s);
+  cudaMemsetAsync(records, 0, (size_t)pixels * 4, s);
   if (rows > 0) {
     GSX_CHECK_ARG(table && map_geometry && gvertex, "gsx_unique_select: null pointer");
-    RowArgs a{table, rows, map_geometry, capacity, gvertex, nullptr, B, H, W, 0.f, 0.f, nullptr, (U128 *)records};
+    RowArgs a{table, rows, map_geometry, capacity, gvertex, nullptr, B, H, W, 0.f, 0.f, nullptr,
+              (unsigned int *)records};
     k_unique_select<<<(unsigned)tb_blocks(rows), kTB, 0, s>>>(a);
   }
-  k_unique_emit<<<(unsigned)tb_blocks(pixels), kTB, 0, s>>>((const U128 *)records, pixels, pixel_flags, pixel_n);
+  k_unique_emit<<<(unsigned)tb_blocks(pixels), kTB, 0, s>>>((const unsigned int *)records, pixels, pixel_flags, pixel_n);
   GSX_CHECK_LAUNCH("gsx_unique_select");
   return 0;
 }
@@ -239,8 +241,9 @@ extern "C" int gsx_records_from_table(const int64_t *table, int64_t rows, int64_
                                       void *workspace, void *stream) {
   if (rows == 0) return 0;
   GSX_CHECK_ARG(table && workspace, "gsx_records_from_table: null pointer");
+  GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_records_from_table: capacity must fit int32");
   RowArgs a{table, rows, nullptr, capacity, nullptr, nullptr, B, H, W, 0.f, 0.f, nullptr,
-            fusion_workspace(workspace, B, H, W).best};
+            fusion_workspace(workspace, B, H, W).win};
   k_records_from_table<<<(unsigned)tb_blocks(rows), kTB, 0, (cudaStream_t)stream>>>(a);
   GSX_CHECK_LAUNCH("gsx_records_from_table");
   return 0;

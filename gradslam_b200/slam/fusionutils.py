@@ -75,7 +75,7 @@ def are_normals_similar(tensor1: torch.Tensor, tensor2: torch.Tensor, dot_th: Un
 
 # --------------------------------------------------------------------------------------------- workspaces
 class _Workspace:
-    """Per (device, stream, B, H, W) scratch of the fusion kernels: frame records, arg-min records, scan state.  Nothing
+    """Per (device, stream, B, H, W) scratch of the fusion kernels: frame records, arg-min slots, scan state.  Nothing
     in it survives from frame to frame (gsx_fusion_frame_records re-arms it), so there is no epoch or "left clean"
     invariant to break; it is keyed by the CUDA stream as well, so maps updated concurrently from different streams or
     threads never share records."""
@@ -337,7 +337,7 @@ def find_best_unique_correspondences(pointclouds: Pointclouds, rgbdimages: RGBDI
                                      pc2im_bnhw: torch.Tensor) -> torch.Tensor:
     """One row per live pixel: among the candidates of a pixel keep the largest confidence count, then the
     smallest ray distance, then the smallest index.  Output sorted by (b, h, w) (fusionutils.py:414-546); the
-    reference's torch.unique(dim=0) row sort becomes a per-pixel 128-bit atomic arg-min."""
+    reference's torch.unique(dim=0) row sort becomes a per-pixel atomic arg-min."""
     _check_pc(pointclouds)
     _check_table(pc2im_bnhw)
     if rgbdimages.shape[1] != 1:
@@ -356,7 +356,7 @@ def find_best_unique_correspondences(pointclouds: Pointclouds, rgbdimages: RGBDI
         raise ValueError("Pointclouds features must be a single confidence count per point.")
     gv = frames.global_vertex_map.contiguous()
     geo = _dense(pointclouds._geo, "pointclouds (geometry rows)", device)
-    records = torch.empty(B * H * W * 2, dtype=torch.int64, device=device)  # 16-byte arg-min records (scratch)
+    records = torch.empty(B * H * W, dtype=torch.int32, device=device)  # 4-byte arg-min slots (scratch)
     pflags = torch.empty(B * H * W, dtype=torch.uint8, device=device)
     pn = torch.empty(B * H * W, dtype=torch.int64, device=device)
     _C.launch("gsx_unique_select", table, table.shape[0], geo, pointclouds.capacity, gv, B, H, W, records, pflags, pn)

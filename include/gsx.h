@@ -71,7 +71,7 @@ int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const
  *   K1r  gsx_fusion_frame_records    re-arms the workspace for this frame and records where its depth image and camera
  *                                    are (from depth nothing per pixel is stored: K2 and K4 re-evaluate the world
  *                                    vertex, world normal and confidence weight from the depth where they need them)
- *   K2   gsx_fusion_project_select   per map row: projection, tests, per-pixel 128-bit arg-min
+ *   K2   gsx_fusion_project_select   per map row: projection, tests, per-pixel atomic arg-min
  *   K4   gsx_fusion_merge_append     per pixel: merge the selected row or append a new surfel
  * replaces update_map_fusion = find_active_map_points + find_similar_map_points +
  *          find_best_unique_correspondences + fuse_with_map (+ Pointclouds.append_points)
@@ -103,8 +103,8 @@ int gsx_fusion_frame_records(const float *depth, int64_t depth_bstride, const fl
 
 /* K2+K3: project every map point into the live camera, keep points that are in the frustum, close to
  * the frame vertex they land on and with a similar normal, and reduce per pixel to the best candidate
- * (largest confidence count, then smallest ray distance, then smallest index) with a 128-bit atomic
- * min.  max_count = host upper bound on counts[b] (sizes the grid).  The frame records of the live frame must be in
+ * (largest confidence count, then smallest ray distance, then smallest index) with an atomic arg-min on a
+ * 4-byte slot per pixel that holds the winning row.  max_count = host upper bound on counts[b] (sizes the grid).  The frame records of the live frame must be in
  * the workspace (gsx_fusion_frame_records), and the depth it was given still valid. */
 int gsx_fusion_project_select(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                               const float *poses, int64_t pose_bstride, const float *intrinsics, int64_t K_bstride,
@@ -263,14 +263,14 @@ int gsx_similar_eval(const int64_t *table, int64_t rows, const float *map_geomet
                      uint8_t *flags, void *stream);
 
 /* per pixel winner among the table rows (largest ccount, then smallest ray distance, then smallest n):
- * pixel_flags (B*H*W) and pixel_n (B*H*W, -1 if none).  records: scratch of B*H*W 16-byte records, 16-byte
- * aligned (cleared by the call). */
+ * pixel_flags (B*H*W) and pixel_n (B*H*W, -1 if none).  records: scratch of B*H*W 4-byte slots, 4-byte aligned
+ * (cleared by the call).  capacity < 2^31. */
 int gsx_unique_select(const int64_t *table, int64_t rows, const float *map_geometry, int64_t capacity,
                       const float *gvertex, int B, int H, int W, void *records, uint8_t *pixel_flags,
                       int64_t *pixel_n, void *stream);
 
 /* stores every table row as its pixel's winner in the fusion workspace: call it AFTER gsx_fusion_frame_records
- * (which re-arms the workspace) and BEFORE gsx_fusion_merge_append. */
+ * (which re-arms the workspace) and BEFORE gsx_fusion_merge_append.  capacity < 2^31. */
 int gsx_records_from_table(const int64_t *table, int64_t rows, int64_t capacity, int B, int H, int W,
                            void *workspace, void *stream);
 
