@@ -57,6 +57,7 @@ SIGNATURES = {
                 c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_vp, c_vp]),
     "gsx_debug_fail_at_frame": (None, [c_int]),
     "gsx_debug_set_k2_grid_cap": (None, [c_int]),
+    "gsx_debug_set_bin_capacity": (None, [c_int]),
     "gsx_peer_export": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "gsx_peer_open": (c_int, [c_vp, c_i64, c_vp]),
     "gsx_peer_close_all": (c_int, []),

@@ -5,10 +5,12 @@
 //                              (fusionutils.py:16-73) from the pixel's depth stencil, bit for bit.  Caller-supplied maps
 //                              (differentiable mode) are packed into per-pixel records instead.
 //   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, gather of the depth
-//                              stencil under the projection, distance / normal tests, then an atomic arg-min per
-//                              pixel on the key (1/ccount, ray distance, row index) into a 4-byte slot holding the
-//                              winning row (argmin_claim / argmin_settle, gsx_common.cuh).
-//   k_merge_append    (K4)     one thread per pixel: confidence-weighted merge of the selected map row, or stable append of
+//                              stencil under the projection, distance / normal tests, then each live candidate, with
+//                              its key (1/ccount, ray distance, row index), is appended to the bin of the K4 tile that
+//                              owns its pixel (a full bin sends it to the pixel's 4-byte arg-min slot instead:
+//                              argmin_claim / argmin_settle, gsx_common.cuh).
+//   k_merge_append    (K4)     per tile, the arg-min of its binned candidates in shared memory, combined with the slots;
+//                              then one thread per pixel: confidence-weighted merge of the selected map row, or stable append of
 //                              unmatched valid pixels (single-pass decoupled look-back scan, row-major order per batch
 //                              element).  No float atomics anywhere.
 // Map rows are sector-packed (DESIGN.md section 2): geometry rows (px,py,pz,nx,ny,nz,ccount,0) of exactly one 32-byte
@@ -109,7 +111,10 @@ __global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records(FrameRecArgs a
   const int tid = threadIdx.y * kRecTW + threadIdx.x;
   // re-arm the scan state of this element for the frame's K4
   const int lin = (blockIdx.y * gridDim.x + blockIdx.x) * (kRecTW * kRecTH) + tid;
-  if (lin < a.ws.tiles) a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
+  if (lin < a.ws.tiles) {
+    a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
+    a.ws.bin_count[(int64_t)b * a.ws.tiles + lin] = 0u;
+  }
   if (lin == 0) {
     a.ws.ticket[b] = 0u;
     store_frame_header(a, b);
@@ -159,12 +164,15 @@ struct ProjectArgs {
   const FrameHeader *hdr;
   unsigned int *win;
   unsigned long long *stats;
+  unsigned int *bin_count;  // (B,T) and (B,T,kBinCap): the candidate bins of K4's tiles
+  uint4 *bin;
+  int tiles;
+  int bin_cap;  // records per bin that K2 fills (<= kBinCap)
 };
 
-// 4 CTAs/SM: the loop holds the normal's re-evaluation; at 5 CTAs/SM (48 registers) it spills 24 bytes
-// (DESIGN.md section 4)
+// 5 CTAs/SM (48 registers, no spill; DESIGN.md section 4)
 #ifndef GSX_K2_MINB
-#define GSX_K2_MINB 4
+#define GSX_K2_MINB 5
 #endif
 
 struct MapRow {  // one geometry row
@@ -184,9 +192,30 @@ __device__ __forceinline__ MapRow load_map_row(const float *geo, int64_t n) {
 //     image, 1.2 MB per element, stays in L2) and re-evaluate K1's world vertex and world normal from it;
 //   * sqrtf(d2) < dist_th is decided as d2 <= d2_max (exact: the correctly rounded square root is monotonic; the
 //     threshold is found on the host, gsx_thresholds.h);
-//   * the result of the arg-min CAS is only looked at one iteration later.
+//   * a live candidate is not resolved here: it is appended to the bin of the K4 tile that owns its pixel, with one
+//     atomicAdd per group of lanes that hit the same tile, and K4 takes the arg-min in shared memory (append_candidate).
 // The grid-stride loop of one CTA over element b's rows; the record kind is a template argument so that each of the two
 // loops only holds the registers of its own kind.
+// Appends candidate row n of pixel pix (key (key_hi, n)) to the bin of the pixel's K4 tile.  The lanes of a warp that
+// hit the same tile share one atomicAdd on the tile's count; each lane then stores its 16-byte record.  A lane whose
+// slot lies past the bin's capacity resolves its candidate on the pixel's arg-min slot instead, as the table API
+// does; the count keeps growing, so K4 knows the tile overflowed.
+__device__ __forceinline__ void append_candidate(unsigned int *bin_count, uint4 *bin, int bin_cap, unsigned int *win,
+                                                 const float *geo, int pix, unsigned int n,
+                                                 unsigned long long key_hi, const float3 &fv) {
+  const int t = pix / kTilePix;
+  const unsigned int grp = __match_any_sync(__activemask(), t);
+  const int lane = (int)(threadIdx.x & 31), leader = __ffs(grp) - 1;
+  unsigned int base = 0u;
+  if (lane == leader) base = atomicAdd(bin_count + t, (unsigned int)__popc(grp));
+  const unsigned int s = __shfl_sync(grp, base, leader) + (unsigned int)__popc(grp & ((1u << lane) - 1u));
+  if (s < (unsigned int)bin_cap)
+    bin[(int64_t)t * kBinCap + s] =
+        make_uint4((unsigned int)key_hi, (unsigned int)(key_hi >> 32), n, (unsigned int)(pix - t * kTilePix));
+  else
+    argmin_settle(win + pix, n, key_hi, fv, geo, argmin_claim(win + pix, n));
+}
+
 template <bool kFromMaps>
 __device__ __forceinline__ void select_rows(const ProjectArgs &a, const LiveCamera &s_cam, const FrameHeader &s_hdr,
                                             unsigned int *s_act, int b, int count) {
@@ -194,13 +223,10 @@ __device__ __forceinline__ void select_rows(const ProjectArgs &a, const LiveCame
   const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   const float4 *nrec = a.nrec + (int64_t)b * P, *vrec = a.vrec + (int64_t)b * P;
   unsigned int *win = a.win + (int64_t)b * P;
+  unsigned int *bin_count = a.bin_count + (int64_t)b * a.tiles;
+  uint4 *bin = a.bin + (int64_t)b * a.tiles * kBinCap;
   const int64_t stride = (int64_t)gridDim.x * kBlock;
   int64_t n = (int64_t)blockIdx.x * kBlock + threadIdx.x;
-  // the pending candidate: its pixel, row, key, the pixel's frame vertex and what its claim returned
-  int pend_pix = -1;
-  unsigned int pend_n = 0u, pend_old = 0u;
-  unsigned long long pend_key = 0ull;
-  float3 pend_fv = make_float3(0.f, 0.f, 0.f);
   MapRow cur = load_map_row(geo, n < count ? n : 0);
   for (; n < count; n += stride) {
     const MapRow m = cur;
@@ -223,20 +249,10 @@ __device__ __forceinline__ void select_rows(const ProjectArgs &a, const LiveCame
       const float3 fv3 = make_float3(fv.x, fv.y, fv.z);
       const float d2 = ray_d2(fv3, m.a.x, m.a.y, m.a.z);
       const bool live = (d2 <= a.d2_max) && (dot > a.dot_th);
-      if (pend_pix >= 0) {  // settle the previous candidate's CAS before re-using the registers
-        argmin_settle(win + pend_pix, pend_n, pend_key, pend_fv, geo, pend_old);
-        pend_pix = -1;
-      }
-      if (live) {
-        pend_n = (unsigned int)n;
-        pend_key = argmin_key_hi(m.b.z, d2);
-        pend_fv = fv3;
-        pend_old = argmin_claim(win + pix, pend_n);
-        pend_pix = pix;
-      }
+      if (live)
+        append_candidate(bin_count, bin, a.bin_cap, win, geo, pix, (unsigned int)n, argmin_key_hi(m.b.z, d2), fv3);
     }
   }
-  if (pend_pix >= 0) argmin_settle(win + pend_pix, pend_n, pend_key, pend_fv, geo, pend_old);
 }
 
 __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectArgs a) {
@@ -274,8 +290,15 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
 // passes.  0 = the shipped cap below.
 static int g_k2_grid_cap = 0;
 
-int launch_project_select(const ProjectArgs &a, int64_t max_count, cudaStream_t stream) {
-  if (a.B == 0 || max_count <= 0) return 0;
+// Test hook (tests/test_gpu_binned_argmin.py): caps the records per candidate bin that K2 fills and K4 reads, so that
+// small frames exercise the overflow to the arg-min slots.  Negative = kBinCap.
+static int g_bin_cap = -1;
+static int bin_capacity() { return g_bin_cap >= 0 && g_bin_cap < kBinCap ? g_bin_cap : kBinCap; }
+
+int launch_project_select(const ProjectArgs &args, int64_t max_count, cudaStream_t stream) {
+  if (args.B == 0 || max_count <= 0) return 0;
+  ProjectArgs a = args;
+  a.bin_cap = bin_capacity();
   int64_t bx = (max_count + kBlock - 1) / kBlock;
   // grid-stride beyond this many CTAs per SM
   const int64_t cap_blocks = g_k2_grid_cap > 0 ? (int64_t)g_k2_grid_cap : (int64_t)kNumSMs * GSX_K2_CTAS_PER_SM;
@@ -299,6 +322,7 @@ struct MergeArgs {
   Workspace ws;
   int32_t *overflow;
   int32_t *assoc;  // optional (B,P): +row+1 appended at `row`, -(row+1) merged into `row`, 0 untouched
+  int bin_cap;     // records per candidate bin that K2 filled (set at launch)
 };
 
 // K1r zeroes K4's tile states before every frame, so K4's scan always runs in epoch 1
@@ -322,11 +346,18 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   __shared__ int s_excl;
   __shared__ __align__(16) float s_rgb[kTilePix * 3];
   __shared__ FrameHeader s_hdr;
+  // the tile's arg-min over its binned candidates: per pixel the smallest key_hi, then the smallest n of that key
+  __shared__ unsigned long long s_key[kTilePix];
+  __shared__ unsigned int s_n[kTilePix];
   // batch element varies fastest in the grid: CTAs resident at the same time belong to different elements, so
   // each element's look-back chain only sees ~1/B of the in-flight tiles
   const int b = blockIdx.x % a.B;
   const int T = a.ws.tiles;
   if (threadIdx.x == 0) s_tile = (int)atomicAdd(a.ws.ticket + b, 1u);  // tiles start in ticket order
+  for (int i = threadIdx.x; i < kTilePix; i += kMB) {
+    s_key[i] = ~0ull;
+    s_n[i] = ~0u;
+  }
   load_frame_header(s_hdr, a.ws.hdr + b);
   const int count_in = a.counts_in[b];  // loaded early: its latency hides behind everything below
   __syncthreads();
@@ -337,6 +368,8 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   const unsigned int *win = a.ws.win + (int64_t)b * P;
   const float4 *nrec = a.ws.nrec + (int64_t)b * P, *vrec = a.ws.vrec + (int64_t)b * P;
   const float *rgb = a.rgb + b * a.rgb_bstride + (int64_t)pix0 * 3;
+  const int n_bin = (int)min(a.ws.bin_count[(int64_t)b * T + tile], (unsigned int)a.bin_cap);
+  const uint4 *bin = a.ws.bin + ((int64_t)b * T + tile) * kBinCap;
 
   // live colours of the tile: coalesced 128-bit loads into shared memory (stride-3 reads are conflict free)
   const int tile_px = min(kTilePix, P - pix0);
@@ -350,7 +383,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   }
 
   int pix[kPix];
-  unsigned int slot[kPix];  // arg-min slot: the matched map row + 1
+  unsigned int slot[kPix];  // the matched map row + 1, 0 for none
   float dep[kPix];
   bool matched[kPix], is_new[kPix];
 #pragma unroll
@@ -361,6 +394,51 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
     if (pix[j] < P) {
       slot[j] = win[pix[j]];
       dep[j] = frame_depth(s_hdr, s_hdr.from_maps, nrec, pix[j]);
+    }
+  }
+
+  // arg-min of the binned candidates, (key_hi, n) lexicographic: the smallest key_hi per pixel, then the smallest n
+  // among the records that carry it.  All of a thread's records are loaded at once and kept for the second pass.
+  static_assert(kBinCap % kMB == 0, "a bin is read in whole rounds of the CTA");
+  constexpr int kRec = kBinCap / kMB;
+  uint4 rec[kRec];
+#pragma unroll
+  for (int k = 0; k < kRec; ++k) {
+    const int i = k * kMB + (int)threadIdx.x;
+    if (i < n_bin) rec[k] = __ldg(bin + i);
+  }
+#pragma unroll
+  for (int k = 0; k < kRec; ++k)
+    if (k * kMB + (int)threadIdx.x < n_bin) atomicMin(s_key + rec[k].w, ((unsigned long long)rec[k].y << 32) | rec[k].x);
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < kRec; ++k)
+    if (k * kMB + (int)threadIdx.x < n_bin &&
+        (((unsigned long long)rec[k].y << 32) | rec[k].x) == s_key[rec[k].w])
+      atomicMin(s_n + rec[k].w, rec[k].z);
+  __syncthreads();
+
+#pragma unroll
+  for (int j = 0; j < kPix; ++j) {
+    const int q = j * kMB + (int)threadIdx.x;
+    const unsigned int bn = s_n[q];
+    if (bn != ~0u) {
+      if (slot[j] == 0u) {
+        slot[j] = bn + 1u;
+      } else {
+        // the pixel also has a winner in its arg-min slot (a bin that overflowed, or gsx_records_from_table): that
+        // row's key, recomputed from the pixel's frame vertex as argmin_settle does, decides
+        const int ph = pix[j] / a.W;
+        float3 gn;
+        float4 fv;
+        frame_values<false>(s_hdr, s_hdr.from_maps, s_hdr.cam.posed ? &s_hdr.cam.pose : nullptr, nrec, vrec, ph,
+                            pix[j] - ph * a.W, a.H, a.W, dep[j], gn, fv);
+        const unsigned int m = slot[j] - 1u;
+        const float4 p = *reinterpret_cast<const float4 *>(a.geo + ((int64_t)b * a.cap + m) * kGeoW);
+        const unsigned long long k = argmin_key_hi(a.geo[((int64_t)b * a.cap + m) * kGeoW + 6],
+                                                   ray_d2(make_float3(fv.x, fv.y, fv.z), p.x, p.y, p.z));
+        if (!(k < s_key[q] || (k == s_key[q] && m < bn))) slot[j] = bn + 1u;
+      }
     }
     matched[j] = a.with_cc && slot[j] != 0u;
     if (matched[j]) {  // the matched row's geometry and colour sectors, gathered below
@@ -478,8 +556,10 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   }
 }
 
-int launch_merge_append(const MergeArgs &a, cudaStream_t stream) {
-  if (a.B == 0) return 0;
+int launch_merge_append(const MergeArgs &args, cudaStream_t stream) {
+  if (args.B == 0) return 0;
+  MergeArgs a = args;
+  a.bin_cap = bin_capacity();
   const dim3 grid((unsigned)(a.ws.tiles * a.B));
   if (a.assoc)
     k_merge_append<true><<<grid, kMB, 0, stream>>>(a);  // differentiable forward
@@ -633,6 +713,8 @@ static Workspace group_workspace(void *workspace, int B_total, int b0, int H, in
   ws.hdr += b0;
   ws.win += (int64_t)b0 * P;
   ws.tile_state += (int64_t)b0 * ws.tiles;
+  ws.bin_count += (int64_t)b0 * ws.tiles;
+  ws.bin += (int64_t)b0 * ws.tiles * kBinCap;
   ws.ticket += b0;
   ws.stats += 2 * b0;
   return ws;
@@ -655,11 +737,11 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
   if (max_count > 0) {
     ProjectArgs pa{ggeo, cin + b0, cap, poses + (int64_t)b0 * pose_bs, pose_bs, K + (int64_t)b0 * K_bs, K_bs, nb,
-                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.win, ws.stats};
+                   image_bounds(H, W), dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.win, ws.stats, ws.bin_count, ws.bin, ws.tiles, 0};
     const int rc = launch_project_select(pa, max_count, st);
     if (rc) return rc;
   }
-  MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow, nullptr};
+  MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow, nullptr, 0};
   return launch_merge_append(ma, st);
 }
 
@@ -714,11 +796,13 @@ extern "C" int gsx_fusion_project_select(const float *map_geometry, const int32_
                 (long long)max_count, (long long)capacity);
   const Workspace ws = fusion_workspace(workspace, B, H, W);
   ProjectArgs a{map_geometry, counts, capacity, poses, pose_bstride, intrinsics, K_bstride, B, image_bounds(H, W),
-                dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.win, ws.stats};
+                dot_th, sqrt_lt_threshold(dist_th), ws.nrec, ws.vrec, ws.hdr, ws.win, ws.stats, ws.bin_count, ws.bin, ws.tiles, 0};
   return launch_project_select(a, max_count, (cudaStream_t)stream);
 }
 
 extern "C" void gsx_debug_set_k2_grid_cap(int ctas) { g_k2_grid_cap = ctas > 0 ? ctas : 0; }
+
+extern "C" void gsx_debug_set_bin_capacity(int records) { g_bin_cap = records >= 0 ? records : -1; }
 
 extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_ccounts,
                                        const int32_t *counts_in, int32_t *counts_out, int64_t capacity,
@@ -733,7 +817,7 @@ extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, i
                 "gsx_fusion_merge_append: map rows and workspace must be 16-byte aligned");
   GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_merge_append: capacity must fit int32 (counts are int32)");
   MergeArgs a{map_geometry, map_colors, with_ccounts ? 1 : 0, counts_in, counts_out, capacity, rgb, rgb_bstride, B, H,
-              W, fusion_workspace(workspace, B, H, W), overflow_flag, assoc_out};
+              W, fusion_workspace(workspace, B, H, W), overflow_flag, assoc_out, 0};
   return launch_merge_append(a, (cudaStream_t)stream);
 }
 

@@ -71,14 +71,17 @@ int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const
  *   K1r  gsx_fusion_frame_records    re-arms the workspace for this frame and records where its depth image and camera
  *                                    are (from depth nothing per pixel is stored: K2 and K4 re-evaluate the world
  *                                    vertex, world normal and confidence weight from the depth where they need them)
- *   K2   gsx_fusion_project_select   per map row: projection, tests, per-pixel atomic arg-min
- *   K4   gsx_fusion_merge_append     per pixel: merge the selected row or append a new surfel
+ *   K2   gsx_fusion_project_select   per map row: projection, tests; live candidates go to the bin of their pixel's
+ *                                    K4 tile
+ *   K4   gsx_fusion_merge_append     per pixel: arg-min over the tile's bin, merge the selected row or append a new
+ *                                    surfel
  * replaces update_map_fusion = find_active_map_points + find_similar_map_points +
  *          find_best_unique_correspondences + fuse_with_map (+ Pointclouds.append_points)
  *          gradslam/slam/fusionutils.py:198-287, 290-411, 414-546, 580-722, 761-789;
  *          gradslam/structures/pointclouds.py:526-614, 1117-1237
  *
- * Workspace: gsx_fusion_workspace_bytes(B,H,W) bytes, 16-byte aligned.  Nothing in it has to survive from one frame
+ * Workspace: gsx_fusion_workspace_bytes(B,H,W) bytes, 16-byte aligned (B * ceil(H*W/512) candidate bins of 16 KB
+ * each, per-pixel arg-min slots and frame records: about 167 MB at B=8, 640x480).  Nothing in it has to survive from one frame
  * to the next: gsx_fusion_frame_records re-arms everything the other two kernels consume, so no zero-fill and no
  * epoch bookkeeping is needed and an abandoned frame cannot poison the next one.  (Only the statistics below
  * accumulate; zero them once if they are read.)                                                            */
@@ -103,8 +106,9 @@ int gsx_fusion_frame_records(const float *depth, int64_t depth_bstride, const fl
 
 /* K2+K3: project every map point into the live camera, keep points that are in the frustum, close to
  * the frame vertex they land on and with a similar normal, and reduce per pixel to the best candidate
- * (largest confidence count, then smallest ray distance, then smallest index) with an atomic arg-min on a
- * 4-byte slot per pixel that holds the winning row.  max_count = host upper bound on counts[b] (sizes the grid).  The frame records of the live frame must be in
+ * (largest confidence count, then smallest ray distance, then smallest index): each candidate is appended to the
+ * workspace's bin of its pixel's 512-pixel tile, which gsx_fusion_merge_append reduces in shared memory (a candidate
+ * that finds its bin full takes an atomic arg-min on a 4-byte slot per pixel instead).  max_count = host upper bound on counts[b] (sizes the grid).  The frame records of the live frame must be in
  * the workspace (gsx_fusion_frame_records), and the depth it was given still valid. */
 int gsx_fusion_project_select(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                               const float *poses, int64_t pose_bstride, const float *intrinsics, int64_t K_bstride,
@@ -198,6 +202,9 @@ void gsx_debug_fail_at_frame(int s);
 /* test hook: caps the total CTA count of the map projection kernel (K2), so that small maps take several grid-stride
  * passes; 0 = the default cap.  Results do not depend on it. */
 void gsx_debug_set_k2_grid_cap(int ctas);
+/* test hook: caps the candidate records per K4 tile that K2 bins and K4 reads (0 = every candidate takes the per-pixel
+ * arg-min slot); negative = the built-in capacity.  Results do not depend on it. */
+void gsx_debug_set_bin_capacity(int records);
 
 /* ------------------------------------------------------------------------------------------------
  * Map exchange between the GPUs of a node through peer memory (SURVEY.md section 8e "Collective": the variable-length
