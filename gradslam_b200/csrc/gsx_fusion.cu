@@ -281,9 +281,12 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
   }
 }
 
-// H100, bench workload: 24 beat 12 by 1.2 % and 9 by 2.3 % (spread 0.2 %, DESIGN.md section 4)
+// K2 runs beside the other batch group's K4 (two groups on concurrent streams); a smaller grid most likely leaves SM
+// slots to that K4 (not measured on its own).
+// H100, bench workload with the binned arg-min: 8 beat 24 by 6.2-6.5 % on the headline, 12 by 1.3-1.5 % and 16 by
+// 2.5-3.4 % (DESIGN.md section 4)
 #ifndef GSX_K2_CTAS_PER_SM
-#define GSX_K2_CTAS_PER_SM 24
+#define GSX_K2_CTAS_PER_SM 8
 #endif
 
 // Test hook (tests/test_gpu_coverage.py): caps K2's total CTA count so that small maps take several grid-stride
