@@ -55,6 +55,13 @@ SIGNATURES = {
     "gsx_pointfusion_sequence_gt_prune": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                 c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_vp, c_vp]),
+    "gsx_fusion_free_space_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_i64]),
+    "gsx_fusion_prune_free_space": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_float, c_int, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64,
+                c_vp, c_i64, c_int, c_int, c_float, c_vp, c_i64, c_vp]),
+    "gsx_pointfusion_sequence_gt_prune_free_space": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_float, c_vp, c_i64, c_vp, c_vp]),
     "gsx_debug_fail_at_frame": (None, [c_int]),
     "gsx_debug_set_k2_grid_cap": (None, [c_int]),
     "gsx_debug_set_bin_capacity": (None, [c_int]),

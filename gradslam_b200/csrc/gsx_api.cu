@@ -4,9 +4,11 @@
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
+#include <algorithm>
 #include <mutex>
 
 #include "gsx_common.cuh"
+#include "gsx_prune.cuh"
 #include "../../include/gsx.h"
 
 namespace gsx {
@@ -30,20 +32,42 @@ int fusion_records_group(const float *poses, int64_t pose_bs, const float *K, in
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
                         int64_t rgb_bs, int B_total, int b0, int nb, int H, int W, float dist_th, float dot_th,
-                        void *workspace, int32_t *overflow, cudaStream_t st);
+                        void *workspace, int32_t *overflow, int32_t *assoc, cudaStream_t st);
 int64_t fusion_workspace_bytes(int B, int H, int W);
-// gsx_prune.cu: removal of unstable surfels for the elements [b0, b0 + nb)
-int prune_group(float *geo, float *col, int32_t *counts, int64_t cap, int32_t *ring, int ring_len, int step, int t_max,
-                float c_stable, int B_total, int b0, int nb, int32_t *keep_map, void *scratch, cudaStream_t st);
-int64_t prune_scratch_bytes(int B, int64_t capacity);
 
-// Pruning of the sequence driver (Keller et al. 2013): frame s of the call is pruned step s; null = pruning off
+// Pruning of the sequence driver (Keller et al. 2013): frame s of the call is pruned step s; null = pruning off.
+// fs_scratch non-null adds the free-space rule: K4 records where each pixel went (its group's slice of the scratch's
+// assoc image, zeroed first) and KFb, KFt and KP<true> run after it.
 struct SequencePrune {
   int32_t *ring;  // (t_max + 2, B)
   int t_max;
   float c_stable;
   void *scratch;
+  float margin;
+  void *fs_scratch;
 };
+
+// one group's pruned step s after its K4 (max_count: the host bound of the counts after that K4)
+static int sequence_prune_group(const SequencePrune *prune, float *geo, float *col, int32_t *cout, int64_t cap,
+                                const float *intrinsics, const float *poses, int64_t pose_bs, int B, int b0, int nb,
+                                int s, int H, int W, int64_t max_count, cudaStream_t st) {
+  if (!prune->fs_scratch)
+    return prune_group(geo, col, cout, cap, prune->ring, prune->t_max + 2, s, prune->t_max, prune->c_stable, B, b0, nb,
+                       nullptr, prune->scratch, st);
+  const FreeSpaceStep fs{free_space_assoc(prune->fs_scratch, B, H, W, cap, 0), intrinsics, 16, poses, pose_bs, H, W,
+                         prune->margin, prune->fs_scratch, max_count};
+  return prune_group(geo, col, cout, cap, prune->ring, prune->t_max + 2, s, prune->t_max, prune->c_stable, B, b0, nb,
+                     nullptr, prune->scratch, st, &fs);
+}
+
+// the group's assoc slice, zeroed for its K4 (null when the free-space rule is off)
+static int32_t *sequence_assoc(const SequencePrune *prune, int B, int b0, int nb, int H, int W, int64_t cap,
+                               cudaStream_t st) {
+  if (!prune || !prune->fs_scratch) return nullptr;
+  int32_t *assoc = free_space_assoc(prune->fs_scratch, B, H, W, cap, 0);
+  cudaMemsetAsync(assoc + (int64_t)b0 * H * W, 0, (size_t)nb * H * W * sizeof(int32_t), st);
+  return assoc;
+}
 
 // Batch elements own independent maps, so the sequence driver splits the batch into groups that walk the frame
 // sequence on their own streams: the kernels of one group overlap those of another instead of alternating on an otherwise
@@ -134,10 +158,12 @@ static int sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, 
         rc = gsx::fusion_update_group(map_geometry, map_colors, counts + (int64_t)(s & 1) * B,
                                       counts + (int64_t)((s + 1) & 1) * B, capacity, max_count, poses + (int64_t)s * 16,
                                       (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, 0, B,
-                                      H, W, dist_th, dot_th, half[0], overflow_flag, user);
+                                      H, W, dist_th, dot_th, half[0], overflow_flag,
+                                      gsx::sequence_assoc(prune, B, 0, B, H, W, capacity, user), user);
       if (rc == 0 && prune)
-        rc = gsx::prune_group(map_geometry, map_colors, counts + (int64_t)((s + 1) & 1) * B, capacity, prune->ring,
-                              prune->t_max + 2, s, prune->t_max, prune->c_stable, B, 0, B, nullptr, prune->scratch, user);
+        rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, counts + (int64_t)((s + 1) & 1) * B, capacity,
+                                       intrinsics, poses + (int64_t)s * 16, (int64_t)L * 16, B, 0, B, s, H, W,
+                                       std::min(max_count + P, capacity), user);
     }
     return rc;
   }
@@ -169,10 +195,13 @@ static int sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, 
       cudaStreamWaitEvent(gs->stream[g], gs->rec_done[g][h], 0);
       rc = gsx::fusion_update_group(map_geometry, map_colors, cin, cout, capacity, max_count, poses + (int64_t)s * 16,
                                     (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, b0,
-                                    b1 - b0, H, W, dist_th, dot_th, half[h], overflow_flag, gs->stream[g]);
+                                    b1 - b0, H, W, dist_th, dot_th, half[h], overflow_flag,
+                                    gsx::sequence_assoc(prune, B, b0, b1 - b0, H, W, capacity, gs->stream[g]),
+                                    gs->stream[g]);
       if (rc == 0 && prune)
-        rc = gsx::prune_group(map_geometry, map_colors, cout, capacity, prune->ring, prune->t_max + 2, s, prune->t_max,
-                              prune->c_stable, B, b0, b1 - b0, nullptr, prune->scratch, gs->stream[g]);
+        rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, cout, capacity, intrinsics,
+                                       poses + (int64_t)s * 16, (int64_t)L * 16, B, b0, b1 - b0, s, H, W,
+                                       std::min(max_count + P, capacity), gs->stream[g]);
       cudaEventRecord(gs->upd_done[g][h], gs->stream[g]);
     }
   }
@@ -210,7 +239,33 @@ extern "C" int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map
                   "gsx_pointfusion_sequence_gt_prune: prune scratch of %lld bytes < gsx_fusion_prune_scratch_bytes",
                   (long long)prune_scratch_bytes);
   }
-  const gsx::SequencePrune prune{ring, t_max, c_stable, prune_scratch};
+  const gsx::SequencePrune prune{ring, t_max, c_stable, prune_scratch, 0.0f, nullptr};
+  return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
+                     s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, &prune, stream);
+}
+
+extern "C" int gsx_pointfusion_sequence_gt_prune_free_space(
+    float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int64_t max_count0, const float *depth,
+    const float *rgb, const float *intrinsics, const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
+    float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring, int t_max, float c_stable,
+    void *prune_scratch, int64_t prune_scratch_bytes, float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+    int32_t *overflow_flag, void *stream) {
+  GSX_CHECK_ARG(t_max >= 0 && c_stable >= 0.0f && margin >= 0.0f,
+                "gsx_pointfusion_sequence_gt_prune_free_space: need t_max >= 0, c_stable >= 0, margin >= 0");
+  if (B > 0 && s_begin < s_end) {
+    GSX_CHECK_ARG(ring && prune_scratch && fs_scratch,
+                  "gsx_pointfusion_sequence_gt_prune_free_space: null ring / scratch pointer");
+    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(fs_scratch) & 15) == 0,
+                  "gsx_pointfusion_sequence_gt_prune_free_space: the free-space scratch must be 16-byte aligned");
+    GSX_CHECK_ARG(prune_scratch_bytes >= gsx::prune_scratch_bytes(B, capacity),
+                  "gsx_pointfusion_sequence_gt_prune_free_space: prune scratch of %lld bytes < "
+                  "gsx_fusion_prune_scratch_bytes", (long long)prune_scratch_bytes);
+    GSX_CHECK_ARG(H >= 0 && W >= 0 && capacity >= 0 &&
+                      fs_scratch_bytes >= gsx::free_space_scratch_bytes(B, H, W, capacity),
+                  "gsx_pointfusion_sequence_gt_prune_free_space: free-space scratch of %lld bytes < "
+                  "gsx_fusion_free_space_scratch_bytes", (long long)fs_scratch_bytes);
+  }
+  const gsx::SequencePrune prune{ring, t_max, c_stable, prune_scratch, margin, fs_scratch};
   return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
                      s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, &prune, stream);
 }

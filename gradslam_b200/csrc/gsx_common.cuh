@@ -316,6 +316,7 @@ __device__ __forceinline__ void load_live_camera(LiveCamera &c, const float *pos
 struct PixelHit {
   bool in_frustum;
   int h, w;  // pixel under the projection, clamped to the image
+  float z;   // camera-frame depth q.z (the free-space test of gsx_prune.cu)
 };
 // world -> camera (pointclouds.py:526-573), pinhole projection with the 4x4 K on the homogeneous point
 // (projutils.py:92-238; z == 0 divides by 1), frustum test, round-half-even like torch.round, then clamp
@@ -330,6 +331,7 @@ __device__ __forceinline__ PixelHit project(const LiveCamera &c, const ImageBoun
   r.in_frustum = (u > -1e-3f) && (u < ib.u_hi) && (v > -1e-3f) && (v < ib.v_hi) && (q.z > 0.0f);
   r.w = min(max((int)rintf(u), 0), ib.W - 1);
   r.h = min(max((int)rintf(v), 0), ib.H - 1);
+  r.z = q.z;
   return r;
 }
 

@@ -735,7 +735,7 @@ int fusion_records_group(const float *poses, int64_t pose_bs, const float *K, in
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
                         int64_t rgb_bs, int B_total, int b0, int nb, int H, int W, float dist_th, float dot_th,
-                        void *workspace, int32_t *overflow, cudaStream_t st) {
+                        void *workspace, int32_t *overflow, int32_t *assoc, cudaStream_t st) {
   const Workspace ws = group_workspace(workspace, B_total, b0, H, W);
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
   if (max_count > 0) {
@@ -744,7 +744,9 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
     const int rc = launch_project_select(pa, max_count, st);
     if (rc) return rc;
   }
-  MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow, nullptr, 0};
+  // assoc (full-batch base, zeroed by the caller, or null): where each pixel went, for the free-space step
+  MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow,
+               assoc ? assoc + (int64_t)b0 * H * W : nullptr, 0};
   return launch_merge_append(ma, st);
 }
 

@@ -7,6 +7,7 @@ table-returning helpers (`find_active_map_points`, `find_similar_map_points`,
 `find_best_unique_correspondences`, `fuse_with_map`) are kept for API parity and run the same arithmetic
 through the table kernels in csrc/gsx_tables.cu.
 """
+import math
 import threading
 import warnings
 from typing import Union
@@ -17,7 +18,7 @@ from .. import _C
 from ..structures.pointclouds import Pointclouds, _PruneHistory
 from ..structures.rgbdimages import RGBDImages, _frame_base
 
-__all__ = ["update_map_fusion", "update_map_aggregate", "prune_unstable"]
+__all__ = ["update_map_fusion", "update_map_aggregate", "prune_unstable", "fuse_and_prune"]
 
 
 # --------------------------------------------------------------------------------------------- small helpers
@@ -86,6 +87,16 @@ class _Workspace:
     def __init__(self, device, B, H, W):
         nbytes = _C.lib().gsx_fusion_workspace_bytes(B, H, W)
         self.buf = torch.zeros(nbytes, dtype=torch.uint8, device=device)  # (zero: the statistics start at 0)
+        self.shape = (B, H * W)
+        self.assoc = None  # K4's per-pixel record for the free-space step (fuse_and_prune), allocated on first use
+
+    def zeroed_assoc(self):
+        """int32 (B, H*W) buffer for K4's assoc_out, zeroed in stream order (K4 writes only merged / appended pixels)."""
+        if self.assoc is None:
+            self.assoc = torch.zeros(self.shape, dtype=torch.int32, device=self.buf.device)
+        else:
+            self.assoc.zero_()
+        return self.assoc
 
     @classmethod
     def get(cls, device, B, H, W):
@@ -207,8 +218,8 @@ def _append_valid_pixels(pointclouds, frames, global_coordinates=True, sigma=0.6
     return pointclouds
 
 
-def _fused_update(pointclouds, frames, dist_th, dot_th, sigma):
-    """K1r, K2/K3 then K4, in place."""
+def _fused_update(pointclouds, frames, dist_th, dot_th, sigma, assoc_out=None):
+    """K1r, K2/K3 then K4, in place.  assoc_out: a list that receives K4's per-pixel record (B, H*W) int32."""
     frames = frames.to_channels_last()
     _C.require_cuda(frames.depth_image, "depth_image")
     if frames.poses is None:
@@ -230,7 +241,11 @@ def _fused_update(pointclouds, frames, dist_th, dot_th, sigma):
         K = _dense(frames.intrinsics, "intrinsics", dev)
         _C.launch("gsx_fusion_project_select", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
                   pointclouds._bound, poses, 16, K, 16, B, H, W, float(dist_th), float(dot_th), ws.buf)
-    _launch_merge_append(pointclouds, frames, ws)
+    if assoc_out is None:
+        _launch_merge_append(pointclouds, frames, ws)
+    else:
+        assoc_out.append(ws.zeroed_assoc())
+        _launch_merge_append(pointclouds, frames, ws, assoc_out[-1])
     return pointclouds
 
 
@@ -430,7 +445,7 @@ class _MergeAppendFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pack, geo, col, gv, gn, rgb, vloc):
-        pointclouds, frames, sigma, ws = pack
+        pointclouds, frames, sigma, ws = pack[:4]
         B, _, H, W = frames.shape
         P = H * W
         dev = geo.device
@@ -448,6 +463,8 @@ class _MergeAppendFn(torch.autograd.Function):
         with_cc = 1 if pointclouds._has_cc else 0
         _C.launch("gsx_fusion_merge_append", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c, P * 3, B,
                   H, W, ws.buf, pointclouds._overflow_flag(), assoc)
+        if len(pack) > 4 and pack[4] is not None:  # (fuse_and_prune's free-space step reads it)
+            pack[4].append(assoc)
         ctx.saved = (assoc, counts_in, geo.detach(), col.detach(), gv_c, gn_c, rgb_c, vloc_c)
         ctx.dims = (B, H, W, cap_in, cap_out, float(sigma), with_cc)
         ctx.shapes = (gv.shape, rgb.shape)
@@ -469,10 +486,12 @@ class _MergeAppendFn(torch.autograd.Function):
                 d_frame[2].view(rgb_shape), d_frame[3].view(gv_shape))
 
 
-def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=None, dot_th=None, table=None):
+def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=None, dot_th=None, table=None,
+                           assoc_out=None):
     """Map update when a gradient is requested: K1 (differentiable op) -> frame records packed from its maps ->
     association (K2 kernel, or the rows of `table`; index-only) -> K4 (differentiable op), out of place so the pre-merge
-    map survives for the backward.  Values equal the in-place kernel path bit for bit."""
+    map survives for the backward.  Values equal the in-place kernel path bit for bit.  assoc_out: a list that receives
+    K4's per-pixel record."""
     frames = frames.to_channels_last()
     _C.require_cuda(frames.depth_image, "depth_image")
     B, _, H, W = frames.shape
@@ -496,8 +515,8 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
         poses = _dense(frames.poses.detach(), "poses", dev)
         _C.launch("gsx_fusion_project_select", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
                   pointclouds._bound, poses, 16, K, 16, B, H, W, float(dist_th), float(dot_th), ws.buf)
-    geo_out, col_out = _MergeAppendFn.apply((pointclouds, frames, sig, ws), pointclouds._geo, pointclouds._col, gv, gn,
-                                            frames.rgb_image, vloc)
+    geo_out, col_out = _MergeAppendFn.apply((pointclouds, frames, sig, ws, assoc_out), pointclouds._geo,
+                                            pointclouds._col, gv, gn, frames.rgb_image, vloc)
     pointclouds._geo, pointclouds._col = geo_out, col_out
     pointclouds._uninit = False
     pointclouds._mark_device_updated(pointclouds._bound + P)
@@ -530,22 +549,27 @@ def _pruned(pointclouds, h):
 
 
 class _PruneFn(torch.autograd.Function):
-    """The prune as one differentiable op on the packed rows: forward = gsx_fusion_prune_unstable on a copy of the rows,
-    recording where every row went (keep_map); backward = gsx_fusion_prune_unstable_bwd, a gather.  The removal itself
-    is a decision on the confidence and carries no gradient, as an index_select would not."""
+    """The prune as one differentiable op on the packed rows: forward = gsx_fusion_prune_unstable (or, with a free-space
+    step in the pack, gsx_fusion_prune_free_space) on a copy of the rows, recording where every row went (keep_map);
+    backward = gsx_fusion_prune_unstable_bwd, a gather.  The removal itself is a decision on the confidence and the
+    geometry and carries no gradient, as an index_select would not."""
 
     @staticmethod
     def forward(ctx, pack, geo, col):
-        pointclouds, h, c_stable = pack
+        pointclouds, h, c_stable = pack[:3]
+        free_space = pack[3] if len(pack) > 3 else None
         B, cap = geo.shape[0], geo.shape[1]
         dev = geo.device
         geo_o, col_o = geo.detach().clone(), col.detach().clone()
         counts = pointclouds._counts_dev[pointclouds._cur]
         counts_in = counts.clone()
-        keep_map = torch.arange(cap, dtype=torch.int32, device=dev).repeat(B, 1)  # rows before the window: identity
+        keep_map = torch.arange(cap, dtype=torch.int32, device=dev).repeat(B, 1)  # rows before the scan: identity
         scratch = _prune_scratch(B, cap, dev)
-        _C.launch("gsx_fusion_prune_unstable", geo_o, col_o, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
-                  float(c_stable), B, keep_map, scratch, scratch.numel())
+        if free_space is None:
+            _C.launch("gsx_fusion_prune_unstable", geo_o, col_o, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
+                      float(c_stable), B, keep_map, scratch, scratch.numel())
+        else:
+            _launch_free_space(free_space, geo_o, col_o, counts, cap, h, c_stable, B, keep_map, scratch)
         ctx.saved = (keep_map, counts_in)
         return geo_o, col_o
 
@@ -579,6 +603,78 @@ def prune_unstable(pointclouds: Pointclouds, stable_confidence: float, max_unsta
         scratch = _prune_scratch(B, pointclouds.capacity, dev)
         _C.launch("gsx_fusion_prune_unstable", geo, col, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
                   h.ring, h.t_max + 2, h.step, h.t_max, float(stable_confidence), B, None, scratch, scratch.numel())
+    _pruned(pointclouds, h)
+    return pointclouds
+
+
+# --------------------------------------------------------------------------------------------- free-space violations
+def _check_free_space_margin(margin):
+    """free_space_margin: a number (not a bool), >= 0 (inf allowed), not NaN."""
+    if isinstance(margin, bool) or not isinstance(margin, (float, int)):
+        raise TypeError("free_space_margin must be of type float or int; but was of type {}.".format(type(margin)))
+    if math.isnan(margin) or margin < 0:
+        raise ValueError("free_space_margin ({}) must be >= 0".format(margin))
+
+
+def _launch_free_space(free_space, geo, col, counts, cap, h, c_stable, B, keep_map, scratch):
+    """One gsx_fusion_prune_free_space call; free_space = (assoc, K, poses, H, W, margin) of the step's K4."""
+    assoc, K, poses, H, W, margin = free_space
+    fs_scratch = torch.empty(_C.lib().gsx_fusion_free_space_scratch_bytes(B, H, W, cap), dtype=torch.uint8,
+                             device=geo.device)
+    _C.launch("gsx_fusion_prune_free_space", geo, col, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
+              float(c_stable), B, keep_map, scratch, scratch.numel(), assoc, K, 16, poses, 16, H, W, float(margin),
+              fs_scratch, fs_scratch.numel())
+
+
+def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Union[float, int],
+                   dot_th: Union[float, int], sigma: Union[torch.Tensor, float, int],
+                   stable_confidence: Union[float, int], max_unstable_age: int,
+                   free_space_margin: Union[float, int], inplace: bool = False) -> Pointclouds:
+    """update_map_fusion followed by one pruned step with both of Keller et al.'s (2013, section 4.3) outlier rules
+    (an extension: gradslam keeps every surfel).  The age rule is prune_unstable's.  The free-space rule: wherever the
+    live frame merged a pixel into a surfel that is stable after the merge (confidence >= stable_confidence), every
+    surfel that projects to that same pixel more than `free_space_margin` (metres, camera z) in front of it is removed,
+    stable or not.  Unlike the paper (a 4x4-supersampled index map), "in front" is decided at image resolution, at the
+    pixel the association's own projection gives.  Both removals are one stable compaction: kept rows keep their order.
+    free_space_margin = inf removes no violator (the result is update_map_fusion + prune_unstable)."""
+    if not isinstance(pointclouds, Pointclouds):
+        raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
+    _check_frame(rgbdimages)
+    _check_free_space_margin(free_space_margin)
+    t_max = int(max_unstable_age)
+    if pointclouds._prune is not None and pointclouds._prune.t_max != t_max:
+        raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
+            t_max, pointclouds._prune.t_max))
+    if pointclouds.has_points and not pointclouds._has_cc:
+        raise ValueError("pruning needs maps with colours and a confidence count per point")
+    if not inplace:
+        pointclouds = pointclouds.clone()
+    got = []
+    grad = _wants_grad(pointclouds, rgbdimages)
+    if grad:
+        if rgbdimages.poses is None:
+            raise ValueError("rgbdimages must have poses for map fusion")
+        if pointclouds.has_points:
+            for what in ("normals", "colors", "features"):
+                if not getattr(pointclouds, "has_" + what):
+                    raise ValueError("Pointclouds must have {} for map fusion, but did not.".format(what))
+        _update_differentiable(pointclouds, rgbdimages, sigma, True, dist_th, dot_th, assoc_out=got)
+    else:
+        _fused_update(pointclouds, rgbdimages, dist_th, dot_th, sigma, assoc_out=got)
+    frames = rgbdimages.to_channels_last()
+    B, _, H, W = frames.shape
+    dev = pointclouds.device
+    h = _prune_history(pointclouds, t_max)
+    free_space = (got[0], _dense(frames.intrinsics.detach(), "intrinsics", dev),
+                  _dense(frames.poses.detach(), "poses", dev), H, W, free_space_margin)
+    if grad:
+        pointclouds._geo, pointclouds._col = _PruneFn.apply((pointclouds, h, stable_confidence, free_space),
+                                                            pointclouds._geo, pointclouds._col)
+    else:
+        geo, col = _map_ptrs(pointclouds, dev)
+        scratch = _prune_scratch(B, pointclouds.capacity, dev)
+        _launch_free_space(free_space, geo, col, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, h,
+                           stable_confidence, B, None, scratch)
     _pruned(pointclouds, h)
     return pointclouds
 

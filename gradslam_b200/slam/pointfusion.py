@@ -13,7 +13,7 @@ from .. import _C
 from ..structures.pointclouds import Pointclouds
 from ..structures.rgbdimages import RGBDImages
 from ..structures.pointclouds import _PruneHistory
-from .fusionutils import _prune_scratch, prune_unstable, update_map_fusion
+from .fusionutils import _check_free_space_margin, _prune_scratch, fuse_and_prune, prune_unstable, update_map_fusion
 from .icpslam import ICPSLAM
 
 __all__ = ["PointFusion"]
@@ -43,13 +43,19 @@ class PointFusion(ICPSLAM):
                  lambda_max: Union[float, int] = 2.0, B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0,
                  nu: Union[float, int] = 200.0, association: str = "nn",
                  device: Union[torch.device, str, None] = None, stable_confidence: Union[float, int, None] = None,
-                 max_unstable_age: Optional[int] = None):
+                 max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None):
         """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
         surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
         (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
         clamp(exp(-|v|^2 / 2 sigma^2), 1e-7, 1.01) of the camera-frame vertex, summed over merges - so a good threshold
         depends on the scene's depth range and on sigma; there is no universal default.  max_unstable_age = 0 tests each
-        surfel in the frame that creates it.  Default: nothing is removed (gradslam's behaviour)."""
+        surfel in the frame that creates it.  Default: nothing is removed (gradslam's behaviour).
+
+        free_space_margin (extension, metres >= 0, inf allowed; needs stable_confidence and max_unstable_age): in the same
+        step, also remove the free-space violations of Keller et al. 2013, section 4.3 - wherever the live frame merged
+        a pixel into a surfel that is stable after the merge, every surfel projecting to that pixel more than the margin
+        (camera z) in front of it.  The paper finds "in front" on a 4x4-supersampled index map; here it is the merged
+        pixel itself, at image resolution.  Default None: no such removal."""
         for name, val, kinds in (("stable_confidence", stable_confidence, (float, int)),
                                  ("max_unstable_age", max_unstable_age, (int,))):
             if val is not None and (isinstance(val, bool) or not isinstance(val, kinds)):
@@ -61,6 +67,10 @@ class PointFusion(ICPSLAM):
             raise ValueError("stable_confidence ({}) must be >= 0".format(stable_confidence))
         if max_unstable_age is not None and max_unstable_age < 0:
             raise ValueError("max_unstable_age ({}) must be >= 0".format(max_unstable_age))
+        if free_space_margin is not None:
+            _check_free_space_margin(free_space_margin)
+            if stable_confidence is None:
+                raise ValueError("free_space_margin needs stable_confidence and max_unstable_age")
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
                          lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device)
         if not isinstance(dist_th, (float, int)):
@@ -78,12 +88,16 @@ class PointFusion(ICPSLAM):
         self.sigma = sigma
         self.stable_confidence = stable_confidence
         self.max_unstable_age = max_unstable_age
+        self.free_space_margin = free_space_margin
 
     def _map(self, pointclouds: Pointclouds, live_frame: RGBDImages, inplace: bool = False):
         if self.stable_confidence is not None and isinstance(pointclouds, Pointclouds):
             if pointclouds._prune is not None and pointclouds._prune.t_max != self.max_unstable_age:
                 raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
                     self.max_unstable_age, pointclouds._prune.t_max))
+        if self.free_space_margin is not None:
+            return fuse_and_prune(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, self.stable_confidence,
+                                  self.max_unstable_age, self.free_space_margin, inplace)
         pointclouds = update_map_fusion(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, inplace)
         if self.stable_confidence is not None:
             prune_unstable(pointclouds, self.stable_confidence, self.max_unstable_age)
@@ -155,6 +169,9 @@ class PointFusion(ICPSLAM):
         if self.stable_confidence is not None:  # a fresh map: frame s of the call is pruned step s
             pc._prune = hist = _PruneHistory.fresh(B, self.max_unstable_age, dev)
             prune_scratch = _prune_scratch(B, pc.capacity, dev)
+            if self.free_space_margin is not None:
+                fs_scratch = torch.empty(_C.lib().gsx_fusion_free_space_scratch_bytes(B, H, W, pc.capacity),
+                                         dtype=torch.uint8, device=dev)
         main = torch.cuda.current_stream(dev)
         ready = []
         if not on_device:
@@ -181,6 +198,12 @@ class PointFusion(ICPSLAM):
                 _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
                           min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
                           float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag())
+            elif self.free_space_margin is not None:
+                _C.launch("gsx_pointfusion_sequence_gt_prune_free_space", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                          min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                          float(self.dot_th), float(self.sigma), ws.buf, hist.ring, self.max_unstable_age,
+                          float(self.stable_confidence), prune_scratch, prune_scratch.numel(),
+                          float(self.free_space_margin), fs_scratch, fs_scratch.numel(), pc._overflow_flag())
             else:
                 _C.launch("gsx_pointfusion_sequence_gt_prune", pc._geo, pc._col, pc._counts_dev, pc.capacity,
                           min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),

@@ -71,6 +71,39 @@ def make_sequence(B, L, H, W, seed=0, hole_fraction=0.02, motion_scale=1.0, pin_
     return rgb, depth, Kt, poses
 
 
+# the box of make_dynamic_sequence, in room coordinates (metres): in front of the far wall (z = 3), in view of camera 0
+DYNAMIC_BOX_CENTER = (0.0, 0.0, 2.0)
+DYNAMIC_BOX_HALF_EXTENTS = (0.5, 0.5, 0.25)
+
+
+def make_dynamic_sequence(B, L, H, W, k0, k1, seed=0, hole_fraction=0.02, motion_scale=1.0, pin_memory=False, yaw0=0.0,
+                          box_center=DYNAMIC_BOX_CENTER, box_half_extents=DYNAMIC_BOX_HALF_EXTENTS):
+    """make_sequence's room with an axis-aligned box that is there only in frames [k0, k1): a scene that changes.
+    Same return values, cameras, colours and holes as make_sequence(B, L, H, W, seed, ...); in frames [k0, k1) a valid
+    pixel whose ray meets the box first sees the box instead of the wall."""
+    rgb, depth, Kt, poses = make_sequence(B, L, H, W, seed=seed, hole_fraction=hole_fraction,
+                                          motion_scale=motion_scale, pin_memory=pin_memory, yaw0=yaw0)
+    K = intrinsics(H, W)
+    dirs = np.stack(
+        np.broadcast_arrays((np.arange(W)[None, :] - K[0, 2]) / K[0, 0], (np.arange(H)[:, None] - K[1, 2]) / K[1, 1],
+                            np.ones((H, W))), -1)
+    lo = np.asarray(box_center) - np.asarray(box_half_extents)
+    hi = np.asarray(box_center) + np.asarray(box_half_extents)
+    for b in range(B):
+        for s in range(max(k0, 0), min(k1, L)):
+            T = _room_from_cam(s, b, motion_scale, yaw0)
+            d_room = dirs @ T[:3, :3].T
+            o = T[:3, 3]
+            with np.errstate(divide="ignore", invalid="ignore"):  # slab test; a ray parallel to a slab gives +-inf
+                t1, t2 = (lo - o) / d_room, (hi - o) / d_room
+                t_in = np.nan_to_num(np.minimum(t1, t2), nan=-np.inf).max(-1)
+                t_out = np.nan_to_num(np.maximum(t1, t2), nan=np.inf).min(-1)
+            t_box = torch.from_numpy(np.where((t_out >= t_in) & (t_in > 0), t_in, np.inf).astype(np.float32))
+            d = depth[b, s, :, :, 0]
+            depth[b, s, :, :, 0] = torch.where((d > 0) & (t_box < d), t_box, d)
+    return rgb, depth, Kt, poses
+
+
 def punch_lattice_holes(depth, row_step=5, col_step=7):
     """Zeroes depth (..., H, W, 1) on a sparse lattice (rows 2, 2+row_step, ...; columns 3, 3+col_step, ...).  No two
     holes touch, not even diagonally, so no valid pixel has BOTH its right and its lower neighbour missing: at such

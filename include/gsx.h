@@ -197,6 +197,39 @@ int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map_colors, in
                                       float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring,
                                       int t_max, float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
                                       int32_t *overflow_flag, void *stream);
+/* ------------------------------------------------------------------------------------------------
+ * Removal of free-space violations (opt-in extension beside the unstable-surfel rule above).  Keller et al. 2013,
+ * section 4.3: when a stable surfel is merged with new data, every surfel in front of it along that ray is removed.
+ * Here "along that ray" is the merged pixel itself: pruned step `step` of the rule above, run after K4 of the live frame
+ * with camera-to-world pose T and intrinsics K (element b at poses + b * pose_bstride, intrinsics + b * K_bstride),
+ * also removes row n < counts[b] when
+ *   - K4 merged some pixel u into row m (assoc[b][u] = -(m+1), as gsx_fusion_merge_append's assoc_out), row m's
+ *     ccount after the merge is >= c_stable, and bound(u) = z of T^-1 p_m (the projection's arithmetic); and
+ *   - row n projects into the frustum at pixel u (the K2 / find_active_map_points rule) with T^-1 p_n . z <
+ *     bound(u) - margin, the difference rounded to fp32.
+ * Pixels without a merge, appended, dropped or merged into an unstable row have no bound.  The removal is one stable
+ * compaction IN PLACE of the union of both rules' rows; counts[b] becomes the kept rows, ring(k) for k in
+ * [step - t_max, step) becomes the number of kept rows whose old index was below the old ring(k), and ring(step) =
+ * counts[b].  margin >= 0 (inf: nothing is a violator, the result equals gsx_fusion_prune_unstable's).
+ * scratch / keep_map as gsx_fusion_prune_unstable (keep_map is written from min(window start, lowest violator) on);
+ * fs_scratch: gsx_fusion_free_space_scratch_bytes(B, H, W, capacity) bytes, 16-byte aligned, re-armed by every call.
+ * The backward is gsx_fusion_prune_unstable_bwd with this call's keep_map. */
+int64_t gsx_fusion_free_space_scratch_bytes(int B, int H, int W, int64_t capacity);
+int gsx_fusion_prune_free_space(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                int32_t *ring, int ring_len, int step, int t_max, float c_stable, int B,
+                                int32_t *keep_map, void *scratch, int64_t scratch_bytes, const int32_t *assoc,
+                                const float *intrinsics, int64_t K_bstride, const float *poses, int64_t pose_bstride,
+                                int H, int W, float margin, void *fs_scratch, int64_t fs_scratch_bytes, void *stream);
+/* gsx_pointfusion_sequence_gt_prune with the free-space rule: after every frame's K4 (which then records each pixel's
+ * merge in the free-space scratch), gsx_fusion_prune_free_space's step on the group stream.  Same driver. */
+int gsx_pointfusion_sequence_gt_prune_free_space(float *map_geometry, float *map_colors, int32_t *counts,
+                                                 int64_t capacity, int64_t max_count0, const float *depth,
+                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
+                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
+                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
+                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                                 float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+                                                 int32_t *overflow_flag, void *stream);
 /* test hook: the next gsx_pointfusion_sequence_gt call reports a launch failure at frame s (once); -1 = off */
 void gsx_debug_fail_at_frame(int s);
 /* test hook: caps the total CTA count of the map projection kernel (K2), so that small maps take several grid-stride
