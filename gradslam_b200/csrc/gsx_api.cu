@@ -124,14 +124,19 @@ extern "C" void gsx_debug_fail_at_frame(int s) { g_fail_at_frame = s; }
 
 extern "C" int gsx_pointfusion_sequence_groups(int B) { return B <= 0 ? 0 : gsx::sequence_groups(B); }
 
-// The one driver behind gsx_pointfusion_sequence_gt (prune == nullptr) and gsx_pointfusion_sequence_gt_prune.
-static int sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int64_t max_count0,
-                       const float *depth, const float *rgb, const float *intrinsics, const float *poses, int B, int L,
-                       int s_begin, int s_end, int H, int W, float dist_th, float dot_th, double sigma, void *workspace,
-                       int32_t *overflow_flag, const gsx::SequencePrune *prune, void *stream) {
+extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                           int64_t max_count0, const float *depth, const float *rgb,
+                                           const float *intrinsics, const float *poses, int B, int L, int s_begin,
+                                           int s_end, int H, int W, float dist_th, float dot_th, double sigma,
+                                           void *workspace, int32_t *ring, int t_max, float c_stable,
+                                           void *prune_scratch, int64_t prune_scratch_bytes, float margin,
+                                           void *fs_scratch, int64_t fs_scratch_bytes, int32_t *overflow_flag,
+                                           void *stream) {
   GSX_CHECK_ARG(B >= 0 && L >= 0 && H >= 2 && W >= 2, "gsx_pointfusion_sequence_gt: bad extents");
   GSX_CHECK_ARG(0 <= s_begin && s_begin <= s_end && s_end <= L, "gsx_pointfusion_sequence_gt: bad frame range");
   GSX_CHECK_ARG(counts && depth && rgb && intrinsics && poses, "gsx_pointfusion_sequence_gt: null pointer");
+  GSX_CHECK_ARG(!ring || (t_max >= 0 && c_stable >= 0.0f && (!fs_scratch || margin >= 0.0f)),
+                "gsx_pointfusion_sequence_gt: need t_max >= 0, c_stable >= 0, margin >= 0");
   if (B == 0 || s_begin == s_end) return 0;
   GSX_CHECK_ARG(map_geometry && map_colors && workspace && overflow_flag,
                 "gsx_pointfusion_sequence_gt: null map / workspace pointer");
@@ -139,6 +144,20 @@ static int sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, 
                   reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
                 "gsx_pointfusion_sequence_gt: map rows and workspace must be 16-byte aligned");
   GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_pointfusion_sequence_gt: capacity must fit int32 (counts are int32)");
+  if (ring) {
+    GSX_CHECK_ARG(prune_scratch, "gsx_pointfusion_sequence_gt: null prune scratch pointer");
+    GSX_CHECK_ARG(prune_scratch_bytes >= gsx::prune_scratch_bytes(B, capacity),
+                  "gsx_pointfusion_sequence_gt: prune scratch of %lld bytes < gsx_fusion_prune_scratch_bytes",
+                  (long long)prune_scratch_bytes);
+    GSX_CHECK_ARG(!fs_scratch || (reinterpret_cast<uintptr_t>(fs_scratch) & 15) == 0,
+                  "gsx_pointfusion_sequence_gt: the free-space scratch must be 16-byte aligned");
+    GSX_CHECK_ARG(!fs_scratch || (capacity >= 0 &&
+                                  fs_scratch_bytes >= gsx::free_space_scratch_bytes(B, H, W, capacity)),
+                  "gsx_pointfusion_sequence_gt: free-space scratch of %lld bytes < "
+                  "gsx_fusion_free_space_scratch_bytes", (long long)fs_scratch_bytes);
+  }
+  const gsx::SequencePrune prune_args{ring, t_max, c_stable, prune_scratch, margin, fs_scratch};
+  const gsx::SequencePrune *prune = ring ? &prune_args : nullptr;
   const int64_t P = (int64_t)H * W;
   cudaStream_t user = (cudaStream_t)stream;
   int G = gsx::sequence_groups(B);
@@ -214,60 +233,6 @@ static int sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, 
     cudaStreamWaitEvent(user, gs->rec_join[g], 0);
   }
   return rc;
-}
-
-extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                           int64_t max_count0, const float *depth, const float *rgb,
-                                           const float *intrinsics, const float *poses, int B, int L, int s_begin,
-                                           int s_end, int H, int W, float dist_th, float dot_th, double sigma,
-                                           void *workspace, int32_t *overflow_flag, void *stream) {
-  return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
-                     s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, nullptr, stream);
-}
-
-extern "C" int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map_colors, int32_t *counts,
-                                                 int64_t capacity, int64_t max_count0, const float *depth,
-                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
-                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
-                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
-                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
-                                                 int32_t *overflow_flag, void *stream) {
-  GSX_CHECK_ARG(t_max >= 0 && c_stable >= 0.0f, "gsx_pointfusion_sequence_gt_prune: need t_max >= 0, c_stable >= 0");
-  if (B > 0 && s_begin < s_end) {
-    GSX_CHECK_ARG(ring && prune_scratch, "gsx_pointfusion_sequence_gt_prune: null ring / scratch pointer");
-    GSX_CHECK_ARG(prune_scratch_bytes >= gsx::prune_scratch_bytes(B, capacity),
-                  "gsx_pointfusion_sequence_gt_prune: prune scratch of %lld bytes < gsx_fusion_prune_scratch_bytes",
-                  (long long)prune_scratch_bytes);
-  }
-  const gsx::SequencePrune prune{ring, t_max, c_stable, prune_scratch, 0.0f, nullptr};
-  return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
-                     s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, &prune, stream);
-}
-
-extern "C" int gsx_pointfusion_sequence_gt_prune_free_space(
-    float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int64_t max_count0, const float *depth,
-    const float *rgb, const float *intrinsics, const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
-    float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring, int t_max, float c_stable,
-    void *prune_scratch, int64_t prune_scratch_bytes, float margin, void *fs_scratch, int64_t fs_scratch_bytes,
-    int32_t *overflow_flag, void *stream) {
-  GSX_CHECK_ARG(t_max >= 0 && c_stable >= 0.0f && margin >= 0.0f,
-                "gsx_pointfusion_sequence_gt_prune_free_space: need t_max >= 0, c_stable >= 0, margin >= 0");
-  if (B > 0 && s_begin < s_end) {
-    GSX_CHECK_ARG(ring && prune_scratch && fs_scratch,
-                  "gsx_pointfusion_sequence_gt_prune_free_space: null ring / scratch pointer");
-    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(fs_scratch) & 15) == 0,
-                  "gsx_pointfusion_sequence_gt_prune_free_space: the free-space scratch must be 16-byte aligned");
-    GSX_CHECK_ARG(prune_scratch_bytes >= gsx::prune_scratch_bytes(B, capacity),
-                  "gsx_pointfusion_sequence_gt_prune_free_space: prune scratch of %lld bytes < "
-                  "gsx_fusion_prune_scratch_bytes", (long long)prune_scratch_bytes);
-    GSX_CHECK_ARG(H >= 0 && W >= 0 && capacity >= 0 &&
-                      fs_scratch_bytes >= gsx::free_space_scratch_bytes(B, H, W, capacity),
-                  "gsx_pointfusion_sequence_gt_prune_free_space: free-space scratch of %lld bytes < "
-                  "gsx_fusion_free_space_scratch_bytes", (long long)fs_scratch_bytes);
-  }
-  const gsx::SequencePrune prune{ring, t_max, c_stable, prune_scratch, margin, fs_scratch};
-  return sequence_gt(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
-                     s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, overflow_flag, &prune, stream);
 }
 
 extern "C" int64_t gsx_pointfusion_sequence_workspace_bytes(int B, int H, int W) {

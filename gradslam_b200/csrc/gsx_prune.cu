@@ -328,7 +328,7 @@ int prune_group(float *geo, float *col, int32_t *counts, int64_t cap, int32_t *r
   // re-arm this group's tile states and tickets
   if (cudaMemsetAsync(sc.tile_state, 0, (size_t)nb * sc.tiles * sizeof(unsigned long long), st) != cudaSuccess ||
       cudaMemsetAsync(sc.ticket, 0, (size_t)nb * sizeof(unsigned int), st) != cudaSuccess) {
-    set_error("gsx_fusion_prune_unstable: re-arming the scratch failed: %s", cudaGetErrorString(cudaGetLastError()));
+    set_error("gsx_fusion_prune: re-arming the scratch failed: %s", cudaGetErrorString(cudaGetLastError()));
     return 2;
   }
   PruneArgs a{geo + (int64_t)b0 * cap * kGeoW, col + (int64_t)b0 * cap * kColW, counts + b0, cap, ring + b0, ring_len,
@@ -342,14 +342,14 @@ int prune_group(float *geo, float *col, int32_t *counts, int64_t cap, int32_t *r
                     c_stable, fs->margin, fsc.bound + (int64_t)b0 * P, fsc.lowest + b0,
                     fsc.flags + (int64_t)b0 * fsc.words, fsc.words};
     k_free_space_bound<<<dim3((unsigned)((P + kFB - 1) / kFB), (unsigned)nb), kFB, 0, st>>>(f);
-    GSX_CHECK_LAUNCH("gsx_fusion_prune_free_space(bound)");
+    GSX_CHECK_LAUNCH("gsx_fusion_prune(free-space bound)");
     if (fs->max_count > 0) {
       int64_t bx = (fs->max_count + kFB - 1) / kFB;
       const int64_t cap_blocks = (int64_t)kNumSMs * kFreeSpaceCtasPerSM;  // grid-stride beyond this many CTAs
       if (bx * nb > cap_blocks) bx = (cap_blocks + nb - 1) / nb;
       if (bx < 1) bx = 1;
       k_free_space_test<<<dim3((unsigned)bx, (unsigned)nb), kFB, 0, st>>>(f);
-      GSX_CHECK_LAUNCH("gsx_fusion_prune_free_space(test)");
+      GSX_CHECK_LAUNCH("gsx_fusion_prune(free-space test)");
     }
     a.flags = f.flags;
     a.words = f.words;
@@ -364,7 +364,7 @@ int prune_group(float *geo, float *col, int32_t *counts, int64_t cap, int32_t *r
     k_prune_unstable<true><<<(unsigned)(per_elem * nb), kPB, 0, st>>>(a);
   else
     k_prune_unstable<false><<<(unsigned)(per_elem * nb), kPB, 0, st>>>(a);
-  GSX_CHECK_LAUNCH(fs ? "gsx_fusion_prune_free_space" : "gsx_fusion_prune_unstable");
+  GSX_CHECK_LAUNCH("gsx_fusion_prune");
   return 0;
 }
 
@@ -412,72 +412,53 @@ extern "C" int64_t gsx_fusion_prune_scratch_bytes(int B, int64_t capacity) {
   return prune_scratch_bytes(B, capacity);
 }
 
-extern "C" int gsx_fusion_prune_unstable(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                         int32_t *ring, int ring_len, int step, int t_max, float c_stable, int B,
-                                         int32_t *keep_map, void *scratch, int64_t scratch_bytes, void *stream) {
-  GSX_CHECK_ARG(B >= 0 && capacity >= 0, "gsx_fusion_prune_unstable: bad extents B=%d capacity=%lld", B,
-                (long long)capacity);
-  GSX_CHECK_ARG(t_max >= 0 && ring_len == t_max + 2 && step >= 0,
-                "gsx_fusion_prune_unstable: need t_max >= 0, ring_len == t_max + 2, step >= 0 (got %d, %d, %d)", t_max,
-                ring_len, step);
-  GSX_CHECK_ARG(c_stable >= 0.0f, "gsx_fusion_prune_unstable: c_stable must be >= 0");
-  if (B == 0) return 0;
-  GSX_CHECK_ARG(map_geometry && map_colors && counts && ring && scratch, "gsx_fusion_prune_unstable: null pointer");
-  GSX_CHECK_ARG(aligned16(map_geometry) && aligned16(map_colors),
-                "gsx_fusion_prune_unstable: map rows must be 16-byte aligned");
-  GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_prune_unstable: capacity must fit int32 (counts are int32)");
-  GSX_CHECK_ARG(scratch_bytes >= prune_scratch_bytes(B, capacity),
-                "gsx_fusion_prune_unstable: scratch of %lld bytes < gsx_fusion_prune_scratch_bytes = %lld",
-                (long long)scratch_bytes, (long long)prune_scratch_bytes(B, capacity));
-  return prune_group(map_geometry, map_colors, counts, capacity, ring, ring_len, step, t_max, c_stable, B, 0, B,
-                     keep_map, scratch, (cudaStream_t)stream);
-}
-
 extern "C" int64_t gsx_fusion_free_space_scratch_bytes(int B, int H, int W, int64_t capacity) {
   if (B < 0 || H < 0 || W < 0 || capacity < 0) return -1;
   return free_space_scratch_bytes(B, H, W, capacity);
 }
 
-extern "C" int gsx_fusion_prune_free_space(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                           int32_t *ring, int ring_len, int step, int t_max, float c_stable, int B,
-                                           int32_t *keep_map, void *scratch, int64_t scratch_bytes,
-                                           const int32_t *assoc, const float *intrinsics, int64_t K_bstride,
-                                           const float *poses, int64_t pose_bstride, int H, int W, float margin,
-                                           void *fs_scratch, int64_t fs_scratch_bytes, void *stream) {
-  GSX_CHECK_ARG(B >= 0 && capacity >= 0 && H >= 2 && W >= 2,
-                "gsx_fusion_prune_free_space: bad extents B=%d capacity=%lld H=%d W=%d", B, (long long)capacity, H, W);
+extern "C" int gsx_fusion_prune(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int32_t *ring,
+                                int ring_len, int step, int t_max, float c_stable, int B, int32_t *keep_map,
+                                void *scratch, int64_t scratch_bytes, const int32_t *assoc, const float *intrinsics,
+                                int64_t K_bstride, const float *poses, int64_t pose_bstride, int H, int W, float margin,
+                                void *fs_scratch, int64_t fs_scratch_bytes, void *stream) {
+  GSX_CHECK_ARG(B >= 0 && capacity >= 0 && (!assoc || (H >= 2 && W >= 2)),
+                "gsx_fusion_prune: bad extents B=%d capacity=%lld H=%d W=%d", B, (long long)capacity, H, W);
   GSX_CHECK_ARG(t_max >= 0 && ring_len == t_max + 2 && step >= 0,
-                "gsx_fusion_prune_free_space: need t_max >= 0, ring_len == t_max + 2, step >= 0 (got %d, %d, %d)", t_max,
-                ring_len, step);
-  GSX_CHECK_ARG(c_stable >= 0.0f, "gsx_fusion_prune_free_space: c_stable must be >= 0");
-  GSX_CHECK_ARG(margin >= 0.0f, "gsx_fusion_prune_free_space: margin must be >= 0 (inf allowed, not NaN)");
+                "gsx_fusion_prune: need t_max >= 0, ring_len == t_max + 2, step >= 0 (got %d, %d, %d)", t_max, ring_len,
+                step);
+  GSX_CHECK_ARG(c_stable >= 0.0f, "gsx_fusion_prune: c_stable must be >= 0");
+  GSX_CHECK_ARG(!assoc || margin >= 0.0f, "gsx_fusion_prune: margin must be >= 0 (inf allowed, not NaN)");
   if (B == 0) return 0;
-  GSX_CHECK_ARG(map_geometry && map_colors && counts && ring && scratch && assoc && intrinsics && poses && fs_scratch,
-                "gsx_fusion_prune_free_space: null pointer");
-  GSX_CHECK_ARG(aligned16(map_geometry) && aligned16(map_colors) && aligned16(fs_scratch),
-                "gsx_fusion_prune_free_space: map rows and scratch must be 16-byte aligned");
-  GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_prune_free_space: capacity must fit int32 (counts are int32)");
+  GSX_CHECK_ARG(map_geometry && map_colors && counts && ring && scratch, "gsx_fusion_prune: null pointer");
+  GSX_CHECK_ARG(aligned16(map_geometry) && aligned16(map_colors), "gsx_fusion_prune: map rows must be 16-byte aligned");
+  GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_prune: capacity must fit int32 (counts are int32)");
   GSX_CHECK_ARG(scratch_bytes >= prune_scratch_bytes(B, capacity),
-                "gsx_fusion_prune_free_space: scratch of %lld bytes < gsx_fusion_prune_scratch_bytes = %lld",
+                "gsx_fusion_prune: scratch of %lld bytes < gsx_fusion_prune_scratch_bytes = %lld",
                 (long long)scratch_bytes, (long long)prune_scratch_bytes(B, capacity));
+  if (!assoc)
+    return prune_group(map_geometry, map_colors, counts, capacity, ring, ring_len, step, t_max, c_stable, B, 0, B,
+                       keep_map, scratch, (cudaStream_t)stream);
+  GSX_CHECK_ARG(intrinsics && poses && fs_scratch, "gsx_fusion_prune: null free-space pointer");
+  GSX_CHECK_ARG(aligned16(fs_scratch), "gsx_fusion_prune: the free-space scratch must be 16-byte aligned");
   GSX_CHECK_ARG(fs_scratch_bytes >= free_space_scratch_bytes(B, H, W, capacity),
-                "gsx_fusion_prune_free_space: free-space scratch of %lld bytes < gsx_fusion_free_space_scratch_bytes = "
-                "%lld", (long long)fs_scratch_bytes, (long long)free_space_scratch_bytes(B, H, W, capacity));
+                "gsx_fusion_prune: free-space scratch of %lld bytes < gsx_fusion_free_space_scratch_bytes = %lld",
+                (long long)fs_scratch_bytes, (long long)free_space_scratch_bytes(B, H, W, capacity));
   const FreeSpaceStep fs{assoc, intrinsics, K_bstride, poses, pose_bstride, H, W, margin, fs_scratch, capacity};
   return prune_group(map_geometry, map_colors, counts, capacity, ring, ring_len, step, t_max, c_stable, B, 0, B,
                      keep_map, scratch, (cudaStream_t)stream, &fs);
 }
 
-extern "C" int gsx_fusion_prune_unstable_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
+extern "C" int gsx_fusion_prune_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
                                              const float *g_geometry, const float *g_colors, int64_t capacity_out,
                                              int B, float *d_map_geometry, float *d_map_colors, void *stream) {
-  GSX_CHECK_ARG(B >= 0 && capacity_in >= 0 && capacity_out >= 0, "gsx_fusion_prune_unstable_bwd: bad extents");
+  GSX_CHECK_ARG(B >= 0 && capacity_in >= 0 && capacity_out >= 0, "gsx_fusion_prune_bwd: bad extents");
   if (B == 0 || capacity_in == 0) return 0;
-  GSX_CHECK_ARG(keep_map && counts_in && d_map_geometry && d_map_colors, "gsx_fusion_prune_unstable_bwd: null pointer");
+  GSX_CHECK_ARG(keep_map && counts_in && d_map_geometry && d_map_colors, "gsx_fusion_prune_bwd: null pointer");
   GSX_CHECK_ARG(aligned16(g_geometry) && aligned16(g_colors) && aligned16(d_map_geometry) && aligned16(d_map_colors),
-                "gsx_fusion_prune_unstable_bwd: map rows must be 16-byte aligned");
+                "gsx_fusion_prune_bwd: map rows must be 16-byte aligned");
   k_prune_bwd_rows<<<dim3((unsigned)((capacity_in + 255) / 256), (unsigned)B), 256, 0, (cudaStream_t)stream>>>(
       keep_map, counts_in, capacity_in, g_geometry, g_colors, capacity_out, d_map_geometry, d_map_colors);
-  GSX_CHECK_LAUNCH("gsx_fusion_prune_unstable_bwd");
+  GSX_CHECK_LAUNCH("gsx_fusion_prune_bwd");
   return 0;
 }

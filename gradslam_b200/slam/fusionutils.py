@@ -213,11 +213,9 @@ def _append_valid_pixels(pointclouds, frames, global_coordinates=True, sigma=0.6
     return pointclouds
 
 
-def _fused_update(pointclouds, frames, dist_th, dot_th, sigma, assoc_out=None):
-    """K1r, K2/K3 then K4, in place.  assoc_out: a list that receives K4's per-pixel record (B, H*W) int32."""
-    frames = frames.to_channels_last()
-    _C.require_cuda(frames.depth_image, "depth_image")
-    if frames.poses is None:
+def _check_fusion_inputs(pointclouds, rgbdimages):
+    """A fused update needs the live frame's poses and a map with normals, colours and one confidence count per point."""
+    if rgbdimages.poses is None:
         raise ValueError("rgbdimages must have poses for map fusion")
     if pointclouds.has_points:
         for what in ("normals", "colors", "features"):
@@ -225,17 +223,24 @@ def _fused_update(pointclouds, frames, dist_th, dot_th, sigma, assoc_out=None):
                 raise ValueError("Pointclouds must have {} for map fusion, but did not.".format(what))
         if pointclouds.num_features != 1:
             raise ValueError("Pointclouds features must be a single confidence count per point for map fusion.")
+
+
+def _update_in_place(pointclouds, frames, sigma, dist_th=None, dot_th=None, table=None, assoc_out=None):
+    """K1r, the association (K2 with dist_th / dot_th, or the rows of `table`), then K4, in place.  assoc_out: a list
+    that receives K4's per-pixel record (B, H*W) int32."""
+    frames = frames.to_channels_last()
+    _C.require_cuda(frames.depth_image, "depth_image")
     B, _, H, W = frames.shape
     _prepare_map(pointclouds, frames, True)
     dev = pointclouds.device
     ws = _Workspace.get(dev, B, H, W)
     _launch_frame_records(ws, frames, _sigma_value(sigma), dev)
-    _launch_association(ws, pointclouds, frames, dist_th=dist_th, dot_th=dot_th)
-    if assoc_out is None:
-        _launch_merge_append(pointclouds, frames, ws)
-    else:
-        assoc_out.append(ws.zeroed_assoc())
-        _launch_merge_append(pointclouds, frames, ws, assoc_out[-1])
+    _launch_association(ws, pointclouds, frames, dist_th=dist_th, dot_th=dot_th, table=table)
+    assoc = None
+    if assoc_out is not None:
+        assoc = ws.zeroed_assoc()
+        assoc_out.append(assoc)
+    _launch_merge_append(pointclouds, frames, ws, assoc)
     return pointclouds
 
 
@@ -396,18 +401,7 @@ def fuse_with_map(pointclouds: Pointclouds, rgbdimages: RGBDImages, pc2im_bnhw: 
     _check_frame(rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
-    if _wants_grad(pointclouds, rgbdimages) and rgbdimages.poses is not None:
-        return _update_differentiable(pointclouds, rgbdimages, sigma, True, table=pc2im_bnhw)
-    frames = rgbdimages.to_channels_last()
-    _C.require_cuda(frames.depth_image, "depth_image")
-    B, _, H, W = frames.shape
-    _prepare_map(pointclouds, frames, True)
-    device = pointclouds.device
-    ws = _Workspace.get(device, B, H, W)
-    _launch_frame_records(ws, frames, _sigma_value(sigma), device)
-    _launch_association(ws, pointclouds, frames, table=pc2im_bnhw)
-    _launch_merge_append(pointclouds, frames, ws)
-    return pointclouds
+    return _fuse(pointclouds, rgbdimages, sigma, table=pc2im_bnhw)
 
 
 def _launch_association(ws, pointclouds, frames, dist_th=None, dot_th=None, table=None):
@@ -519,54 +513,39 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
     return pointclouds
 
 
+def _fuse(pointclouds, frames, sigma, dist_th=None, dot_th=None, table=None, assoc_out=None):
+    """The fused map update: the differentiable op chain when a gradient is requested, else in place.  A frame without
+    poses (only fuse_with_map accepts one) has no world-frame maps for the differentiable chain and is fused in place."""
+    if _wants_grad(pointclouds, frames) and frames.poses is not None:
+        return _update_differentiable(pointclouds, frames, sigma, True, dist_th, dot_th, table, assoc_out)
+    return _update_in_place(pointclouds, frames, sigma, dist_th, dot_th, table, assoc_out)
+
+
 # --------------------------------------------------------------------------------------------- unstable surfels
-def _prune_history(pointclouds, t_max):
-    """The map's pruning history, created at its first pruned step (rows already in the map count as created then)."""
+def _check_history(pointclouds, t_max):
+    """Raises before anything is launched if the map was pruned with another max_unstable_age."""
     h = pointclouds._prune
-    if h is None:
-        h = pointclouds._prune = _PruneHistory.fresh(len(pointclouds), t_max, pointclouds.device)
-    elif h.t_max != t_max:
+    if h is not None and h.t_max != t_max:
         raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
             t_max, h.t_max))
-    return h
 
 
 def _prune_scratch(B, capacity, device):
     return torch.empty(_C.lib().gsx_fusion_prune_scratch_bytes(B, capacity), dtype=torch.uint8, device=device)
 
 
-def _pruned(pointclouds, h):
-    """Bookkeeping after a prune launch: one more pruned step, sizes changed on the device (the host bound stays an upper
-    bound), and rows past the new sizes hold stale values until a padded view zeroes them."""
-    h.step += 1
-    pointclouds._counts_host = None
-    pointclouds._list_cache = {}
-    pointclouds._uninit = pointclouds._tail_dirty = True
-
-
 class _PruneFn(torch.autograd.Function):
-    """The prune as one differentiable op on the packed rows: forward = gsx_fusion_prune_unstable (or, with a free-space
-    step in the pack, gsx_fusion_prune_free_space) on a copy of the rows, recording where every row went (keep_map);
-    backward = gsx_fusion_prune_unstable_bwd, a gather.  The removal itself is a decision on the confidence and the
-    geometry and carries no gradient, as an index_select would not."""
+    """The prune as one differentiable op on the packed rows: forward = `prune` (a gsx_fusion_prune launch) on a copy of
+    the rows, recording where every row went (keep_map); backward = gsx_fusion_prune_bwd, a gather.  The removal itself
+    is a decision on the confidence and the geometry and carries no gradient, as an index_select would not."""
 
     @staticmethod
-    def forward(ctx, pack, geo, col):
-        pointclouds, h, c_stable = pack[:3]
-        free_space = pack[3] if len(pack) > 3 else None
+    def forward(ctx, prune, counts, geo, col):
         B, cap = geo.shape[0], geo.shape[1]
-        dev = geo.device
         geo_o, col_o = geo.detach().clone(), col.detach().clone()
-        counts = pointclouds._counts_dev[pointclouds._cur]
-        counts_in = counts.clone()
-        keep_map = torch.arange(cap, dtype=torch.int32, device=dev).repeat(B, 1)  # rows before the scan: identity
-        scratch = _prune_scratch(B, cap, dev)
-        if free_space is None:
-            _C.launch("gsx_fusion_prune_unstable", geo_o, col_o, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
-                      float(c_stable), B, keep_map, scratch, scratch.numel())
-        else:
-            _launch_free_space(free_space, geo_o, col_o, counts, cap, h, c_stable, B, keep_map, scratch)
-        ctx.saved = (keep_map, counts_in)
+        keep_map = torch.arange(cap, dtype=torch.int32, device=geo.device).repeat(B, 1)  # rows before the scan: identity
+        ctx.saved = (keep_map, counts.clone())
+        prune(geo_o, col_o, keep_map)
         return geo_o, col_o
 
     @staticmethod
@@ -576,8 +555,41 @@ class _PruneFn(torch.autograd.Function):
         gs = [None if g is None else g.contiguous().float() for g in (g_geo, g_col)]
         d_geo = torch.empty((B, cap, 8), dtype=torch.float32, device=keep_map.device)
         d_col = torch.empty((B, cap, 4), dtype=torch.float32, device=keep_map.device)
-        _C.launch("gsx_fusion_prune_unstable_bwd", keep_map, counts_in, cap, gs[0], gs[1], cap, B, d_geo, d_col)
-        return None, d_geo, d_col
+        _C.launch("gsx_fusion_prune_bwd", keep_map, counts_in, cap, gs[0], gs[1], cap, B, d_geo, d_col)
+        return None, None, d_geo, d_col
+
+
+def _prune(pointclouds, stable_confidence, t_max, free_space=None):
+    """One pruned step of the map, in place: the age rule and, with free_space = (assoc, K, poses, H, W, margin) of the
+    step's K4, the free-space rule.  A differentiable op when the map's rows require grad.  The map's pruning history is
+    created at its first pruned step (rows already in the map count as created then)."""
+    h = pointclouds._prune
+    if h is None:
+        h = pointclouds._prune = _PruneHistory.fresh(len(pointclouds), t_max, pointclouds.device)
+    B, cap, dev = len(pointclouds), pointclouds.capacity, pointclouds.device
+    counts = pointclouds._counts_dev[pointclouds._cur]
+    scratch = _prune_scratch(B, cap, dev)
+    fs = (None, None, 0, None, 0, 0, 0, 0.0, None, 0)  # the age rule alone
+    if free_space is not None:
+        assoc, K, poses, H, W, margin = free_space
+        fs_scratch = torch.empty(_C.lib().gsx_fusion_free_space_scratch_bytes(B, H, W, cap), dtype=torch.uint8,
+                                 device=dev)
+        fs = (assoc, K, 16, poses, 16, H, W, float(margin), fs_scratch, fs_scratch.numel())
+
+    def launch(geo, col, keep_map):
+        _C.launch("gsx_fusion_prune", geo, col, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
+                  float(stable_confidence), B, keep_map, scratch, scratch.numel(), *fs)
+
+    if torch.is_grad_enabled() and any(t.requires_grad for t in pointclouds._grad_tensors()):
+        pointclouds._geo, pointclouds._col = _PruneFn.apply(launch, counts, pointclouds._geo, pointclouds._col)
+    else:
+        launch(*_map_ptrs(pointclouds, dev), None)
+    # one more pruned step; the sizes changed on the device (the host bound stays an upper bound), and rows past the new
+    # sizes hold stale values until a padded view zeroes them
+    h.step += 1
+    pointclouds._counts_host = None
+    pointclouds._list_cache = {}
+    pointclouds._uninit = pointclouds._tail_dirty = True
 
 
 def prune_unstable(pointclouds: Pointclouds, stable_confidence: float, max_unstable_age: int) -> Pointclouds:
@@ -589,17 +601,8 @@ def prune_unstable(pointclouds: Pointclouds, stable_confidence: float, max_unsta
         return pointclouds
     if not pointclouds._has_cc or pointclouds._col is None:
         raise ValueError("pruning needs maps with colours and a confidence count per point")
-    h = _prune_history(pointclouds, int(max_unstable_age))
-    B, dev = len(pointclouds), pointclouds.device
-    if torch.is_grad_enabled() and any(t.requires_grad for t in pointclouds._grad_tensors()):
-        pointclouds._geo, pointclouds._col = _PruneFn.apply((pointclouds, h, stable_confidence), pointclouds._geo,
-                                                            pointclouds._col)
-    else:
-        geo, col = _map_ptrs(pointclouds, dev)
-        scratch = _prune_scratch(B, pointclouds.capacity, dev)
-        _C.launch("gsx_fusion_prune_unstable", geo, col, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
-                  h.ring, h.t_max + 2, h.step, h.t_max, float(stable_confidence), B, None, scratch, scratch.numel())
-    _pruned(pointclouds, h)
+    _check_history(pointclouds, int(max_unstable_age))
+    _prune(pointclouds, stable_confidence, int(max_unstable_age))
     return pointclouds
 
 
@@ -610,16 +613,6 @@ def _check_free_space_margin(margin):
         raise TypeError("free_space_margin must be of type float or int; but was of type {}.".format(type(margin)))
     if math.isnan(margin) or margin < 0:
         raise ValueError("free_space_margin ({}) must be >= 0".format(margin))
-
-
-def _launch_free_space(free_space, geo, col, counts, cap, h, c_stable, B, keep_map, scratch):
-    """One gsx_fusion_prune_free_space call; free_space = (assoc, K, poses, H, W, margin) of the step's K4."""
-    assoc, K, poses, H, W, margin = free_space
-    fs_scratch = torch.empty(_C.lib().gsx_fusion_free_space_scratch_bytes(B, H, W, cap), dtype=torch.uint8,
-                             device=geo.device)
-    _C.launch("gsx_fusion_prune_free_space", geo, col, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
-              float(c_stable), B, keep_map, scratch, scratch.numel(), assoc, K, 16, poses, 16, H, W, float(margin),
-              fs_scratch, fs_scratch.numel())
 
 
 def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Union[float, int],
@@ -638,40 +631,20 @@ def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Un
     _check_frame(rgbdimages)
     _check_free_space_margin(free_space_margin)
     t_max = int(max_unstable_age)
-    if pointclouds._prune is not None and pointclouds._prune.t_max != t_max:
-        raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
-            t_max, pointclouds._prune.t_max))
+    _check_history(pointclouds, t_max)
     if pointclouds.has_points and not pointclouds._has_cc:
         raise ValueError("pruning needs maps with colours and a confidence count per point")
+    _check_fusion_inputs(pointclouds, rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
     got = []
-    grad = _wants_grad(pointclouds, rgbdimages)
-    if grad:
-        if rgbdimages.poses is None:
-            raise ValueError("rgbdimages must have poses for map fusion")
-        if pointclouds.has_points:
-            for what in ("normals", "colors", "features"):
-                if not getattr(pointclouds, "has_" + what):
-                    raise ValueError("Pointclouds must have {} for map fusion, but did not.".format(what))
-        _update_differentiable(pointclouds, rgbdimages, sigma, True, dist_th, dot_th, assoc_out=got)
-    else:
-        _fused_update(pointclouds, rgbdimages, dist_th, dot_th, sigma, assoc_out=got)
+    _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th, assoc_out=got)
     frames = rgbdimages.to_channels_last()
-    B, _, H, W = frames.shape
+    _, _, H, W = frames.shape
     dev = pointclouds.device
-    h = _prune_history(pointclouds, t_max)
     free_space = (got[0], _dense(frames.intrinsics.detach(), "intrinsics", dev),
                   _dense(frames.poses.detach(), "poses", dev), H, W, free_space_margin)
-    if grad:
-        pointclouds._geo, pointclouds._col = _PruneFn.apply((pointclouds, h, stable_confidence, free_space),
-                                                            pointclouds._geo, pointclouds._col)
-    else:
-        geo, col = _map_ptrs(pointclouds, dev)
-        scratch = _prune_scratch(B, pointclouds.capacity, dev)
-        _launch_free_space(free_space, geo, col, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, h,
-                           stable_confidence, B, None, scratch)
-    _pruned(pointclouds, h)
+    _prune(pointclouds, stable_confidence, t_max, free_space)
     return pointclouds
 
 
@@ -702,14 +675,7 @@ def update_map_fusion(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th:
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     _check_frame(rgbdimages)
+    _check_fusion_inputs(pointclouds, rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
-    if _wants_grad(pointclouds, rgbdimages):
-        if rgbdimages.poses is None:
-            raise ValueError("rgbdimages must have poses for map fusion")
-        if pointclouds.has_points:
-            for what in ("normals", "colors", "features"):
-                if not getattr(pointclouds, "has_" + what):
-                    raise ValueError("Pointclouds must have {} for map fusion, but did not.".format(what))
-        return _update_differentiable(pointclouds, rgbdimages, sigma, True, dist_th, dot_th)
-    return _fused_update(pointclouds, rgbdimages, dist_th, dot_th, sigma)
+    return _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th)

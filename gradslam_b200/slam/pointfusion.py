@@ -13,7 +13,8 @@ from .. import _C
 from ..structures.pointclouds import Pointclouds
 from ..structures.rgbdimages import RGBDImages
 from ..structures.pointclouds import _PruneHistory
-from .fusionutils import _check_free_space_margin, _prune_scratch, fuse_and_prune, prune_unstable, update_map_fusion
+from .fusionutils import (_check_free_space_margin, _check_history, _prune_scratch, fuse_and_prune, prune_unstable,
+                          update_map_fusion)
 from .icpslam import ICPSLAM
 
 __all__ = ["PointFusion"]
@@ -92,9 +93,7 @@ class PointFusion(ICPSLAM):
 
     def _map(self, pointclouds: Pointclouds, live_frame: RGBDImages, inplace: bool = False):
         if self.stable_confidence is not None and isinstance(pointclouds, Pointclouds):
-            if pointclouds._prune is not None and pointclouds._prune.t_max != self.max_unstable_age:
-                raise ValueError("max_unstable_age ({}) differs from the one this map was pruned with ({})".format(
-                    self.max_unstable_age, pointclouds._prune.t_max))
+            _check_history(pointclouds, self.max_unstable_age)
         if self.free_space_margin is not None:
             return fuse_and_prune(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, self.stable_confidence,
                                   self.max_unstable_age, self.free_space_margin, inplace)
@@ -166,12 +165,16 @@ class PointFusion(ICPSLAM):
             pc = Pointclouds(device=dev)
             pc._allocate(B, L * P, 1, zero=False)
         ws = _SequenceWorkspace.get(dev, B, H, W)
+        prune = (None, 0, 0.0, None, 0)  # ring, t_max, c_stable, scratch, its bytes: pruning off
+        free_space = (0.0, None, 0)  # margin, scratch, its bytes: the age rule alone
         if self.stable_confidence is not None:  # a fresh map: frame s of the call is pruned step s
             pc._prune = hist = _PruneHistory.fresh(B, self.max_unstable_age, dev)
-            prune_scratch = _prune_scratch(B, pc.capacity, dev)
+            scratch = _prune_scratch(B, pc.capacity, dev)
+            prune = (hist.ring, self.max_unstable_age, float(self.stable_confidence), scratch, scratch.numel())
             if self.free_space_margin is not None:
                 fs_scratch = torch.empty(_C.lib().gsx_fusion_free_space_scratch_bytes(B, H, W, pc.capacity),
                                          dtype=torch.uint8, device=dev)
+                free_space = (float(self.free_space_margin), fs_scratch, fs_scratch.numel())
         main = torch.cuda.current_stream(dev)
         ready = []
         if not on_device:
@@ -194,21 +197,9 @@ class PointFusion(ICPSLAM):
                 for b in range(B):
                     _C.launch("gsx_ingest_raw", raw_rgb[b, s0:s1], raw_depth[b, s0:s1], (s1 - s0) * P,
                               frames.scaling_factor, 1 if frames.normalize_color else 0, rgb[b, s0:s1], depth[b, s0:s1])
-            if self.stable_confidence is None:
-                _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                          min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                          float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag())
-            elif self.free_space_margin is not None:
-                _C.launch("gsx_pointfusion_sequence_gt_prune_free_space", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                          min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                          float(self.dot_th), float(self.sigma), ws.buf, hist.ring, self.max_unstable_age,
-                          float(self.stable_confidence), prune_scratch, prune_scratch.numel(),
-                          float(self.free_space_margin), fs_scratch, fs_scratch.numel(), pc._overflow_flag())
-            else:
-                _C.launch("gsx_pointfusion_sequence_gt_prune", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                          min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                          float(self.dot_th), float(self.sigma), ws.buf, hist.ring, self.max_unstable_age,
-                          float(self.stable_confidence), prune_scratch, prune_scratch.numel(), pc._overflow_flag())
+            _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                      min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                      float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag())
         if not on_device:
             for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
                 t.record_stream(copy_stream)

@@ -147,7 +147,13 @@ int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, 
  * current sizes are in row (s_end & 1).  max_count0 = host upper bound of the sizes on entry.
  * Splitting a sequence into several calls (s_begin..s_end chunks) lets the caller overlap host->device copies of
  * later frames with the fusion of earlier ones.  On a launch failure the internal streams are still joined to
- * `stream` before the error is returned. */
+ * `stream` before the error is returned.
+ * Pruning (Keller et al. 2013, see gsx_fusion_prune below): ring == NULL turns it off, and t_max, c_stable,
+ * prune_scratch, margin and fs_scratch are then neither read nor checked.  Otherwise every frame's K4 is followed, on its
+ * group stream, by gsx_fusion_prune's step: frame s of the call is pruned step s, so a call with s_begin > 0 continues
+ * the same ring.  ring int32 (t_max + 2, B); prune_scratch: gsx_fusion_prune_scratch_bytes(B, capacity) bytes.
+ * fs_scratch == NULL: the age rule alone; otherwise the free-space rule as well, with margin >= 0, and K4 records each
+ * pixel's merge in fs_scratch: gsx_fusion_free_space_scratch_bytes(B, H, W, capacity) bytes, 16-byte aligned. */
 /* number of independent batch groups gsx_pointfusion_sequence_gt runs on concurrent internal streams for a batch of
  * B (default 2, environment GSX_SEQ_GROUPS = 1..4 overrides; never more than B).  Kernel launches per call =
  * groups * (3 * frames - [map empty on entry]). */
@@ -158,7 +164,9 @@ int64_t gsx_pointfusion_sequence_workspace_bytes(int B, int H, int W);
 int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
                                 int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
                                 const float *poses, int B, int L, int s_begin, int s_end, int H, int W, float dist_th,
-                                float dot_th, double sigma, void *workspace, int32_t *overflow_flag, void *stream);
+                                float dot_th, double sigma, void *workspace, int32_t *ring, int t_max, float c_stable,
+                                void *prune_scratch, int64_t prune_scratch_bytes, float margin, void *fs_scratch,
+                                int64_t fs_scratch_bytes, int32_t *overflow_flag, void *stream);
 /* ------------------------------------------------------------------------------------------------
  * Removal of unstable surfels (opt-in extension; gradslam has no such step, so no reference line is replaced).
  * Keller et al. 2013, "Real-time 3D reconstruction in dynamic scenes using point-based fusion", section 4.3: a surfel
@@ -175,28 +183,7 @@ int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t 
  * or -1 if removed; entries before the window start are not written (the differentiable mode fills them with the
  * identity). */
 int64_t gsx_fusion_prune_scratch_bytes(int B, int64_t capacity);
-int gsx_fusion_prune_unstable(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int32_t *ring,
-                              int ring_len, int step, int t_max, float c_stable, int B, int32_t *keep_map,
-                              void *scratch, int64_t scratch_bytes, void *stream);
-/* Backward of gsx_fusion_prune_unstable (Keller et al. 2013, as above): a gather.  d_map[b][n] = g[b][keep_map[b][n]]
- * for n < counts_in[b] with keep_map >= 0, else zero (removed and padding rows; padding slots zero).  keep_map
- * (B, capacity_in) as the forward left it over an identity fill; upstream gradients (B, capacity_out, 8 / 4), either
- * may be NULL = zero; outputs (B, capacity_in, 8 / 4), every row written.  No atomics. */
-int gsx_fusion_prune_unstable_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
-                                  const float *g_geometry, const float *g_colors, int64_t capacity_out, int B,
-                                  float *d_map_geometry, float *d_map_colors, void *stream);
-/* gsx_pointfusion_sequence_gt followed, after every frame's K4, by gsx_fusion_prune_unstable (Keller et al. 2013, as
- * above) on the group stream: frame s of the call is pruned step s, so a call with s_begin > 0 continues the same ring.
- * ring int32 (t_max + 2, B); prune_scratch: gsx_fusion_prune_scratch_bytes(B, capacity) bytes.  Both entry points run
- * one driver; gsx_pointfusion_sequence_gt is this one with pruning off. */
-int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                      int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
-                                      const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
-                                      float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring,
-                                      int t_max, float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
-                                      int32_t *overflow_flag, void *stream);
-/* ------------------------------------------------------------------------------------------------
- * Removal of free-space violations (opt-in extension beside the unstable-surfel rule above).  Keller et al. 2013,
+/* Removal of free-space violations (opt-in, beside the unstable-surfel rule above).  Keller et al. 2013,
  * section 4.3: when a stable surfel is merged with new data, every surfel in front of it along that ray is removed.
  * Here "along that ray" is the merged pixel itself: pruned step `step` of the rule above, run after K4 of the live frame
  * with camera-to-world pose T and intrinsics K (element b at poses + b * pose_bstride, intrinsics + b * K_bstride),
@@ -208,26 +195,24 @@ int gsx_pointfusion_sequence_gt_prune(float *map_geometry, float *map_colors, in
  * Pixels without a merge, appended, dropped or merged into an unstable row have no bound.  The removal is one stable
  * compaction IN PLACE of the union of both rules' rows; counts[b] becomes the kept rows, ring(k) for k in
  * [step - t_max, step) becomes the number of kept rows whose old index was below the old ring(k), and ring(step) =
- * counts[b].  margin >= 0 (inf: nothing is a violator, the result equals gsx_fusion_prune_unstable's).
- * scratch / keep_map as gsx_fusion_prune_unstable (keep_map is written from min(window start, lowest violator) on);
- * fs_scratch: gsx_fusion_free_space_scratch_bytes(B, H, W, capacity) bytes, 16-byte aligned, re-armed by every call.
- * The backward is gsx_fusion_prune_unstable_bwd with this call's keep_map. */
+ * counts[b].  margin >= 0 (inf: nothing is a violator, the result equals the age rule's); keep_map is then written from
+ * min(window start, lowest violator) on.  fs_scratch: gsx_fusion_free_space_scratch_bytes(B, H, W, capacity) bytes,
+ * 16-byte aligned, re-armed by every call. */
 int64_t gsx_fusion_free_space_scratch_bytes(int B, int H, int W, int64_t capacity);
-int gsx_fusion_prune_free_space(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                int32_t *ring, int ring_len, int step, int t_max, float c_stable, int B,
-                                int32_t *keep_map, void *scratch, int64_t scratch_bytes, const int32_t *assoc,
-                                const float *intrinsics, int64_t K_bstride, const float *poses, int64_t pose_bstride,
-                                int H, int W, float margin, void *fs_scratch, int64_t fs_scratch_bytes, void *stream);
-/* gsx_pointfusion_sequence_gt_prune with the free-space rule: after every frame's K4 (which then records each pixel's
- * merge in the free-space scratch), gsx_fusion_prune_free_space's step on the group stream.  Same driver. */
-int gsx_pointfusion_sequence_gt_prune_free_space(float *map_geometry, float *map_colors, int32_t *counts,
-                                                 int64_t capacity, int64_t max_count0, const float *depth,
-                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
-                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
-                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
-                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
-                                                 float margin, void *fs_scratch, int64_t fs_scratch_bytes,
-                                                 int32_t *overflow_flag, void *stream);
+/* One pruned step.  assoc == NULL: the age rule alone, and the free-space arguments after it are neither read nor
+ * checked; otherwise both rules, with the live frame's camera, K4's assoc (B, H*W) and margin. */
+int gsx_fusion_prune(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int32_t *ring,
+                     int ring_len, int step, int t_max, float c_stable, int B, int32_t *keep_map, void *scratch,
+                     int64_t scratch_bytes, const int32_t *assoc, const float *intrinsics, int64_t K_bstride,
+                     const float *poses, int64_t pose_bstride, int H, int W, float margin, void *fs_scratch,
+                     int64_t fs_scratch_bytes, void *stream);
+/* Backward of gsx_fusion_prune (either rule): a gather.  d_map[b][n] = g[b][keep_map[b][n]]
+ * for n < counts_in[b] with keep_map >= 0, else zero (removed and padding rows; padding slots zero).  keep_map
+ * (B, capacity_in) as the forward left it over an identity fill; upstream gradients (B, capacity_out, 8 / 4), either
+ * may be NULL = zero; outputs (B, capacity_in, 8 / 4), every row written.  No atomics. */
+int gsx_fusion_prune_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
+                         const float *g_geometry, const float *g_colors, int64_t capacity_out, int B,
+                         float *d_map_geometry, float *d_map_colors, void *stream);
 /* test hook: the next gsx_pointfusion_sequence_gt call reports a launch failure at frame s (once); -1 = off */
 void gsx_debug_fail_at_frame(int s);
 /* test hook: caps the total CTA count of the map projection kernel (K2), so that small maps take several grid-stride

@@ -189,8 +189,8 @@ def test_full_size_match_oracle():
 
 
 def test_infinite_margin_equals_the_age_rule_entry_points():
-    """margin = inf: gsx_pointfusion_sequence_gt_prune_free_space and gsx_fusion_prune_free_space give exactly what
-    gsx_pointfusion_sequence_gt_prune and gsx_fusion_prune_unstable give, ring included."""
+    """margin = inf: the free-space rule of gsx_pointfusion_sequence_gt and gsx_fusion_prune gives exactly what their
+    age rule alone gives, ring included."""
     import gradslam_b200 as gs
 
     rgb, depth, K, poses, c = _scene("dynamic")

@@ -319,8 +319,8 @@ def test_differentiable_prune_wrt_previous_map():
 
 
 @pytest.mark.parametrize("B,cap", [(3, 70001), (2, 5 * 512 + 17)])
-def test_backward_kernel_matches_float64_gather(B, cap):
-    """gsx_fusion_prune_unstable_bwd against float64 autograd of the gather, at large and ragged sizes, with one element
+def test_prune_bwd_kernel_matches_float64_gather(B, cap):
+    """gsx_fusion_prune_bwd against float64 autograd of the gather, at large and ragged sizes, with one element
     whose window is empty (rows before the window pass through)."""
     from gradslam_b200 import _C
     from gradslam_b200.slam.fusionutils import _prune_scratch
@@ -340,13 +340,13 @@ def test_backward_kernel_matches_float64_gather(B, cap):
     cnt = torch.tensor(counts, dtype=torch.int32, device=DEV)
     keep_map = torch.arange(cap, dtype=torch.int32, device=DEV).repeat(B, 1)
     scratch = _prune_scratch(B, cap, DEV)
-    _C.launch("gsx_fusion_prune_unstable", geo_d, col_d, cnt, cap, ring_d, t_max + 2, step, t_max, 0.5, B, keep_map,
-              scratch, scratch.numel())
+    _C.launch("gsx_fusion_prune", geo_d, col_d, cnt, cap, ring_d, t_max + 2, step, t_max, 0.5, B, keep_map, scratch,
+              scratch.numel(), None, None, 0, None, 0, 0, 0, 0.0, None, 0)
     g_geo, g_col = torch.randn(B, cap, 8, generator=g), torch.randn(B, cap, 4, generator=g)
     d_geo = torch.empty(B, cap, 8, device=DEV)
     d_col = torch.empty(B, cap, 4, device=DEV)
     cin = torch.tensor(counts, dtype=torch.int32, device=DEV)
-    _C.launch("gsx_fusion_prune_unstable_bwd", keep_map, cin, cap, g_geo.to(DEV), g_col.to(DEV), cap, B, d_geo, d_col)
+    _C.launch("gsx_fusion_prune_bwd", keep_map, cin, cap, g_geo.to(DEV), g_col.to(DEV), cap, B, d_geo, d_col)
     for b in range(B):
         x64 = torch.cat([geo[b], col[b]], 1).double().requires_grad_(True)
         n = torch.arange(cap)
