@@ -36,6 +36,8 @@ SIGNATURES = {
     "gsx_fusion_workspace_stats_offset": (c_i64, [c_int, c_int, c_int]),
     "gsx_fusion_frame_records": (
         c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_double, c_vp, c_vp]),
+    "gsx_fusion_sequence_frame": (
+        c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_double, c_int, c_vp, c_vp]),
     "gsx_fusion_project_select": (
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_float, c_float, c_vp, c_vp]),
     "gsx_fusion_merge_append": (

@@ -8,6 +8,7 @@
 #include <mutex>
 
 #include "gsx_common.cuh"
+#include "gsx_fusion_ws.cuh"
 #include "gsx_prune.cuh"
 #include "../../include/gsx.h"
 
@@ -25,15 +26,16 @@ extern "C" int gsx_version(void) { return GSX_VERSION; }
 extern "C" const char *gsx_last_error(void) { return gsx::g_err; }
 
 namespace gsx {
-// gsx_fusion.cu: the two halves of one frame for the batch elements [b0, b0 + nb) of a B_total-element problem
-int fusion_records_group(const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *depth,
-                         int64_t d_bs, int B_total, int b0, int nb, int H, int W, double sigma, void *workspace,
-                         cudaStream_t st);
+// gsx_fusion.cu: the sequence workspace, its per-call re-arm, the frame headers of frames [s, s + F) and the map update
+// of frame s (K2 + K4) for the batch elements [b0, b0 + nb) of a B_total-element problem
+int64_t sequence_workspace_bytes(int B, int H, int W);
+int sequence_rearm(void *workspace, int B, int H, int W, cudaStream_t st);
+int sequence_headers_group(const float *poses, const float *K, const float *depth, int L, int s, int F, int B_total,
+                           int b0, int nb, int H, int W, double sigma, void *workspace, cudaStream_t st);
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
-                        int64_t rgb_bs, int B_total, int b0, int nb, int H, int W, float dist_th, float dot_th,
+                        int64_t rgb_bs, int B_total, int b0, int nb, int s, int H, int W, float dist_th, float dot_th,
                         void *workspace, int32_t *overflow, int32_t *assoc, cudaStream_t st);
-int64_t fusion_workspace_bytes(int B, int H, int W);
 
 // Pruning of the sequence driver (Keller et al. 2013): frame s of the call is pruned step s; null = pruning off.
 // fs_scratch non-null adds the free-space rule: K4 records where each pixel went (its group's slice of the scratch's
@@ -71,15 +73,13 @@ static int32_t *sequence_assoc(const SequencePrune *prune, int B, int b0, int nb
 
 // Batch elements own independent maps, so the sequence driver splits the batch into groups that walk the frame
 // sequence on their own streams: the kernels of one group overlap those of another instead of alternating on an otherwise
-// idle GPU (none of them saturates a unit on its own: they are bound by memory latency).  Inside a group the frame
-// records of frame s+1 (K1r: independent of the map) are computed on a second stream while K2 / K4 of
-// frame s (latency-bound) run: the workspace has two halves used alternately, events order
-//     K1r(s) -> K2(s), K4(s)      and      K4(s) -> K1r(s+2)  (same half).
+// idle GPU (none of them saturates a unit on its own: they are bound by memory latency).  Per frame a group runs K2 and
+// K4 only: the frame headers are written kSeqFrames frames at a time, and K4 re-arms what the next frame consumes.
 constexpr int kMaxGroups = 4, kMaxDevices = 16;
 struct GroupStreams {
   bool ready = false;
-  cudaStream_t stream[kMaxGroups], rec_stream[kMaxGroups];
-  cudaEvent_t fork, join[kMaxGroups], rec_join[kMaxGroups], rec_done[kMaxGroups][2], upd_done[kMaxGroups][2];
+  cudaStream_t stream[kMaxGroups];
+  cudaEvent_t fork, join[kMaxGroups];
 };
 static GroupStreams g_groups[kMaxDevices];
 // The group streams and their fork / join events are shared by every caller on a device: one enqueue (event record ->
@@ -102,13 +102,7 @@ static GroupStreams *group_streams() {
   if (!gs.ready) {
     for (int i = 0; i < kMaxGroups; ++i) {
       if (cudaStreamCreateWithFlags(&gs.stream[i], cudaStreamNonBlocking) != cudaSuccess) return nullptr;
-      if (cudaStreamCreateWithFlags(&gs.rec_stream[i], cudaStreamNonBlocking) != cudaSuccess) return nullptr;
       if (cudaEventCreateWithFlags(&gs.join[i], cudaEventDisableTiming) != cudaSuccess) return nullptr;
-      if (cudaEventCreateWithFlags(&gs.rec_join[i], cudaEventDisableTiming) != cudaSuccess) return nullptr;
-      for (int h = 0; h < 2; ++h) {
-        if (cudaEventCreateWithFlags(&gs.rec_done[i][h], cudaEventDisableTiming) != cudaSuccess) return nullptr;
-        if (cudaEventCreateWithFlags(&gs.upd_done[i][h], cudaEventDisableTiming) != cudaSuccess) return nullptr;
-      }
     }
     if (cudaEventCreateWithFlags(&gs.fork, cudaEventDisableTiming) != cudaSuccess) return nullptr;
     gs.ready = true;
@@ -159,25 +153,36 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
   const gsx::SequencePrune prune_args{ring, t_max, c_stable, prune_scratch, margin, fs_scratch};
   const gsx::SequencePrune *prune = ring ? &prune_args : nullptr;
   const int64_t P = (int64_t)H * W;
+  // K4's scan epoch is ticket / tiles + 1 and must fit the 30 bits of a look-back state word
+  const int64_t tiles = (P + gsx::kTilePix - 1) / gsx::kTilePix;
+  GSX_CHECK_ARG((int64_t)(s_end - s_begin) * tiles < (1ll << 30),
+                "gsx_pointfusion_sequence_gt: %d frames of %lld K4 tiles in one call; split the call",
+                s_end - s_begin, (long long)tiles);
   cudaStream_t user = (cudaStream_t)stream;
   int G = gsx::sequence_groups(B);
-  // the group / record streams and their events are shared by every caller on the device: serialise the enqueue
+  // the group streams and their events are shared by every caller on the device: serialise the enqueue
   std::unique_lock<std::mutex> lock(gsx::g_groups_mutex);
   gsx::GroupStreams *gs = gsx::group_streams();
-  char *half[2] = {(char *)workspace, (char *)workspace + gsx::fusion_workspace_bytes(B, H, W)};
-  int rc = 0;
+  // slots, bin counts, scan states, tickets and table flags: zero once per call, so that nothing a failed or abandoned
+  // call left behind reaches this one
+  int rc = gsx::sequence_rearm(workspace, B, H, W, user);
+  if (rc) return rc;
+  // frames [s, s + F) of a header block: from s to the end of its kSeqFrames-aligned block or of the call
+  auto header_frames = [&](int s) {
+    return (s == s_begin || s % gsx::kSeqFrames == 0) ? std::min(gsx::kSeqFrames - s % gsx::kSeqFrames, s_end - s) : 0;
+  };
   if (!gs) {
     // no side streams available: everything in order on the caller's stream
     for (int s = s_begin; s < s_end && rc == 0; ++s) {
       int64_t max_count = max_count0 + (int64_t)(s - s_begin) * P;
       if (max_count > capacity) max_count = capacity;
-      rc = gsx::fusion_records_group(poses + (int64_t)s * 16, (int64_t)L * 16, intrinsics, 16, depth + (int64_t)s * P,
-                                     (int64_t)L * P, B, 0, B, H, W, sigma, half[0], user);
+      if (const int F = header_frames(s))
+        rc = gsx::sequence_headers_group(poses, intrinsics, depth, L, s, F, B, 0, B, H, W, sigma, workspace, user);
       if (rc == 0)
         rc = gsx::fusion_update_group(map_geometry, map_colors, counts + (int64_t)(s & 1) * B,
                                       counts + (int64_t)((s + 1) & 1) * B, capacity, max_count, poses + (int64_t)s * 16,
                                       (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, 0, B,
-                                      H, W, dist_th, dot_th, half[0], overflow_flag,
+                                      s, H, W, dist_th, dot_th, workspace, overflow_flag,
                                       gsx::sequence_assoc(prune, B, 0, B, H, W, capacity, user), user);
       if (rc == 0 && prune)
         rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, counts + (int64_t)((s + 1) & 1) * B, capacity,
@@ -187,12 +192,8 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
     return rc;
   }
   cudaEventRecord(gs->fork, user);
-  for (int g = 0; g < G; ++g) {
-    cudaStreamWaitEvent(gs->stream[g], gs->fork, 0);
-    cudaStreamWaitEvent(gs->rec_stream[g], gs->fork, 0);
-  }
+  for (int g = 0; g < G; ++g) cudaStreamWaitEvent(gs->stream[g], gs->fork, 0);
   for (int s = s_begin; s < s_end && rc == 0; ++s) {
-    const int h = s & 1;
     int32_t *cin = counts + (int64_t)(s & 1) * B;
     int32_t *cout = counts + (int64_t)((s + 1) & 1) * B;
     int64_t max_count = max_count0 + (int64_t)(s - s_begin) * P;
@@ -205,23 +206,20 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
         rc = 2;
         break;
       }
-      // frame records of frame s into half h, as soon as K4(s-2) has released that half
-      if (s >= s_begin + 2) cudaStreamWaitEvent(gs->rec_stream[g], gs->upd_done[g][h], 0);
-      rc = gsx::fusion_records_group(poses + (int64_t)s * 16, (int64_t)L * 16, intrinsics, 16, depth + (int64_t)s * P,
-                                     (int64_t)L * P, B, b0, b1 - b0, H, W, sigma, half[h], gs->rec_stream[g]);
+      // the group's headers of the next block, after its K4 of the frames that read the block's slots before
+      if (const int F = header_frames(s))
+        rc = gsx::sequence_headers_group(poses, intrinsics, depth, L, s, F, B, b0, b1 - b0, H, W, sigma, workspace,
+                                         gs->stream[g]);
       if (rc) break;
-      cudaEventRecord(gs->rec_done[g][h], gs->rec_stream[g]);
-      cudaStreamWaitEvent(gs->stream[g], gs->rec_done[g][h], 0);
       rc = gsx::fusion_update_group(map_geometry, map_colors, cin, cout, capacity, max_count, poses + (int64_t)s * 16,
                                     (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, b0,
-                                    b1 - b0, H, W, dist_th, dot_th, half[h], overflow_flag,
+                                    b1 - b0, s, H, W, dist_th, dot_th, workspace, overflow_flag,
                                     gsx::sequence_assoc(prune, B, b0, b1 - b0, H, W, capacity, gs->stream[g]),
                                     gs->stream[g]);
       if (rc == 0 && prune)
         rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, cout, capacity, intrinsics,
                                        poses + (int64_t)s * 16, (int64_t)L * 16, B, b0, b1 - b0, s, H, W,
                                        std::min(max_count + P, capacity), gs->stream[g]);
-      cudaEventRecord(gs->upd_done[g][h], gs->stream[g]);
     }
   }
   // join ALWAYS, also after a failed launch: whatever was already enqueued on the internal streams stays ordered before
@@ -229,13 +227,11 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
   for (int g = 0; g < G; ++g) {
     cudaEventRecord(gs->join[g], gs->stream[g]);
     cudaStreamWaitEvent(user, gs->join[g], 0);
-    cudaEventRecord(gs->rec_join[g], gs->rec_stream[g]);
-    cudaStreamWaitEvent(user, gs->rec_join[g], 0);
   }
   return rc;
 }
 
 extern "C" int64_t gsx_pointfusion_sequence_workspace_bytes(int B, int H, int W) {
   if (B < 0 || H < 0 || W < 0) return -1;
-  return 2 * gsx::fusion_workspace_bytes(B, H, W);
+  return gsx::sequence_workspace_bytes(B, H, W);
 }

@@ -1,8 +1,10 @@
 // Fused PointFusion map update for sm_90a.
-//   k_frame_records   (K1r)    one thread per live pixel: re-arms the per-frame workspace and writes the element's header
-//                              (camera, depth image).  Nothing per pixel is stored: the consumers re-evaluate the world
-//                              vertex, world normal (rgbdimages.py:643-762) and confidence weight (fusionutils.py:16-73)
-//                              from the pixel's depth stencil, bit for bit.
+//   k_frame_records   (K1r)    step API only, one CTA per K4 tile: re-arms the tile's bin count and scan state, clears
+//                              slots an abandoned frame left, and writes the element's header (camera, depth image).
+//                              The sequence driver writes the headers with k_frame_headers instead.  Nothing per pixel
+//                              is stored: the consumers re-evaluate the world vertex, world normal
+//                              (rgbdimages.py:643-762) and confidence weight (fusionutils.py:16-73) from the pixel's
+//                              depth stencil, bit for bit.
 //   k_project_select  (K2+K3)  one thread per map row: project into the live camera, frustum test, gather of the depth
 //                              stencil under the projection, distance / normal tests, then each live candidate, with
 //                              its key (1/ccount, ray distance, row index), is appended to the bin of the K4 tile that
@@ -37,32 +39,52 @@ __device__ __forceinline__ float confidence_alpha(float sq_norm, float two_sigma
   return fminf(fmaxf(confidence_exp(sq_norm, two_sigma_sq), 1e-7f), 1.01f);
 }
 
-// ---- K1r ------------------------------------------------------------------------------------------------
-struct FrameRecArgs {
-  const float *depth;  // (B,H,W) live depth
-  int64_t depth_bstride;
+// ---- K1r and the frame headers ----------------------------------------------------------------------------
+// Where the frames of a (B, F) block are: element b's frame f starts at base + b * bstride + f * fstride.
+struct FrameSource {
+  const float *depth;  // (H,W) live depth images
+  int64_t depth_bstride, depth_fstride;
   const float *K;
   int64_t K_bstride;
   const float *poses;  // camera-to-world, or null: world frame == camera frame
-  int64_t pose_bstride;
-  int B, H, W;
+  int64_t pose_bstride, pose_fstride;
   float two_sigma_sq;
-  Workspace ws;
 };
 
-constexpr int kRecTW = 32, kRecTH = 8;  // pixel tile of one K1r CTA
-
-// element b's FrameHeader, by one thread of the element's first K1r CTA.  Without poses world frame == camera frame
-// (the pose stays zero).
-__device__ __forceinline__ void store_frame_header(const FrameRecArgs &a, int b) {
+// Element b's header of frame f.  Without poses world frame == camera frame (the pose stays zero).
+__device__ __forceinline__ FrameHeader make_frame_header(const FrameSource &a, int b, int f) {
   FrameHeader hd = {};
   hd.cam.k = load_kinv(a.K + b * a.K_bstride);
-  if (a.poses) hd.cam.pose = load_rigid(a.poses + b * a.pose_bstride);
+  if (a.poses) hd.cam.pose = load_rigid(a.poses + b * a.pose_bstride + f * a.pose_fstride);
   hd.cam.posed = a.poses != nullptr;
   hd.two_sigma_sq = a.two_sigma_sq;
-  hd.depth = a.depth + b * a.depth_bstride;
-  a.ws.hdr[b] = hd;
+  hd.depth = a.depth + b * a.depth_bstride + f * a.depth_fstride;
+  return hd;
 }
+
+// hdr[f * hdr_fstride + b] for the F frames of B elements, one thread each
+__global__ void __launch_bounds__(128) k_frame_headers(FrameSource a, int B, int F, FrameHeader *hdr,
+                                                       int64_t hdr_fstride) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * F) return;
+  const int b = i % B, f = i / B;
+  hdr[f * hdr_fstride + b] = make_frame_header(a, b, f);
+}
+
+int launch_frame_headers(const FrameSource &a, int B, int F, FrameHeader *hdr, int64_t hdr_fstride,
+                         cudaStream_t stream) {
+  if (B == 0 || F == 0) return 0;
+  k_frame_headers<<<(unsigned)((B * F + 127) / 128), 128, 0, stream>>>(a, B, F, hdr, hdr_fstride);
+  GSX_CHECK_LAUNCH("gsx_fusion_frame_headers");
+  return 0;
+}
+
+struct FrameRecArgs {
+  FrameSource src;  // frame 0 of each element
+  int B, H, W;
+  int bin_cap;  // records per candidate bin (set at launch): a count above it means the tile's slots may be dirty
+  Workspace ws;
+};
 
 // Pixel (h,w)'s world normal gn and world vertex fv.xyz (and, if kAlpha, its confidence weight fv.w): the values K1
 // computes for that pixel, bit for bit.  The stencil is gathered (its centre dc = hd.depth[h * W + w] already loaded)
@@ -85,32 +107,41 @@ __device__ __forceinline__ void load_frame_header(FrameHeader &s, const FrameHea
   if (i >= 0 && i < kWords) reinterpret_cast<int *>(&s)[i] = __ldg(reinterpret_cast<const int *>(g) + i);
 }
 
-// K1r only re-arms the workspace for the frame and writes the header: K2 and K4 evaluate what they need from the depth
-// image itself.
-__global__ void __launch_bounds__(kRecTW *kRecTH) k_frame_records(FrameRecArgs a) {
-  const int b = blockIdx.z;
-  const int tid = threadIdx.y * kRecTW + threadIdx.x;
-  // re-arm the scan state of this element for the frame's K4
-  const int lin = (blockIdx.y * gridDim.x + blockIdx.x) * (kRecTW * kRecTH) + tid;
-  if (lin < a.ws.tiles) {
-    a.ws.tile_state[(int64_t)b * a.ws.tiles + lin] = 0ull;
-    a.ws.bin_count[(int64_t)b * a.ws.tiles + lin] = 0u;
+// K1r re-arms the workspace for one frame of the step API and writes the header: K2 and K4 evaluate what they need
+// from the depth image itself.  One CTA per K4 tile.  A tile's slots are zero after every complete frame (K4 restores
+// them); they can be dirty only when an earlier frame stopped before its K4, with the tile's bin overflowed or the
+// element's table flag set, and only then are they cleared here.  The flag itself stays set until a K4 clears it.
+__global__ void __launch_bounds__(kMB) k_frame_records(FrameRecArgs a) {
+  __shared__ int s_dirty;
+  const int t = blockIdx.x, b = blockIdx.y;
+  const int64_t bt = (int64_t)b * a.ws.tiles + t;
+  if (threadIdx.x == 0) {
+    s_dirty = a.ws.table[b] != 0u || a.ws.bin_count[bt] > (unsigned int)a.bin_cap;
+    a.ws.bin_count[bt] = 0u;
+    a.ws.tile_state[bt] = 0ull;
+    if (t == 0) {
+      a.ws.ticket[b] = 0u;
+      a.ws.hdr[b] = make_frame_header(a.src, b, 0);
+    }
   }
-  if (lin == 0) {
-    a.ws.ticket[b] = 0u;
-    store_frame_header(a, b);
-  }
-  const int w = blockIdx.x * kRecTW + threadIdx.x, h = blockIdx.y * kRecTH + threadIdx.y;
-  if (w >= a.W || h >= a.H) return;
+  __syncthreads();
+  if (!s_dirty) return;
   const int P = a.H * a.W;
-  a.ws.win[(int64_t)b * P + h * a.W + w] = 0u;
+  const int end = min(P, (t + 1) * kTilePix);
+  for (int p = t * kTilePix + (int)threadIdx.x; p < end; p += kMB) a.ws.win[(int64_t)b * P + p] = 0u;
 }
 
-int launch_frame_records(const FrameRecArgs &a, cudaStream_t stream) {
-  if (a.B == 0) return 0;
-  const dim3 grid((unsigned)((a.W + kRecTW - 1) / kRecTW), (unsigned)((a.H + kRecTH - 1) / kRecTH), (unsigned)a.B);
-  const dim3 block(kRecTW, kRecTH);
-  k_frame_records<<<grid, block, 0, stream>>>(a);
+// Test hook (tests/test_gpu_binned_argmin.py): caps the records per candidate bin that K2 fills and K4 reads, so that
+// small frames exercise the overflow to the arg-min slots.  Negative = kBinCap.  K1r judges an abandoned frame's tiles
+// against the capacity in force, so change it only between complete frames.
+static int g_bin_cap = -1;
+static int bin_capacity() { return g_bin_cap >= 0 && g_bin_cap < kBinCap ? g_bin_cap : kBinCap; }
+
+int launch_frame_records(const FrameRecArgs &args, cudaStream_t stream) {
+  if (args.B == 0) return 0;
+  FrameRecArgs a = args;
+  a.bin_cap = bin_capacity();
+  k_frame_records<<<dim3((unsigned)a.ws.tiles, (unsigned)a.B), kMB, 0, stream>>>(a);
   GSX_CHECK_LAUNCH("gsx_fusion_frame_records");
   return 0;
 }
@@ -260,11 +291,6 @@ __global__ void __launch_bounds__(kBlock, GSX_K2_MINB) k_project_select(ProjectA
 // passes.  0 = the shipped cap below.
 static int g_k2_grid_cap = 0;
 
-// Test hook (tests/test_gpu_binned_argmin.py): caps the records per candidate bin that K2 fills and K4 reads, so that
-// small frames exercise the overflow to the arg-min slots.  Negative = kBinCap.
-static int g_bin_cap = -1;
-static int bin_capacity() { return g_bin_cap >= 0 && g_bin_cap < kBinCap ? g_bin_cap : kBinCap; }
-
 int launch_project_select(const ProjectArgs &args, int64_t max_count, cudaStream_t stream) {
   if (args.B == 0 || max_count <= 0) return 0;
   ProjectArgs a = args;
@@ -295,9 +321,6 @@ struct MergeArgs {
   int bin_cap;     // records per candidate bin that K2 filled (set at launch)
 };
 
-// K1r zeroes K4's tile states before every frame, so K4's scan always runs in epoch 1
-constexpr unsigned int kMergeEpoch = 1u;
-
 #ifndef GSX_K4_MINB
 #define GSX_K4_MINB 4
 #endif
@@ -310,7 +333,7 @@ __device__ __forceinline__ void prefetch_l2(const float *p) { asm volatile("pref
 
 template <bool kAssoc>
 __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) {
-  __shared__ int s_tile;
+  __shared__ unsigned int s_ticket, s_table;
   __shared__ int s_warp_sums[kPix][kMB / 32];
   __shared__ int s_matched[kMB / 32];
   __shared__ int s_excl;
@@ -323,7 +346,8 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   // each element's look-back chain only sees ~1/B of the in-flight tiles
   const int b = blockIdx.x % a.B;
   const int T = a.ws.tiles;
-  if (threadIdx.x == 0) s_tile = (int)atomicAdd(a.ws.ticket + b, 1u);  // tiles start in ticket order
+  if (threadIdx.x == 0) s_ticket = atomicAdd(a.ws.ticket + b, 1u);  // tiles start in ticket order
+  if (threadIdx.x == 32) s_table = a.ws.table[b];
   for (int i = threadIdx.x; i < kTilePix; i += kMB) {
     s_key[i] = ~0ull;
     s_n[i] = ~0u;
@@ -331,13 +355,19 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   load_frame_header(s_hdr, a.ws.hdr + b);
   const int count_in = a.counts_in[b];  // loaded early: its latency hides behind everything below
   __syncthreads();
-  const int tile = s_tile;
+  // the ticket counts on over the frames of a sequence call: each frame's scan runs in its own epoch, so no tile state
+  // has to be re-armed between frames
+  const int tile = (int)(s_ticket % (unsigned int)T);
+  const unsigned int epoch = s_ticket / (unsigned int)T + 1u;
   const int P = a.H * a.W;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int pix0 = tile * kTilePix;
-  const unsigned int *win = a.ws.win + (int64_t)b * P;
+  unsigned int *win = a.ws.win + (int64_t)b * P;
   const float *rgb = a.rgb + b * a.rgb_bstride + (int64_t)pix0 * 3;
-  const int n_bin = (int)min(a.ws.bin_count[(int64_t)b * T + tile], (unsigned int)a.bin_cap);
+  const unsigned int bin_count = a.ws.bin_count[(int64_t)b * T + tile];
+  const int n_bin = (int)min(bin_count, (unsigned int)a.bin_cap);
+  // the tile's slots can be non-zero only if its bin overflowed or gsx_records_from_table filled the element's slots
+  const bool read_slots = bin_count > (unsigned int)a.bin_cap || s_table != 0u;
   const uint4 *bin = a.ws.bin + ((int64_t)b * T + tile) * kBinCap;
 
   // live colours of the tile: coalesced 128-bit loads into shared memory (stride-3 reads are conflict free)
@@ -361,7 +391,10 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
     slot[j] = 0u;
     dep[j] = 0.0f;
     if (pix[j] < P) {
-      slot[j] = win[pix[j]];
+      if (read_slots) {
+        slot[j] = win[pix[j]];
+        if (slot[j] != 0u) win[pix[j]] = 0u;  // every slot is zero again when the next frame's K2 starts
+      }
       dep[j] = __ldg(s_hdr.depth + pix[j]);
     }
   }
@@ -437,7 +470,10 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
         }
       });
   unsigned long long *state = a.ws.tile_state + (int64_t)b * T;
-  if (threadIdx.x == 0) publish_tile(state, tile, T, kMergeEpoch, kTileAggregate, (unsigned)block_total);
+  if (threadIdx.x == 0) {
+    if (bin_count != 0u) a.ws.bin_count[(int64_t)b * T + tile] = 0u;  // every thread has read it (barrier above)
+    publish_tile(state, tile, T, epoch, kTileAggregate, (unsigned)block_total);
+  }
 
   float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
   float *col = a.col + (int64_t)b * a.cap * kColW;
@@ -498,7 +534,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
 
   // decoupled look-back (warp 0): exclusive prefix of new-point counts over preceding tiles of this element
   if (warp == 0) {
-    const unsigned int excl = lookback_warp(state, tile, T, kMergeEpoch, (unsigned)block_total);
+    const unsigned int excl = lookback_warp(state, tile, T, epoch, (unsigned)block_total);
     if (lane == 0) s_excl = (int)excl;
   }
   __syncthreads();
@@ -523,6 +559,9 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   if (tile == T - 1 && threadIdx.x == 0) {
     const int64_t total = base + block_total;
     a.counts_out[b] = (int32_t)(total < a.cap ? total : a.cap);
+    // every other tile of the element read the flag before it published its state, and this tile's look-back has
+    // seen all of them (directly or through an inclusive prefix)
+    if (s_table != 0u) a.ws.table[b] = 0u;
   }
 }
 
@@ -671,10 +710,47 @@ __global__ void __launch_bounds__(256) k_merge_bwd_pixels(MergeBwdArgs a) {
   }
 }
 
-// The two halves of one frame for the batch elements [b0, b0 + nb) of a B_total-element problem, on `st`: the frame
-// records (K1r), and the map update that consumes them (K2 + K4).  All pointers are the FULL-batch base pointers; batch
-// elements are independent, so disjoint groups may run concurrently on different streams, and the records of the next
-// frame may be computed (into another workspace) while this frame's update runs (gsx_pointfusion_sequence_gt).
+// The sequence driver (gsx_pointfusion_sequence_gt) runs no K1r.  Its workspace is one fusion workspace followed by
+// the frame headers of kSeqFrames consecutive frames, hdr[f][B]: frame s of element b reads header [s % kSeqFrames][b],
+// written by one k_frame_headers launch per group and kSeqFrames frames, in the group's stream order.  The re-arm
+// state is zeroed once per call (sequence_rearm); from then on K4 keeps it armed from frame to frame.
+int64_t fusion_workspace_bytes(int B, int H, int W) {
+  int64_t bytes;
+  fusion_workspace(nullptr, B, H, W, &bytes);
+  return bytes;
+}
+
+static FrameHeader *seq_headers(void *workspace, int B, int H, int W) {
+  return reinterpret_cast<FrameHeader *>((char *)workspace + fusion_workspace_bytes(B, H, W));
+}
+
+int64_t sequence_workspace_bytes(int B, int H, int W) {
+  return fusion_workspace_bytes(B, H, W) + ((int64_t)kSeqFrames * B * (int64_t)sizeof(FrameHeader) + 255) / 256 * 256;
+}
+
+int sequence_rearm(void *workspace, int B, int H, int W, cudaStream_t st) {
+  int64_t rearm = 0;
+  const Workspace ws = fusion_workspace(workspace, B, H, W, nullptr, &rearm);
+  if (cudaMemsetAsync(ws.win, 0, (size_t)rearm, st) != cudaSuccess) {
+    set_error("gsx_pointfusion_sequence_gt: re-arm memset failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  return 0;
+}
+
+// the frames [s, s + F) of the group's elements; s % kSeqFrames + F <= kSeqFrames
+int sequence_headers_group(const float *poses, const float *K, const float *depth, int L, int s, int F, int B_total,
+                           int b0, int nb, int H, int W, double sigma, void *workspace, cudaStream_t st) {
+  const int64_t P = (int64_t)H * W;
+  const FrameSource src{depth + ((int64_t)b0 * L + s) * P, (int64_t)L * P, P, K + (int64_t)b0 * 16, 16,
+                        poses + ((int64_t)b0 * L + s) * 16, (int64_t)L * 16, 16, (float)(2.0 * (sigma * sigma))};
+  return launch_frame_headers(src, nb, F, seq_headers(workspace, B_total, H, W) + (int64_t)(s % kSeqFrames) * B_total + b0,
+                              B_total, st);
+}
+
+// The map update of one frame (K2 + K4) for the batch elements [b0, b0 + nb) of a B_total-element problem, on `st`.
+// All pointers are the FULL-batch base pointers; batch elements are independent, so disjoint groups may run
+// concurrently on different streams.
 static Workspace group_workspace(void *workspace, int B_total, int b0, int H, int W) {
   const int64_t P = (int64_t)H * W;
   Workspace ws = fusion_workspace(workspace, B_total, H, W);
@@ -684,23 +760,17 @@ static Workspace group_workspace(void *workspace, int B_total, int b0, int H, in
   ws.bin_count += (int64_t)b0 * ws.tiles;
   ws.bin += (int64_t)b0 * ws.tiles * kBinCap;
   ws.ticket += b0;
+  ws.table += b0;
   ws.stats += 2 * b0;
   return ws;
 }
 
-int fusion_records_group(const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *depth,
-                         int64_t d_bs, int B_total, int b0, int nb, int H, int W, double sigma, void *workspace,
-                         cudaStream_t st) {
-  FrameRecArgs fa{depth + (int64_t)b0 * d_bs, d_bs, K + (int64_t)b0 * K_bs, K_bs, poses + (int64_t)b0 * pose_bs, pose_bs,
-                  nb, H, W, (float)(2.0 * (sigma * sigma)), group_workspace(workspace, B_total, b0, H, W)};
-  return launch_frame_records(fa, st);
-}
-
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
-                        int64_t rgb_bs, int B_total, int b0, int nb, int H, int W, float dist_th, float dot_th,
+                        int64_t rgb_bs, int B_total, int b0, int nb, int s, int H, int W, float dist_th, float dot_th,
                         void *workspace, int32_t *overflow, int32_t *assoc, cudaStream_t st) {
-  const Workspace ws = group_workspace(workspace, B_total, b0, H, W);
+  Workspace ws = group_workspace(workspace, B_total, b0, H, W);
+  ws.hdr = seq_headers(workspace, B_total, H, W) + (int64_t)(s % kSeqFrames) * B_total + b0;
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
   if (max_count > 0) {
     ProjectArgs pa{ggeo, cin + b0, cap, poses + (int64_t)b0 * pose_bs, pose_bs, K + (int64_t)b0 * K_bs, K_bs, nb,
@@ -713,12 +783,6 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow,
                assoc ? assoc + (int64_t)b0 * H * W : nullptr, 0};
   return launch_merge_append(ma, st);
-}
-
-int64_t fusion_workspace_bytes(int B, int H, int W) {
-  int64_t bytes;
-  fusion_workspace(nullptr, B, H, W, &bytes);
-  return bytes;
 }
 
 }  // namespace gsx
@@ -744,9 +808,26 @@ extern "C" int gsx_fusion_frame_records(const float *depth, int64_t depth_bstrid
   if (B == 0) return 0;
   GSX_CHECK_ARG(depth && intrinsics && workspace, "gsx_fusion_frame_records: null pointer");
   GSX_CHECK_ARG(aligned16(workspace), "gsx_fusion_frame_records: the workspace must be 16-byte aligned");
-  FrameRecArgs a{depth, depth_bstride, intrinsics, K_bstride, poses, pose_bstride, B, H, W,
-                 (float)(2.0 * (sigma * sigma)), fusion_workspace(workspace, B, H, W)};
+  FrameRecArgs a{{depth, depth_bstride, 0, intrinsics, K_bstride, poses, pose_bstride, 0, (float)(2.0 * (sigma * sigma))},
+                 B, H, W, 0, fusion_workspace(workspace, B, H, W)};
   return launch_frame_records(a, (cudaStream_t)stream);
+}
+
+extern "C" int gsx_fusion_sequence_frame(const float *depth, int64_t depth_bstride, const float *intrinsics,
+                                         int64_t K_bstride, const float *poses, int64_t pose_bstride, int B, int H,
+                                         int W, double sigma, int rearm, void *workspace, void *stream) {
+  GSX_CHECK_ARG(B >= 0 && H >= 2 && W >= 2, "gsx_fusion_sequence_frame: bad extents B=%d H=%d W=%d", B, H, W);
+  if (B == 0) return 0;
+  GSX_CHECK_ARG(depth && intrinsics && poses && workspace, "gsx_fusion_sequence_frame: null pointer");
+  GSX_CHECK_ARG(aligned16(workspace), "gsx_fusion_sequence_frame: the workspace must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rearm) {
+    const int rc = sequence_rearm(workspace, B, H, W, st);
+    if (rc) return rc;
+  }
+  const FrameSource src{depth, depth_bstride, 0, intrinsics, K_bstride, poses, pose_bstride, 0,
+                        (float)(2.0 * (sigma * sigma))};
+  return launch_frame_headers(src, B, 1, fusion_workspace(workspace, B, H, W).hdr, 0, st);
 }
 
 extern "C" int gsx_fusion_project_select(const float *map_geometry, const int32_t *counts, int64_t capacity,

@@ -20,6 +20,9 @@ constexpr int kTilePix = kMB * kPix;  // pixels per merge tile
 #endif
 constexpr int kBinCap = GSX_BIN_CAP;
 
+// frames whose headers the sequence driver's workspace holds at a time (gsx_fusion.cu: sequence_workspace_bytes)
+constexpr int kSeqFrames = 64;
+
 // How K2 / K4 get a pixel's world vertex, world normal and confidence weight, per batch element (written by K1r).
 // Nothing per pixel is stored: K2 and K4 gather the pixel's depth stencil from the caller's depth image and re-evaluate
 // vertex, normal and weight with K1r's camera and device functions, bit for bit.  The 1.2 MB depth image of an element
@@ -31,38 +34,52 @@ struct FrameHeader {
 };
 
 //   FrameHeader hdr[B]         where the depth is, how to re-evaluate vertex / normal / weight  written by K1r
-//   uint32 win[B][P]           arg-min slot: n + 1 of the winning row, 0 = none; only K2's      cleared by K1r
+//   uint32 win[B][P]           arg-min slot: n + 1 of the winning row, 0 = none; only K2's      zero when K2 starts
 //                              bin overflow and gsx_records_from_table write it
-//   uint64 tile_state[B][T]    look-back state of K4's scan (epoch 1), T = ceil(P / kTilePix)  cleared by K1r
-//   uint32 bin_count[B][T]     candidates K2 appended to the tile's bin (may exceed kBinCap)    cleared by K1r
+//   uint64 tile_state[B][T]    look-back state of K4's scan, T = ceil(P / kTilePix)            epoch from the ticket
+//   uint32 bin_count[B][T]     candidates K2 appended to the tile's bin (may exceed kBinCap)    zeroed by K4
+//   uint32 ticket[B]           K4's tickets: tile = ticket % T, scan epoch = ticket / T + 1
+//   uint32 table[B]            non-zero: gsx_records_from_table filled slots of the element    cleared by K4
 //   uint4  bin[B][T][kBinCap]  candidates (key_hi lo, key_hi hi, n, pixel offset in the tile)  written by K2
-//   uint32 ticket[B]           dynamic tile ids of K4                                           cleared by K1r
 //   uint64 stats[B][2]         running totals: {active map rows (in frustum), merged rows}      caller zeroes once
-// Nothing in here has to survive from one frame to the next (the stats are bookkeeping only): every frame's K1r
-// re-arms what K2 / K4 of that frame consume, so a failed or abandoned call cannot poison a later one.
+// win .. table form the re-arm state, one contiguous byte range (rearm_bytes): all zero is a valid start, and the
+// step API's workspace must start so (zero-filled once before first use: no kernel clears the slots per frame).  The
+// invariant is kept by the consumer: every slot is zero when a frame's K2 starts.  K4 reads a tile's slots only when
+// the tile's bin overflowed or the element's table flag is set, and stores zero to the slots it read; so on a frame
+// without overflow no slot is read or written.  K4 zeroes its tile's bin count once it has read it, and the scan's last
+// tile clears the table flag.  A frame abandoned before its K4 (K2 or the table fill ran, K4 did not) leaves
+// dirty slots: K1r (the per-frame step API) clears the slots of every tile whose bin count exceeds the capacity, and of
+// the whole element while its table flag is set, before it re-arms the counts.  The sequence driver runs no K1r: it
+// zeroes the re-arm state once per call, so nothing survives from one call to the next.
 struct Workspace {
   FrameHeader *hdr;
   unsigned int *win;
   unsigned long long *tile_state;
   unsigned int *bin_count;
-  uint4 *bin;
   unsigned int *ticket;
+  unsigned int *table;
+  uint4 *bin;
   unsigned long long *stats;
   int tiles;
 };
 
-// the workspace at `base` (nullptr: byte offsets); `bytes`, if given, receives its size
-inline Workspace fusion_workspace(void *base, int B, int H, int W, int64_t *bytes = nullptr) {
+// the workspace at `base` (nullptr: byte offsets); `bytes`, if given, receives its size; `rearm_bytes`, if given, the
+// size of the re-arm state that starts at win
+inline Workspace fusion_workspace(void *base, int B, int H, int W, int64_t *bytes = nullptr,
+                                  int64_t *rearm_bytes = nullptr) {
   const int64_t P = (int64_t)H * W;
   Carver c(base);
   Workspace w;
   w.tiles = (int)((P + kTilePix - 1) / kTilePix);
   w.hdr = c.take<FrameHeader>(B);
+  const int64_t rearm0 = c.bytes;
   w.win = c.take<unsigned int>(B * P);
   w.tile_state = c.take<unsigned long long>((int64_t)B * w.tiles);
   w.bin_count = c.take<unsigned int>((int64_t)B * w.tiles);
-  w.bin = c.take<uint4>((int64_t)B * w.tiles * kBinCap);
   w.ticket = c.take<unsigned int>(B);
+  w.table = c.take<unsigned int>(B);
+  if (rearm_bytes) *rearm_bytes = c.bytes - rearm0;
+  w.bin = c.take<uint4>((int64_t)B * w.tiles * kBinCap);
   w.stats = c.take<unsigned long long>(2 * (int64_t)B);
   if (bytes) *bytes = c.bytes;
   return w;

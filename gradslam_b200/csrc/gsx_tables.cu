@@ -242,8 +242,13 @@ extern "C" int gsx_records_from_table(const int64_t *table, int64_t rows, int64_
   if (rows == 0) return 0;
   GSX_CHECK_ARG(table && workspace, "gsx_records_from_table: null pointer");
   GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_records_from_table: capacity must fit int32");
-  RowArgs a{table, rows, nullptr, capacity, nullptr, nullptr, B, H, W, 0.f, 0.f, nullptr,
-            fusion_workspace(workspace, B, H, W).win};
+  const Workspace ws = fusion_workspace(workspace, B, H, W);
+  RowArgs a{table, rows, nullptr, capacity, nullptr, nullptr, B, H, W, 0.f, 0.f, nullptr, ws.win};
+  // the table flags tell K4 to read the slots (and K1r, should this frame stop before its K4, to clear them)
+  if (cudaMemsetAsync(ws.table, 0xff, (size_t)B * sizeof(unsigned int), (cudaStream_t)stream) != cudaSuccess) {
+    set_error("gsx_records_from_table: table-flag memset failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
   k_records_from_table<<<(unsigned)tb_blocks(rows), kTB, 0, (cudaStream_t)stream>>>(a);
   GSX_CHECK_LAUNCH("gsx_records_from_table");
   return 0;

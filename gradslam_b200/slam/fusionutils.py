@@ -76,17 +76,19 @@ def are_normals_similar(tensor1: torch.Tensor, tensor2: torch.Tensor, dot_th: Un
 
 # --------------------------------------------------------------------------------------------- workspaces
 class _Workspace:
-    """Per (device, stream, B, H, W) scratch of the fusion kernels: frame records, arg-min slots, scan state.  Nothing
-    in it survives from frame to frame (gsx_fusion_frame_records re-arms it), so there is no epoch or "left clean"
-    invariant to break; it is keyed by the CUDA stream as well, so maps updated concurrently from different streams or
-    threads never share records."""
+    """Per (device, stream, B, H, W) scratch of the fusion kernels: frame header, arg-min slots, candidate bins, scan
+    state.  gsx_fusion_frame_records re-arms it for every frame; the arg-min slots are kept zero by the merge kernel,
+    and K1r clears those a frame abandoned before its merge left behind.  It is keyed by the CUDA stream as well, so
+    maps updated concurrently from different streams or threads never share records."""
 
     _cache = {}
     _lock = threading.Lock()
 
     def __init__(self, device, B, H, W):
         nbytes = _C.lib().gsx_fusion_workspace_bytes(B, H, W)
-        self.buf = torch.zeros(nbytes, dtype=torch.uint8, device=device)  # (zero: the statistics start at 0)
+        # zeroed once: the arg-min slots are never cleared per frame (a non-zero slot reads as a winning map row), and
+        # the statistics start at 0
+        self.buf = torch.zeros(nbytes, dtype=torch.uint8, device=device)
         self.shape = (B, H * W)
         self.assoc = None  # K4's per-pixel record for the free-space step (fuse_and_prune), allocated on first use
 

@@ -21,7 +21,8 @@ __all__ = ["PointFusion"]
 
 
 class _SequenceWorkspace:
-    """Scratch of gsx_pointfusion_sequence_gt (two frame workspaces used alternately), per (device, stream, B, H, W)."""
+    """Scratch of gsx_pointfusion_sequence_gt (one frame workspace and a block of frame headers, re-armed by every
+    call), per (device, stream, B, H, W)."""
 
     _cache = {}
 
@@ -116,7 +117,7 @@ class PointFusion(ICPSLAM):
         return super().forward(frames, out)
 
     def _forward_sequence(self, frames, chunk: int = 4, raw: bool = False, out=None):
-        """odom='gt': the whole (B, L) sequence runs as C calls chaining K1 -> K2/K3 -> K4 per frame with no
+        """odom='gt': the whole (B, L) sequence runs as C calls chaining K2/K3 -> K4 per frame with no
         host synchronisation.  Frames that live in HOST memory are uploaded `chunk` frames at a time on a side
         stream, so the copy of chunk i+1 overlaps the fusion of chunk i (pin the host tensors for this)."""
         if self.odom != "gt" or frames.poses is None or torch.is_tensor(self.sigma):

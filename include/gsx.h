@@ -81,9 +81,12 @@ int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const
  *          gradslam/structures/pointclouds.py:526-614, 1117-1237
  *
  * Workspace: gsx_fusion_workspace_bytes(B,H,W) bytes, 16-byte aligned (B * ceil(H*W/512) candidate bins of 16 KB
- * each, per-pixel arg-min slots and frame headers: about 88.5 MB at B=8, 640x480).  Nothing in it has to survive from one frame
- * to the next: gsx_fusion_frame_records re-arms everything the other two kernels consume, so no zero-fill and no
- * epoch bookkeeping is needed and an abandoned frame cannot poison the next one.  (Only the statistics below
+ * each, per-pixel arg-min slots and frame headers: about 88.5 MB at B=8, 640x480).  Zero-fill it ONCE before its
+ * first use (cudaMemsetAsync to 0): the per-pixel arg-min slots are not cleared per frame, so a fresh allocation's
+ * contents would be read as winning map rows.  From then on gsx_fusion_frame_records re-arms what the other two
+ * kernels consume (bin counts, scan states, tickets, the frame header).  The per-pixel arg-min slots are kept zero by gsx_fusion_merge_append, which clears the slots it reads; an
+ * abandoned frame (project_select or gsx_records_from_table ran, merge_append did not) cannot poison the next one,
+ * because gsx_fusion_frame_records clears the slots such a frame may have left.  (Only the statistics below
  * accumulate; zero them once if they are read.)                                                            */
 int64_t gsx_fusion_workspace_bytes(int B, int H, int W);
 /* byte offset inside the workspace of uint64 stats[B][2] = running totals of {map points inside the
@@ -101,6 +104,14 @@ int64_t gsx_fusion_workspace_stats_offset(int B, int H, int W);
 int gsx_fusion_frame_records(const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
                              const float *poses, int64_t pose_bstride, int B, int H, int W, double sigma,
                              void *workspace, void *stream);
+
+/* How gsx_pointfusion_sequence_gt prepares a frame, for timing its K2 / K4 through gsx_fusion_project_select and
+ * gsx_fusion_merge_append: writes the live frame's header (as gsx_fusion_frame_records does) and re-arms nothing,
+ * except that rearm != 0 first zeroes the workspace's re-arm state (slots, bin counts, scan states, tickets), as the
+ * driver does once per call.  Same depth lifetime as gsx_fusion_frame_records. */
+int gsx_fusion_sequence_frame(const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
+                              const float *poses, int64_t pose_bstride, int B, int H, int W, double sigma, int rearm,
+                              void *workspace, void *stream);
 
 /* K2+K3: project every map point into the live camera, keep points that are in the frustum, close to
  * the frame vertex they land on and with a similar normal, and reduce per pixel to the best candidate
@@ -139,7 +150,9 @@ int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, 
                                 int B, int H, int W, double sigma, float *d_map_geometry, float *d_map_colors,
                                 float *d_gvertex, float *d_gnormal, float *d_rgb, float *d_vertex, void *stream);
 
-/* Whole-sequence driver with ground-truth poses: for s in [s_begin,s_end): K1r -> K2/K3 -> K4, no host sync.
+/* Whole-sequence driver with ground-truth poses: for s in [s_begin,s_end): K2/K3 -> K4, no host sync and no K1r.  The
+ * workspace's re-arm state is zeroed once per call and then kept armed by K4 from frame to frame, so nothing survives
+ * from one call to the next, also after a failed call.  Frame headers are written for blocks of 64 frames.
  * replaces ICPSLAM.forward with odom='gt' + PointFusion._map   gradslam/slam/icpslam.py:99-138,
  *          gradslam/slam/pointfusion.py:107-112
  * depth (B,L,H,W), rgb (B,L,H,W,3) dense; poses (B,L,4,4) dense; intrinsics (B,4,4) dense.
@@ -156,10 +169,11 @@ int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, 
  * pixel's merge in fs_scratch: gsx_fusion_free_space_scratch_bytes(B, H, W, capacity) bytes, 16-byte aligned. */
 /* number of independent batch groups gsx_pointfusion_sequence_gt runs on concurrent internal streams for a batch of
  * B (default 2, environment GSX_SEQ_GROUPS = 1..4 overrides; never more than B).  Kernel launches per call =
- * groups * (3 * frames - [map empty on entry]). */
+ * groups * (2 * frames - [map empty on entry] + header launches), plus one memset; a group launches one header
+ * launch for each 64-frame block (frames [64k, 64k + 64)) that [s_begin, s_end) touches. */
 int gsx_pointfusion_sequence_groups(int B);
-/* workspace of the sequence driver: two frame workspaces used alternately (the records of frame s+1 are computed on a
- * side stream while frame s is fused), 16-byte aligned, no initialisation needed */
+/* workspace of the sequence driver: one frame workspace (gsx_fusion_workspace_bytes) plus the headers of 64 frames
+ * (about 88.5 MB at B=8, 640x480), 16-byte aligned, no initialisation needed */
 int64_t gsx_pointfusion_sequence_workspace_bytes(int B, int H, int W);
 int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
                                 int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
