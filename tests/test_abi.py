@@ -74,6 +74,27 @@ def test_host_only_entry_points():
     assert rc != 0 and b"null" in lib.gsx_last_error()
 
 
+@pytest.mark.parametrize("H,W,s_begin,frames", [(2, 2, 0, 1 << 30), (480, 640, 5, 1_789_570)],
+                         ids=["one_tile", "600_tiles"])
+def test_sequence_call_refuses_more_scan_epochs_than_a_state_word_holds(H, W, s_begin, frames):
+    """K4's scan epoch is ticket / tiles + 1 and the ticket counts on through a call: gsx_pointfusion_sequence_gt refuses
+    a call of (s_end - s_begin) * tiles >= 2^30 before any CUDA call, and leaves every buffer as it was.
+    1 789 570 frames of 600 tiles is the first frame count past the bound (1 789 569 * 600 < 2^30)."""
+    tiles = (H * W + 511) // 512
+    assert frames * tiles >= 1 << 30 > (frames - 1) * tiles
+    bufs = [torch.full((256,), -7.25) for _ in range(9)]  # geometry, colours, counts, depth, rgb, K, poses, ws, flag
+    assert all(t.data_ptr() % 16 == 0 for t in bufs)
+    geo, col, counts, depth, rgb, K, poses, ws, flag = (t.data_ptr() for t in bufs)
+    s_end = s_begin + frames
+    rc = _C.lib().gsx_pointfusion_sequence_gt(geo, col, counts, 16, 0, depth, rgb, K, poses, 1, s_end, s_begin, s_end,
+                                              H, W, 0.05, 0.94, 0.6, ws, None, 0, 0.0, None, 0, 0.0, None, 0, flag,
+                                              None)
+    assert rc != 0
+    assert b"split the call" in _C.lib().gsx_last_error()
+    for t in bufs:
+        assert torch.equal(t, torch.full((256,), -7.25))
+
+
 def test_no_oracle_import_in_product_package():
     """The product never routes through the oracle (or any CPU fallback)."""
     pkg = os.path.join(ROOT, "gradslam_b200")
