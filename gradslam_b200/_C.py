@@ -42,6 +42,8 @@ SIGNATURES = {
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_float, c_float, c_vp, c_vp]),
     "gsx_fusion_merge_append": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "gsx_fusion_merge_append_radii": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_int, c_vp]),
     "gsx_fusion_merge_append_bwd": (
         c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int,
                 c_double, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -50,6 +52,10 @@ SIGNATURES = {
     "gsx_pointfusion_sequence_gt": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                 c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_float, c_vp, c_i64, c_vp, c_vp]),
+    "gsx_pointfusion_sequence_gt_radii": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_float, c_vp, c_i64, c_vp, c_int,
+                c_vp]),
     "gsx_fusion_prune_scratch_bytes": (c_i64, [c_int, c_i64]),
     "gsx_fusion_free_space_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_i64]),
     "gsx_fusion_prune": (
@@ -113,6 +119,12 @@ SIGNATURES = {
     "gsx_render_views": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                 c_vp, c_vp, c_vp]),
+    "gsx_render_splats": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                c_vp, c_vp, c_int, c_vp]),
+    "gsx_render_splats_bwd": (
+        c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "gsx_render_views_bwd_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
     "gsx_render_views_bwd": (
         c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,

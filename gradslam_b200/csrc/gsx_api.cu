@@ -35,7 +35,7 @@ int sequence_headers_group(const float *poses, const float *K, const float *dept
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
                         int64_t rgb_bs, int B_total, int b0, int nb, int s, int H, int W, float dist_th, float dot_th,
-                        void *workspace, int32_t *overflow, int32_t *assoc, cudaStream_t st);
+                        void *workspace, int32_t *overflow, int32_t *assoc, bool radii, cudaStream_t st);
 
 // Pruning of the sequence driver (Keller et al. 2013): frame s of the call is pruned step s; null = pruning off.
 // fs_scratch non-null adds the free-space rule: K4 records where each pixel went (its group's slice of the scratch's
@@ -118,15 +118,18 @@ extern "C" void gsx_debug_fail_at_frame(int s) { g_fail_at_frame = s; }
 
 extern "C" int gsx_pointfusion_sequence_groups(int B) { return B <= 0 ? 0 : gsx::sequence_groups(B); }
 
-extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
-                                           int64_t max_count0, const float *depth, const float *rgb,
-                                           const float *intrinsics, const float *poses, int B, int L, int s_begin,
-                                           int s_end, int H, int W, float dist_th, float dot_th, double sigma,
-                                           void *workspace, int32_t *ring, int t_max, float c_stable,
-                                           void *prune_scratch, int64_t prune_scratch_bytes, float margin,
-                                           void *fs_scratch, int64_t fs_scratch_bytes, int32_t *overflow_flag,
-                                           void *stream) {
+extern "C" int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map_colors, int32_t *counts,
+                                                 int64_t capacity, int64_t max_count0, const float *depth,
+                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
+                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
+                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
+                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                                 float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+                                                 int32_t *overflow_flag, int surfel_radii, void *stream) {
   GSX_CHECK_ARG(B >= 0 && L >= 0 && H >= 2 && W >= 2, "gsx_pointfusion_sequence_gt: bad extents");
+  GSX_CHECK_ARG(surfel_radii == 0 || surfel_radii == 1,
+                "gsx_pointfusion_sequence_gt: surfel_radii must be 0 or 1, not %d", surfel_radii);
+  const bool radii = surfel_radii != 0;
   GSX_CHECK_ARG(0 <= s_begin && s_begin <= s_end && s_end <= L, "gsx_pointfusion_sequence_gt: bad frame range");
   GSX_CHECK_ARG(counts && depth && rgb && intrinsics && poses, "gsx_pointfusion_sequence_gt: null pointer");
   GSX_CHECK_ARG(!ring || (t_max >= 0 && c_stable >= 0.0f && (!fs_scratch || margin >= 0.0f)),
@@ -183,7 +186,7 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
                                       counts + (int64_t)((s + 1) & 1) * B, capacity, max_count, poses + (int64_t)s * 16,
                                       (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, 0, B,
                                       s, H, W, dist_th, dot_th, workspace, overflow_flag,
-                                      gsx::sequence_assoc(prune, B, 0, B, H, W, capacity, user), user);
+                                      gsx::sequence_assoc(prune, B, 0, B, H, W, capacity, user), radii, user);
       if (rc == 0 && prune)
         rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, counts + (int64_t)((s + 1) & 1) * B, capacity,
                                        intrinsics, poses + (int64_t)s * 16, (int64_t)L * 16, B, 0, B, s, H, W,
@@ -214,7 +217,7 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
       rc = gsx::fusion_update_group(map_geometry, map_colors, cin, cout, capacity, max_count, poses + (int64_t)s * 16,
                                     (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, b0,
                                     b1 - b0, s, H, W, dist_th, dot_th, workspace, overflow_flag,
-                                    gsx::sequence_assoc(prune, B, b0, b1 - b0, H, W, capacity, gs->stream[g]),
+                                    gsx::sequence_assoc(prune, B, b0, b1 - b0, H, W, capacity, gs->stream[g]), radii,
                                     gs->stream[g]);
       if (rc == 0 && prune)
         rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, cout, capacity, intrinsics,
@@ -229,6 +232,20 @@ extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_color
     cudaStreamWaitEvent(user, gs->join[g], 0);
   }
   return rc;
+}
+
+extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                           int64_t max_count0, const float *depth, const float *rgb,
+                                           const float *intrinsics, const float *poses, int B, int L, int s_begin,
+                                           int s_end, int H, int W, float dist_th, float dot_th, double sigma,
+                                           void *workspace, int32_t *ring, int t_max, float c_stable,
+                                           void *prune_scratch, int64_t prune_scratch_bytes, float margin,
+                                           void *fs_scratch, int64_t fs_scratch_bytes, int32_t *overflow_flag,
+                                           void *stream) {
+  return gsx_pointfusion_sequence_gt_radii(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb,
+                                           intrinsics, poses, B, L, s_begin, s_end, H, W, dist_th, dot_th, sigma,
+                                           workspace, ring, t_max, c_stable, prune_scratch, prune_scratch_bytes, margin,
+                                           fs_scratch, fs_scratch_bytes, overflow_flag, 0, stream);
 }
 
 extern "C" int64_t gsx_pointfusion_sequence_workspace_bytes(int B, int H, int W) {

@@ -30,7 +30,7 @@ void set_error(const char *fmt, ...);
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
-// floats per packed map row (DESIGN.md section 2): geometry (px,py,pz,nx,ny,nz,ccount,0), colour (r,g,b,0)
+// floats per packed map row (DESIGN.md section 2): geometry (px,py,pz,nx,ny,nz,ccount,radius), colour (r,g,b,0)
 constexpr int kGeoW = 8, kColW = 4;
 
 // Scratch and workspace layouts are each written once, as a function that walks a Carver over the allocation:
@@ -250,6 +250,17 @@ __device__ __forceinline__ FrameSample frame_sample(const float *__restrict__ di
   s.gv = world_vertex(pose, s.v, dc);
   s.gn = (pose && kWantNormal) ? rotate(*pose, s.n.x, s.n.y, s.n.z) : s.n;
   return s;
+}
+
+// Radius of the surfel a pixel with centre depth d and camera-frame normal z component nz creates (Keller et al. 2013,
+// section 3; ElasticFusion): r0 = sqrt(2) d / f with 1/f the mean of K^-1's diagonal, grown by 1/|n_z| as the surface
+// tilts away from the camera and capped at 2 r0.  2|n_z| <= 1 is decided exactly (a zero normal takes the cap).
+constexpr float kSqrt2F = 1.41421356237309504880f;
+__device__ __forceinline__ float surfel_radius(float d, float nz, float k00, float k11) {
+  const float s = 0.5f * (k00 + k11);
+  const float r0 = (kSqrt2F * d) * s;
+  const float a = fabsf(nz);
+  return (2.0f * a <= 1.0f) ? 2.0f * r0 : r0 / a;
 }
 
 // High word of the arg-min key of find_best_unique_correspondences (fusionutils.py:491-517): 1/(cc+1e-20), then the

@@ -14,8 +14,8 @@
 //                              then one thread per pixel: confidence-weighted merge of the selected map row, or stable append of
 //                              unmatched valid pixels (single-pass decoupled look-back scan, row-major order per batch
 //                              element).  No float atomics anywhere.
-// Map rows are sector-packed (DESIGN.md section 2): geometry rows (px,py,pz,nx,ny,nz,ccount,0) of exactly one 32-byte
-// sector, colour rows (r,g,b,0) of 16 bytes; every row access is a 128-bit load / store.
+// Map rows are sector-packed (DESIGN.md section 2): geometry rows (px,py,pz,nx,ny,nz,ccount,radius) of exactly one
+// 32-byte sector, colour rows (r,g,b,0) of 16 bytes; every row access is a 128-bit load / store.
 // Reference op chains: gradslam/slam/fusionutils.py:198-722 (see include/gsx.h).
 #include "gsx_common.cuh"
 #include "gsx_exp.cuh"
@@ -90,11 +90,13 @@ struct FrameRecArgs {
 // computes for that pixel, bit for bit.  The stencil is gathered (its centre dc = hd.depth[h * W + w] already loaded)
 // and re-evaluated with K1r's camera and the same device functions and operands.  pose is
 // hd.cam.posed ? &hd.cam.pose : nullptr, passed separately so that a caller may make it a compile-time constant.
+// nz, if not null, receives the camera-frame normal's z component (the surfel radius's tilt).
 template <bool kAlpha>
 __device__ __forceinline__ void frame_values(const FrameHeader &hd, const Rigid *pose, int h, int w, int H, int W,
-                                             float dc, float3 &gn, float4 &fv) {
+                                             float dc, float3 &gn, float4 &fv, float *nz = nullptr) {
   const FrameSample f = frame_sample_from(load_stencil_around(hd.depth, dc, h, w, H, W), hd.cam.k, pose, h, w, H, W);
   gn = f.gn;
+  if (nz) *nz = f.n.z;
   // alpha from the LOCAL vertex (fusionutils.py:657, 69-72)
   fv = make_float4(f.gv.x, f.gv.y, f.gv.z,
                    kAlpha ? confidence_alpha((f.v.x * f.v.x + f.v.y * f.v.y) + f.v.z * f.v.z, hd.two_sigma_sq) : 0.0f);
@@ -331,7 +333,10 @@ struct MergeArgs {
 // 400 W, bench workload: K4 185 -> 178 us per launch, 21.6-21.7 k -> 21.9-22.0 k frames/s (DESIGN.md section 4).
 __device__ __forceinline__ void prefetch_l2(const float *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-template <bool kAssoc>
+// kRadii: slot 7 of every merged or appended row holds the surfel radius (surfel_radius of the pixel; a merge takes the
+// confidence-weighted mean of the row's radius and the pixel's, as for the position, and a row of radius 0 adopts the
+// pixel's).  Nothing else depends on it: slots 0-6 and the colour rows are those of kRadii = false, bit for bit.
+template <bool kAssoc, bool kRadii>
 __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) {
   __shared__ unsigned int s_ticket, s_table;
   __shared__ int s_warp_sums[kPix][kMB / 32];
@@ -342,6 +347,9 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   // the tile's arg-min over its binned candidates: per pixel the smallest key_hi, then the smallest n of that key
   __shared__ unsigned long long s_key[kTilePix];
   __shared__ unsigned int s_n[kTilePix];
+  // kRadii: each pixel's surfel radius, written and read back by the pixel's own thread (held in registers across the
+  // look-back, it would spill)
+  __shared__ float s_rad[kRadii ? kTilePix : 1];
   // batch element varies fastest in the grid: CTAs resident at the same time belong to different elements, so
   // each element's look-back chain only sees ~1/B of the in-flight tiles
   const int b = blockIdx.x % a.B;
@@ -486,8 +494,10 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   for (int j = 0; j < kPix; ++j) {
     if (matched[j] || is_new[j]) {
       const int ph = pix[j] / a.W;
+      float nz = 0.0f;
       frame_values<true>(s_hdr, s_hdr.cam.posed ? &s_hdr.cam.pose : nullptr, ph, pix[j] - ph * a.W, a.H, a.W, dep[j],
-                         fn[j], fv[j]);
+                         fn[j], fv[j], kRadii ? &nz : nullptr);
+      if (kRadii) s_rad[j * kMB + (int)threadIdx.x] = surfel_radius(dep[j], nz, s_hdr.cam.k.k00, s_hdr.cam.k.k11);
     }
   }
 
@@ -520,7 +530,12 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
       o1.x = ((c0 * g1[j].x) + (alpha * fn[j].y)) * inv;
       o1.y = ((c0 * g1[j].y) + (alpha * fn[j].z)) * inv;
       o1.z = tot;
-      o1.w = 0.0f;
+      if (kRadii) {
+        const float r = s_rad[j * kMB + (int)threadIdx.x];
+        o1.w = (g1[j].w == 0.0f) ? r : ((c0 * g1[j].w) + (alpha * r)) * inv;
+      } else {
+        o1.w = 0.0f;
+      }
       oc.x = ((c0 * c4[j].x) + (alpha * fc[0])) * inv;
       oc.y = ((c0 * c4[j].y) + (alpha * fc[1])) * inv;
       oc.z = ((c0 * c4[j].z) + (alpha * fc[2])) * inv;
@@ -548,7 +563,8 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
         const float *fc = s_rgb + (j * kMB + (int)threadIdx.x) * 3;
         *reinterpret_cast<float4 *>(geo + n * kGeoW) = make_float4(fv[j].x, fv[j].y, fv[j].z, fn[j].x);
         *reinterpret_cast<float4 *>(geo + n * kGeoW + 4) =
-            make_float4(fn[j].y, fn[j].z, a.with_cc ? fv[j].w : 0.0f, 0.0f);
+            make_float4(fn[j].y, fn[j].z, a.with_cc ? fv[j].w : 0.0f,
+                        kRadii ? s_rad[j * kMB + (int)threadIdx.x] : 0.0f);
         *reinterpret_cast<float4 *>(col + n * kColW) = make_float4(fc[0], fc[1], fc[2], 0.0f);
         if (kAssoc) a.assoc[(int64_t)b * P + pix[j]] = (int32_t)(n + 1);
       } else {
@@ -565,15 +581,22 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
   }
 }
 
-int launch_merge_append(const MergeArgs &args, cudaStream_t stream) {
+int launch_merge_append(const MergeArgs &args, bool radii, cudaStream_t stream) {
   if (args.B == 0) return 0;
   MergeArgs a = args;
   a.bin_cap = bin_capacity();
   const dim3 grid((unsigned)(a.ws.tiles * a.B));
-  if (a.assoc)
-    k_merge_append<true><<<grid, kMB, 0, stream>>>(a);  // differentiable forward
-  else
-    k_merge_append<false><<<grid, kMB, 0, stream>>>(a);
+  if (a.assoc) {  // differentiable forward, or the free-space step's record
+    if (radii)
+      k_merge_append<true, true><<<grid, kMB, 0, stream>>>(a);
+    else
+      k_merge_append<true, false><<<grid, kMB, 0, stream>>>(a);
+  } else {
+    if (radii)
+      k_merge_append<false, true><<<grid, kMB, 0, stream>>>(a);
+    else
+      k_merge_append<false, false><<<grid, kMB, 0, stream>>>(a);
+  }
   GSX_CHECK_LAUNCH("gsx_fusion_merge_append");
   return 0;
 }
@@ -768,7 +791,7 @@ static Workspace group_workspace(void *workspace, int B_total, int b0, int H, in
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
                         int64_t rgb_bs, int B_total, int b0, int nb, int s, int H, int W, float dist_th, float dot_th,
-                        void *workspace, int32_t *overflow, int32_t *assoc, cudaStream_t st) {
+                        void *workspace, int32_t *overflow, int32_t *assoc, bool radii, cudaStream_t st) {
   Workspace ws = group_workspace(workspace, B_total, b0, H, W);
   ws.hdr = seq_headers(workspace, B_total, H, W) + (int64_t)(s % kSeqFrames) * B_total + b0;
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
@@ -782,7 +805,7 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
   // assoc (full-batch base, zeroed by the caller, or null): where each pixel went, for the free-space step
   MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow,
                assoc ? assoc + (int64_t)b0 * H * W : nullptr, 0};
-  return launch_merge_append(ma, st);
+  return launch_merge_append(ma, radii, st);
 }
 
 }  // namespace gsx
@@ -852,11 +875,14 @@ extern "C" void gsx_debug_set_k2_grid_cap(int ctas) { g_k2_grid_cap = ctas > 0 ?
 
 extern "C" void gsx_debug_set_bin_capacity(int records) { g_bin_cap = records >= 0 ? records : -1; }
 
-extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_ccounts,
-                                       const int32_t *counts_in, int32_t *counts_out, int64_t capacity,
-                                       const float *rgb, int64_t rgb_bstride, int B, int H, int W, void *workspace,
-                                       int32_t *overflow_flag, int32_t *assoc_out, void *stream) {
+extern "C" int gsx_fusion_merge_append_radii(float *map_geometry, float *map_colors, int with_ccounts,
+                                             const int32_t *counts_in, int32_t *counts_out, int64_t capacity,
+                                             const float *rgb, int64_t rgb_bstride, int B, int H, int W,
+                                             void *workspace, int32_t *overflow_flag, int32_t *assoc_out,
+                                             int surfel_radii, void *stream) {
   GSX_CHECK_ARG(B >= 0 && H >= 2 && W >= 2, "gsx_fusion_merge_append: bad extents B=%d H=%d W=%d", B, H, W);
+  GSX_CHECK_ARG(surfel_radii == 0 || surfel_radii == 1, "gsx_fusion_merge_append: surfel_radii must be 0 or 1, not %d",
+                surfel_radii);
   if (B == 0) return 0;
   GSX_CHECK_ARG(map_geometry && map_colors && counts_in && counts_out, "gsx_fusion_merge_append: null map pointer");
   GSX_CHECK_ARG(counts_in != counts_out, "gsx_fusion_merge_append: counts_in and counts_out must not alias");
@@ -866,7 +892,15 @@ extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, i
   GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_merge_append: capacity must fit int32 (counts are int32)");
   MergeArgs a{map_geometry, map_colors, with_ccounts ? 1 : 0, counts_in, counts_out, capacity, rgb, rgb_bstride, B, H,
               W, fusion_workspace(workspace, B, H, W), overflow_flag, assoc_out, 0};
-  return launch_merge_append(a, (cudaStream_t)stream);
+  return launch_merge_append(a, surfel_radii != 0, (cudaStream_t)stream);
+}
+
+extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_ccounts,
+                                       const int32_t *counts_in, int32_t *counts_out, int64_t capacity,
+                                       const float *rgb, int64_t rgb_bstride, int B, int H, int W, void *workspace,
+                                       int32_t *overflow_flag, int32_t *assoc_out, void *stream) {
+  return gsx_fusion_merge_append_radii(map_geometry, map_colors, with_ccounts, counts_in, counts_out, capacity, rgb,
+                                       rgb_bstride, B, H, W, workspace, overflow_flag, assoc_out, 0, stream);
 }
 
 extern "C" int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, const float *map_geometry,

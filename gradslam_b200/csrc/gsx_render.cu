@@ -14,6 +14,13 @@
 //                              pixel's upstream gradients in view order (a row wins at most one pixel per view: no atomics).
 //   k_render_bwd_pose    (R3)  per pixel tile: d/d(camera-to-world pose) of depth and normals, reduced per tile, then
 //                              summed in tile order by k_pose_grad_reduce (gsx_frame.cu).
+//   k_render_splat       (R1d) max_splat_px >= 1: R1 where a row with a radius (slot 7 > 0) and a non-zero normal is an
+//                              oriented disk: every pixel of a box of +-max_splat_px around its projected centre whose
+//                              ray meets the disk takes the key (bits(t) << 32 | n), t the ray's depth on the disk's
+//                              plane.  Other rows keep R1's one-pixel rule.
+//   k_render_splat_bwd_rows / k_render_splat_bwd_pose  the backward of R1d at the fixed index: a disk row re-enumerates
+//                              its footprint per view and sums the pixels it won in (view, h, w) order; the pose kernel
+//                              takes the plane depth's derivative per pixel.
 // Positive floats order like their bit patterns, so the 64-bit key orders like (z, n).
 #include "gsx_common.cuh"
 #include "../../include/gsx.h"
@@ -258,6 +265,247 @@ __global__ void __launch_bounds__(kRB) k_render_bwd_pose(RenderBwdArgs a) {
 
 static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// ---- disk splats (R1d) -----------------------------------------------------------------------------------------
+// A row is a disk when it has a radius and a normal; everything else renders as one pixel.
+__device__ __forceinline__ bool is_disk(const float4 &g0, const float4 &g1) {
+  return g1.w > 0.0f && (g0.w != 0.0f || g1.x != 0.0f || g1.y != 0.0f);
+}
+
+// K^-1 of a camera staged as LiveCamera::k (the first three rows of the 4x4 K), as load_kinv computes it
+__device__ __forceinline__ KInv kinv_of(const float *k) {
+  KInv r;
+  r.k00 = 1.0f / (k[0] + 1e-6f);
+  r.k11 = 1.0f / (k[5] + 1e-6f);
+  r.k02 = (-1.0f * k[2]) / (k[0] + 1e-6f);
+  r.k12 = (-1.0f * k[6]) / (k[5] + 1e-6f);
+  return r;
+}
+
+// The disk of a row in one camera: q = T^-1 p, m = R^T n, mq = m.q, rr = r^2, and the box of pixels around the
+// projected centre (rint of project()'s u, v; the box is +-M pixels, clipped to the image).
+struct Disk {
+  float3 q, m;
+  float mq, rr;
+  int h0, h1, w0, w1;
+};
+__device__ __forceinline__ Disk make_disk(const LiveCamera &c, const ImageBounds &ib, int M, const float4 &g0,
+                                          const float4 &g1) {
+  Disk d;
+  d.q = rigid_apply(c.tinv, g0.x, g0.y, g0.z);
+  d.m = rotate(c.tinv, g0.w, g1.x, g1.y);
+  d.mq = dot3(d.m.x, d.m.y, d.m.z, d.q.x, d.q.y, d.q.z);
+  d.rr = g1.w * g1.w;
+  const float hx = ((c.k[0] * d.q.x + c.k[1] * d.q.y) + c.k[2] * d.q.z) + c.k[3];
+  const float hy = ((c.k[4] * d.q.x + c.k[5] * d.q.y) + c.k[6] * d.q.z) + c.k[7];
+  const float hz = ((c.k[8] * d.q.x + c.k[9] * d.q.y) + c.k[10] * d.q.z) + c.k[11];
+  const float den = (hz != 0.0f) ? hz : 1.0f;
+  // clamped first so that the conversion is defined; a centre past the clamp has an empty box either way
+  const int cu = (int)rintf(fminf(fmaxf(hx / den, (float)(-M - 2)), (float)(ib.W + M + 1)));
+  const int cv = (int)rintf(fminf(fmaxf(hy / den, (float)(-M - 2)), (float)(ib.H + M + 1)));
+  d.w0 = max(cu - M, 0);
+  d.w1 = min(cu + M, ib.W - 1);
+  d.h0 = max(cv - M, 0);
+  d.h1 = min(cv + M, ib.H - 1);
+  if (!(d.q.z > 0.0f)) d.h1 = d.h0 - 1;  // behind the camera: no pixel
+  return d;
+}
+
+// Pixel (h,w)'s ray d = K^-1 (w, h, 1) against the disk: true, with the plane depth t and m.d, if it meets the disk.
+__device__ __forceinline__ bool disk_hit(const Disk &d, const KInv &k, int h, int w, float &t, float &md, float3 &ray) {
+  ray = make_float3(k.k00 * (float)w + k.k02, k.k11 * (float)h + k.k12, 1.0f);
+  md = dot3(d.m.x, d.m.y, d.m.z, ray.x, ray.y, ray.z);
+  if (md == 0.0f) return false;
+  t = d.mq / md;
+  if (!(t > 0.0f)) return false;
+  const float ex = t * ray.x - d.q.x, ey = t * ray.y - d.q.y, ez = t * ray.z - d.q.z;
+  return ((ex * ex + ey * ey) + ez * ez) <= d.rr;
+}
+
+// Every covered pixel takes the atomicMin directly: a plain load of the key first, skipping the atomic when it could not
+// lower the key, was measured 17-22 % slower on the bench's map (DESIGN.md section 4).
+__global__ void __launch_bounds__(kRB) k_render_splat(RenderArgs a, int M) {
+  __shared__ LiveCamera s_cam[kViews];
+  __shared__ KInv s_kinv;
+  const int b = blockIdx.y, l0 = blockIdx.z * kViews;
+  const int nv = min(kViews, a.L - l0);
+  const int count = a.counts[b];
+  if ((int64_t)blockIdx.x * kRB >= count) return;
+  load_view_cameras(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b, l0, nv);
+  if (threadIdx.x == 0) s_kinv = load_kinv(a.K + b * a.K_bstride);
+  __syncthreads();
+  const int64_t P = (int64_t)a.ib.H * a.ib.W;
+  const float *geo = a.geo + (int64_t)b * a.cap * kGeoW;
+  unsigned long long *key = a.key + ((int64_t)b * a.L + l0) * P;
+  const int64_t stride = (int64_t)gridDim.x * kRB;
+  for (int64_t n = (int64_t)blockIdx.x * kRB + threadIdx.x; n < count; n += stride) {
+    const float4 g0 = __ldg(reinterpret_cast<const float4 *>(geo + n * kGeoW));
+    const float4 g1 = __ldg(reinterpret_cast<const float4 *>(geo + n * kGeoW + 4));
+    const bool disk = is_disk(g0, g1);
+    for (int v = 0; v < nv; ++v) {
+      if (!disk) {  // R1's rule
+        const PixelHit hit = project(s_cam[v], a.ib, g0.x, g0.y, g0.z);
+        if (hit.in_frustum) {
+          const float z = rigid_apply(s_cam[v].tinv, g0.x, g0.y, g0.z).z;
+          atomicMin(key + v * P + hit.h * a.ib.W + hit.w,
+                    ((unsigned long long)__float_as_uint(z) << 32) | (unsigned long long)n);
+        }
+        continue;
+      }
+      const Disk d = make_disk(s_cam[v], a.ib, M, g0, g1);
+      for (int h = d.h0; h <= d.h1; ++h)
+        for (int w = d.w0; w <= d.w1; ++w) {
+          float t, md;
+          float3 ray;
+          if (!disk_hit(d, s_kinv, h, w, t, md, ray)) continue;
+          const unsigned long long k = ((unsigned long long)__float_as_uint(t) << 32) | (unsigned long long)n;
+          atomicMin(key + v * P + h * a.ib.W + w, k);
+        }
+    }
+  }
+}
+
+// Rows: a row's gradient sums, in (view, h, w) order, the gradients of the pixels it won.  Disk rows: depth = t =
+// (m.q) / (m.d), so dt/dq = m / (m.d) and dt/dm = (q - t d) / (m.d); q = R^T (p - c) and m = R^T n give d/dp = R dt/dq
+// and d/dn = R (dt/dm + g_normals).
+__global__ void __launch_bounds__(kRB) k_render_splat_bwd_rows(RenderBwdArgs a, int M) {
+  __shared__ LiveCamera s_cam[kViews];
+  __shared__ KInv s_kinv;
+  const int b = blockIdx.y;
+  const int64_t n = (int64_t)blockIdx.x * kRB + threadIdx.x;
+  const bool live = n < a.counts[b];
+  const int64_t P = (int64_t)a.ib.H * a.ib.W;
+  float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
+  if (live) {
+    g0 = __ldg(reinterpret_cast<const float4 *>(a.geo + ((int64_t)b * a.cap + n) * kGeoW));
+    g1 = __ldg(reinterpret_cast<const float4 *>(a.geo + ((int64_t)b * a.cap + n) * kGeoW + 4));
+  }
+  const bool disk = is_disk(g0, g1);
+  if (threadIdx.x == 0) s_kinv = load_kinv(a.K + b * a.K_bstride);
+  float dp[3] = {0.f, 0.f, 0.f}, dn[3] = {0.f, 0.f, 0.f}, dc[3] = {0.f, 0.f, 0.f}, dcc = 0.f;
+  for (int l0 = 0; l0 < a.L; l0 += kViews) {
+    const int nv = min(kViews, a.L - l0);
+    __syncthreads();
+    load_view_cameras(s_cam, a.poses, a.pose_bstride, a.K, a.K_bstride, b, l0, nv);
+    __syncthreads();
+    if (!live) continue;
+    for (int v = 0; v < nv; ++v) {
+      const float *r = s_cam[v].tinv.r;  // R^T of the camera-to-world pose
+      // one pixel's gradients: gq = dL/dq, gm = dL/dm (camera frame)
+      auto add = [&](int64_t i, float gq0, float gq1, float gq2, float gm0, float gm1, float gm2) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          dp[j] += dot3(r[j], r[3 + j], r[6 + j], gq0, gq1, gq2);
+          dn[j] += dot3(r[j], r[3 + j], r[6 + j], gm0, gm1, gm2);
+        }
+        if (a.g_rgb) {
+          dc[0] += __ldg(a.g_rgb + i * 3); dc[1] += __ldg(a.g_rgb + i * 3 + 1); dc[2] += __ldg(a.g_rgb + i * 3 + 2);
+        }
+        if (a.g_confidence) dcc += __ldg(a.g_confidence + i);
+      };
+      auto g_normal = [&](int64_t i, int j) { return a.g_normals ? __ldg(a.g_normals + i * 3 + j) : 0.0f; };
+      if (!disk) {
+        const PixelHit hit = project(s_cam[v], a.ib, g0.x, g0.y, g0.z);
+        if (!hit.in_frustum) continue;
+        const int64_t i = ((int64_t)b * a.L + l0 + v) * P + hit.h * a.ib.W + hit.w;
+        if (__ldg(a.index + i) != n) continue;
+        const float gd = a.g_depth ? __ldg(a.g_depth + i) : 0.0f;
+        add(i, 0.0f, 0.0f, gd, g_normal(i, 0), g_normal(i, 1), g_normal(i, 2));
+        continue;
+      }
+      const Disk d = make_disk(s_cam[v], a.ib, M, g0, g1);
+      for (int h = d.h0; h <= d.h1; ++h)
+        for (int w = d.w0; w <= d.w1; ++w) {
+          const int64_t i = ((int64_t)b * a.L + l0 + v) * P + h * a.ib.W + w;
+          if (__ldg(a.index + i) != n) continue;
+          float t, md;
+          float3 ray;
+          disk_hit(d, s_kinv, h, w, t, md, ray);  // the row won the pixel, so its ray meets the disk
+          const float s = (a.g_depth ? __ldg(a.g_depth + i) : 0.0f) / md;
+          add(i, s * d.m.x, s * d.m.y, s * d.m.z, g_normal(i, 0) + s * (d.q.x - t * ray.x),
+              g_normal(i, 1) + s * (d.q.y - t * ray.y), g_normal(i, 2) + s * (d.q.z - t * ray.z));
+        }
+    }
+  }
+  if (n >= a.cap) return;
+  const int64_t row = (int64_t)b * a.cap + n;
+  if (a.d_geo) {
+    float4 *o = reinterpret_cast<float4 *>(a.d_geo + row * kGeoW);
+    o[0] = make_float4(dp[0], dp[1], dp[2], dn[0]);
+    o[1] = make_float4(dn[1], dn[2], dcc, 0.f);
+  }
+  if (a.d_col) reinterpret_cast<float4 *>(a.d_col + row * kColW)[0] = make_float4(dc[0], dc[1], dc[2], 0.f);
+}
+
+// Pose: per pixel, with gq = dL/dq and gm = dL/dm of the winning row (as in the rows kernel),
+//   dL/dR = (p - c) gq^T + n gm^T,  dL/dc = -R gq;  reduced per tile as k_render_bwd_pose does.
+__global__ void __launch_bounds__(kRB) k_render_splat_bwd_pose(RenderBwdArgs a) {
+  __shared__ Rigid s_pose, s_tinv;
+  __shared__ KInv s_kinv;
+  __shared__ float s_red[kRB / 32][12];
+  const int img = blockIdx.y;
+  const int b = img / a.L, l = img - b * a.L;
+  if (threadIdx.x == 0) {
+    s_pose = load_rigid(a.poses + b * a.pose_bstride + (int64_t)l * 16);
+    s_tinv = rigid_inverse(s_pose);
+    s_kinv = load_kinv(a.K + b * a.K_bstride);
+  }
+  __syncthreads();
+  const int64_t P = (int64_t)a.ib.H * a.ib.W;
+  const int64_t pix = (int64_t)blockIdx.x * kRB + threadIdx.x;
+  float acc[12];
+#pragma unroll
+  for (int j = 0; j < 12; ++j) acc[j] = 0.0f;
+  const int64_t i = img * P + pix;
+  const int64_t n = pix < P ? __ldg(a.index + i) : -1;
+  if (n >= 0) {
+    const float *row = a.geo + ((int64_t)b * a.cap + n) * kGeoW;
+    const float4 g0 = __ldg(reinterpret_cast<const float4 *>(row));
+    const float4 g1 = __ldg(reinterpret_cast<const float4 *>(row + 4));
+    const float gd = a.g_depth ? __ldg(a.g_depth + i) : 0.0f;
+    float gm[3] = {0.f, 0.f, 0.f}, gq[3] = {0.f, 0.f, gd};
+    if (a.g_normals) {
+      gm[0] = __ldg(a.g_normals + i * 3); gm[1] = __ldg(a.g_normals + i * 3 + 1); gm[2] = __ldg(a.g_normals + i * 3 + 2);
+    }
+    if (is_disk(g0, g1)) {
+      const int h = (int)(pix / a.ib.W), w = (int)(pix - (int64_t)h * a.ib.W);
+      const float3 q = rigid_apply(s_tinv, g0.x, g0.y, g0.z);
+      const float3 m = rotate(s_tinv, g0.w, g1.x, g1.y);
+      const float3 ray = make_float3(s_kinv.k00 * (float)w + s_kinv.k02, s_kinv.k11 * (float)h + s_kinv.k12, 1.0f);
+      const float md = dot3(m.x, m.y, m.z, ray.x, ray.y, ray.z);
+      const float t = dot3(m.x, m.y, m.z, q.x, q.y, q.z) / md;
+      const float s = gd / md;
+      gq[0] = s * m.x; gq[1] = s * m.y; gq[2] = s * m.z;
+      gm[0] += s * (q.x - t * ray.x); gm[1] += s * (q.y - t * ray.y); gm[2] += s * (q.z - t * ray.z);
+    }
+    const Rigid &T = s_pose;
+    const float pt[3] = {g0.x - T.t[0], g0.y - T.t[1], g0.z - T.t[2]};
+    const float nw[3] = {g0.w, g1.x, g1.y};
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) acc[r * 4 + c] = pt[r] * gq[c] + nw[r] * gm[c];
+      acc[r * 4 + 3] = -dot3(T.r[r * 3 + 0], T.r[r * 3 + 1], T.r[r * 3 + 2], gq[0], gq[1], gq[2]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 12; ++j) {
+    float x = acc[j];
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) x += __shfl_xor_sync(0xffffffffu, x, s);
+    acc[j] = x;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0)
+#pragma unroll
+    for (int j = 0; j < 12; ++j) s_red[warp][j] = acc[j];
+  __syncthreads();
+  if (threadIdx.x < 12) {
+    float x = 0.0f;
+    for (int w = 0; w < kRB / 32; ++w) x += s_red[w][threadIdx.x];
+    a.pose_partials[((int64_t)img * a.tiles + blockIdx.x) * 12 + threadIdx.x] = x;
+  }
+}
+
 }  // namespace gsx
 
 using namespace gsx;
@@ -275,22 +523,43 @@ static inline unsigned pixel_tiles(int H, int W) { return (unsigned)(((int64_t)H
 
 // Fills the index image with empty keys, then runs R1 over the rows of every element (max_count = host bound on the
 // element sizes; no row pass when it is 0).
-static void launch_zbuffer(const RenderArgs &a, int B, int64_t max_count, cudaStream_t s) {
+// max_splat_px = 0: R1 (one pixel per row); >= 1: R1d (disks of the rows' radii, boxes of +-max_splat_px pixels).
+static void launch_zbuffer(const RenderArgs &a, int B, int64_t max_count, cudaStream_t s, int max_splat_px = 0) {
   cudaMemsetAsync(a.key, 0xFF, (size_t)B * a.L * a.ib.H * a.ib.W * sizeof(int64_t), s);
   if (max_count > 0) {
     const unsigned chunks = (unsigned)((a.L + kViews - 1) / kViews);
     int64_t bx = (max_count + kRB - 1) / kRB;
     const int64_t cap_blocks = (int64_t)kNumSMs * kRenderCtasPerSM;  // grid-stride beyond
     if (bx * B * chunks > cap_blocks) bx = (cap_blocks + B * chunks - 1) / (B * chunks);
-    k_render_zbuffer<<<dim3((unsigned)bx, (unsigned)B, chunks), kRB, 0, s>>>(a);
+    const dim3 grid((unsigned)bx, (unsigned)B, chunks);
+    if (max_splat_px == 0)
+      k_render_zbuffer<<<grid, kRB, 0, s>>>(a);
+    else
+      k_render_splat<<<grid, kRB, 0, s>>>(a, max_splat_px);
   }
+}
+
+static int check_splat_px(const char *fn, int max_splat_px) {
+  GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX, "%s: max_splat_px %d outside [0, %d]", fn,
+                max_splat_px, GSX_MAX_SPLAT_PX);
+  return 0;
 }
 
 extern "C" int gsx_render_views(const float *map_geometry, const float *map_colors, const int32_t *counts,
                                 int64_t capacity, int64_t max_count, const float *intrinsics, int64_t K_bstride,
                                 const float *poses, int64_t pose_bstride, int B, int L, int H, int W, int64_t *index,
                                 float *depth, float *rgb, float *normals, float *confidence, void *stream) {
+  return gsx_render_splats(map_geometry, map_colors, counts, capacity, max_count, intrinsics, K_bstride, poses,
+                           pose_bstride, B, L, H, W, index, depth, rgb, normals, confidence, 0, stream);
+}
+
+extern "C" int gsx_render_splats(const float *map_geometry, const float *map_colors, const int32_t *counts,
+                                 int64_t capacity, int64_t max_count, const float *intrinsics, int64_t K_bstride,
+                                 const float *poses, int64_t pose_bstride, int B, int L, int H, int W, int64_t *index,
+                                 float *depth, float *rgb, float *normals, float *confidence, int max_splat_px,
+                                 void *stream) {
   if (check_render_extents("gsx_render_views", B, L, H, W, capacity)) return 1;
+  if (check_splat_px("gsx_render_splats", max_splat_px)) return 1;
   GSX_CHECK_ARG(intrinsics && poses && index, "gsx_render_views: null pointer");
   GSX_CHECK_ARG(max_count >= 0 && max_count <= capacity, "gsx_render_views: max_count %lld outside [0, capacity %lld]",
                 (long long)max_count, (long long)capacity);
@@ -301,7 +570,7 @@ extern "C" int gsx_render_views(const float *map_geometry, const float *map_colo
   cudaStream_t s = (cudaStream_t)stream;
   RenderArgs a{map_geometry, map_colors, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, L,
                image_bounds(H, W), reinterpret_cast<unsigned long long *>(index), depth, rgb, normals, confidence};
-  launch_zbuffer(a, B, max_count, s);
+  launch_zbuffer(a, B, max_count, s, max_splat_px);
   k_render_resolve<<<dim3(pixel_tiles(H, W), (unsigned)(B * L)), kRB, 0, s>>>(a);
   GSX_CHECK_LAUNCH("gsx_render_views");
   return 0;
@@ -339,7 +608,19 @@ extern "C" int gsx_render_views_bwd(const float *map_geometry, const int32_t *co
                                     const float *g_depth, const float *g_rgb, const float *g_normals,
                                     const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses,
                                     void *scratch, int64_t scratch_bytes, void *stream) {
+  return gsx_render_splats_bwd(map_geometry, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, index, B, L,
+                               H, W, g_depth, g_rgb, g_normals, g_confidence, d_geometry, d_colors, d_poses, scratch,
+                               scratch_bytes, 0, stream);
+}
+
+extern "C" int gsx_render_splats_bwd(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                     const float *intrinsics, int64_t K_bstride, const float *poses,
+                                     int64_t pose_bstride, const int64_t *index, int B, int L, int H, int W,
+                                     const float *g_depth, const float *g_rgb, const float *g_normals,
+                                     const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses,
+                                     void *scratch, int64_t scratch_bytes, int max_splat_px, void *stream) {
   if (check_render_extents("gsx_render_views_bwd", B, L, H, W, capacity)) return 1;
+  if (check_splat_px("gsx_render_splats_bwd", max_splat_px)) return 1;
   GSX_CHECK_ARG(intrinsics && poses && index, "gsx_render_views_bwd: null pointer");
   const bool want_rows = (d_geometry || d_colors) && capacity > 0;
   if (capacity > 0 && (want_rows || d_poses))
@@ -354,10 +635,14 @@ extern "C" int gsx_render_views_bwd(const float *map_geometry, const int32_t *co
   RenderBwdArgs a{map_geometry, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, index, L,
                   image_bounds(H, W), g_depth, g_rgb, g_normals, g_confidence, d_geometry, d_colors,
                   (float *)scratch, (int)tiles};
-  if (want_rows)
-    k_render_bwd_rows<<<dim3((unsigned)((capacity + kRB - 1) / kRB), (unsigned)B), kRB, 0, s>>>(a);
+  const dim3 row_grid((unsigned)((capacity + kRB - 1) / kRB), (unsigned)B);
+  if (want_rows && max_splat_px == 0) k_render_bwd_rows<<<row_grid, kRB, 0, s>>>(a);
+  if (want_rows && max_splat_px > 0) k_render_splat_bwd_rows<<<row_grid, kRB, 0, s>>>(a, max_splat_px);
   if (d_poses) {
-    k_render_bwd_pose<<<dim3(tiles, (unsigned)(B * L)), kRB, 0, s>>>(a);
+    if (max_splat_px == 0)
+      k_render_bwd_pose<<<dim3(tiles, (unsigned)(B * L)), kRB, 0, s>>>(a);
+    else
+      k_render_splat_bwd_pose<<<dim3(tiles, (unsigned)(B * L)), kRB, 0, s>>>(a);
     k_pose_grad_reduce<<<B * L, 16, 0, s>>>((const float *)scratch, (int)tiles, d_poses, B * L);
   }
   GSX_CHECK_LAUNCH("gsx_render_views_bwd");

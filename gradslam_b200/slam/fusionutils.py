@@ -167,8 +167,8 @@ def _dense_frame(t, name, device):
     return t
 
 
-def _launch_merge_append(pointclouds, frames, ws, assoc=None):
-    """K4 on the current workspace state (frame records + per-pixel winners)."""
+def _launch_merge_append(pointclouds, frames, ws, assoc=None, radii=False):
+    """K4 on the current workspace state (frame records + per-pixel winners); radii: write surfel radii (slot 7)."""
     B, _, H, W = frames.shape
     P = H * W
     dev = pointclouds.device
@@ -176,8 +176,8 @@ def _launch_merge_append(pointclouds, frames, ws, assoc=None):
     geo, col = _map_ptrs(pointclouds, dev)
     cin = pointclouds._counts_dev[pointclouds._cur]
     cout = pointclouds._counts_dev[pointclouds._cur ^ 1]
-    _C.launch("gsx_fusion_merge_append", geo, col, 1 if pointclouds._has_cc else 0, cin, cout, pointclouds.capacity, rgb,
-              c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc)
+    _C.launch("gsx_fusion_merge_append_radii", geo, col, 1 if pointclouds._has_cc else 0, cin, cout,
+              pointclouds.capacity, rgb, c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, 1 if radii else 0)
     pointclouds._mark_device_updated(pointclouds._bound + P)
 
 
@@ -227,9 +227,9 @@ def _check_fusion_inputs(pointclouds, rgbdimages):
             raise ValueError("Pointclouds features must be a single confidence count per point for map fusion.")
 
 
-def _update_in_place(pointclouds, frames, sigma, dist_th=None, dot_th=None, table=None, assoc_out=None):
+def _update_in_place(pointclouds, frames, sigma, dist_th=None, dot_th=None, table=None, assoc_out=None, radii=False):
     """K1r, the association (K2 with dist_th / dot_th, or the rows of `table`), then K4, in place.  assoc_out: a list
-    that receives K4's per-pixel record (B, H*W) int32."""
+    that receives K4's per-pixel record (B, H*W) int32; radii: K4 writes surfel radii."""
     frames = frames.to_channels_last()
     _C.require_cuda(frames.depth_image, "depth_image")
     B, _, H, W = frames.shape
@@ -242,8 +242,13 @@ def _update_in_place(pointclouds, frames, sigma, dist_th=None, dot_th=None, tabl
     if assoc_out is not None:
         assoc = ws.zeroed_assoc()
         assoc_out.append(assoc)
-    _launch_merge_append(pointclouds, frames, ws, assoc)
+    _launch_merge_append(pointclouds, frames, ws, assoc, radii)
     return pointclouds
+
+
+def _check_surfel_radii(surfel_radii):
+    if not isinstance(surfel_radii, bool):
+        raise TypeError("surfel_radii must be of type bool; but was of type {}.".format(type(surfel_radii)))
 
 
 # --------------------------------------------------------------------------------------------- table API
@@ -386,10 +391,12 @@ def find_correspondences(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_
 
 
 def fuse_with_map(pointclouds: Pointclouds, rgbdimages: RGBDImages, pc2im_bnhw: torch.Tensor,
-                  sigma: Union[torch.Tensor, float, int], inplace: bool = False) -> Pointclouds:
+                  sigma: Union[torch.Tensor, float, int], inplace: bool = False, *,
+                  surfel_radii: bool = False) -> Pointclouds:
     """Merges the corresponding points of `pc2im_bnhw` (unique rows) and appends the unmatched valid pixels
-    (fusionutils.py:580-722)."""
+    (fusionutils.py:580-722).  surfel_radii (extension): as in update_map_fusion."""
     _check_pc(pointclouds)
+    _check_surfel_radii(surfel_radii)
     if not isinstance(rgbdimages, RGBDImages):
         raise TypeError("Expected rgbdimages to be of type gradslam.RGBDImages. Got {0}.".format(type(rgbdimages)))
     _check_table(pc2im_bnhw)
@@ -403,7 +410,7 @@ def fuse_with_map(pointclouds: Pointclouds, rgbdimages: RGBDImages, pc2im_bnhw: 
     _check_frame(rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
-    return _fuse(pointclouds, rgbdimages, sigma, table=pc2im_bnhw)
+    return _fuse(pointclouds, rgbdimages, sigma, table=pc2im_bnhw, radii=surfel_radii)
 
 
 def _launch_association(ws, pointclouds, frames, dist_th=None, dot_th=None, table=None):
@@ -436,15 +443,16 @@ def _wants_grad(pointclouds, frames):
 
 class _MergeAppendFn(torch.autograd.Function):
     """K4 as one differentiable op: (pre-merge map rows, frame maps) -> updated map rows.  forward =
-    gsx_fusion_merge_append on a copy of the map (also records where every pixel went), backward =
-    gsx_fusion_merge_append_bwd; both hand-written kernels, both on the packed row layout (the public
-    points / normals / colors / features tensors are slices of the rows, so autograd carries the gradients in and out
-    of the rows by itself).  The frame records and the per-pixel winners must already sit in the fusion workspace
+    gsx_fusion_merge_append_radii (surfel radii on or off) on a copy of the map (also records where every pixel went),
+    backward = gsx_fusion_merge_append_bwd; both hand-written kernels, both on the packed row layout (the public
+    points / normals / colors / features / radii tensors are slices of the rows, so autograd carries the gradients in
+    and out of the rows by itself).  The radii carry no gradient: the gradient w.r.t. `radii_padded` is identically
+    zero.  The frame records and the per-pixel winners must already sit in the fusion workspace
     (K1r; K2, or gsx_records_from_table); the winners are index-only, as in the reference (fusionutils.py:523)."""
 
     @staticmethod
     def forward(ctx, pack, geo, col, gv, gn, rgb, vloc):
-        pointclouds, frames, sigma, ws = pack[:4]
+        pointclouds, frames, sigma, ws, _, radii = pack
         B, _, H, W = frames.shape
         P = H * W
         dev = geo.device
@@ -460,9 +468,9 @@ class _MergeAppendFn(torch.autograd.Function):
         counts_out = pointclouds._counts_dev[pointclouds._cur ^ 1]
         assoc = torch.zeros((B, P), dtype=torch.int32, device=dev)
         with_cc = 1 if pointclouds._has_cc else 0
-        _C.launch("gsx_fusion_merge_append", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c, P * 3, B,
-                  H, W, ws.buf, pointclouds._overflow_flag(), assoc)
-        if len(pack) > 4 and pack[4] is not None:  # (fuse_and_prune's free-space step reads it)
+        _C.launch("gsx_fusion_merge_append_radii", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c,
+                  P * 3, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, 1 if radii else 0)
+        if pack[4] is not None:  # (fuse_and_prune's free-space step reads it)
             pack[4].append(assoc)
         ctx.saved = (assoc, counts_in, geo.detach(), col.detach(), gv_c, gn_c, rgb_c, vloc_c)
         ctx.dims = (B, H, W, cap_in, cap_out, float(sigma), with_cc)
@@ -486,7 +494,7 @@ class _MergeAppendFn(torch.autograd.Function):
 
 
 def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=None, dot_th=None, table=None,
-                           assoc_out=None):
+                           assoc_out=None, radii=False):
     """Map update when a gradient is requested: K1 (differentiable op, for the backward) -> frame records ->
     association (K2 kernel, or the rows of `table`; index-only) -> K4 (differentiable op), out of place so the pre-merge
     map survives for the backward.  K4's forward re-evaluates the frame values from depth, as the in-place path does,
@@ -507,7 +515,7 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
     ws = _Workspace.get(dev, B, H, W)
     _launch_frame_records(ws, frames, sig, dev)
     _launch_association(ws, pointclouds, frames, dist_th=dist_th, dot_th=dot_th, table=table)
-    geo_out, col_out = _MergeAppendFn.apply((pointclouds, frames, sig, ws, assoc_out), pointclouds._geo,
+    geo_out, col_out = _MergeAppendFn.apply((pointclouds, frames, sig, ws, assoc_out, radii), pointclouds._geo,
                                             pointclouds._col, gv, gn, frames.rgb_image, vloc)
     pointclouds._geo, pointclouds._col = geo_out, col_out
     pointclouds._uninit = False
@@ -515,12 +523,12 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
     return pointclouds
 
 
-def _fuse(pointclouds, frames, sigma, dist_th=None, dot_th=None, table=None, assoc_out=None):
+def _fuse(pointclouds, frames, sigma, dist_th=None, dot_th=None, table=None, assoc_out=None, radii=False):
     """The fused map update: the differentiable op chain when a gradient is requested, else in place.  A frame without
     poses (only fuse_with_map accepts one) has no world-frame maps for the differentiable chain and is fused in place."""
     if _wants_grad(pointclouds, frames) and frames.poses is not None:
-        return _update_differentiable(pointclouds, frames, sigma, True, dist_th, dot_th, table, assoc_out)
-    return _update_in_place(pointclouds, frames, sigma, dist_th, dot_th, table, assoc_out)
+        return _update_differentiable(pointclouds, frames, sigma, True, dist_th, dot_th, table, assoc_out, radii)
+    return _update_in_place(pointclouds, frames, sigma, dist_th, dot_th, table, assoc_out, radii)
 
 
 # --------------------------------------------------------------------------------------------- unstable surfels
@@ -620,17 +628,20 @@ def _check_free_space_margin(margin):
 def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Union[float, int],
                    dot_th: Union[float, int], sigma: Union[torch.Tensor, float, int],
                    stable_confidence: Union[float, int], max_unstable_age: int,
-                   free_space_margin: Union[float, int], inplace: bool = False) -> Pointclouds:
+                   free_space_margin: Union[float, int], inplace: bool = False, *,
+                   surfel_radii: bool = False) -> Pointclouds:
     """update_map_fusion followed by one pruned step with both of Keller et al.'s (2013, section 4.3) outlier rules
     (an extension: gradslam keeps every surfel).  The age rule is prune_unstable's.  The free-space rule: wherever the
     live frame merged a pixel into a surfel that is stable after the merge (confidence >= stable_confidence), every
     surfel that projects to that same pixel more than `free_space_margin` (metres, camera z) in front of it is removed,
     stable or not.  Unlike the paper (a 4x4-supersampled index map), "in front" is decided at image resolution, at the
     pixel the association's own projection gives.  Both removals are one stable compaction: kept rows keep their order.
-    free_space_margin = inf removes no violator (the result is update_map_fusion + prune_unstable)."""
+    free_space_margin = inf removes no violator (the result is update_map_fusion + prune_unstable).  surfel_radii: as in
+    update_map_fusion; the pruning moves whole rows, radius included."""
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     _check_frame(rgbdimages)
+    _check_surfel_radii(surfel_radii)
     _check_free_space_margin(free_space_margin)
     t_max = int(max_unstable_age)
     _check_history(pointclouds, t_max)
@@ -640,7 +651,7 @@ def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Un
     if not inplace:
         pointclouds = pointclouds.clone()
     got = []
-    _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th, assoc_out=got)
+    _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th, assoc_out=got, radii=surfel_radii)
     frames = rgbdimages.to_channels_last()
     _, _, H, W = frames.shape
     dev = pointclouds.device
@@ -672,12 +683,19 @@ def update_map_aggregate(pointclouds: Pointclouds, rgbdimages: RGBDImages, inpla
 
 def update_map_fusion(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Union[float, int],
                       dot_th: Union[float, int], sigma: Union[torch.Tensor, float, int],
-                      inplace: bool = False) -> Pointclouds:
-    """PointFusion update of the maps with one live frame (fusionutils.py:761-789)."""
+                      inplace: bool = False, *, surfel_radii: bool = False) -> Pointclouds:
+    """PointFusion update of the maps with one live frame (fusionutils.py:761-789).
+
+    surfel_radii (extension, default False): every merged or appended surfel also gets a radius, readable as
+    `radii_padded` / `radii_list`: min(2 r0, r0 / |n_z|) with r0 = sqrt(2) d / f, from the pixel's depth d, camera-frame
+    normal n and the mean 1/f of the live camera (Keller et al. 2013); a merge averages it with the confidence weights, as
+    it does the position, and a surfel without a radius (0) takes the pixel's.  No association, merge or append
+    decision depends on it: every other value of the map is what surfel_radii=False gives.  Radii carry no gradient."""
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     _check_frame(rgbdimages)
+    _check_surfel_radii(surfel_radii)
     _check_fusion_inputs(pointclouds, rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
-    return _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th)
+    return _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th, radii=surfel_radii)

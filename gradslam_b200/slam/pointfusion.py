@@ -45,7 +45,8 @@ class PointFusion(ICPSLAM):
                  lambda_max: Union[float, int] = 2.0, B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0,
                  nu: Union[float, int] = 200.0, association: str = "nn",
                  device: Union[torch.device, str, None] = None, stable_confidence: Union[float, int, None] = None,
-                 max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None):
+                 max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None,
+                 surfel_radii: bool = False):
         """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
         surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
         (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
@@ -57,7 +58,13 @@ class PointFusion(ICPSLAM):
         step, also remove the free-space violations of Keller et al. 2013, section 4.3 - wherever the live frame merged
         a pixel into a surfel that is stable after the merge, every surfel projecting to that pixel more than the margin
         (camera z) in front of it.  The paper finds "in front" on a 4x4-supersampled index map; here it is the merged
-        pixel itself, at image resolution.  Default None: no such removal."""
+        pixel itself, at image resolution.  Default None: no such removal.
+
+        surfel_radii (extension, default False): every fused surfel also gets a radius (`radii_padded`), as
+        fusionutils.update_map_fusion(surfel_radii=True) gives it, in the whole-sequence call, the step API, the
+        differentiable mode and with pruning.  Nothing else in the map changes."""
+        if not isinstance(surfel_radii, bool):
+            raise TypeError("surfel_radii must be of type bool; but was of type {}.".format(type(surfel_radii)))
         for name, val, kinds in (("stable_confidence", stable_confidence, (float, int)),
                                  ("max_unstable_age", max_unstable_age, (int,))):
             if val is not None and (isinstance(val, bool) or not isinstance(val, kinds)):
@@ -91,14 +98,17 @@ class PointFusion(ICPSLAM):
         self.stable_confidence = stable_confidence
         self.max_unstable_age = max_unstable_age
         self.free_space_margin = free_space_margin
+        self.surfel_radii = surfel_radii
 
     def _map(self, pointclouds: Pointclouds, live_frame: RGBDImages, inplace: bool = False):
         if self.stable_confidence is not None and isinstance(pointclouds, Pointclouds):
             _check_history(pointclouds, self.max_unstable_age)
         if self.free_space_margin is not None:
             return fuse_and_prune(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, self.stable_confidence,
-                                  self.max_unstable_age, self.free_space_margin, inplace)
-        pointclouds = update_map_fusion(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, inplace)
+                                  self.max_unstable_age, self.free_space_margin, inplace,
+                                  surfel_radii=self.surfel_radii)
+        pointclouds = update_map_fusion(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, inplace,
+                                        surfel_radii=self.surfel_radii)
         if self.stable_confidence is not None:
             prune_unstable(pointclouds, self.stable_confidence, self.max_unstable_age)
         return pointclouds
@@ -198,9 +208,10 @@ class PointFusion(ICPSLAM):
                 for b in range(B):
                     _C.launch("gsx_ingest_raw", raw_rgb[b, s0:s1], raw_depth[b, s0:s1], (s1 - s0) * P,
                               frames.scaling_factor, 1 if frames.normalize_color else 0, rgb[b, s0:s1], depth[b, s0:s1])
-            _C.launch("gsx_pointfusion_sequence_gt", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+            _C.launch("gsx_pointfusion_sequence_gt_radii", pc._geo, pc._col, pc._counts_dev, pc.capacity,
                       min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                      float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag())
+                      float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag(),
+                      1 if self.surfel_radii else 0)
         if not on_device:
             for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
                 t.record_stream(copy_stream)

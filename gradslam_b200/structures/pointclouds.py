@@ -6,14 +6,15 @@ list / padded views, arithmetic helpers, `append_points`, `transform`, `pinhole_
 reference's list <-> padded duality, rebuilt with `torch.cat` on every append, the map lives in ONE
 capacity-backed store of SECTOR-PACKED rows that the fusion kernels update IN PLACE:
 
-    geometry  (B, capacity, 8)  float32   (px, py, pz, nx, ny, nz, ccount, 0)   one 32-byte DRAM sector per surfel
+    geometry  (B, capacity, 8)  float32   (px, py, pz, nx, ny, nz, ccount, radius)   one 32-byte DRAM sector per surfel
     colours   (B, capacity, 4)  float32   (r, g, b, 0)
     counts    (2, B)            int32     ping-pong: kernels read row `cur`, write row `cur ^ 1`
 
 so a kernel touches a surfel with two (geometry) or three (+ colour) 128-bit accesses instead of ten scalar ones
 spread over four arrays.  gradslam's tensors are STRIDED VIEWS of these rows: `points_padded = geometry[:, :N, 0:3]`,
 `normals_padded = geometry[:, :N, 3:6]`, `features_padded = geometry[:, :N, 6:7]` (the confidence count),
-`colors_padded = colours[:, :N, 0:3]`; `*_list[b]` are the same views cut at `counts[b]`.  (Features with more than
+`colors_padded = colours[:, :N, 0:3]`, `radii_padded = geometry[:, :N, 7:8]` (the surfel radius: 0 unless the map
+was fused with surfel_radii=True); `*_list[b]` are the same views cut at `counts[b]`.  (Features with more than
 one channel are not part of the fusion path; they live in a separate dense (B, capacity, C) tensor.)  Rows >=
 counts[b] are always zero inside the padded width.  The per-element sizes live on the device (the kernels bump them);
 the host copy is refreshed lazily, only when a caller asks for a shape-dependent view.  Everything is float32: other
@@ -163,6 +164,8 @@ class Pointclouds(object):
             return None if self._col is None else self._col[..., 0:3]
         if key == "features":
             return self._geo[..., 6:7] if self._has_cc else self._feat
+        if key == "radii":
+            return self._geo[..., 7:8]
         raise KeyError(key)
 
     def _grad_tensors(self):
@@ -356,6 +359,10 @@ class Pointclouds(object):
     normals_list = property(lambda self: self._list("normals"))
     colors_list = property(lambda self: self._list("colors"))
     features_list = property(lambda self: self._list("features"))
+    # surfel radii (B, N, 1) / [(N_b, 1)]: written by the fused map update with surfel_radii=True, 0 otherwise; they carry
+    # no gradient through the fusion ops
+    radii_padded = property(lambda self: self._padded("radii"))
+    radii_list = property(lambda self: self._list("radii"))
 
     @property
     def nonpad_mask(self):
@@ -384,7 +391,7 @@ class Pointclouds(object):
         """Fresh (out-of-place, autograd friendly: never mutate a tensor a caller may still hold) full-capacity view of
         attribute `key` with `channels` channels, creating / re-shaping its buffer if needed."""
         cap = max(self.capacity, self._N)
-        if key in ("points", "normals") or (key == "features" and channels == 1):
+        if key in ("points", "normals", "radii") or (key == "features" and channels == 1):
             self._geo = self._geo.clone()
             if key == "normals":
                 self._has_normals = True
@@ -435,6 +442,20 @@ class Pointclouds(object):
     normals_list = normals_list.setter(lambda self, v: self._set_list("normals", v))
     colors_list = colors_list.setter(lambda self, v: self._set_list("colors", v))
     features_list = features_list.setter(lambda self, v: self._set_list("features", v, True))
+    radii_padded = radii_padded.setter(lambda self, v: self._set_radii_padded(v))
+    radii_list = radii_list.setter(lambda self, v: self._set_radii_list(v))
+
+    def _set_radii_padded(self, value):
+        self._assert_set_padded(value, True)
+        if value.shape[-1] != 1:
+            raise ValueError("radii must have one channel. Got {}".format(value.shape[-1]))
+        self._set_padded("radii", value, True)
+
+    def _set_radii_list(self, value):
+        self._assert_set_list(value, True)
+        if any(v.shape[1] != 1 for v in value):
+            raise ValueError("radii must have one channel")
+        self._set_list("radii", value, True)
 
     # ------------------------------------------------------------------ indexing
     def __getitem__(self, index):

@@ -41,8 +41,8 @@ class RenderedViews(NamedTuple):
     index: torch.Tensor                 # (B, L, H, W) int64 map row of the pixel, or -1
 
 
-def _render(geo, col, counts, bound, K, poses, H, W, want_normals, want_conf):
-    """gsx_render_views on dense CUDA tensors -> (depth, rgb, normals, confidence, index)."""
+def _render(geo, col, counts, bound, K, poses, H, W, want_normals, want_conf, splat=0):
+    """gsx_render_splats on dense CUDA tensors -> (depth, rgb, normals, confidence, index); splat = max_splat_px."""
     B, L = poses.shape[:2]
     dev = poses.device
     cap = 0 if geo is None else geo.shape[1]
@@ -50,30 +50,31 @@ def _render(geo, col, counts, bound, K, poses, H, W, want_normals, want_conf):
     index = torch.empty((B, L, H, W), dtype=torch.int64, device=dev)
     depth, rgb = img(1), None if col is None else img(3)
     normals, conf = img(3) if want_normals else None, img(1) if want_conf else None
-    _C.launch("gsx_render_views", geo, col, counts, cap, bound, K, 16, poses, L * 16, B, L, H, W, index, depth, rgb,
-              normals, conf)
+    _C.launch("gsx_render_splats", geo, col, counts, cap, bound, K, 16, poses, L * 16, B, L, H, W, index, depth, rgb,
+              normals, conf, splat)
     return depth, rgb, normals, conf, index
 
 
 class _RenderFn(torch.autograd.Function):
-    """gsx_render_views as one differentiable op over (geometry rows, colour rows, poses); backward =
-    gsx_render_views_bwd at the forward's index (the association carries no gradient)."""
+    """gsx_render_splats as one differentiable op over (geometry rows, colour rows, poses); backward =
+    gsx_render_splats_bwd at the forward's index (the association and the footprint carry no gradient, the radius
+    none either)."""
 
     @staticmethod
     def forward(ctx, pack, geo, col, poses):
-        counts, bound, K, H, W, want_normals, want_conf = pack
+        counts, bound, K, H, W, want_normals, want_conf, splat = pack
         outs = _render(geo.detach(), None if col is None else col.detach(), counts, bound, K, poses.detach(), H, W,
-                       want_normals, want_conf)
+                       want_normals, want_conf, splat)
         ctx.mark_non_differentiable(outs[4])
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(geo, poses, outs[4])
-        ctx.pack = (counts, K, H, W)
+        ctx.pack = (counts, K, H, W, splat)
         return outs
 
     @staticmethod
     def backward(ctx, g_depth, g_rgb, g_normals, g_conf, _g_index):
         geo, poses, index = ctx.saved_tensors
-        counts, K, H, W = ctx.pack
+        counts, K, H, W, splat = ctx.pack
         _, need_geo, need_col, need_pose = ctx.needs_input_grad
         B, L = poses.shape[:2]
         dev, cap = geo.device, geo.shape[1]
@@ -85,8 +86,8 @@ class _RenderFn(torch.autograd.Function):
             scratch = torch.empty(_C.lib().gsx_render_views_bwd_scratch_bytes(B, L, H, W), dtype=torch.uint8,
                                   device=dev)
         gs = [None if g is None else g.contiguous() for g in (g_depth, g_rgb, g_normals, g_conf)]
-        _C.launch("gsx_render_views_bwd", geo.detach(), counts, cap, K, 16, poses.detach(), L * 16, index, B, L, H, W, *gs,
-                  d_geo, d_col, d_poses, scratch, 0 if scratch is None else scratch.numel())
+        _C.launch("gsx_render_splats_bwd", geo.detach(), counts, cap, K, 16, poses.detach(), L * 16, index, B, L, H, W,
+                  *gs, d_geo, d_col, d_poses, scratch, 0 if scratch is None else scratch.numel(), splat)
         return None, d_geo, d_col, d_poses
 
 
@@ -99,8 +100,11 @@ def _camera(t, name, B):
         raise ValueError("Expected equal batch sizes for {} and poses. Got {} and {}.".format(name, t.shape[0], B))
 
 
+MAX_SPLAT_PX = 16  # GSX_MAX_SPLAT_PX (include/gsx.h)
+
+
 def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses: torch.Tensor, height: int,
-                       width: int) -> RenderedViews:
+                       width: int, max_splat_px: int = 0) -> RenderedViews:
     """Renders every map of the batch from L cameras: a map row covers the one pixel it projects to (the projection of
     find_active_map_points) and each pixel shows the covering row with the smallest camera-frame depth, ties to the
     lowest row index.
@@ -108,7 +112,13 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
     intrinsics (B, 1, 4, 4) as in RGBDImages; poses (B, L, 4, 4) camera-to-world.  `RGBDImages(out.rgb, out.depth,
     intrinsics, poses)` turns the result into frames.  Differentiable w.r.t. the map rows (points, normals, colours,
     confidence counts) and the poses, at the fixed pixel assignment; not w.r.t. the intrinsics.  No host
-    synchronisation."""
+    synchronisation.
+
+    max_splat_px (extension, 0 .. 16, default 0 = the one-pixel rule above for every row): a row with a surfel radius
+    (`radii_padded` > 0, PointFusion(surfel_radii=True)) and a non-zero normal is drawn as an oriented disk: every pixel
+    within max_splat_px pixels of its projected centre whose ray meets the disk shows it, at the depth where the ray
+    meets the disk's plane.  Rows without a radius keep the one-pixel rule.  The footprint carries no gradient, and
+    the radius none either.  Cost grows with (2 max_splat_px + 1)^2 per disk row and view."""
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     for name, v in (("height", height), ("width", width)):
@@ -116,6 +126,10 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
             raise TypeError("Expected {} to be of type int. Got {}.".format(name, type(v)))
         if v < 1:
             raise ValueError("Expected {} >= 1. Got {}.".format(name, v))
+    if not isinstance(max_splat_px, int) or isinstance(max_splat_px, bool):
+        raise TypeError("Expected max_splat_px to be of type int. Got {}.".format(type(max_splat_px)))
+    if not 0 <= max_splat_px <= MAX_SPLAT_PX:
+        raise ValueError("Expected 0 <= max_splat_px <= {}. Got {}.".format(MAX_SPLAT_PX, max_splat_px))
     _camera(poses, "poses", None)
     B = poses.shape[0]
     _camera(intrinsics, "intrinsics", B)
@@ -147,8 +161,9 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
     from ..odometry.icputils import _wants_grad
 
     if _wants_grad(geo, col, poses_c):
-        outs = _RenderFn.apply((counts.clone(), pointclouds._bound, K, height, width) + want, geo, col, poses_c)
+        outs = _RenderFn.apply((counts.clone(), pointclouds._bound, K, height, width) + want + (max_splat_px,), geo, col,
+                               poses_c)
     else:
         outs = _render(geo.detach(), None if col is None else col.detach(), counts, pointclouds._bound, K,
-                       poses_c.detach(), height, width, *want)
+                       poses_c.detach(), height, width, *want, max_splat_px)
     return RenderedViews(*outs)

@@ -16,7 +16,8 @@
  *     a base pointer for the frame plus the element stride (`*_bstride`, in floats) between batch elements,
  *     so frame s of a (B,L,H,W,C) tensor is addressed without a copy.
  *   - the surfel map has a fixed capacity and SECTOR-PACKED rows: map_geometry (B,cap,8) float32 rows
- *     (px,py,pz,nx,ny,nz,ccount,0) - exactly one 32-byte DRAM sector per surfel - and map_colors (B,cap,4) rows
+ *     (px,py,pz,nx,ny,nz,ccount,radius) - exactly one 32-byte DRAM sector per surfel; the radius is 0 unless the map
+ *     is fused with surfel radii on - and map_colors (B,cap,4) rows
  *     (r,g,b,0); both 16-byte aligned, every row access is a 128-bit load / store.  counts int32 (B,).  Rows
  *     >= counts[b] are never read.  (gradslam's padded tensors points / normals / colors / features are the
  *     strided views [..., 0:3], [..., 3:6], colours [..., 0:3], [..., 6:7] of these two arrays.)
@@ -135,6 +136,18 @@ int gsx_fusion_project_select(const float *map_geometry, const int32_t *counts, 
 int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_ccounts, const int32_t *counts_in,
                             int32_t *counts_out, int64_t capacity, const float *rgb, int64_t rgb_bstride, int B, int H,
                             int W, void *workspace, int32_t *overflow_flag, int32_t *assoc_out, void *stream);
+/* gsx_fusion_merge_append with surfel radii (surfel_radii = 1; 0 is gsx_fusion_merge_append itself).  Slot 7 of every
+ * merged or appended geometry row becomes the surfel radius (Keller et al. 2013; ElasticFusion) of the pixel, from its
+ * depth d, its camera-frame normal n and the live camera's K^-1 diagonal k00 = 1/(fx+1e-6), k11 = 1/(fy+1e-6), each
+ * operation rounded separately:
+ *   s = 0.5 * (k00 + k11),  r0 = (sqrt(2) * d) * s,  r = (2|n_z| <= 1) ? 2 * r0 : r0 / |n_z|
+ * appended: slot 7 = r; merged: slot 7 = ((c0 * r_row) + (alpha * r)) * inv with the merge's c0, alpha and inv, except
+ * that a row of radius 0 (appended without radii) takes r.  No decision depends on the radius: slots 0-6, the colour
+ * rows, counts and assoc_out equal those of surfel_radii = 0 bit for bit.  surfel_radii other than 0 / 1 is refused. */
+int gsx_fusion_merge_append_radii(float *map_geometry, float *map_colors, int with_ccounts, const int32_t *counts_in,
+                                  int32_t *counts_out, int64_t capacity, const float *rgb, int64_t rgb_bstride, int B,
+                                  int H, int W, void *workspace, int32_t *overflow_flag, int32_t *assoc_out,
+                                  int surfel_radii, void *stream);
 
 /* Backward of K4 (autograd.Function backward of the differentiable mode).
  * replaces the tape PyTorch builds through fuse_with_map   gradslam/slam/fusionutils.py:654-720 (merge),
@@ -142,7 +155,8 @@ int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_cco
  * upstream gradients of the updated map in the packed row layout (B,capacity_out,8 / 4) (either may be NULL = zero)
  * -> gradients of the pre-merge map (B,capacity_in,8 / 4) (every row written; padding rows and padding slots zero) and
  * of the frame values: world vertex / normal maps, colours and - through the confidence weight alpha - the
- * camera-frame vertex map, all (B,H,W,3). */
+ * camera-frame vertex map, all (B,H,W,3).  Surfel radii (slot 7) carry no gradient: d_map_geometry's slot 7 is zero and
+ * slot 7 of g_geometry is not read. */
 int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, const float *map_geometry,
                                 const float *map_colors, int with_ccounts, int64_t capacity_in,
                                 const float *g_geometry, const float *g_colors, int64_t capacity_out,
@@ -181,6 +195,15 @@ int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t 
                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max, float c_stable,
                                 void *prune_scratch, int64_t prune_scratch_bytes, float margin, void *fs_scratch,
                                 int64_t fs_scratch_bytes, int32_t *overflow_flag, void *stream);
+/* gsx_pointfusion_sequence_gt with surfel radii: every frame's K4 runs as gsx_fusion_merge_append_radii with
+ * surfel_radii (0 or 1; 0 is gsx_pointfusion_sequence_gt itself).  Pruning moves whole rows, radius included. */
+int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                      int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
+                                      const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
+                                      float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring,
+                                      int t_max, float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                      float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+                                      int32_t *overflow_flag, int surfel_radii, void *stream);
 /* ------------------------------------------------------------------------------------------------
  * Removal of unstable surfels (opt-in extension; gradslam has no such step, so no reference line is replaced).
  * Keller et al. 2013, "Real-time 3D reconstruction in dynamic scenes using point-based fusion", section 4.3: a surfel
@@ -477,12 +500,34 @@ int gsx_render_views(const float *map_geometry, const float *map_colors, const i
  * 3x4 block; bottom row zero), reduced per pixel tile then summed in tile order.  Any of the three may be NULL.
  * Deterministic, no atomics; no gradient w.r.t. the intrinsics.  scratch: gsx_render_views_bwd_scratch_bytes(B,L,H,W)
  * bytes (only needed for d_poses). */
+/* gsx_render_views with disk splats (max_splat_px = 0 is gsx_render_views itself; 1 .. GSX_MAX_SPLAT_PX, others are
+ * refused).  A row n with radius r = slot 7 > 0 and a non-zero normal is an oriented disk: with q = T^-1 p and m = R^T n
+ * (skipped unless q.z > 0), the pixels (h,w) of the box of +-max_splat_px pixels around rint(u), rint(v) of its projected
+ * centre (the projection above; the box clipped to the image) whose ray d = K^-1 (w,h,1) (k00 = 1/(fx+1e-6) ...) meets
+ * the disk's plane at t = (m.q)/(m.d) with m.d != 0, t > 0 and |t d - q|^2 <= r^2 take the key bits(t) << 32 | n; the
+ * z-buffer, ties and fill are unchanged, and depth = t.  Other rows (radius 0, zero normal) cover one pixel as above.
+ * Each disk row tests up to (2 max_splat_px + 1)^2 pixels per view. */
+#define GSX_MAX_SPLAT_PX 16
+int gsx_render_splats(const float *map_geometry, const float *map_colors, const int32_t *counts, int64_t capacity,
+                      int64_t max_count, const float *intrinsics, int64_t K_bstride, const float *poses,
+                      int64_t pose_bstride, int B, int L, int H, int W, int64_t *index, float *depth, float *rgb,
+                      float *normals, float *confidence, int max_splat_px, void *stream);
+
 int64_t gsx_render_views_bwd_scratch_bytes(int B, int L, int H, int W);
 int gsx_render_views_bwd(const float *map_geometry, const int32_t *counts, int64_t capacity, const float *intrinsics,
                          int64_t K_bstride, const float *poses, int64_t pose_bstride, const int64_t *index, int B,
                          int L, int H, int W, const float *g_depth, const float *g_rgb, const float *g_normals,
                          const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses, void *scratch,
                          int64_t scratch_bytes, void *stream);
+/* Backward of gsx_render_splats at a fixed index (max_splat_px = 0 is gsx_render_views_bwd itself).  A disk row's
+ * depth is t: dt/dq = m/(m.d), dt/dm = (q - t d)/(m.d) carry the gradient to its position, its normal and the pose; a
+ * row sums, in (view, h, w) order, the gradients of the pixels of its footprint that it won.  No gradient w.r.t. the
+ * radius (slot 7 of d_geometry is zero), the footprint or the intrinsics.  Deterministic, no atomics. */
+int gsx_render_splats_bwd(const float *map_geometry, const int32_t *counts, int64_t capacity, const float *intrinsics,
+                          int64_t K_bstride, const float *poses, int64_t pose_bstride, const int64_t *index, int B,
+                          int L, int H, int W, const float *g_depth, const float *g_rgb, const float *g_normals,
+                          const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses, void *scratch,
+                          int64_t scratch_bytes, int max_splat_px, void *stream);
 
 #ifdef __cplusplus
 }
