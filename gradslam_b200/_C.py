@@ -56,12 +56,22 @@ SIGNATURES = {
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                 c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_float, c_vp, c_i64, c_vp, c_int,
                 c_vp]),
+    "gsx_pointfusion_sequence_gt_merge": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                c_float, c_float, c_double, c_vp, c_vp, c_int, c_float, c_vp, c_i64, c_float, c_vp, c_i64, c_vp, c_int,
+                c_vp, c_i64, c_vp]),
     "gsx_fusion_prune_scratch_bytes": (c_i64, [c_int, c_i64]),
     "gsx_fusion_free_space_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_i64]),
     "gsx_fusion_prune": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_float, c_int, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64,
                 c_vp, c_i64, c_int, c_int, c_float, c_vp, c_i64, c_vp]),
     "gsx_fusion_prune_bwd": (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp]),
+    "gsx_fusion_merge_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_i64]),
+    "gsx_fusion_prune_merge": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_float, c_int, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64,
+                c_vp, c_i64, c_int, c_int, c_float, c_vp, c_i64, c_float, c_vp, c_i64, c_vp, c_vp]),
+    "gsx_fusion_prune_merge_bwd": (
+        c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp]),
     "gsx_debug_fail_at_frame": (None, [c_int]),
     "gsx_debug_set_k2_grid_cap": (None, [c_int]),
     "gsx_debug_set_bin_capacity": (None, [c_int]),

@@ -47,6 +47,8 @@ struct SequencePrune {
   void *scratch;
   float margin;
   void *fs_scratch;
+  void *merge_scratch;  // null: no merging of overlapping surfels
+  float dot_th;
 };
 
 // one group's pruned step s after its K4 (max_count: the host bound of the counts after that K4)
@@ -57,7 +59,7 @@ static int sequence_prune_group(const SequencePrune *prune, float *geo, float *c
     return prune_group(geo, col, cout, cap, prune->ring, prune->t_max + 2, s, prune->t_max, prune->c_stable, B, b0, nb,
                        nullptr, prune->scratch, st);
   const FreeSpaceStep fs{free_space_assoc(prune->fs_scratch, B, H, W, cap, 0), intrinsics, 16, poses, pose_bs, H, W,
-                         prune->margin, prune->fs_scratch, max_count};
+                         prune->margin, prune->fs_scratch, max_count, prune->merge_scratch, prune->dot_th, nullptr};
   return prune_group(geo, col, cout, cap, prune->ring, prune->t_max + 2, s, prune->t_max, prune->c_stable, B, b0, nb,
                      nullptr, prune->scratch, st, &fs);
 }
@@ -118,14 +120,15 @@ extern "C" void gsx_debug_fail_at_frame(int s) { g_fail_at_frame = s; }
 
 extern "C" int gsx_pointfusion_sequence_groups(int B) { return B <= 0 ? 0 : gsx::sequence_groups(B); }
 
-extern "C" int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map_colors, int32_t *counts,
+extern "C" int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map_colors, int32_t *counts,
                                                  int64_t capacity, int64_t max_count0, const float *depth,
                                                  const float *rgb, const float *intrinsics, const float *poses, int B,
                                                  int L, int s_begin, int s_end, int H, int W, float dist_th,
                                                  float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
                                                  float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
                                                  float margin, void *fs_scratch, int64_t fs_scratch_bytes,
-                                                 int32_t *overflow_flag, int surfel_radii, void *stream) {
+                                                 int32_t *overflow_flag, int surfel_radii, void *merge_scratch,
+                                                 int64_t merge_scratch_bytes, void *stream) {
   GSX_CHECK_ARG(B >= 0 && L >= 0 && H >= 2 && W >= 2, "gsx_pointfusion_sequence_gt: bad extents");
   GSX_CHECK_ARG(surfel_radii == 0 || surfel_radii == 1,
                 "gsx_pointfusion_sequence_gt: surfel_radii must be 0 or 1, not %d", surfel_radii);
@@ -152,8 +155,16 @@ extern "C" int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map
                                   fs_scratch_bytes >= gsx::free_space_scratch_bytes(B, H, W, capacity)),
                   "gsx_pointfusion_sequence_gt: free-space scratch of %lld bytes < "
                   "gsx_fusion_free_space_scratch_bytes", (long long)fs_scratch_bytes);
+    GSX_CHECK_ARG(!merge_scratch || fs_scratch,
+                  "gsx_pointfusion_sequence_gt_merge: merging needs the free-space scratch (margin = inf removes no "
+                  "violator)");
+    GSX_CHECK_ARG(!merge_scratch || (reinterpret_cast<uintptr_t>(merge_scratch) & 15) == 0,
+                  "gsx_pointfusion_sequence_gt_merge: the merge scratch must be 16-byte aligned");
+    GSX_CHECK_ARG(!merge_scratch || merge_scratch_bytes >= gsx::merge_scratch_bytes(B, H, W, capacity),
+                  "gsx_pointfusion_sequence_gt_merge: merge scratch of %lld bytes < gsx_fusion_merge_scratch_bytes",
+                  (long long)merge_scratch_bytes);
   }
-  const gsx::SequencePrune prune_args{ring, t_max, c_stable, prune_scratch, margin, fs_scratch};
+  const gsx::SequencePrune prune_args{ring, t_max, c_stable, prune_scratch, margin, fs_scratch, merge_scratch, dot_th};
   const gsx::SequencePrune *prune = ring ? &prune_args : nullptr;
   const int64_t P = (int64_t)H * W;
   // K4's scan epoch is ticket / tiles + 1 and must fit the 30 bits of a look-back state word
@@ -232,6 +243,21 @@ extern "C" int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map
     cudaStreamWaitEvent(user, gs->join[g], 0);
   }
   return rc;
+}
+
+extern "C" int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map_colors, int32_t *counts,
+                                                 int64_t capacity, int64_t max_count0, const float *depth,
+                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
+                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
+                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
+                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                                 float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+                                                 int32_t *overflow_flag, int surfel_radii, void *stream) {
+  return gsx_pointfusion_sequence_gt_merge(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb,
+                                           intrinsics, poses, B, L, s_begin, s_end, H, W, dist_th, dot_th, sigma,
+                                           workspace, ring, t_max, c_stable, prune_scratch, prune_scratch_bytes, margin,
+                                           fs_scratch, fs_scratch_bytes, overflow_flag, surfel_radii, nullptr, 0,
+                                           stream);
 }
 
 extern "C" int gsx_pointfusion_sequence_gt(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,

@@ -16,6 +16,10 @@ struct FreeSpaceStep {
   float margin;
   void *scratch;        // free_space_scratch_bytes(B_total, H, W, cap)
   int64_t max_count;    // host-side upper bound of the counts (KFt's grid)
+  // merging of overlapping surfels: null merge_scratch = off
+  void *merge_scratch;  // merge_scratch_bytes(B_total, H, W, cap)
+  float dot_th;
+  int32_t *absorbed;    // optional (B_total, cap), full-batch base pointer
 };
 
 // removal of unstable surfels (and, with fs, of free-space violations) for the elements [b0, b0 + nb)
@@ -24,6 +28,7 @@ int prune_group(float *geo, float *col, int32_t *counts, int64_t cap, int32_t *r
                 const FreeSpaceStep *fs = nullptr);
 int64_t prune_scratch_bytes(int B, int64_t capacity);
 int64_t free_space_scratch_bytes(int B, int H, int W, int64_t capacity);
+int64_t merge_scratch_bytes(int B, int H, int W, int64_t capacity);
 // the group's slice of the free-space scratch's assoc image (the sequence driver's K4 writes it)
 int32_t *free_space_assoc(void *scratch, int B_total, int H, int W, int64_t capacity, int b0);
 

@@ -569,10 +569,47 @@ class _PruneFn(torch.autograd.Function):
         return None, None, d_geo, d_col
 
 
-def _prune(pointclouds, stable_confidence, t_max, free_space=None):
+class _PruneMergeFn(torch.autograd.Function):
+    """_PruneFn with merging of overlapping surfels: the forward also records every absorbed pair and keeps the pairs'
+    pre-step rows (b, m, n and rows m, n: 104 bytes per pair, about 1 % of the map's rows at 640x480), and the backward
+    (gsx_fusion_prune_merge_bwd) adds the quotient rule of each absorption to the gather.  Finding the pairs costs one
+    host synchronisation per pruned step (their number sizes the record)."""
+
+    @staticmethod
+    def forward(ctx, prune, counts, geo, col):
+        B, cap = geo.shape[0], geo.shape[1]
+        geo_o, col_o = geo.detach().clone(), col.detach().clone()
+        keep_map = torch.arange(cap, dtype=torch.int32, device=geo.device).repeat(B, 1)  # rows before the scan: identity
+        absorbed = torch.full((B, cap), -1, dtype=torch.int32, device=geo.device)
+        counts_in = counts.clone()
+        prune(geo_o, col_o, keep_map, absorbed)
+        bm = torch.nonzero(absorbed >= 0)
+        b, m = bm[:, 0], bm[:, 1]
+        n = absorbed[b, m].long()
+        rows = torch.stack([m, n], 1)
+        pair_geo = geo.detach()[b.unsqueeze(1), rows].contiguous()  # (A, 2, 8)
+        pair_col = col.detach()[b.unsqueeze(1), rows].contiguous()  # (A, 2, 4)
+        pairs = torch.stack([b, m, n], 1).to(torch.int32).contiguous()
+        ctx.saved = (keep_map, counts_in, pairs, pair_geo, pair_col)
+        return geo_o, col_o
+
+    @staticmethod
+    def backward(ctx, g_geo, g_col):
+        keep_map, counts_in, pairs, pair_geo, pair_col = ctx.saved
+        B, cap = keep_map.shape
+        gs = [None if g is None else g.contiguous().float() for g in (g_geo, g_col)]
+        d_geo = torch.empty((B, cap, 8), dtype=torch.float32, device=keep_map.device)
+        d_col = torch.empty((B, cap, 4), dtype=torch.float32, device=keep_map.device)
+        _C.launch("gsx_fusion_prune_merge_bwd", keep_map, counts_in, cap, pairs, pair_geo, pair_col, pairs.shape[0],
+                  gs[0], gs[1], cap, B, d_geo, d_col)
+        return None, None, d_geo, d_col
+
+
+def _prune(pointclouds, stable_confidence, t_max, free_space=None, merge_dot_th=None):
     """One pruned step of the map, in place: the age rule and, with free_space = (assoc, K, poses, H, W, margin) of the
-    step's K4, the free-space rule.  A differentiable op when the map's rows require grad.  The map's pruning history is
-    created at its first pruned step (rows already in the map count as created then)."""
+    step's K4, the free-space rule, and with merge_dot_th as well, merging of overlapping surfels.  A differentiable op
+    when the map's rows require grad.  The map's pruning history is created at its first pruned step (rows already in
+    the map count as created then)."""
     h = pointclouds._prune
     if h is None:
         h = pointclouds._prune = _PruneHistory.fresh(len(pointclouds), t_max, pointclouds.device)
@@ -586,12 +623,22 @@ def _prune(pointclouds, stable_confidence, t_max, free_space=None):
                                  device=dev)
         fs = (assoc, K, 16, poses, 16, H, W, float(margin), fs_scratch, fs_scratch.numel())
 
-    def launch(geo, col, keep_map):
-        _C.launch("gsx_fusion_prune", geo, col, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
-                  float(stable_confidence), B, keep_map, scratch, scratch.numel(), *fs)
+    if merge_dot_th is None:
+        def launch(geo, col, keep_map):
+            _C.launch("gsx_fusion_prune", geo, col, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
+                      float(stable_confidence), B, keep_map, scratch, scratch.numel(), *fs)
+        fn = _PruneFn
+    else:
+        ms = torch.empty(_C.lib().gsx_fusion_merge_scratch_bytes(B, H, W, cap), dtype=torch.uint8, device=dev)
+
+        def launch(geo, col, keep_map, absorbed=None):
+            _C.launch("gsx_fusion_prune_merge", geo, col, counts, cap, h.ring, h.t_max + 2, h.step, h.t_max,
+                      float(stable_confidence), B, keep_map, scratch, scratch.numel(), *fs, float(merge_dot_th), ms,
+                      ms.numel(), absorbed)
+        fn = _PruneMergeFn
 
     if torch.is_grad_enabled() and any(t.requires_grad for t in pointclouds._grad_tensors()):
-        pointclouds._geo, pointclouds._col = _PruneFn.apply(launch, counts, pointclouds._geo, pointclouds._col)
+        pointclouds._geo, pointclouds._col = fn.apply(launch, counts, pointclouds._geo, pointclouds._col)
     else:
         launch(*_map_ptrs(pointclouds, dev), None)
     # one more pruned step; the sizes changed on the device (the host bound stays an upper bound), and rows past the new
@@ -625,11 +672,18 @@ def _check_free_space_margin(margin):
         raise ValueError("free_space_margin ({}) must be >= 0".format(margin))
 
 
+def _check_merge_overlapping(merge_overlapping, surfel_radii):
+    if not isinstance(merge_overlapping, bool):
+        raise TypeError("merge_overlapping must be of type bool; but was of type {}.".format(type(merge_overlapping)))
+    if merge_overlapping and not surfel_radii:
+        raise ValueError("merge_overlapping needs surfel_radii=True (it merges surfels whose disks overlap)")
+
+
 def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Union[float, int],
                    dot_th: Union[float, int], sigma: Union[torch.Tensor, float, int],
                    stable_confidence: Union[float, int], max_unstable_age: int,
                    free_space_margin: Union[float, int], inplace: bool = False, *,
-                   surfel_radii: bool = False) -> Pointclouds:
+                   surfel_radii: bool = False, merge_overlapping: bool = False) -> Pointclouds:
     """update_map_fusion followed by one pruned step with both of Keller et al.'s (2013, section 4.3) outlier rules
     (an extension: gradslam keeps every surfel).  The age rule is prune_unstable's.  The free-space rule: wherever the
     live frame merged a pixel into a surfel that is stable after the merge (confidence >= stable_confidence), every
@@ -637,11 +691,22 @@ def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Un
     stable or not.  Unlike the paper (a 4x4-supersampled index map), "in front" is decided at image resolution, at the
     pixel the association's own projection gives.  Both removals are one stable compaction: kept rows keep their order.
     free_space_margin = inf removes no violator (the result is update_map_fusion + prune_unstable).  surfel_radii: as in
-    update_map_fusion; the pruning moves whole rows, radius included."""
+    update_map_fusion; the pruning moves whole rows, radius included.
+
+    merge_overlapping (extension, default False; needs surfel_radii=True): in the same step, Keller et al.'s third rule,
+    "merge surfels with similar position and normal and overlapping radii".  At every pixel the live frame merged into
+    a surfel m that is stable after the merge (and that the free-space rule keeps), the other surfels projecting to that
+    pixel are candidates when no pixel merged into them, neither rule removes them, both radii are positive, the normals'
+    dot product exceeds dot_th and the disks overlap (centre distance <= r_m + r_n).  The closest candidate (ties: the
+    lower index) is absorbed: m becomes the confidence-weighted mean of both surfels (position, normal, colour, radius;
+    the confidences add up) and the candidate is removed.  As the free-space rule, this works at the merged pixel, at
+    image resolution, not on the paper's 4x4-supersampled index map.  Merging runs with free_space_margin = inf as
+    well, which removes no violator.  Gradients flow through the absorption's weighted mean."""
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     _check_frame(rgbdimages)
     _check_surfel_radii(surfel_radii)
+    _check_merge_overlapping(merge_overlapping, surfel_radii)
     _check_free_space_margin(free_space_margin)
     t_max = int(max_unstable_age)
     _check_history(pointclouds, t_max)
@@ -657,7 +722,7 @@ def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Un
     dev = pointclouds.device
     free_space = (got[0], _dense(frames.intrinsics.detach(), "intrinsics", dev),
                   _dense(frames.poses.detach(), "poses", dev), H, W, free_space_margin)
-    _prune(pointclouds, stable_confidence, t_max, free_space)
+    _prune(pointclouds, stable_confidence, t_max, free_space, dot_th if merge_overlapping else None)
     return pointclouds
 
 

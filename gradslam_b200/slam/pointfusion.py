@@ -13,8 +13,8 @@ from .. import _C
 from ..structures.pointclouds import Pointclouds
 from ..structures.rgbdimages import RGBDImages
 from ..structures.pointclouds import _PruneHistory
-from .fusionutils import (_check_free_space_margin, _check_history, _prune_scratch, fuse_and_prune, prune_unstable,
-                          update_map_fusion)
+from .fusionutils import (_check_free_space_margin, _check_history, _check_merge_overlapping, _prune_scratch,
+                          fuse_and_prune, prune_unstable, update_map_fusion)
 from .icpslam import ICPSLAM
 
 __all__ = ["PointFusion"]
@@ -46,7 +46,7 @@ class PointFusion(ICPSLAM):
                  nu: Union[float, int] = 200.0, association: str = "nn",
                  device: Union[torch.device, str, None] = None, stable_confidence: Union[float, int, None] = None,
                  max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None,
-                 surfel_radii: bool = False):
+                 surfel_radii: bool = False, merge_overlapping: bool = False):
         """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
         surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
         (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
@@ -62,9 +62,18 @@ class PointFusion(ICPSLAM):
 
         surfel_radii (extension, default False): every fused surfel also gets a radius (`radii_padded`), as
         fusionutils.update_map_fusion(surfel_radii=True) gives it, in the whole-sequence call, the step API, the
-        differentiable mode and with pruning.  Nothing else in the map changes."""
+        differentiable mode and with pruning.  Nothing else in the map changes.
+
+        merge_overlapping (extension, default False; needs surfel_radii=True, stable_confidence and max_unstable_age): in
+        every pruned step, also merge overlapping surfels (Keller et al. 2013, section 4.3, the third rule), as
+        fusionutils.fuse_and_prune(merge_overlapping=True) does: a surfel that projects to a pixel the live frame merged
+        into a stable surfel, with a similar normal (dot > cos(angle_th)) and a disk that overlaps the stable surfel's,
+        is folded into it (confidence-weighted mean) and removed; one per pixel, the closest.  Without
+        free_space_margin no free-space violation is removed.  stable_confidence=0 makes the age rule a no-op (every
+        surfel is stable), so merging can run alone; the stable surfels are then every surfel the frame merged into."""
         if not isinstance(surfel_radii, bool):
             raise TypeError("surfel_radii must be of type bool; but was of type {}.".format(type(surfel_radii)))
+        _check_merge_overlapping(merge_overlapping, surfel_radii)
         for name, val, kinds in (("stable_confidence", stable_confidence, (float, int)),
                                  ("max_unstable_age", max_unstable_age, (int,))):
             if val is not None and (isinstance(val, bool) or not isinstance(val, kinds)):
@@ -80,6 +89,9 @@ class PointFusion(ICPSLAM):
             _check_free_space_margin(free_space_margin)
             if stable_confidence is None:
                 raise ValueError("free_space_margin needs stable_confidence and max_unstable_age")
+        if merge_overlapping and stable_confidence is None:
+            raise ValueError("merge_overlapping needs stable_confidence and max_unstable_age (stable_confidence=0 makes "
+                             "the age rule a no-op)")
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
                          lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device)
         if not isinstance(dist_th, (float, int)):
@@ -99,14 +111,16 @@ class PointFusion(ICPSLAM):
         self.max_unstable_age = max_unstable_age
         self.free_space_margin = free_space_margin
         self.surfel_radii = surfel_radii
+        self.merge_overlapping = merge_overlapping
 
     def _map(self, pointclouds: Pointclouds, live_frame: RGBDImages, inplace: bool = False):
         if self.stable_confidence is not None and isinstance(pointclouds, Pointclouds):
             _check_history(pointclouds, self.max_unstable_age)
-        if self.free_space_margin is not None:
+        if self.free_space_margin is not None or self.merge_overlapping:
+            margin = math.inf if self.free_space_margin is None else self.free_space_margin
             return fuse_and_prune(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, self.stable_confidence,
-                                  self.max_unstable_age, self.free_space_margin, inplace,
-                                  surfel_radii=self.surfel_radii)
+                                  self.max_unstable_age, margin, inplace, surfel_radii=self.surfel_radii,
+                                  merge_overlapping=self.merge_overlapping)
         pointclouds = update_map_fusion(pointclouds, live_frame, self.dist_th, self.dot_th, self.sigma, inplace,
                                         surfel_radii=self.surfel_radii)
         if self.stable_confidence is not None:
@@ -178,14 +192,20 @@ class PointFusion(ICPSLAM):
         ws = _SequenceWorkspace.get(dev, B, H, W)
         prune = (None, 0, 0.0, None, 0)  # ring, t_max, c_stable, scratch, its bytes: pruning off
         free_space = (0.0, None, 0)  # margin, scratch, its bytes: the age rule alone
+        merge = (None, 0)  # merge scratch, its bytes: no merging
         if self.stable_confidence is not None:  # a fresh map: frame s of the call is pruned step s
             pc._prune = hist = _PruneHistory.fresh(B, self.max_unstable_age, dev)
             scratch = _prune_scratch(B, pc.capacity, dev)
             prune = (hist.ring, self.max_unstable_age, float(self.stable_confidence), scratch, scratch.numel())
-            if self.free_space_margin is not None:
+            if self.free_space_margin is not None or self.merge_overlapping:
                 fs_scratch = torch.empty(_C.lib().gsx_fusion_free_space_scratch_bytes(B, H, W, pc.capacity),
                                          dtype=torch.uint8, device=dev)
-                free_space = (float(self.free_space_margin), fs_scratch, fs_scratch.numel())
+                margin = math.inf if self.free_space_margin is None else float(self.free_space_margin)
+                free_space = (margin, fs_scratch, fs_scratch.numel())
+            if self.merge_overlapping:
+                ms = torch.empty(_C.lib().gsx_fusion_merge_scratch_bytes(B, H, W, pc.capacity), dtype=torch.uint8,
+                                 device=dev)
+                merge = (ms, ms.numel())
         main = torch.cuda.current_stream(dev)
         ready = []
         if not on_device:
@@ -208,10 +228,10 @@ class PointFusion(ICPSLAM):
                 for b in range(B):
                     _C.launch("gsx_ingest_raw", raw_rgb[b, s0:s1], raw_depth[b, s0:s1], (s1 - s0) * P,
                               frames.scaling_factor, 1 if frames.normalize_color else 0, rgb[b, s0:s1], depth[b, s0:s1])
-            _C.launch("gsx_pointfusion_sequence_gt_radii", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+            _C.launch("gsx_pointfusion_sequence_gt_merge", pc._geo, pc._col, pc._counts_dev, pc.capacity,
                       min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
                       float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag(),
-                      1 if self.surfel_radii else 0)
+                      1 if self.surfel_radii else 0, *merge)
         if not on_device:
             for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
                 t.record_stream(copy_stream)

@@ -184,7 +184,9 @@ int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, 
 /* number of independent batch groups gsx_pointfusion_sequence_gt runs on concurrent internal streams for a batch of
  * B (default 2, environment GSX_SEQ_GROUPS = 1..4 overrides; never more than B).  Kernel launches per call =
  * groups * (2 * frames - [map empty on entry] + header launches), plus one memset; a group launches one header
- * launch for each 64-frame block (frames [64k, 64k + 64)) that [s_begin, s_end) touches. */
+ * launch for each 64-frame block (frames [64k, 64k + 64)) that [s_begin, s_end) touches.  Pruning adds, per group and
+ * frame, KP and two memsets (the age rule), KFb, KFt and one more memset (the free-space rule: KFt only once the map
+ * has rows), and KM and one more memset (merging). */
 int gsx_pointfusion_sequence_groups(int B);
 /* workspace of the sequence driver: one frame workspace (gsx_fusion_workspace_bytes) plus the headers of 64 frames
  * (about 88.5 MB at B=8, 640x480), 16-byte aligned, no initialisation needed */
@@ -204,6 +206,19 @@ int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map_colors, in
                                       int t_max, float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
                                       float margin, void *fs_scratch, int64_t fs_scratch_bytes,
                                       int32_t *overflow_flag, int surfel_radii, void *stream);
+/* gsx_pointfusion_sequence_gt_radii with merging of overlapping surfels (gsx_fusion_prune_merge below) in every pruned
+ * step: merge_scratch NULL turns it off (and is gsx_pointfusion_sequence_gt_radii itself); otherwise it needs ring and
+ * fs_scratch (margin = inf removes no violator), is gsx_fusion_merge_scratch_bytes(B, H, W, capacity) bytes, 16-byte
+ * aligned, and the merge's normal test uses the fusion's dot_th.  Merging reads the radii: run it with
+ * surfel_radii = 1 (rows of radius 0 are never merged). */
+int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                      int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
+                                      const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
+                                      float dist_th, float dot_th, double sigma, void *workspace, int32_t *ring,
+                                      int t_max, float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                      float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+                                      int32_t *overflow_flag, int surfel_radii, void *merge_scratch,
+                                      int64_t merge_scratch_bytes, void *stream);
 /* ------------------------------------------------------------------------------------------------
  * Removal of unstable surfels (opt-in extension; gradslam has no such step, so no reference line is replaced).
  * Keller et al. 2013, "Real-time 3D reconstruction in dynamic scenes using point-based fusion", section 4.3: a surfel
@@ -250,6 +265,41 @@ int gsx_fusion_prune(float *map_geometry, float *map_colors, int32_t *counts, in
 int gsx_fusion_prune_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
                          const float *g_geometry, const float *g_colors, int64_t capacity_out, int B,
                          float *d_map_geometry, float *d_map_colors, void *stream);
+/* Merging of overlapping surfels (opt-in, in the same pruned step as both rules above; Keller et al. 2013, section 4.3:
+ * "merge surfels with similar position and normal and overlapping radii").  As the free-space rule, it works at the
+ * pixel the live frame merged, at image resolution, not on the paper's 4x4-supersampled index map.  Every test is
+ * decided on the map K4 left, before any absorption, with each operation rounded to fp32 on its own:
+ *   - absorber: a pixel u with assoc[b][u] = -(m+1) and ccount_m >= c_stable (the pixels that have a free-space bound),
+ *     unless the free-space rule removes m in this step;
+ *   - candidate n < counts[b] at u: project() puts n in the frustum at u, n != m, no pixel merged into n, neither rule
+ *     removes n, r_m > 0 and r_n > 0 (slot 7), dot = (nm.x nn.x + nm.y nn.y) + nm.z nn.z > dot_th, and with
+ *     d = p_n - p_m, d2 = (d.x d.x + d.y d.y) + d.z d.z <= (r_m + r_n)^2;
+ *   - the candidate of smallest (d2, n) is absorbed: c = c_m + c_n, inv = 1 / c (1 / 1 if c == 0), and position,
+ *     normal, colour and radius of m become ((c_m x_m) + (c_n x_n)) * inv, its ccount c; row n is removed.
+ * The step's one stable compaction removes the age rule's rows, the violators and the absorbed rows (the ring update of
+ * the free-space rule; m keeps its index).  Pairs are disjoint, so the result is deterministic.
+ * merge_scratch: gsx_fusion_merge_scratch_bytes(B, H, W, capacity) bytes, 16-byte aligned, re-armed by every call.
+ * Four launches per pruned step with merging (KFb, KFt, KM, KP) plus three memsets. */
+int64_t gsx_fusion_merge_scratch_bytes(int B, int H, int W, int64_t capacity);
+/* gsx_fusion_prune plus merging: merge_scratch NULL is gsx_fusion_prune itself (dot_th and absorbed are not read);
+ * otherwise assoc and the free-space arguments are required.  absorbed: NULL, or int32 (B, capacity) filled with -1 by
+ * the caller, that receives absorbed[b][m] = n (pre-step row indices) for every pair, for the backward. */
+int gsx_fusion_prune_merge(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity, int32_t *ring,
+                           int ring_len, int step, int t_max, float c_stable, int B, int32_t *keep_map, void *scratch,
+                           int64_t scratch_bytes, const int32_t *assoc, const float *intrinsics, int64_t K_bstride,
+                           const float *poses, int64_t pose_bstride, int H, int W, float margin, void *fs_scratch,
+                           int64_t fs_scratch_bytes, float dot_th, void *merge_scratch, int64_t merge_scratch_bytes,
+                           int32_t *absorbed, void *stream);
+/* Backward of gsx_fusion_prune_merge: gsx_fusion_prune_bwd's gather, then, for every absorbed pair, the quotient rule of
+ * the absorption applied to the upstream gradient of m's destination row gives the gradients of both rows' position,
+ * normal, colour and ccount (the radius carries none).  pairs int32 (n_pairs, 3) = (b, m, n) in pre-step row indices
+ * (from the forward's `absorbed`); pair_geometry (n_pairs, 2, 8) / pair_colors (n_pairs, 2, 4): rows m and n as the
+ * forward read them (before the step), 16-byte aligned, so the caller keeps only the pairs' rows, not the whole map.
+ * Every argument is checked before anything is written.  One thread writes both rows of a pair; no atomics. */
+int gsx_fusion_prune_merge_bwd(const int32_t *keep_map, const int32_t *counts_in, int64_t capacity_in,
+                               const int32_t *pairs, const float *pair_geometry, const float *pair_colors,
+                               int64_t n_pairs, const float *g_geometry, const float *g_colors, int64_t capacity_out,
+                               int B, float *d_map_geometry, float *d_map_colors, void *stream);
 /* test hook: the next gsx_pointfusion_sequence_gt call reports a launch failure at frame s (once); -1 = off */
 void gsx_debug_fail_at_frame(int s);
 /* test hook: caps the total CTA count of the map projection kernel (K2), so that small maps take several grid-stride
