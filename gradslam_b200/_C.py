@@ -123,6 +123,12 @@ SIGNATURES = {
     "gsx_icp_localize_projective": (
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
                 c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_vp]),
+    "gsx_icp_localize_projective_splats": (
+        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
+                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_int,
+                c_vp]),
+    "gsx_icp_projective_targets": (
+        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "gsx_icp_project_associate": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp,
                 c_vp]),

@@ -18,7 +18,9 @@
 //                        smooth gates (icputils.py:527-543), pose accumulation
 // Projective association (an extension, no reference counterpart; gsx_icp_localize_projective):
 //   render_icp_targets   (gsx_render.cu) the map seen from the previous pose through R1's z-buffer: index image and the
-//                        winning rows' world-frame points / normals at full resolution
+//                        winning rows' world-frame points / normals at full resolution; with max_splat_px >= 1
+//                        through R1d's, a disk row's point being the surface point its pixel sees
+//                        (gsx_icp_localize_projective_splats)
 //   k_icp_proj_linearize a source point is associated with the pixel it projects to in the previous camera (the fusion
 //                        step's project()) if a row covers that pixel; the same rows, reduction and partials layout as
 //                        k_icp_knn_linearize, so k_icp_solve / k_icp_update run unchanged
@@ -1119,7 +1121,7 @@ inline ProjectiveWorkspace projective_workspace_layout(Carver &c, int B, int H, 
 // defined in gsx_render.cu
 int render_icp_targets(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                        const float *intrinsics, int64_t K_bstride, const float *poses, int64_t pose_bstride, int B,
-                       int H, int W, int64_t *index, float *tgt_p, float *tgt_n, cudaStream_t s);
+                       int H, int W, int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n, cudaStream_t s);
 
 }  // namespace gsx
 
@@ -1334,6 +1336,22 @@ extern "C" int gsx_icp_localize_projective(const float *map_geometry, const int3
                                            float lambda_max, float Bp, float B2p, float nu, float *poses_out,
                                            int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
                                            void *stream) {
+  return gsx_icp_localize_projective_splats(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics,
+                                            K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters,
+                                            damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu, poses_out,
+                                            poses_out_bstride, workspace, workspace_bytes, 0, stream);
+}
+
+extern "C" int gsx_icp_localize_projective_splats(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                                  int64_t max_count, const float *depth, int64_t depth_bstride,
+                                                  const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                                  int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
+                                                  int numiters, float damp, int use_dist_thresh, float dist_thresh,
+                                                  float lambda_max, float Bp, float B2p, float nu, float *poses_out,
+                                                  int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
+                                                  int max_splat_px, void *stream) {
+  GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX,
+                "gsx_icp_localize_projective: max_splat_px %d outside [0, %d]", max_splat_px, GSX_MAX_SPLAT_PX);
   GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace,
                 "gsx_icp_localize_projective: null pointer");
   GSX_CHECK_ARG(B >= 1 && H >= 2 && W >= 2 && ds >= 1 && numiters >= 0, "gsx_icp_localize_projective: bad extents");
@@ -1347,7 +1365,7 @@ extern "C" int gsx_icp_localize_projective(const float *map_geometry, const int3
                    w.src, w.src_count, w.ns_cap};
   k_icp_gather_src<<<B, 1024, 0, s>>>(gs);
   if (render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
-                         prev_pose_bstride, B, H, W, w.index, w.tgt_p, w.tgt_n, s))
+                         prev_pose_bstride, B, H, W, max_splat_px, w.index, w.tgt_p, w.tgt_n, s))
     return 1;
   ProjLinearize lin{ProjLinArgs{w.src, w.src_count, w.ns_cap, nullptr, 0,
                                 ProjTargets{prev_poses, prev_pose_bstride, intrinsics, K_bstride, image_bounds(H, W),

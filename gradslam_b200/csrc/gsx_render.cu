@@ -9,7 +9,8 @@
 //                              the outputs requested.
 //   k_render_resolve_world (R2w) per pixel of one view per element: key -> n or -1 in place, the winning row's
 //                              world-frame point and normal (two 128-bit row loads), zeros where uncovered: the target
-//                              images of the projective ICP (gsx_icp.cu, render_icp_targets).
+//                              images of the projective ICP (gsx_icp.cu, render_icp_targets).  <true> after R1d: a
+//                              disk row's target point is K1's global vertex of the pixel's plane depth.
 //   k_render_bwd_rows    (R3)  per map row: re-projects the row into every view; where it won the pixel, accumulates the
 //                              pixel's upstream gradients in view order (a row wins at most one pixel per view: no atomics).
 //   k_render_bwd_pose    (R3)  per pixel tile: d/d(camera-to-world pose) of depth and normals, reduced per tile, then
@@ -122,9 +123,27 @@ __global__ void __launch_bounds__(kRB) k_render_resolve(RenderArgs a) {
   }
 }
 
+// A row is a disk when it has a radius and a normal; everything else renders as one pixel.
+__device__ __forceinline__ bool is_disk(const float4 &g0, const float4 &g1) {
+  return g1.w > 0.0f && (g0.w != 0.0f || g1.x != 0.0f || g1.y != 0.0f);
+}
+
+// kSplat (the key came from R1d): at a pixel a disk row won, the target point is the surface point the pixel sees,
+// K1's global vertex of the plane depth t in the key, world_vertex(prev, backproject(K^-1, w, h, t), t), with the
+// same operands as K1 (load_kinv of K, load_rigid of the previous pose).  K .. W are read only then.
+template <bool kSplat>
 __global__ void __launch_bounds__(kRB) k_render_resolve_world(unsigned long long *key, const float *geo, int64_t cap,
-                                                           int64_t P, float *tgt_p, float *tgt_n) {
+                                                           int64_t P, float *tgt_p, float *tgt_n, const float *K,
+                                                           int64_t K_bstride, const float *poses,
+                                                           int64_t pose_bstride, int W) {
+  __shared__ KInv s_kinv;
+  __shared__ Rigid s_pose;
   const int b = blockIdx.y;
+  if constexpr (kSplat) {
+    if (threadIdx.x == 0) s_kinv = load_kinv(K + b * K_bstride);
+    if (threadIdx.x == 32) s_pose = load_rigid(poses + b * pose_bstride);
+    __syncthreads();
+  }
   const int64_t pix = (int64_t)blockIdx.x * kRB + threadIdx.x;
   if (pix >= P) return;
   const int64_t i = b * P + pix;
@@ -138,7 +157,17 @@ __global__ void __launch_bounds__(kRB) k_render_resolve_world(unsigned long long
     g0 = __ldg(reinterpret_cast<const float4 *>(row));
     g1 = __ldg(reinterpret_cast<const float4 *>(row + 4));
   }
-  st3(tgt_p + i * 3, g0.x, g0.y, g0.z);
+  if constexpr (kSplat) {
+    float3 p = make_float3(g0.x, g0.y, g0.z);
+    if (is_disk(g0, g1)) {  // (an uncovered pixel's zeros are no disk)
+      const int h = (int)(pix / W), w = (int)(pix - (int64_t)h * W);
+      const float t = __uint_as_float((unsigned int)(k >> 32));
+      p = world_vertex(&s_pose, backproject(s_kinv, (float)w, (float)h, t), t);
+    }
+    st3(tgt_p + i * 3, p.x, p.y, p.z);
+  } else {
+    st3(tgt_p + i * 3, g0.x, g0.y, g0.z);
+  }
   st3(tgt_n + i * 3, g0.w, g1.x, g1.y);
 }
 
@@ -266,11 +295,6 @@ __global__ void __launch_bounds__(kRB) k_render_bwd_pose(RenderBwdArgs a) {
 static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // ---- disk splats (R1d) -----------------------------------------------------------------------------------------
-// A row is a disk when it has a radius and a normal; everything else renders as one pixel.
-__device__ __forceinline__ bool is_disk(const float4 &g0, const float4 &g1) {
-  return g1.w > 0.0f && (g0.w != 0.0f || g1.x != 0.0f || g1.y != 0.0f);
-}
-
 // K^-1 of a camera staged as LiveCamera::k (the first three rows of the 4x4 K), as load_kinv computes it
 __device__ __forceinline__ KInv kinv_of(const float *k) {
   KInv r;
@@ -578,24 +602,43 @@ extern "C" int gsx_render_splats(const float *map_geometry, const float *map_col
 
 namespace gsx {
 // Target images of the projective ICP (declared in gsx_icp.cu): one view per element from `poses`, resolved to the
-// index image (B, H*W) and the winning rows' world-frame points and normals (B, H*W, 3).  Same checks as
-// gsx_render_views; returns non-zero (error set) if they fail.
+// index image (B, H*W) and the winning rows' world-frame points and normals (B, H*W, 3); max_splat_px >= 1 renders
+// through R1d and takes a disk row's surface point at the pixel.  Same checks as gsx_render_views; returns non-zero
+// (error set) if they fail.
 int render_icp_targets(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                        const float *intrinsics, int64_t K_bstride, const float *poses, int64_t pose_bstride, int B,
-                       int H, int W, int64_t *index, float *tgt_p, float *tgt_n, cudaStream_t s) {
+                       int H, int W, int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n, cudaStream_t s) {
   if (check_render_extents("render_icp_targets", B, 1, H, W, capacity)) return 1;
+  if (check_splat_px("render_icp_targets", max_splat_px)) return 1;
   GSX_CHECK_ARG(max_count >= 0 && max_count <= capacity, "render_icp_targets: max_count %lld outside [0, capacity %lld]",
                 (long long)max_count, (long long)capacity);
   GSX_CHECK_ARG(aligned16(map_geometry), "render_icp_targets: map rows must be 16-byte aligned");
   RenderArgs a{map_geometry, nullptr, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, 1,
                image_bounds(H, W), reinterpret_cast<unsigned long long *>(index), nullptr, nullptr, nullptr, nullptr};
-  launch_zbuffer(a, B, max_count, s);
-  k_render_resolve_world<<<dim3(pixel_tiles(H, W), (unsigned)B), kRB, 0, s>>>(a.key, map_geometry, capacity,
-                                                                             (int64_t)H * W, tgt_p, tgt_n);
+  launch_zbuffer(a, B, max_count, s, max_splat_px);
+  const dim3 grid(pixel_tiles(H, W), (unsigned)B);
+  if (max_splat_px == 0)
+    k_render_resolve_world<false><<<grid, kRB, 0, s>>>(a.key, map_geometry, capacity, (int64_t)H * W, tgt_p, tgt_n,
+                                                       intrinsics, K_bstride, poses, pose_bstride, W);
+  else
+    k_render_resolve_world<true><<<grid, kRB, 0, s>>>(a.key, map_geometry, capacity, (int64_t)H * W, tgt_p, tgt_n,
+                                                      intrinsics, K_bstride, poses, pose_bstride, W);
   GSX_CHECK_LAUNCH("render_icp_targets");
   return 0;
 }
 }  // namespace gsx
+
+extern "C" int gsx_icp_projective_targets(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                          int64_t max_count, const float *intrinsics, int64_t K_bstride,
+                                          const float *prev_poses, int64_t pose_bstride, int B, int H, int W,
+                                          int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n,
+                                          void *stream) {
+  if (check_splat_px("gsx_icp_projective_targets", max_splat_px)) return 1;
+  GSX_CHECK_ARG(intrinsics && prev_poses && index && tgt_p && tgt_n, "gsx_icp_projective_targets: null pointer");
+  if (max_count > 0) GSX_CHECK_ARG(map_geometry && counts, "gsx_icp_projective_targets: null map pointer");
+  return render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses, pose_bstride,
+                            B, H, W, max_splat_px, index, tgt_p, tgt_n, (cudaStream_t)stream);
+}
 
 extern "C" int64_t gsx_render_views_bwd_scratch_bytes(int B, int L, int H, int W) {
   if (B < 1 || L < 1 || H < 1 || W < 1) return -1;

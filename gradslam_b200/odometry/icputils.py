@@ -667,11 +667,34 @@ def _solver_params(odomprov):
             float(getattr(odomprov, "B", 1.0)), float(getattr(odomprov, "B2", 1.0)), float(getattr(odomprov, "nu", 200.0)))
 
 
-def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov):
-    """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective): the source is the
-    live frame on the ds lattice at the previous pose, the target is the map rendered from the previous pose at full
-    resolution, each source point is associated with the pixel it projects to.  Returns the new poses (B,1,4,4) =
-    T_icp · prev pose.  No host synchronisation."""
+def projective_targets(pointclouds, K, prev_poses, H, W, target_splat_px=0):
+    """The target images of the projective ICP, the map's predicted vertex and normal maps seen from prev_poses (B,4,4)
+    with intrinsics K (B,4,4): (index (B,H*W) int64, -1 = uncovered; points, normals (B,H*W,3) world frame, zeros where
+    uncovered).  target_splat_px >= 1 renders the surfels with radii as disks (render_pointclouds(max_splat_px)) and a
+    disk's point is the surface point the pixel sees.  Forward only (gsx_icp_projective_targets)."""
+    _C.require_cuda(K, "K")
+    _C.require_cuda(prev_poses, "prev_poses")
+    B = prev_poses.numel() // 16
+    dev = prev_poses.device
+    index = torch.empty((B, H * W), dtype=torch.int64, device=dev)
+    tgt_p = torch.empty((B, H * W, 3), dtype=torch.float32, device=dev)
+    tgt_n = torch.empty_like(tgt_p)
+    geo, counts, cap, bound = None, None, 0, 0
+    if pointclouds.has_points:
+        _C.require_cuda(pointclouds._geo, "pointclouds (geometry rows)")
+        geo, counts = pointclouds._geo.detach().contiguous(), pointclouds._counts_dev[pointclouds._cur]
+        cap, bound = pointclouds.capacity, pointclouds._bound
+    _C.launch("gsx_icp_projective_targets", geo, counts, cap, bound, K.detach().contiguous(), 16,
+              prev_poses.detach().contiguous(), 16, B, int(H), int(W), int(target_splat_px), index, tgt_p, tgt_n)
+    return index, tgt_p, tgt_n
+
+
+def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0):
+    """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective_splats): the source
+    is the live frame on the ds lattice at the previous pose, the target is the map rendered from the previous pose at
+    full resolution (surfels with radii as disks when target_splat_px >= 1, see projective_targets), each source point
+    is associated with the pixel it projects to.  Returns the new poses (B,1,4,4) = T_icp · prev pose.  No host
+    synchronisation."""
     live = live_frame.to_channels_last()
     B, _, H, W = live.shape
     dev = pointclouds.device
@@ -684,19 +707,25 @@ def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov):
     out = torch.empty((B, 1, 4, 4), dtype=torch.float32, device=dev)
     mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
     dth = odomprov.dist_thresh
-    _C.launch("gsx_icp_localize_projective", pointclouds._geo.contiguous(), pointclouds._counts_dev[pointclouds._cur],
-              pointclouds.capacity, pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode,
-              int(odomprov.numiters), float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth),
-              lambda_max, Bp, B2p, nu, out, 16, ws, ws.numel())
+    _C.launch("gsx_icp_localize_projective_splats", pointclouds._geo.contiguous(),
+              pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, pointclouds._bound, depth, d_bs, K, 16,
+              prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters), float(odomprov.damp),
+              0 if dth is None else 1, 0.0 if dth is None else float(dth), lambda_max, Bp, B2p, nu, out, 16, ws,
+              ws.numel(), int(target_splat_px))
     return out
 
 
-def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov):
+def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0):
     """The differentiable counterpart of `localize_projective`, bit-identical poses: the index image comes from
     gsx_render_views, the target images are gathers of the map rows at that index (so the gradient reaches the rows that
-    won a pixel, each at most one), and the batched ICP chain runs with the projective association.  live_frame.poses
-    must be the previous poses.  Returns (B,1,4,4)."""
+    won a pixel, each at most one), and the batched ICP chain runs with the projective association.  With
+    target_splat_px >= 1 the index and depth come from render_pointclouds(max_splat_px=target_splat_px), and at a pixel
+    a disk row won the target point is the K1 global vertex of that depth from the previous pose (the gradient reaches
+    the live depth, the previous pose and the winning rows' positions and normals; the radius gets none).
+    live_frame.poses must be the previous poses.  Returns (B,1,4,4)."""
     from ..slam.icpslam import _compose_canonical
+    from ..structures.rgbdimages import RGBDImages
+    from ..structures.utils import render_pointclouds
 
     frames_pc = downsample_rgbdimages(live_frame, dsratio)
     live = live_frame.to_channels_last()
@@ -705,9 +734,14 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     K = live.intrinsics.detach().contiguous()
     prev = prev_frame.poses
     prev_d = prev.detach().contiguous()
-    index = torch.empty((B, H * W), dtype=torch.int64, device=dev)
-    _C.launch("gsx_render_views", pointclouds._geo.detach().contiguous(), None, pointclouds._counts_dev[pointclouds._cur],
-              pointclouds.capacity, pointclouds._bound, K, 16, prev_d, 16, B, 1, H, W, index, None, None, None, None)
+    if target_splat_px:
+        splat = render_pointclouds(pointclouds, K, prev, H, W, max_splat_px=target_splat_px)
+        index = splat.index.view(B, H * W)
+    else:
+        index = torch.empty((B, H * W), dtype=torch.int64, device=dev)
+        _C.launch("gsx_render_views", pointclouds._geo.detach().contiguous(), None,
+                  pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, pointclouds._bound, K, 16, prev_d, 16,
+                  B, 1, H, W, index, None, None, None, None)
     covered = (index >= 0).unsqueeze(-1)
     rows = index.clamp(min=0).unsqueeze(-1).expand(B, H * W, 3)
 
@@ -716,6 +750,13 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
         return torch.where(covered, torch.gather(padded, 1, rows), torch.zeros((), dtype=padded.dtype, device=dev))
 
     tgt_p, tgt_n = target(pointclouds.points_padded), target(pointclouds.normals_padded)
+    if target_splat_px:
+        # the pixels a disk row (radius > 0, normal != 0) won, decided on the detached rows: no gradient
+        radii = pointclouds.radii_padded.detach()[..., 0]
+        radius = torch.gather(torch.cat([radii, radii.new_zeros(B, 1)], 1), 1, index.clamp(min=0))
+        disk = covered[..., 0] & (radius > 0) & (tgt_n.detach() != 0).any(-1)
+        surface = RGBDImages(splat.depth.new_zeros(B, 1, H, W, 3), splat.depth, K, prev).global_vertex_map
+        tgt_p = torch.where(disk.unsqueeze(-1), surface.reshape(B, H * W, 3), tgt_p)
     src_counts = frames_pc._counts_dev[frames_pc._cur]
     dth = odomprov.dist_thresh
     tgt_p_d = tgt_p.detach().contiguous()

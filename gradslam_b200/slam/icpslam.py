@@ -13,6 +13,7 @@ import torch.nn as nn
 
 from ..structures.pointclouds import Pointclouds
 from ..structures.rgbdimages import RGBDImages
+from ..structures.utils import MAX_SPLAT_PX
 from .fusionutils import update_map_aggregate
 
 __all__ = ["ICPSLAM"]
@@ -42,16 +43,29 @@ class ICPSLAM(nn.Module):
     def __init__(self, *, odom: str = "gradicp", dsratio: int = 4, numiters: int = 20, damp: float = 1e-8,
                  dist_thresh: Union[float, int, None] = None, lambda_max: Union[float, int] = 2.0,
                  B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0, nu: Union[float, int] = 200.0,
-                 association: str = "nn", device: Union[torch.device, str, None] = None):
+                 association: str = "nn", device: Union[torch.device, str, None] = None, target_splat_px: int = 0):
         """association (extension): how the ICP odometry pairs live points with the map.  'nn' (default, the
         reference's) = exact 1-NN between the lattice-thinned live cloud and the lattice-active map points; 'projective'
         = each live point with the map row visible at the pixel it projects to in the map rendered from the previous
-        pose (Keller et al.'s PointFusion, KinectFusion).  The two give different poses.  No effect with odom='gt'."""
+        pose (Keller et al.'s PointFusion, KinectFusion).  The two give different poses.  No effect with odom='gt'.
+
+        target_splat_px (extension, 0 .. 16, needs association='projective' when > 0): the projective targets are the
+        map rendered with surfels that have a radius (PointFusion(surfel_radii=True)) drawn as oriented disks, as
+        render_pointclouds(max_splat_px=target_splat_px) draws them, and at a pixel a disk won the target point is the
+        point of the disk the pixel's ray meets (Keller et al. 2013's predicted vertex map).  Disks leave fewer pixels
+        empty, so fewer live points pair with a row further back.  0 (default) = one pixel per surfel; a map without
+        radii gives the same poses at any value.  No effect with odom='gt'."""
         super().__init__()
         if not isinstance(association, str):
             raise TypeError("Expected association to be of type str. Got {0}.".format(type(association)))
         if association not in ("nn", "projective"):
             raise ValueError("association must be 'nn' or 'projective'. Got {!r}.".format(association))
+        if not isinstance(target_splat_px, int) or isinstance(target_splat_px, bool):
+            raise TypeError("Expected target_splat_px to be of type int. Got {0}.".format(type(target_splat_px)))
+        if not 0 <= target_splat_px <= MAX_SPLAT_PX:
+            raise ValueError("Expected 0 <= target_splat_px <= {}. Got {}.".format(MAX_SPLAT_PX, target_splat_px))
+        if target_splat_px > 0 and association != "projective":
+            raise ValueError("target_splat_px > 0 needs association='projective'")
         if odom not in ["gt", "icp", "gradicp"]:
             msg = "odometry method ({}) not supported for PointFusion. ".format(odom)
             msg += "Currently supported odometry modules for PointFusion are: 'gt', 'icp', 'gradicp'"
@@ -69,6 +83,7 @@ class ICPSLAM(nn.Module):
         self.odomprov = odomprov
         self.dsratio = dsratio
         self.association = association
+        self.target_splat_px = target_splat_px
         self.device = _normalize_device(device if device is not None else "cuda")
 
     # ------------------------------------------------------------------ sequence driver
@@ -152,7 +167,7 @@ class ICPSLAM(nn.Module):
             if not pointclouds.has_normals:
                 raise ValueError("projective ICP association needs a map with normals")
             fn = localize_projective_taped if wants_grad else localize_projective
-            return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov)
+            return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov, self.target_splat_px)
         if wants_grad:
             # differentiable mode (reference op order, slam/icpslam.py:238-247): the K1 maps carry their hand-written
             # backward, the association kernels are index-only, the ICP algebra is taped.

@@ -517,6 +517,31 @@ int gsx_icp_localize_projective(const float *map_geometry, const int32_t *counts
                                 float lambda_max, float Bp, float B2p, float nu, float *poses_out,
                                 int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes, void *stream);
 
+/* gsx_icp_localize_projective against the disk-splat render of the map (max_splat_px = 0 is gsx_icp_localize_projective
+ * itself; 1 .. GSX_MAX_SPLAT_PX, others are refused before any launch).  The target images are rendered with the
+ * z-buffer, keys, ties and fill of gsx_render_splats at max_splat_px; at a pixel j = h*W + w won by a disk row (radius
+ * > 0 and a non-zero normal) the target point is the surface point the pixel sees, (R v + t) with v = t_j K^-1 (w,h,1)
+ * (the K^-1 and arithmetic of gsx_backproject_normals_fwd) for the plane depth t_j and the previous pose [R | t], and
+ * the target normal the row's; other rows and uncovered pixels as in gsx_icp_localize_projective.  The source, the
+ * association (the distance test measures against the surface point) and the loop are unchanged; so is the workspace.
+ * A map without radii gives the max_splat_px = 0 poses. */
+int gsx_icp_localize_projective_splats(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                       int64_t max_count, const float *depth, int64_t depth_bstride,
+                                       const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                       int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
+                                       float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                                       float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
+                                       void *workspace, int64_t workspace_bytes, int max_splat_px, void *stream);
+
+/* The target images of gsx_icp_localize_projective_splats alone, the model's predicted vertex and normal maps seen from
+ * prev_poses: index int64 (B, H*W) = the winning row or -1, tgt_p / tgt_n (B, H*W, 3) = the world-frame target point
+ * and normal, zeros where uncovered.  index is the z-buffer while the call runs.  The map pointers may be NULL when
+ * max_count is 0.  No host synchronisation. */
+int gsx_icp_projective_targets(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                               const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                               int64_t pose_bstride, int B, int H, int W, int max_splat_px, int64_t *index,
+                               float *tgt_p, float *tgt_n, void *stream);
+
 /* The association of gsx_icp_localize_projective alone (the index-only op of the differentiable mode): for the source
  * rows i < src_count[b] of src_points (B, ns_stride, 3), world frame, idx_out int64 (B, ns_stride) = the pixel
  * j = h*W + w of the target images they are associated with, or -1; d2_out (may be NULL) = |s - tgt_points[b, j]|^2
