@@ -129,6 +129,20 @@ SIGNATURES = {
                 c_vp]),
     "gsx_icp_projective_targets": (
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "gsx_icp_projective_rgb_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
+    "gsx_icp_localize_projective_rgb": (
+        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
+                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_int,
+                c_vp, c_vp, c_i64, c_float, c_vp]),
+    "gsx_icp_projective_targets_rgb": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                c_vp, c_vp]),
+    "gsx_icp_joint_normal_eq_batched_fwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
+                c_vp, c_i64, c_vp]),
+    "gsx_icp_joint_normal_eq_batched_bwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
+                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gsx_icp_project_associate": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp,
                 c_vp]),

@@ -25,6 +25,15 @@
 //                        step's project()) if a row covers that pixel; the same rows, reduction and partials layout as
 //                        k_icp_knn_linearize, so k_icp_solve / k_icp_update run unchanged
 //   k_icp_project_associate  the association alone (index-only op of the differentiable mode)
+// Photometric term (gsx_icp_localize_projective_rgb, photometric_weight w > 0): E_icp + w E_rgb as in ElasticFusion.
+//   k_icp_gather_src<true>    also the intensity I_s of each source point's live colour
+//   k_icp_model_intensity     after the target build: I_m, the intensity of the colour of each pixel's winning row
+//   k_icp_proj_linearize<true> an associated point whose pixel is photometrically valid (off the border, it and its
+//                        four neighbours covered) adds w times the products of its photometric row (photometric_row)
+//                        to its 28 sums before the same reduction
+//   k_icp_joint_linearize_idx / _bwd  the geometric + photometric sums at a given association and their backward
+//                        (gsx_icp_joint_normal_eq_batched_fwd / _bwd, the op of the differentiable mode; the same
+//                        photometric_row, the backward through dual numbers)
 #include "gsx_common.cuh"
 #include "../../include/gsx.h"
 
@@ -50,7 +59,17 @@ struct GatherSrcArgs {
   int ns_cap;
 };
 
-__global__ void __launch_bounds__(1024) k_icp_gather_src(GatherSrcArgs a) {
+// intensity of a colour, every product and sum rounded on its own (the library is built without FMA contraction)
+__device__ __forceinline__ float intensity(float r, float g, float b) { return (0.299f * r + 0.587f * g) + 0.114f * b; }
+
+struct GatherRgbArgs {  // of k_icp_gather_src<true>
+  const float *rgb;     // live colour, channels-last (H, W, 3) per element, element stride rgb_bstride
+  int64_t rgb_bstride;
+  float *I_s;           // (B, ns_cap) intensity of each source point's colour
+};
+
+template <bool kRgb>
+__global__ void __launch_bounds__(1024) k_icp_gather_src(GatherSrcArgs a, GatherRgbArgs rgbc) {
   __shared__ int s_warp[32];
   __shared__ int s_base;
   __shared__ KInv s_k;
@@ -91,6 +110,11 @@ __global__ void __launch_bounds__(1024) k_icp_gather_src(GatherSrcArgs a) {
       out[(int64_t)excl * 3 + 0] = gv.x;
       out[(int64_t)excl * 3 + 1] = gv.y;
       out[(int64_t)excl * 3 + 2] = gv.z;
+      if constexpr (kRgb) {
+        const int hs = i / Ws, ws = i - hs * Ws;
+        const float *px = rgbc.rgb + b * rgbc.rgb_bstride + ((int64_t)(hs * a.ds) * a.W + ws * a.ds) * 3;
+        rgbc.I_s[(int64_t)b * a.ns_cap + excl] = intensity(__ldg(px), __ldg(px + 1), __ldg(px + 2));
+      }
     }
     __syncthreads();
     if (threadIdx.x == 0) s_base += tot;
@@ -581,7 +605,91 @@ struct ProjLinArgs {
   float *partials;  // (B, gridDim.x, 28)
 };
 
-__global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a) {
+struct ProjRgb {       // photometric inputs of k_icp_proj_linearize<true>
+  const float *I_s;    // (B, ns_stride) source intensities
+  const float *I_m;    // (B, H*W) model image, 0 where uncovered
+  float w;             // photometric weight
+};
+
+// Photometric validity of pixel j (covered, as the caller knows) of an element's index image idx: off the image border
+// and its four neighbours covered.  Then the central differences of the model image.
+__device__ __forceinline__ bool model_gradient(const int64_t *idx, const float *Im, const ImageBounds &ib, int j,
+                                               float &gu, float &gv) {
+  const int h = j / ib.W, w = j - h * ib.W;
+  if (h < 1 || h > ib.H - 2 || w < 1 || w > ib.W - 2) return false;
+  if (__ldg(idx + j - 1) < 0 || __ldg(idx + j + 1) < 0 || __ldg(idx + j - ib.W) < 0 || __ldg(idx + j + ib.W) < 0)
+    return false;
+  gu = 0.5f * (__ldg(Im + j + 1) - __ldg(Im + j - 1));
+  gv = 0.5f * (__ldg(Im + j + ib.W) - __ldg(Im + j - ib.W));
+  return true;
+}
+
+// The photometric row A = [c, s x c] of the world-frame source point s at a pixel with model gradient (gu, gv):
+// q = T_prev^-1 s, u, v, den with project()'s arithmetic, du/dq_i = (k[i] - u k[8+i]) / den,
+// dv/dq_i = (k[4+i] - v k[8+i]) / den, c = R_prev (gu du/dq + gv dv/dq), R_prev = tinv^T.  -c is the derivative of the
+// residual I_s - I_m(pi(q(s))) with respect to s.
+// T = float, or Dual for the backward (one input direction per evaluation); r, t: T^-1 of the previous pose, k: the
+// first three rows of K (no derivative).
+struct Dual {  // value and one directional derivative; the value is computed with exactly the float operations
+  float v, d;
+};
+__device__ __forceinline__ Dual operator+(Dual a, Dual b) { return Dual{a.v + b.v, a.d + b.d}; }
+__device__ __forceinline__ Dual operator-(Dual a, Dual b) { return Dual{a.v - b.v, a.d - b.d}; }
+__device__ __forceinline__ Dual operator*(Dual a, Dual b) { return Dual{a.v * b.v, a.d * b.v + a.v * b.d}; }
+__device__ __forceinline__ Dual operator/(Dual a, Dual b) {
+  const float q = a.v / b.v;
+  return Dual{q, (a.d - q * b.d) / b.v};
+}
+__device__ __forceinline__ Dual operator+(Dual a, float b) { return Dual{a.v + b, a.d}; }
+__device__ __forceinline__ Dual operator*(float a, Dual b) { return Dual{a * b.v, a * b.d}; }
+__device__ __forceinline__ Dual operator*(Dual a, float b) { return Dual{a.v * b, a.d * b}; }
+__device__ __forceinline__ Dual operator-(float a, Dual b) { return Dual{a - b.v, -b.d}; }
+__device__ __forceinline__ float value(float x) { return x; }
+__device__ __forceinline__ float value(Dual x) { return x.v; }
+
+template <class T>
+__device__ __forceinline__ void photometric_row_t(const T *r, const T *t, const float *k, T sx, T sy, T sz, T gu, T gv,
+                                                  T *A) {
+  const T qx = ((r[0] * sx + r[1] * sy) + r[2] * sz) + t[0];
+  const T qy = ((r[3] * sx + r[4] * sy) + r[5] * sz) + t[1];
+  const T qz = ((r[6] * sx + r[7] * sy) + r[8] * sz) + t[2];
+  const T hx = ((k[0] * qx + k[1] * qy) + k[2] * qz) + k[3];
+  const T hy = ((k[4] * qx + k[5] * qy) + k[6] * qz) + k[7];
+  const T hz = ((k[8] * qx + k[9] * qy) + k[10] * qz) + k[11];
+  T den = hz;
+  if (value(hz) == 0.0f) den = T{1.0f};
+  const T u = hx / den, v = hy / den;
+  T cc[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) cc[i] = gu * ((k[i] - u * k[8 + i]) / den) + gv * ((k[4 + i] - v * k[8 + i]) / den);
+  const T cx = (r[0] * cc[0] + r[3] * cc[1]) + r[6] * cc[2];
+  const T cy = (r[1] * cc[0] + r[4] * cc[1]) + r[7] * cc[2];
+  const T cz = (r[2] * cc[0] + r[5] * cc[1]) + r[8] * cc[2];
+  A[0] = cx; A[1] = cy; A[2] = cz;
+  A[3] = cz * sy - cy * sz;
+  A[4] = cx * sz - cz * sx;
+  A[5] = cy * sx - cx * sy;
+}
+
+__device__ __forceinline__ void photometric_row(const LiveCamera &c, float sx, float sy, float sz, float gu, float gv,
+                                                float *A) {
+  photometric_row_t<float>(c.tinv.r, c.tinv.t, c.k, sx, sy, sz, gu, gv, A);
+}
+
+// acc[k] += w (A_p A_q), w (A_p r), w (r r) in the order of row_products
+__device__ __forceinline__ void add_weighted_products(const float *A, float r, float w, float *acc) {
+  int k = 0;
+#pragma unroll
+  for (int p = 0; p < 6; ++p)
+#pragma unroll
+    for (int q = p; q < 6; ++q, ++k) acc[k] = acc[k] + w * (A[p] * A[q]);
+#pragma unroll
+  for (int p = 0; p < 6; ++p) acc[21 + p] = acc[21 + p] + w * (A[p] * r);
+  acc[27] = acc[27] + w * (r * r);
+}
+
+template <bool kRgb>
+__global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a, ProjRgb pm) {
   __shared__ float s_red[kIcpBlock / 32][kNumSums];
   __shared__ Rigid s_pre;
   __shared__ LiveCamera s_cam;
@@ -605,7 +713,18 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a)
     const float *tp = a.t.tgt_p + b * P * 3;
     float d2;
     const int j = project_associate(s_cam, a.t, a.t.idx + b * P, tp, q.x, q.y, q.z, d2);
-    if (j >= 0) row_products(q.x, q.y, q.z, tp, a.t.tgt_n + b * P * 3, (int64_t)j, acc);
+    if (j >= 0) {
+      row_products(q.x, q.y, q.z, tp, a.t.tgt_n + b * P * 3, (int64_t)j, acc);
+      if constexpr (kRgb) {
+        float gu, gv;
+        const float *Im = pm.I_m + b * P;
+        if (model_gradient(a.t.idx + b * P, Im, a.t.ib, j, gu, gv)) {
+          float A[6];
+          photometric_row(s_cam, q.x, q.y, q.z, gu, gv, A);
+          add_weighted_products(A, __ldg(pm.I_s + (int64_t)b * a.ns_stride + i) - __ldg(Im + j), pm.w, acc);
+        }
+      }
+    }
   }
   block_reduce_sums(acc, s_red, a.partials + ((int64_t)b * gridDim.x + blockIdx.x) * kNumSums);
 }
@@ -625,6 +744,22 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_project_associate(const float
   const int j = project_associate(s_cam, t, t.idx + b * P, t.tgt_p + b * P * 3, s[0], s[1], s[2], d2);
   idx_out[(int64_t)b * ns_stride + i] = j;
   if (d2_out) d2_out[(int64_t)b * ns_stride + i] = d2;
+}
+
+// I_m of the photometric term: per pixel of the resolved index image, the intensity of the winning row's colour, 0 where
+// uncovered.  col: (B, cap, kColW) colour rows.
+__global__ void __launch_bounds__(kIcpBlock) k_icp_model_intensity(const int64_t *idx, const float *col, int64_t cap,
+                                                                  int64_t P, float *I_m) {
+  const int b = blockIdx.y;
+  const int64_t pix = (int64_t)blockIdx.x * kIcpBlock + threadIdx.x;
+  if (pix >= P) return;
+  const int64_t n = idx[b * P + pix];
+  float I = 0.0f;
+  if (n >= 0) {
+    const float4 c = __ldg(reinterpret_cast<const float4 *>(col + ((int64_t)b * cap + n) * kColW));
+    I = intensity(c.x, c.y, c.z);
+  }
+  I_m[b * P + pix] = I;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -727,6 +862,205 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_linearize_bwd(const float *sr
     g_src[(int64_t)i * 3 + c] = gs[c];
     g_tp[(int64_t)i * 3 + c] = gp[c];
     g_tn[(int64_t)i * 3 + c] = gn[c];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// joint geometric + photometric normal equations for a GIVEN association (the differentiable op of the taped mode)
+// ---------------------------------------------------------------------------------------------------------
+struct JointArgs {
+  const float *src;        // (B, ns_stride, 3) world frame
+  const int32_t *counts;   // (B)
+  int ns_stride;
+  const float *src_col;    // (B, ns_stride, 3) the source points' live colours
+  const float *tp, *tn;    // (B, H*W, 3) target images
+  const float *mcol;       // (B, H*W, 3) model colour image (the winning rows' colours, zeros where uncovered)
+  const int64_t *index;    // (B, H*W) index image, -1 = uncovered
+  const int64_t *idx;      // (B, ns_stride) associated pixel, -1 = none
+  const float *poses;      // (B, 4, 4) previous camera-to-world poses
+  const float *K;          // (B, 4, 4)
+  ImageBounds ib;
+  float w;
+};
+
+__device__ __forceinline__ float intensity3(const float *c) { return intensity(c[0], c[1], c[2]); }
+
+// model_gradient on the model colour image: the same validity and, since I_m = intensity(colour), the same values
+__device__ __forceinline__ bool model_gradient_rgb(const int64_t *index, const float *mcol, const ImageBounds &ib, int j,
+                                                   float &gu, float &gv) {
+  const int h = j / ib.W, w = j - h * ib.W;
+  if (h < 1 || h > ib.H - 2 || w < 1 || w > ib.W - 2) return false;
+  if (index[j - 1] < 0 || index[j + 1] < 0 || index[j - ib.W] < 0 || index[j + ib.W] < 0) return false;
+  gu = 0.5f * (intensity3(mcol + (int64_t)(j + 1) * 3) - intensity3(mcol + (int64_t)(j - 1) * 3));
+  gv = 0.5f * (intensity3(mcol + (int64_t)(j + ib.W) * 3) - intensity3(mcol + (int64_t)(j - ib.W) * 3));
+  return true;
+}
+
+__global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_idx(JointArgs a, float *partials) {
+  __shared__ float s_red[kIcpBlock / 32][kNumSums];
+  __shared__ LiveCamera s_cam;
+  const int b = blockIdx.y;
+  load_live_camera(s_cam, a.poses, 16, a.K, 16, b);
+  __syncthreads();
+  const int64_t P = (int64_t)a.ib.H * a.ib.W;
+  const int i = blockIdx.x * kIcpBlock + threadIdx.x;
+  float acc[kNumSums];
+#pragma unroll
+  for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0f;
+  if (i < a.counts[b]) {
+    const int64_t row = (int64_t)b * a.ns_stride + i;
+    const int64_t j = a.idx[row];
+    if (j >= 0) {
+      const float sx = a.src[row * 3], sy = a.src[row * 3 + 1], sz = a.src[row * 3 + 2];
+      row_products(sx, sy, sz, a.tp + b * P * 3, a.tn + b * P * 3, j, acc);
+      const float *mcol = a.mcol + b * P * 3;
+      float gu, gv;
+      if (model_gradient_rgb(a.index + b * P, mcol, a.ib, (int)j, gu, gv)) {
+        float A[6];
+        photometric_row(s_cam, sx, sy, sz, gu, gv, A);
+        add_weighted_products(A, intensity3(a.src_col + row * 3) - intensity3(mcol + j * 3), a.w, acc);
+      }
+    }
+  }
+  block_reduce_sums(acc, s_red, partials + ((int64_t)b * gridDim.x + blockIdx.x) * kNumSums);
+}
+
+// dL/dA_p and dL/dr of one row A, r whose products enter the 28 sums with weight wt, from g = dL/d(sums)
+__device__ __forceinline__ void row_adjoint(const float *g, const float *A, float r, float wt, float *a, float &gr) {
+  gr = 2.0f * g[27] * r;
+#pragma unroll
+  for (int p = 0; p < 6; ++p) {
+    float v = g[21 + p] * r;
+    gr += g[21 + p] * A[p];
+#pragma unroll
+    for (int q = 0; q < 6; ++q) {
+      const int lo = p < q ? p : q, hi = p < q ? q : p;
+      v += g[lo * 6 - lo * (lo - 1) / 2 + (hi - lo)] * A[q] * ((p == q) ? 2.0f : 1.0f);
+    }
+    a[p] = wt * v;
+  }
+  gr *= wt;
+}
+
+// Per source row: d/d(source point), d/d(source colour), d/d(target point and normal at the associated pixel), d/d(the
+// colours of the five stencil pixels j, j-1, j+1, j-W, j+W) (rows written per source row, the caller scatters them),
+// and the previous pose's gradient reduced per block in a fixed order (pose_partials (B, gridDim.x, 12), summed by
+// k_pose_grad_reduce).  No atomics.
+__global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs a, const float *g, float *g_src,
+                                                                      float *g_scol, float *g_tp, float *g_tn,
+                                                                      float *g_stencil, float *pose_partials) {
+  __shared__ float s_g[kNumSums];
+  __shared__ LiveCamera s_cam;
+  __shared__ Rigid s_pose;
+  __shared__ float s_red[kIcpBlock / 32][12];
+  const int b = blockIdx.y;
+  load_live_camera(s_cam, a.poses, 16, a.K, 16, b);
+  if (threadIdx.x == 64) s_pose = load_rigid(a.poses + b * 16);
+  if (threadIdx.x < kNumSums) s_g[threadIdx.x] = g[(int64_t)b * kNumSums + threadIdx.x];
+  __syncthreads();
+  const int64_t P = (int64_t)a.ib.H * a.ib.W;
+  const int i = blockIdx.x * kIcpBlock + threadIdx.x;
+  float gs[3] = {0.f, 0.f, 0.f}, gc[3] = {0.f, 0.f, 0.f}, gp[3] = {0.f, 0.f, 0.f}, gn[3] = {0.f, 0.f, 0.f};
+  float gst[15], gT[12];
+#pragma unroll
+  for (int k = 0; k < 15; ++k) gst[k] = 0.0f;
+#pragma unroll
+  for (int k = 0; k < 12; ++k) gT[k] = 0.0f;
+  const int64_t row = (int64_t)b * a.ns_stride + i;
+  if (i < a.ns_stride && i < a.counts[b] && a.idx[row] >= 0) {
+    const int64_t j = a.idx[row];
+    const float sx = a.src[row * 3], sy = a.src[row * 3 + 1], sz = a.src[row * 3 + 2];
+    const float *tp = a.tp + (b * P + j) * 3, *tn = a.tn + (b * P + j) * 3;
+    const float px = tp[0], py = tp[1], pz = tp[2], nx = tn[0], ny = tn[1], nz = tn[2];
+    // geometric row (as k_icp_linearize_bwd)
+    const float A[6] = {nx, ny, nz, nz * sy - ny * sz, nx * sz - nz * sx, ny * sx - nx * sy};
+    const float r = (nx * (px - sx) + ny * (py - sy)) + nz * (pz - sz);
+    float ad[6], gr;
+    row_adjoint(s_g, A, r, 1.0f, ad, gr);
+    gs[0] = (-nz * ad[4] + ny * ad[5]) - gr * nx;
+    gs[1] = (nz * ad[3] - nx * ad[5]) - gr * ny;
+    gs[2] = (-ny * ad[3] + nx * ad[4]) - gr * nz;
+    gn[0] = (ad[0] + sz * ad[4] - sy * ad[5]) + gr * (px - sx);
+    gn[1] = (ad[1] - sz * ad[3] + sx * ad[5]) + gr * (py - sy);
+    gn[2] = (ad[2] + sy * ad[3] - sx * ad[4]) + gr * (pz - sz);
+    gp[0] = gr * nx; gp[1] = gr * ny; gp[2] = gr * nz;
+    // photometric row
+    const float *mcol = a.mcol + b * P * 3;
+    float gu, gv;
+    if (model_gradient_rgb(a.index + b * P, mcol, a.ib, (int)j, gu, gv)) {
+      const LiveCamera &c = s_cam;
+      float Ap[6];
+      photometric_row(c, sx, sy, sz, gu, gv, Ap);
+      const float rp = intensity3(a.src_col + row * 3) - intensity3(mcol + j * 3);
+      float ap[6], grp;
+      row_adjoint(s_g, Ap, rp, a.w, ap, grp);
+      // d(sum_p ap[p] A_p)/d(input) for the 17 inputs s (3), gu, gv, T^-1 rotation (9) and translation (3)
+      float gin[17];
+#pragma unroll 1
+      for (int e = 0; e < 17; ++e) {
+        Dual r9[9], t3[3], in[5] = {{sx, 0.f}, {sy, 0.f}, {sz, 0.f}, {gu, 0.f}, {gv, 0.f}};
+#pragma unroll
+        for (int k = 0; k < 9; ++k) r9[k] = Dual{c.tinv.r[k], e == 5 + k ? 1.0f : 0.0f};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) t3[k] = Dual{c.tinv.t[k], e == 14 + k ? 1.0f : 0.0f};
+#pragma unroll
+        for (int k = 0; k < 5; ++k) in[k].d = e == k ? 1.0f : 0.0f;
+        Dual Ad[6];
+        photometric_row_t<Dual>(r9, t3, c.k, in[0], in[1], in[2], in[3], in[4], Ad);
+        float v = 0.0f;
+#pragma unroll
+        for (int p = 0; p < 6; ++p) v += ap[p] * Ad[p].d;
+        gin[e] = v;
+      }
+      gs[0] += gin[0]; gs[1] += gin[1]; gs[2] += gin[2];
+      // r_p = I_s - I_m[j]; g_u = (I_m[j+1] - I_m[j-1]) / 2, g_v = (I_m[j+W] - I_m[j-W]) / 2; I = 0.299 r + 0.587 g + 0.114 b
+      const float wI[3] = {0.299f, 0.587f, 0.114f};
+      const float dI[5] = {-grp, -0.5f * gin[3], 0.5f * gin[3], -0.5f * gin[4], 0.5f * gin[4]};
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        gc[k] = grp * wI[k];
+#pragma unroll
+        for (int m = 0; m < 5; ++m) gst[m * 3 + k] = dI[m] * wI[k];
+      }
+      // T^-1 = [R^T, -R^T t]: dL/dR[rr][cc] = G_r[cc][rr] - t[rr] G_t[cc], dL/dt[rr] = -sum_cc R[rr][cc] G_t[cc]
+      const Rigid &T = s_pose;
+      const float *Gr = gin + 5, *Gt = gin + 14;
+#pragma unroll
+      for (int rr = 0; rr < 3; ++rr) {
+#pragma unroll
+        for (int cc = 0; cc < 3; ++cc) gT[rr * 4 + cc] = Gr[cc * 3 + rr] - T.t[rr] * Gt[cc];
+        gT[rr * 4 + 3] = -dot3(T.r[rr * 3 + 0], T.r[rr * 3 + 1], T.r[rr * 3 + 2], Gt[0], Gt[1], Gt[2]);
+      }
+    }
+  }
+  if (i < a.ns_stride) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      g_src[row * 3 + k] = gs[k];
+      g_scol[row * 3 + k] = gc[k];
+      g_tp[row * 3 + k] = gp[k];
+      g_tn[row * 3 + k] = gn[k];
+    }
+#pragma unroll
+    for (int k = 0; k < 15; ++k) g_stencil[row * 15 + k] = gst[k];
+  }
+  // the pose gradient: butterfly inside the warp, then warps in index order
+#pragma unroll
+  for (int k = 0; k < 12; ++k) {
+    float x = gT[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    gT[k] = x;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0)
+#pragma unroll
+    for (int k = 0; k < 12; ++k) s_red[warp][k] = gT[k];
+  __syncthreads();
+  if (threadIdx.x < 12) {
+    float x = 0.0f;
+    for (int w = 0; w < kIcpBlock / 32; ++w) x += s_red[w][threadIdx.x];
+    pose_partials[((int64_t)b * gridDim.x + blockIdx.x) * 12 + threadIdx.x] = x;
   }
 }
 
@@ -1071,13 +1405,16 @@ struct KnnLinearize {
 };
 
 // projective association against target images rendered from the previous pose
+// (with the photometric term when pm.w > 0)
 struct ProjLinearize {
   ProjLinArgs pa;
+  ProjRgb pm;
   void prepare(cudaStream_t) {}
   void operator()(const float *pre, int write_back, bool, dim3 grid, cudaStream_t s) {
     pa.pre = pre;
     pa.write_back = write_back;
-    k_icp_proj_linearize<<<grid, kIcpBlock, 0, s>>>(pa);
+    if (pm.w > 0.0f) k_icp_proj_linearize<true><<<grid, kIcpBlock, 0, s>>>(pa, pm);
+    else k_icp_proj_linearize<false><<<grid, kIcpBlock, 0, s>>>(pa, pm);
   }
 };
 
@@ -1100,10 +1437,12 @@ struct ProjectiveWorkspace {  // of gsx_icp_localize_projective; nothing in it o
   IcpState st;
   int64_t *index;        // (B, H*W) z-buffer, then the index image
   float *tgt_p, *tgt_n;  // (B, H*W, 3)
+  float *I_s, *I_m;      // (B, ns_cap) source and (B, H*W) model intensities, with_rgb only
   int ns_cap, nblk;
 };
 
-inline ProjectiveWorkspace projective_workspace_layout(Carver &c, int B, int H, int W, int ds) {
+// with_rgb: the layout of gsx_icp_localize_projective_rgb, the geometric layout followed by the intensity arrays
+inline ProjectiveWorkspace projective_workspace_layout(Carver &c, int B, int H, int W, int ds, bool with_rgb = false) {
   ProjectiveWorkspace w;
   const int64_t P = (int64_t)H * W;
   w.ns_cap = ((H + ds - 1) / ds) * ((W + ds - 1) / ds);
@@ -1115,6 +1454,8 @@ inline ProjectiveWorkspace projective_workspace_layout(Carver &c, int B, int H, 
   w.index = c.take<int64_t>((int64_t)B * P);
   w.tgt_p = c.take<float>((int64_t)B * P * 3);
   w.tgt_n = c.take<float>((int64_t)B * P * 3);
+  w.I_s = with_rgb ? c.take<float>((int64_t)B * w.ns_cap) : nullptr;
+  w.I_m = with_rgb ? c.take<float>((int64_t)B * P) : nullptr;
   return w;
 }
 
@@ -1198,7 +1539,7 @@ extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts
   const TargetScratch tgt = target_scratch_layout(ct, B, tgt_capacity);
   GatherSrcArgs gs{depth, depth_bstride, intrinsics, K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds,
                    w.src, w.src_count, w.ns_cap};
-  k_icp_gather_src<<<B, 1024, 0, s>>>(gs);
+  k_icp_gather_src<false><<<B, 1024, 0, s>>>(gs, GatherRgbArgs{});
   int tiles = (int)((max_count + 1023) / 1024);
   if (tiles > w.tiles_cap) tiles = w.tiles_cap;
   if (tiles == 0) cudaMemsetAsync(w.tgt_count, 0, (size_t)B * 4, s);
@@ -1342,6 +1683,61 @@ extern "C" int gsx_icp_localize_projective(const float *map_geometry, const int3
                                             poses_out_bstride, workspace, workspace_bytes, 0, stream);
 }
 
+namespace gsx {
+// colours of the photometric term (gsx_icp_localize_projective_rgb); w == 0 runs the geometric kernels
+struct PhotometricInputs {
+  const float *map_colours;  // (B, capacity, 4)
+  const float *rgb;          // live colour, channels-last, element stride rgb_bstride
+  int64_t rgb_bstride;
+  float w;
+};
+
+// gsx_icp_localize_projective_splats (pm == nullptr, the geometric workspace) and gsx_icp_localize_projective_rgb
+static int localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                               const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
+                               const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
+                               int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max,
+                               float Bp, float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
+                               void *workspace, int64_t workspace_bytes, int max_splat_px, const PhotometricInputs *pm,
+                               void *stream) {
+  GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX,
+                "gsx_icp_localize_projective: max_splat_px %d outside [0, %d]", max_splat_px, GSX_MAX_SPLAT_PX);
+  GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace,
+                "gsx_icp_localize_projective: null pointer");
+  GSX_CHECK_ARG(B >= 1 && H >= 2 && W >= 2 && ds >= 1 && numiters >= 0, "gsx_icp_localize_projective: bad extents");
+  GSX_CHECK_ARG(mode == 0 || mode == 1, "gsx_icp_localize_projective: mode must be 0 (ICP) or 1 (gradICP)");
+  Carver c(workspace);
+  const ProjectiveWorkspace w = projective_workspace_layout(c, B, H, W, ds, pm != nullptr);
+  GSX_CHECK_ARG(workspace_bytes >= c.bytes, "gsx_icp_localize_projective: workspace too small (%lld < %lld)",
+                (long long)workspace_bytes, (long long)c.bytes);
+  const bool rgb = pm && pm->w > 0.0f;
+  cudaStream_t s = (cudaStream_t)stream;
+  GatherSrcArgs gs{depth, depth_bstride, intrinsics, K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds,
+                   w.src, w.src_count, w.ns_cap};
+  if (rgb) k_icp_gather_src<true><<<B, 1024, 0, s>>>(gs, GatherRgbArgs{pm->rgb, pm->rgb_bstride, w.I_s});
+  else k_icp_gather_src<false><<<B, 1024, 0, s>>>(gs, GatherRgbArgs{});
+  if (render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
+                         prev_pose_bstride, B, H, W, max_splat_px, w.index, w.tgt_p, w.tgt_n, s))
+    return 1;
+  const int64_t P = (int64_t)H * W;
+  if (rgb)
+    k_icp_model_intensity<<<dim3((unsigned)((P + kIcpBlock - 1) / kIcpBlock), (unsigned)B), kIcpBlock, 0, s>>>(
+        w.index, pm->map_colours, capacity, P, w.I_m);
+  ProjLinearize lin{ProjLinArgs{w.src, w.src_count, w.ns_cap, nullptr, 0,
+                                ProjTargets{prev_poses, prev_pose_bstride, intrinsics, K_bstride, image_bounds(H, W),
+                                            w.index, w.tgt_p, w.tgt_n, dist_thresh, use_dist_thresh},
+                                w.partials},
+                    ProjRgb{w.I_s, w.I_m, rgb ? pm->w : 0.0f}};
+  const int rc = icp_iterations(lin, w.ns_cap, B, nullptr, mode, numiters, damp, lambda_max, Bp, B2p, nu, w.partials,
+                                w.nblk, w.st, s);
+  if (rc) return rc;
+  k_pose_compose<<<(B + 63) / 64, 64, 0, s>>>(w.st.T_total, prev_poses, prev_pose_bstride, poses_out,
+                                              poses_out_bstride, B);
+  GSX_CHECK_LAUNCH("gsx_icp_localize_projective");
+  return 0;
+}
+}  // namespace gsx
+
 extern "C" int gsx_icp_localize_projective_splats(const float *map_geometry, const int32_t *counts, int64_t capacity,
                                                   int64_t max_count, const float *depth, int64_t depth_bstride,
                                                   const float *intrinsics, int64_t K_bstride, const float *prev_poses,
@@ -1350,33 +1746,61 @@ extern "C" int gsx_icp_localize_projective_splats(const float *map_geometry, con
                                                   float lambda_max, float Bp, float B2p, float nu, float *poses_out,
                                                   int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
                                                   int max_splat_px, void *stream) {
-  GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX,
-                "gsx_icp_localize_projective: max_splat_px %d outside [0, %d]", max_splat_px, GSX_MAX_SPLAT_PX);
-  GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace,
-                "gsx_icp_localize_projective: null pointer");
-  GSX_CHECK_ARG(B >= 1 && H >= 2 && W >= 2 && ds >= 1 && numiters >= 0, "gsx_icp_localize_projective: bad extents");
-  GSX_CHECK_ARG(mode == 0 || mode == 1, "gsx_icp_localize_projective: mode must be 0 (ICP) or 1 (gradICP)");
-  Carver c(workspace);
-  const ProjectiveWorkspace w = projective_workspace_layout(c, B, H, W, ds);
-  GSX_CHECK_ARG(workspace_bytes >= c.bytes, "gsx_icp_localize_projective: workspace too small (%lld < %lld)",
-                (long long)workspace_bytes, (long long)c.bytes);
-  cudaStream_t s = (cudaStream_t)stream;
-  GatherSrcArgs gs{depth, depth_bstride, intrinsics, K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds,
-                   w.src, w.src_count, w.ns_cap};
-  k_icp_gather_src<<<B, 1024, 0, s>>>(gs);
-  if (render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
-                         prev_pose_bstride, B, H, W, max_splat_px, w.index, w.tgt_p, w.tgt_n, s))
+  return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
+                             prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
+                             dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
+                             workspace_bytes, max_splat_px, nullptr, stream);
+}
+
+extern "C" int64_t gsx_icp_projective_rgb_workspace_bytes(int B, int H, int W, int ds) {
+  if (B < 1 || H < 1 || W < 1 || ds < 1) return -1;
+  Carver c(nullptr);
+  projective_workspace_layout(c, B, H, W, ds, true);
+  return c.bytes;
+}
+
+extern "C" int gsx_icp_localize_projective_rgb(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                               int64_t max_count, const float *depth, int64_t depth_bstride,
+                                               const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                               int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
+                                               int numiters, float damp, int use_dist_thresh, float dist_thresh,
+                                               float lambda_max, float Bp, float B2p, float nu, float *poses_out,
+                                               int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
+                                               int max_splat_px, const float *map_colours, const float *rgb,
+                                               int64_t rgb_bstride, float photometric_weight, void *stream) {
+  GSX_CHECK_ARG(photometric_weight >= 0.0f && photometric_weight <= 3.402823466e38f,
+                "gsx_icp_localize_projective_rgb: photometric_weight %g must be finite and >= 0",
+                (double)photometric_weight);
+  if (photometric_weight > 0.0f) {
+    GSX_CHECK_ARG(map_colours && rgb, "gsx_icp_localize_projective_rgb: null colour pointer");
+    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
+                  "gsx_icp_localize_projective_rgb: colour rows must be 16-byte aligned");
+  }
+  const PhotometricInputs pm{map_colours, rgb, rgb_bstride, photometric_weight};
+  return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
+                             prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
+                             dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
+                             workspace_bytes, max_splat_px, &pm, stream);
+}
+
+extern "C" int gsx_icp_projective_targets_rgb(const float *map_geometry, const float *map_colours,
+                                              const int32_t *counts, int64_t capacity, int64_t max_count,
+                                              const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                              int64_t pose_bstride, int B, int H, int W, int max_splat_px,
+                                              int64_t *index, float *tgt_p, float *tgt_n, float *I_m, void *stream) {
+  GSX_CHECK_ARG(I_m, "gsx_icp_projective_targets_rgb: null pointer");
+  if (max_count > 0) {
+    GSX_CHECK_ARG(map_colours, "gsx_icp_projective_targets_rgb: null colour pointer");
+    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
+                  "gsx_icp_projective_targets_rgb: colour rows must be 16-byte aligned");
+  }
+  if (gsx_icp_projective_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
+                                 pose_bstride, B, H, W, max_splat_px, index, tgt_p, tgt_n, stream))
     return 1;
-  ProjLinearize lin{ProjLinArgs{w.src, w.src_count, w.ns_cap, nullptr, 0,
-                                ProjTargets{prev_poses, prev_pose_bstride, intrinsics, K_bstride, image_bounds(H, W),
-                                            w.index, w.tgt_p, w.tgt_n, dist_thresh, use_dist_thresh},
-                                w.partials}};
-  const int rc = icp_iterations(lin, w.ns_cap, B, nullptr, mode, numiters, damp, lambda_max, Bp, B2p, nu, w.partials,
-                                w.nblk, w.st, s);
-  if (rc) return rc;
-  k_pose_compose<<<(B + 63) / 64, 64, 0, s>>>(w.st.T_total, prev_poses, prev_pose_bstride, poses_out,
-                                              poses_out_bstride, B);
-  GSX_CHECK_LAUNCH("gsx_icp_localize_projective");
+  const int64_t P = (int64_t)H * W;
+  k_icp_model_intensity<<<dim3((unsigned)((P + kIcpBlock - 1) / kIcpBlock), (unsigned)B), kIcpBlock, 0,
+                          (cudaStream_t)stream>>>(index, map_colours, capacity, P, I_m);
+  GSX_CHECK_LAUNCH("gsx_icp_projective_targets_rgb");
   return 0;
 }
 
@@ -1395,5 +1819,73 @@ extern "C" int gsx_icp_project_associate(const float *src_points, const int32_t 
   k_icp_project_associate<<<grid, kIcpBlock, 0, (cudaStream_t)stream>>>(src_points, src_count, ns_stride, t, idx_out,
                                                                         d2_out);
   GSX_CHECK_LAUNCH("gsx_icp_project_associate");
+  return 0;
+}
+
+// defined in gsx_frame.cu: partials (img, tile, 12) summed in tile order -> (img, 4, 4), bottom row zero
+namespace gsx {
+__global__ void k_pose_grad_reduce(const float *partials, int tiles, float *g_poses, int n_img);
+}
+
+static int joint_args(const char *fn, const float *src_points, const int32_t *src_count, int ns_stride,
+                      const float *src_colours, const float *tgt_points, const float *tgt_normals,
+                      const float *model_colours, const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                      const float *prev_poses, const float *intrinsics, float w, JointArgs &a) {
+  GSX_CHECK_ARG(src_points && src_count && src_colours && tgt_points && tgt_normals && model_colours && index && nn_idx &&
+                    prev_poses && intrinsics,
+                "%s: null pointer", fn);
+  GSX_CHECK_ARG(B >= 1 && B <= 65535 && ns_stride >= 1 && H >= 1 && W >= 1 && (int64_t)H * W <= INT32_MAX,
+                "%s: bad extents", fn);
+  GSX_CHECK_ARG(w >= 0.0f && w <= 3.402823466e38f, "%s: photometric_weight %g must be finite and >= 0", fn, (double)w);
+  a = JointArgs{src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, nn_idx,
+                prev_poses, intrinsics, image_bounds(H, W), w};
+  return 0;
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                                   const float *src_colours, const float *tgt_points,
+                                                   const float *tgt_normals, const float *model_colours,
+                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                                                   const float *prev_poses, const float *intrinsics,
+                                                   float photometric_weight, float *sums_out, void *scratch,
+                                                   int64_t scratch_bytes, void *stream) {
+  JointArgs a;
+  if (joint_args("gsx_icp_joint_normal_eq_batched_fwd", src_points, src_count, ns_stride, src_colours, tgt_points,
+                 tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
+    return 1;
+  GSX_CHECK_ARG(sums_out && scratch && scratch_bytes >= (int64_t)B * gsx_icp_normal_eq_scratch_bytes(ns_stride),
+                "gsx_icp_joint_normal_eq_batched_fwd: bad scratch");
+  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
+  cudaStream_t s = (cudaStream_t)stream;
+  k_icp_joint_linearize_idx<<<dim3((unsigned)nblk, (unsigned)B), kIcpBlock, 0, s>>>(a, (float *)scratch);
+  k_icp_reduce_partials<<<B, 32, 0, s>>>((const float *)scratch, nblk, sums_out);
+  GSX_CHECK_LAUNCH("gsx_icp_joint_normal_eq_batched_fwd");
+  return 0;
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                                   const float *src_colours, const float *tgt_points,
+                                                   const float *tgt_normals, const float *model_colours,
+                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                                                   const float *prev_poses, const float *intrinsics,
+                                                   float photometric_weight, const float *g_sums, float *g_src,
+                                                   float *g_src_colours, float *g_tgt_points_rows,
+                                                   float *g_tgt_normals_rows, float *g_stencil_colours_rows,
+                                                   float *g_prev_poses, void *scratch, int64_t scratch_bytes,
+                                                   void *stream) {
+  JointArgs a;
+  if (joint_args("gsx_icp_joint_normal_eq_batched_bwd", src_points, src_count, ns_stride, src_colours, tgt_points,
+                 tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
+    return 1;
+  GSX_CHECK_ARG(g_sums && g_src && g_src_colours && g_tgt_points_rows && g_tgt_normals_rows && g_stencil_colours_rows &&
+                    g_prev_poses && scratch,
+                "gsx_icp_joint_normal_eq_batched_bwd: null pointer");
+  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
+  GSX_CHECK_ARG(scratch_bytes >= (int64_t)B * nblk * 12 * 4, "gsx_icp_joint_normal_eq_batched_bwd: scratch too small");
+  cudaStream_t s = (cudaStream_t)stream;
+  k_icp_joint_linearize_bwd<<<dim3((unsigned)nblk, (unsigned)B), kIcpBlock, 0, s>>>(
+      a, g_sums, g_src, g_src_colours, g_tgt_points_rows, g_tgt_normals_rows, g_stencil_colours_rows, (float *)scratch);
+  k_pose_grad_reduce<<<B, 16, 0, s>>>((const float *)scratch, nblk, g_prev_poses, B);
+  GSX_CHECK_LAUNCH("gsx_icp_joint_normal_eq_batched_bwd");
   return 0;
 }

@@ -372,7 +372,55 @@ class _RigidTransformBatchedFn(torch.autograd.Function):
         return g_p, g_T, None
 
 
-def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, target_cache=None, associate=None):
+class _JointNormalEqBatchedFn(torch.autograd.Function):
+    """The joint geometric + photometric normal equations of the projective ICP at a given association (idx (B,Ns) pixel
+    or -1): (src, src_col (B,Ns,3), tgt, tgt_n, model_col (B,H*W,3), prev (B,4,4)) -> (B,28).  forward =
+    gsx_icp_joint_normal_eq_batched_fwd, backward = gsx_icp_joint_normal_eq_batched_bwd; the gradients of the model
+    colours come per source row for the five stencil pixels and are scattered here."""
+
+    @staticmethod
+    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W):
+        ins = [t.detach().contiguous().float() for t in (src, src_col, tgt, tgt_n, model_col, prev)]
+        _C.require_cuda(ins[0], "src")
+        Bn, Ns = ins[0].shape[:2]
+        idx_c, index_c, K_c = idx.contiguous(), index.contiguous(), K.detach().contiguous()
+        sums = torch.empty((Bn, 28), dtype=torch.float32, device=src.device)
+        nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=src.device)
+        _C.launch("gsx_icp_joint_normal_eq_batched_fwd", ins[0], src_counts, Ns, ins[1], ins[2], ins[3], ins[4], index_c,
+                  Bn, int(H), int(W), idx_c, ins[5], K_c, float(w), sums, scratch, nbytes)
+        ctx.saved = (ins, idx_c, index_c, src_counts, K_c, float(w), int(H), int(W), prev.shape)
+        return sums
+
+    @staticmethod
+    def backward(ctx, g):
+        (src, src_col, tgt, tgt_n, model_col, prev), idx, index, src_counts, K, w, H, W, prev_shape = ctx.saved
+        Bn, Ns = src.shape[:2]
+        P, dev = H * W, src.device
+        g = g.contiguous().float()
+        g_src, g_col, rows_p, rows_n = (torch.empty_like(src) for _ in range(4))
+        rows_st = torch.empty((Bn, Ns, 5, 3), dtype=torch.float32, device=dev)
+        g_prev = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
+        nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _C.launch("gsx_icp_joint_normal_eq_batched_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col, index, Bn,
+                  H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, scratch, nbytes)
+        base = torch.arange(Bn, device=dev).view(Bn, 1) * P
+        flat = (idx.clamp(min=0) + base).view(-1)  # rows with idx < 0 carry zero gradients
+        g_tgt = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_p.view(-1, 3))
+        g_tn = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_n.view(-1, 3))
+        offs = torch.tensor([0, -1, 1, -W, W], device=dev)
+        st = ((idx.clamp(min=0).unsqueeze(-1) + offs).clamp(0, P - 1) + base.unsqueeze(-1)).view(-1)
+        g_model = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, st, rows_st.view(-1, 3))
+        return (g_src, g_col, g_tgt.view(Bn, P, 3), g_tn.view(Bn, P, 3), g_model.view(Bn, P, 3),
+                g_prev.view(prev_shape), None, None, None, None, None, None, None)
+
+
+def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, target_cache=None, associate=None,
+                              normal_eq=None):
+    if normal_eq is not None:  # (the projective association with the photometric term)
+        idx = associate(src.detach())
+        return normal_eq(src, tgt, tgt_n, idx), idx
     if associate is None:
         d2, idx = knn1(src.detach(), tgt.detach(), src_counts, tgt_counts, target_cache)
         if dist_thresh is not None:
@@ -383,12 +431,14 @@ def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thre
 
 
 def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numiters, damp, dist_thresh, lambda_max=2.0,
-                       B=1.0, B2=1.0, nu=200.0, associate=None):
+                       B=1.0, B2=1.0, nu=200.0, associate=None, normal_eq=None):
     """The differentiable ICP / gradICP loop of `_taped_icp` for a padded batch: src (Bn,Ns,3), tgt / tgt_n (Bn,Nt,3),
     int32 sizes (Bn,).  One chain of batched ops for all elements; returns (T (Bn,4,4), last nn idx (Bn,Ns), -1 = none).
     Per element the values are bit-identical to the per-element chain and to the fused no-grad loop.
     associate: None = exact 1-NN in tgt (thresholded by dist_thresh); otherwise a function of the current source
-    (Bn,Ns,3), detached, returning the int64 target row per source row (-1 = none) - the projective association."""
+    (Bn,Ns,3), detached, returning the int64 target row per source row (-1 = none) - the projective association.
+    normal_eq: None = _NormalEqBatchedFn; otherwise a function (src, tgt, tgt_n, idx) -> (Bn,28) sums (the joint op of
+    the photometric term)."""
     dev = src.device
     Bn, Ns = src.shape[0], src.shape[1]
     # No valid source (or target) point in any element gives a padded width of 0, which the kernels reject.  One zero
@@ -403,11 +453,12 @@ def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numite
     idx = None
     grid = {}  # the target's search grid: built by the first of the 2 * numiters associations
     for _ in range(numiters):
-        sums, idx = _normal_equations_batched(cur, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid, associate)
+        sums, idx = _normal_equations_batched(cur, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid, associate,
+                                              normal_eq)
         xi, dT = _SolveBatchedFn.apply(sums, dampt)
         one_step = _RigidTransformBatchedFn.apply(cur, dT, src_counts)
         sums_next, _ = _normal_equations_batched(one_step, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid,
-                                                 associate)
+                                                 associate, normal_eq)
         dampt, dT_applied, T = _UpdateBatchedFn.apply(xi, sums[:, 27], sums_next[:, 27], dampt, T, mode, lambda_max, B,
                                                       B2, nu)
         cur = _RigidTransformBatchedFn.apply(cur, dT_applied, src_counts)
@@ -689,12 +740,52 @@ def projective_targets(pointclouds, K, prev_poses, H, W, target_splat_px=0):
     return index, tgt_p, tgt_n
 
 
-def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0):
+def projective_intensity(pointclouds, K, prev_poses, H, W, target_splat_px=0):
+    """The model image of the photometric term: (index (B,H*W) int64 as projective_targets gives it, I_m (B,H*W) the
+    intensity (0.299 r + 0.587 g) + 0.114 b of the colour of each pixel's winning row, 0 where uncovered).  Forward only
+    (gsx_icp_projective_targets_rgb)."""
+    _C.require_cuda(K, "K")
+    _C.require_cuda(prev_poses, "prev_poses")
+    B = prev_poses.numel() // 16
+    dev = prev_poses.device
+    index = torch.empty((B, H * W), dtype=torch.int64, device=dev)
+    tgt_p = torch.empty((B, H * W, 3), dtype=torch.float32, device=dev)
+    tgt_n, I_m = torch.empty_like(tgt_p), torch.empty((B, H * W), dtype=torch.float32, device=dev)
+    geo, col, counts, cap, bound = None, None, None, 0, 0
+    if pointclouds.has_points:
+        if not pointclouds.has_colors:
+            raise ValueError("the photometric term needs a map with colours")
+        _C.require_cuda(pointclouds._geo, "pointclouds (geometry rows)")
+        geo, col = pointclouds._geo.detach().contiguous(), pointclouds._col.detach().contiguous()
+        counts, cap, bound = pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, pointclouds._bound
+    _C.launch("gsx_icp_projective_targets_rgb", geo, col, counts, cap, bound, K.detach().contiguous(), 16,
+              prev_poses.detach().contiguous(), 16, B, int(H), int(W), int(target_splat_px), index, tgt_p, tgt_n, I_m)
+    return index, I_m
+
+
+class _ProjectiveRgbWorkspace:
+    """Workspace of gsx_icp_localize_projective_rgb per (device, B, H, W, ds), as _ProjectiveWorkspace."""
+    _cache = {}
+
+    @classmethod
+    def get(cls, device, B, H, W, ds):
+        key = (str(device), B, H, W, ds)
+        buf = cls._cache.get(key)
+        if buf is None:
+            buf = torch.empty(_C.lib().gsx_icp_projective_rgb_workspace_bytes(B, H, W, ds), dtype=torch.uint8,
+                              device=device)
+            cls._cache[key] = buf
+        return buf
+
+
+def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0,
+                        photometric_weight=0.0):
     """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective_splats): the source
     is the live frame on the ds lattice at the previous pose, the target is the map rendered from the previous pose at
     full resolution (surfels with radii as disks when target_splat_px >= 1, see projective_targets), each source point
     is associated with the pixel it projects to.  Returns the new poses (B,1,4,4) = T_icp · prev pose.  No host
-    synchronisation."""
+    synchronisation.  photometric_weight w > 0 adds the photometric term of gsx_icp_localize_projective_rgb (the live
+    frame's and the map's colours); w = 0 is the geometric call."""
     live = live_frame.to_channels_last()
     B, _, H, W = live.shape
     dev = pointclouds.device
@@ -703,25 +794,38 @@ def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, 
     depth, d_bs = _frame_base(live.depth_image, H * W)
     K = live.intrinsics.contiguous()
     prev = prev_frame.poses.contiguous()
-    ws = _ProjectiveWorkspace.get(dev, B, H, W, int(dsratio))
     out = torch.empty((B, 1, 4, 4), dtype=torch.float32, device=dev)
     mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
     dth = odomprov.dist_thresh
-    _C.launch("gsx_icp_localize_projective_splats", pointclouds._geo.contiguous(),
-              pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, pointclouds._bound, depth, d_bs, K, 16,
-              prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters), float(odomprov.damp),
-              0 if dth is None else 1, 0.0 if dth is None else float(dth), lambda_max, Bp, B2p, nu, out, 16, ws,
-              ws.numel(), int(target_splat_px))
+    args = (pointclouds._geo.contiguous(), pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
+            pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters),
+            float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth), lambda_max, Bp, B2p, nu,
+            out, 16)
+    if photometric_weight == 0:
+        ws = _ProjectiveWorkspace.get(dev, B, H, W, int(dsratio))
+        _C.launch("gsx_icp_localize_projective_splats", *args, ws, ws.numel(), int(target_splat_px))
+        return out
+    if not pointclouds.has_colors or live.rgb_image is None:
+        raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
+    _C.require_cuda(live.rgb_image, "rgb_image")
+    rgb, rgb_bs = _frame_base(live.rgb_image, H * W * 3)
+    ws = _ProjectiveRgbWorkspace.get(dev, B, H, W, int(dsratio))
+    _C.launch("gsx_icp_localize_projective_rgb", *args, ws, ws.numel(), int(target_splat_px),
+              pointclouds._col.contiguous(), rgb, rgb_bs, float(photometric_weight))
     return out
 
 
-def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0):
+def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0,
+                              photometric_weight=0.0):
     """The differentiable counterpart of `localize_projective`, bit-identical poses: the index image comes from
     gsx_render_views, the target images are gathers of the map rows at that index (so the gradient reaches the rows that
     won a pixel, each at most one), and the batched ICP chain runs with the projective association.  With
     target_splat_px >= 1 the index and depth come from render_pointclouds(max_splat_px=target_splat_px), and at a pixel
     a disk row won the target point is the K1 global vertex of that depth from the previous pose (the gradient reaches
     the live depth, the previous pose and the winning rows' positions and normals; the radius gets none).
+    photometric_weight w > 0 adds the photometric term through _JointNormalEqBatchedFn: the model colour image is the
+    gather of the map's colours at the index image (the gradient reaches the colours of the winning rows), the source
+    colours are the live rgb on the lattice, and the previous pose gets the gradient of q = T_prev^-1 s and R_prev too.
     live_frame.poses must be the previous poses.  Returns (B,1,4,4)."""
     from ..slam.icpslam import _compose_canonical
     from ..structures.rgbdimages import RGBDImages
@@ -762,6 +866,17 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     tgt_p_d = tgt_p.detach().contiguous()
     assoc = lambda cur: project_associate(cur, src_counts, tgt_p_d, index, prev_d.view(B, 4, 4), K, H, W, dth)[1]
     mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
+    normal_eq = None
+    if photometric_weight:
+        if not pointclouds.has_colors or live.rgb_image is None:
+            raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
+        model_col = target(pointclouds.colors_padded)
+        src_col = frames_pc.colors_padded
+        if src_col.shape[1] == 0:  # _taped_icp_batched pads an empty source with one zero row; so do its colours
+            src_col = src_col.new_zeros(B, 1, 3)
+        prev_v = prev.reshape(B, 4, 4)
+        normal_eq = lambda cur, t_p, t_n, idx: _JointNormalEqBatchedFn.apply(
+            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, K, photometric_weight, H, W)
     T, _ = _taped_icp_batched(frames_pc.points_padded, src_counts, tgt_p, tgt_n, None, None, mode, odomprov.numiters,
-                              odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc)
+                              odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc, normal_eq=normal_eq)
     return _compose_canonical(T, prev.squeeze(1)).unsqueeze(1)

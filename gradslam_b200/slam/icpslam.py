@@ -5,6 +5,7 @@ defaults, `forward(frames) -> (Pointclouds, poses[B,L,4,4])`, `step(pointclouds,
 inplace)`.  The per-frame work runs in the sm_90a kernels of libgsx; with `odom='gt'` a whole sequence is
 one C call (gsx_pointfusion_sequence_gt) with no host synchronisation between frames.
 """
+import math
 import warnings
 from typing import Optional, Union
 
@@ -31,6 +32,23 @@ def _compose_canonical(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return torch.cat([top, bottom], -2)
 
 
+_FLT_MAX = 3.4028234663852886e38
+
+
+def _check_photometric_weight(w, association):
+    """photometric_weight: a real number (not a bool), finite and >= 0; > 0 needs the projective association."""
+    if isinstance(w, bool) or not isinstance(w, (float, int)):
+        raise TypeError("Expected photometric_weight to be of type float or int. Got {0}.".format(type(w)))
+    try:
+        wf = float(w)
+    except OverflowError:  # an int beyond float range
+        wf = math.inf
+    if not math.isfinite(wf) or wf < 0 or wf > _FLT_MAX:  # (the kernels take it as a float32)
+        raise ValueError("Expected a finite float32 photometric_weight >= 0. Got {}.".format(w))
+    if w > 0 and association != "projective":
+        raise ValueError("photometric_weight > 0 needs association='projective'")
+
+
 def _normalize_device(device):
     """torch.device with an explicit index for CUDA (the engine's default device is CUDA, not CPU)."""
     device = torch.device(device)
@@ -43,7 +61,8 @@ class ICPSLAM(nn.Module):
     def __init__(self, *, odom: str = "gradicp", dsratio: int = 4, numiters: int = 20, damp: float = 1e-8,
                  dist_thresh: Union[float, int, None] = None, lambda_max: Union[float, int] = 2.0,
                  B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0, nu: Union[float, int] = 200.0,
-                 association: str = "nn", device: Union[torch.device, str, None] = None, target_splat_px: int = 0):
+                 association: str = "nn", device: Union[torch.device, str, None] = None, target_splat_px: int = 0,
+                 photometric_weight: Union[float, int] = 0.0):
         """association (extension): how the ICP odometry pairs live points with the map.  'nn' (default, the
         reference's) = exact 1-NN between the lattice-thinned live cloud and the lattice-active map points; 'projective'
         = each live point with the map row visible at the pixel it projects to in the map rendered from the previous
@@ -54,7 +73,14 @@ class ICPSLAM(nn.Module):
         render_pointclouds(max_splat_px=target_splat_px) draws them, and at a pixel a disk won the target point is the
         point of the disk the pixel's ray meets (Keller et al. 2013's predicted vertex map).  Disks leave fewer pixels
         empty, so fewer live points pair with a row further back.  0 (default) = one pixel per surfel; a map without
-        radii gives the same poses at any value.  No effect with odom='gt'."""
+        radii gives the same poses at any value.  No effect with odom='gt'.
+
+        photometric_weight (extension, float >= 0, needs association='projective' when > 0): w of ElasticFusion's joint
+        tracking energy E_icp + w E_rgb.  Each live point associated with a map pixel also compares its intensity
+        (0.299 r + 0.587 g) + 0.114 b with the intensity of the map's colour rendered there, linearised with the central
+        differences of that model image; w absorbs the colours' scale.  Texture then pins the motions geometry cannot see
+        (sliding along a wall).  0 (default) = depth alone, exactly as without the keyword.  In the differentiable mode the
+        gradient also reaches the live rgb and the map's colours.  No effect with odom='gt'."""
         super().__init__()
         if not isinstance(association, str):
             raise TypeError("Expected association to be of type str. Got {0}.".format(type(association)))
@@ -66,6 +92,7 @@ class ICPSLAM(nn.Module):
             raise ValueError("Expected 0 <= target_splat_px <= {}. Got {}.".format(MAX_SPLAT_PX, target_splat_px))
         if target_splat_px > 0 and association != "projective":
             raise ValueError("target_splat_px > 0 needs association='projective'")
+        _check_photometric_weight(photometric_weight, association)
         if odom not in ["gt", "icp", "gradicp"]:
             msg = "odometry method ({}) not supported for PointFusion. ".format(odom)
             msg += "Currently supported odometry modules for PointFusion are: 'gt', 'icp', 'gradicp'"
@@ -84,6 +111,7 @@ class ICPSLAM(nn.Module):
         self.dsratio = dsratio
         self.association = association
         self.target_splat_px = target_splat_px
+        self.photometric_weight = float(photometric_weight)
         self.device = _normalize_device(device if device is not None else "cuda")
 
     # ------------------------------------------------------------------ sequence driver
@@ -161,12 +189,17 @@ class ICPSLAM(nn.Module):
 
         live_frame.poses = prev_frame.poses
         wants_grad = _wants_grad(live_frame.depth_image, prev_frame.poses, *pointclouds._grad_tensors())
+        if self.photometric_weight > 0:
+            wants_grad = wants_grad or _wants_grad(live_frame.rgb_image)
         if self.association == "projective":
             from ..odometry.icputils import localize_projective, localize_projective_taped
 
             if not pointclouds.has_normals:
                 raise ValueError("projective ICP association needs a map with normals")
             fn = localize_projective_taped if wants_grad else localize_projective
+            if self.photometric_weight > 0:
+                return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov, self.target_splat_px,
+                          self.photometric_weight)
             return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov, self.target_splat_px)
         if wants_grad:
             # differentiable mode (reference op order, slam/icpslam.py:238-247): the K1 maps carry their hand-written

@@ -46,7 +46,8 @@ class PointFusion(ICPSLAM):
                  nu: Union[float, int] = 200.0, association: str = "nn",
                  device: Union[torch.device, str, None] = None, stable_confidence: Union[float, int, None] = None,
                  max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None,
-                 surfel_radii: bool = False, merge_overlapping: bool = False, target_splat_px: int = 0):
+                 surfel_radii: bool = False, merge_overlapping: bool = False, target_splat_px: int = 0,
+                 photometric_weight: Union[float, int] = 0.0):
         """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
         surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
         (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
@@ -73,7 +74,10 @@ class PointFusion(ICPSLAM):
         surfel is stable), so merging can run alone; the stable surfels are then every surfel the frame merged into.
 
         target_splat_px (extension, default 0; > 0 needs association='projective' and surfel_radii=True): track against
-        the map rendered with its surfels as oriented disks, see ICPSLAM."""
+        the map rendered with its surfels as oriented disks, see ICPSLAM.
+
+        photometric_weight (extension, default 0; > 0 needs association='projective'): joint geometric and photometric
+        tracking against the map's colours, see ICPSLAM."""
         if not isinstance(surfel_radii, bool):
             raise TypeError("surfel_radii must be of type bool; but was of type {}.".format(type(surfel_radii)))
         _check_merge_overlapping(merge_overlapping, surfel_radii)
@@ -97,7 +101,7 @@ class PointFusion(ICPSLAM):
                              "the age rule a no-op)")
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
                          lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device,
-                         target_splat_px=target_splat_px)
+                         target_splat_px=target_splat_px, photometric_weight=photometric_weight)
         if target_splat_px > 0 and not surfel_radii:
             raise ValueError("target_splat_px > 0 needs surfel_radii=True (a map without radii has no disks)")
         if not isinstance(dist_th, (float, int)):

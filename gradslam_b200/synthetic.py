@@ -33,6 +33,25 @@ def _room_from_cam(s, b, motion_scale=1.0, yaw0=0.0):
     return T
 
 
+def _camera_rays(H, W):
+    """(H,W,3) camera-frame ray directions of intrinsics(H, W) with unit z, so a ray's parameter is its z-depth."""
+    K = intrinsics(H, W)
+    fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
+    return np.stack(
+        np.broadcast_arrays((np.arange(W)[None, :] - cx) / fx, (np.arange(H)[:, None] - cy) / fy, np.ones((H, W))), -1
+    )
+
+
+def _wall_exit(T, dirs):
+    """(H,W,3) ray parameter at which each ray of the camera T (camera-to-room) leaves the room through the pair of walls
+    normal to room axis 0, 1, 2; the depth is the minimum over the axes."""
+    d_room = dirs @ T[:3, :3].T
+    o = T[:3, 3]
+    half = np.asarray(ROOM_HALF_EXTENTS)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(d_room > 0, (half - o) / d_room, np.where(d_room < 0, (-half - o) / d_room, np.inf))
+
+
 def make_sequence(B, L, H, W, seed=0, hole_fraction=0.02, motion_scale=1.0, pin_memory=False,
                   yaw0=0.0):
     """Returns (rgb (B,L,H,W,3), depth (B,L,H,W,1), intrinsics (B,1,4,4), poses (B,L,4,4)), all float32 CPU.
@@ -44,30 +63,57 @@ def make_sequence(B, L, H, W, seed=0, hole_fraction=0.02, motion_scale=1.0, pin_
     freedom and drifts (the reference drifts identically); yaw0 ~ 0.6 looks into a corner (two walls + floor /
     ceiling) and makes ICP well conditioned."""
     gen = torch.Generator().manual_seed(int(seed))
-    K = intrinsics(H, W)
-    fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
-    dirs = np.stack(
-        np.broadcast_arrays((np.arange(W)[None, :] - cx) / fx, (np.arange(H)[:, None] - cy) / fy, np.ones((H, W))), -1
-    )  # (H,W,3) camera-frame ray directions with unit z => ray parameter == z-depth
-    half = np.asarray(ROOM_HALF_EXTENTS)
+    dirs = _camera_rays(H, W)
     depth = torch.empty((B, L, H, W, 1), dtype=torch.float32, pin_memory=pin_memory)
     poses = torch.empty((B, L, 4, 4), dtype=torch.float32)
     for b in range(B):
         T0_inv = np.linalg.inv(_room_from_cam(0, b, motion_scale, yaw0))
         for s in range(L):
             T = _room_from_cam(s, b, motion_scale, yaw0)
-            d_room = dirs @ T[:3, :3].T
-            o = T[:3, 3]
-            with np.errstate(divide="ignore", invalid="ignore"):
-                t_exit = np.where(d_room > 0, (half - o) / d_room, np.where(d_room < 0, (-half - o) / d_room, np.inf))
-            depth[b, s, :, :, 0] = torch.from_numpy(t_exit.min(-1).astype(np.float32))
+            depth[b, s, :, :, 0] = torch.from_numpy(_wall_exit(T, dirs).min(-1).astype(np.float32))
             poses[b, s] = torch.from_numpy((T0_inv @ T).astype(np.float32))
     if hole_fraction > 0:
         holes = torch.rand((B, L, H, W, 1), generator=gen) < hole_fraction
         depth[holes] = 0.0
     rgb = torch.empty((B, L, H, W, 3), dtype=torch.float32, pin_memory=pin_memory)
     torch.rand((B, L, H, W, 3), generator=gen, out=rgb)
-    Kt = torch.from_numpy(K.astype(np.float32)).view(1, 1, 4, 4).repeat(B, 1, 1, 1)
+    Kt = torch.from_numpy(intrinsics(H, W).astype(np.float32)).view(1, 1, 4, 4).repeat(B, 1, 1, 1)
+    return rgb, depth, Kt, poses
+
+
+# wall texture of make_textured_sequence: channel c at in-wall coordinates (a, b) (metres) is
+# 0.5 + 0.4 sin(2 pi a / la_c + pa_c) sin(2 pi b / lb_c + pb_c)
+TEXTURE_WAVELENGTHS = ((0.30, 0.45), (0.40, 0.25), (0.55, 0.35))
+TEXTURE_PHASES = ((0.3, 1.1), (2.0, 0.4), (1.3, 2.6))
+
+
+def make_textured_sequence(B, L, H, W, seed=0, hole_fraction=0.02, motion_scale=1.0, yaw0=0.0):
+    """make_sequence(B, L, H, W, seed, ...) with a painted room: the same depth, holes, poses and intrinsics, but the
+    colour of a pixel is a smooth function of the room-frame point its ray meets (products of sinusoids of the two
+    in-wall coordinates, TEXTURE_WAVELENGTHS / TEXTURE_PHASES), so a surface point has the same colour in every frame.
+    Hole pixels are coloured as if they had depth.  Everything is deterministic; seed only drives make_sequence's holes."""
+    for name, v in (("B", B), ("L", L), ("H", H), ("W", W)):
+        if isinstance(v, bool) or not isinstance(v, int):
+            raise TypeError("{} must be an int; got {}".format(name, type(v)))
+        if v < 1:
+            raise ValueError("{} must be >= 1; got {}".format(name, v))
+    if not math.isfinite(float(yaw0)) or not math.isfinite(float(motion_scale)):
+        raise ValueError("yaw0 and motion_scale must be finite")
+    _, depth, Kt, poses = make_sequence(B, L, H, W, seed=seed, hole_fraction=hole_fraction, motion_scale=motion_scale,
+                                        yaw0=yaw0)
+    dirs = _camera_rays(H, W)
+    rgb = torch.empty((B, L, H, W, 3), dtype=torch.float32)
+    for b in range(B):
+        for s in range(L):
+            T = _room_from_cam(s, b, motion_scale, yaw0)
+            t_exit = _wall_exit(T, dirs)
+            axis = t_exit.argmin(-1)  # the wall the ray meets
+            p = T[:3, 3] + t_exit.min(-1)[..., None] * (dirs @ T[:3, :3].T)  # room-frame surface point
+            a = np.where(axis == 0, p[..., 1], p[..., 0])
+            c = np.where(axis == 2, p[..., 1], p[..., 2])
+            col = [0.5 + 0.4 * np.sin(2 * math.pi * a / la + pa) * np.sin(2 * math.pi * c / lb + pb)
+                   for (la, lb), (pa, pb) in zip(TEXTURE_WAVELENGTHS, TEXTURE_PHASES)]
+            rgb[b, s] = torch.from_numpy(np.stack(col, -1).astype(np.float32))
     return rgb, depth, Kt, poses
 
 

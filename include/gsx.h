@@ -542,6 +542,62 @@ int gsx_icp_projective_targets(const float *map_geometry, const int32_t *counts,
                                int64_t pose_bstride, int B, int H, int W, int max_splat_px, int64_t *index,
                                float *tgt_p, float *tgt_n, void *stream);
 
+/* Joint geometric and photometric projective ICP (ElasticFusion's E_icp + w E_rgb): gsx_icp_localize_projective_splats
+ * plus a photometric term of weight photometric_weight = w.  I(r, g, b) = (0.299 r + 0.587 g) + 0.114 b; the model image
+ * I_m is the intensity of map_colours (B, capacity, 4) of each pixel's winning row in the target index image, and a
+ * source point's I_s the intensity of the live colour at its lattice pixel (rgb: channels-last (H, W, 3) per element,
+ * element stride rgb_bstride floats).  A source point associated (geometrically, dist_thresh included) with a pixel j
+ * that is off the image border, with j and its four neighbours covered, also has the row A_p = [c, s x c],
+ * r_p = I_s - I_m[j], c = R_prev (g_u du/dq + g_v dv/dq) with the central differences g_u, g_v of I_m at j and the
+ * derivatives of the projection at q = T_prev^-1 s; its 28 sums become geo + w (A_p A_p), geo + w (A_p r_p),
+ * geo + w (r_p r_p).  w = 0 computes exactly what gsx_icp_localize_projective_splats computes.  A negative or non-finite
+ * w, and null colour pointers with w > 0, are refused before any launch.  workspace:
+ * gsx_icp_projective_rgb_workspace_bytes(B,H,W,ds) bytes (it also serves gsx_icp_localize_projective_splats). */
+int64_t gsx_icp_projective_rgb_workspace_bytes(int B, int H, int W, int ds);
+int gsx_icp_localize_projective_rgb(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                    int64_t max_count, const float *depth, int64_t depth_bstride,
+                                    const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                    int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
+                                    float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                                    float B2p, float nu, float *poses_out, int64_t poses_out_bstride, void *workspace,
+                                    int64_t workspace_bytes, int max_splat_px, const float *map_colours,
+                                    const float *rgb, int64_t rgb_bstride, float photometric_weight, void *stream);
+
+/* gsx_icp_projective_targets plus the model image I_m (B, H*W) of gsx_icp_localize_projective_rgb, 0 where uncovered.
+ * map_colours may be NULL when max_count is 0. */
+int gsx_icp_projective_targets_rgb(const float *map_geometry, const float *map_colours, const int32_t *counts,
+                                   int64_t capacity, int64_t max_count, const float *intrinsics, int64_t K_bstride,
+                                   const float *prev_poses, int64_t pose_bstride, int B, int H, int W,
+                                   int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n, float *I_m,
+                                   void *stream);
+
+/* The joint normal equations of gsx_icp_localize_projective_rgb at a GIVEN association (the op of the differentiable
+ * mode; its rows are computed by the fused call's device functions, so the sums are the fused call's bit for bit).
+ * Source rows i < src_count[b] of src_points / src_colours (B, ns_stride, 3), world frame and live colour; nn_idx
+ * (B, ns_stride) the associated pixel or -1; tgt_points / tgt_normals / model_colours (B, H*W, 3) the target images and
+ * the colour of each pixel's winning row (zeros where uncovered); index (B, H*W) the index image (-1 = uncovered);
+ * prev_poses / intrinsics (B, 4, 4).  sums_out (B, 28): the geometric sums plus photometric_weight times the
+ * photometric products.  scratch: B * gsx_icp_normal_eq_scratch_bytes(ns_stride) bytes.
+ * The backward takes g_sums (B, 28) and writes per SOURCE row: g_src, g_src_colours, g_tgt_points_rows,
+ * g_tgt_normals_rows (B, ns_stride, 3) and g_stencil_colours_rows (B, ns_stride, 5, 3), the gradients of the model
+ * colours at pixels j, j-1, j+1, j-W, j+W (zeros where the row has none; the caller scatters them), and g_prev_poses
+ * (B, 4, 4), reduced in a fixed order without atomics (bottom row zero).  No gradient w.r.t. the intrinsics.  A negative
+ * or non-finite weight is refused before any launch. */
+int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                        const float *src_colours, const float *tgt_points, const float *tgt_normals,
+                                        const float *model_colours, const int64_t *index, int B, int H, int W,
+                                        const int64_t *nn_idx, const float *prev_poses, const float *intrinsics,
+                                        float photometric_weight, float *sums_out, void *scratch,
+                                        int64_t scratch_bytes, void *stream);
+int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                        const float *src_colours, const float *tgt_points, const float *tgt_normals,
+                                        const float *model_colours, const int64_t *index, int B, int H, int W,
+                                        const int64_t *nn_idx, const float *prev_poses, const float *intrinsics,
+                                        float photometric_weight, const float *g_sums, float *g_src,
+                                        float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
+                                        float *g_stencil_colours_rows, float *g_prev_poses, void *scratch,
+                                        int64_t scratch_bytes, void *stream);
+
 /* The association of gsx_icp_localize_projective alone (the index-only op of the differentiable mode): for the source
  * rows i < src_count[b] of src_points (B, ns_stride, 3), world frame, idx_out int64 (B, ns_stride) = the pixel
  * j = h*W + w of the target images they are associated with, or -1; d2_out (may be NULL) = |s - tgt_points[b, j]|^2
