@@ -32,6 +32,10 @@ SIGNATURES = {
     "gsx_backproject_normals_bwd": (
         c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                 c_vp, c_i64, c_vp]),
+    "gsx_backproject_normals_bwd_intrinsics_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
+    "gsx_backproject_normals_bwd_intrinsics": (
+        c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                c_vp, c_vp, c_i64, c_vp]),
     "gsx_fusion_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
     "gsx_fusion_workspace_stats_offset": (c_i64, [c_int, c_int, c_int]),
     "gsx_fusion_frame_records": (
@@ -143,6 +147,10 @@ SIGNATURES = {
     "gsx_icp_joint_normal_eq_batched_bwd": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
                 c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes": (c_i64, [c_int, c_int]),
+    "gsx_icp_joint_normal_eq_batched_bwd_intrinsics": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
+                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gsx_icp_project_associate": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp,
                 c_vp]),
@@ -155,6 +163,10 @@ SIGNATURES = {
     "gsx_render_splats_bwd": (
         c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
                 c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
+    "gsx_render_splats_bwd_intrinsics_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
+    "gsx_render_splats_bwd_intrinsics": (
+        c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
     "gsx_render_views_bwd_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
     "gsx_render_views_bwd": (
         c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,

@@ -107,6 +107,22 @@ __device__ __forceinline__ KInv load_kinv(const float *__restrict__ K) {
   return k;
 }
 
+// Chain rule of load_kinv: the gradients g.k00 .. g.k12 of the four K^-1 entries become the gradients of the 4x4 K's
+// fx, cx, fy, cy (K[0], K[2], K[5], K[6]; no other entry is read).  With e = fx + 1e-6: dk00/dfx = -1/e^2,
+// dk02/dfx = cx/e^2, dk02/dcx = -1/e, and the same for y.
+struct KGrad {
+  float fx, cx, fy, cy;
+};
+__device__ __forceinline__ KGrad kinv_chain(const float *__restrict__ K, const KInv &g) {
+  const float ex = __ldg(K + 0) + 1e-6f, ey = __ldg(K + 5) + 1e-6f, cx = __ldg(K + 2), cy = __ldg(K + 6);
+  KGrad o;
+  o.fx = (g.k02 * cx - g.k00) / (ex * ex);
+  o.cx = -g.k02 / ex;
+  o.fy = (g.k12 * cy - g.k11) / (ey * ey);
+  o.cy = -g.k12 / ey;
+  return o;
+}
+
 // local vertex of pixel (u=w, v=h) with depth d, zeroed where d <= 0 (rgbdimages.py:672-679)
 __device__ __forceinline__ float3 backproject(const KInv &k, float u, float v, float d) {
   const float vf = d > 0.0f ? 1.0f : 0.0f;

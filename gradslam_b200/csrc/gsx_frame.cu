@@ -114,7 +114,9 @@ extern "C" int gsx_backproject_normals_fwd(const float *depth, int64_t depth_bst
 // Autograd counterpart of gradslam/structures/rgbdimages.py:643-762 (the reference gets it from PyTorch's tape).
 // Gather formulation, no atomics: every pixel q re-evaluates the normal-branch terms of the (at most five)
 // pixels whose finite-difference stencil touches q.  Pose gradients are reduced per CTA and summed in tile
-// order by a second kernel (deterministic).
+// order by a second kernel (deterministic).  The kWantK instantiation also reduces each pixel's K^-1 partials
+// (v = ((k00 u + k02) d, (k11 v + k12) d, d) valid) per CTA; a third kernel sums them over the tiles and the L frames of
+// each element in a fixed order and maps them to fx, cx, fy, cy.
 // =============================================================================================================
 namespace gsx {
 
@@ -184,7 +186,10 @@ __device__ __forceinline__ void normal_terms(const FrameBwdArgs &a, const float 
   g_dv = cross3(gc, dh);
 }
 
-__global__ void __launch_bounds__(kTile) k_backproject_normals_bwd(FrameBwdArgs a) {
+// k_partials: (B*L, tiles, 4) per-CTA sums of dL/d(k00, k02, k11, k12), written only by the kWantK instantiation (a
+// separate parameter, so that the instantiation without K compiles to the kernel it was before)
+template <bool kWantK>
+__global__ void __launch_bounds__(kTile) k_backproject_normals_bwd(FrameBwdArgs a, float *k_partials) {
   __shared__ KInv s_k;
   __shared__ Rigid s_pose;
   __shared__ float s_red[kTile / 32][12];
@@ -206,6 +211,7 @@ __global__ void __launch_bounds__(kTile) k_backproject_normals_bwd(FrameBwdArgs 
   float acc[12];
 #pragma unroll
   for (int i = 0; i < 12; ++i) acc[i] = 0.0f;
+  float kacc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
   if (pix < P) {
     const int h = pix / a.W, w = pix - h * a.W;
     const int W = a.W, H = a.H;
@@ -255,6 +261,13 @@ __global__ void __launch_bounds__(kTile) k_backproject_normals_bwd(FrameBwdArgs 
       }
     }
     a.g_depth[(int64_t)img * P + pix] = vf * (ray.x * GV.x + ray.y * GV.y + ray.z * GV.z);
+    if constexpr (kWantK) {
+      const float dd = vf * d;
+      kacc[0] = (dd * (float)w) * GV.x;
+      kacc[1] = dd * GV.x;
+      kacc[2] = (dd * (float)h) * GV.y;
+      kacc[3] = dd * GV.y;
+    }
     if (a.pose_partials && pose) {
       // dL/dR = ggv (x) v + ggn (x) n ;  dL/dt = ggv
       float3 ggn = make_float3(0.f, 0.f, 0.f);
@@ -288,6 +301,26 @@ __global__ void __launch_bounds__(kTile) k_backproject_normals_bwd(FrameBwdArgs 
       a.pose_partials[((int64_t)img * a.tiles + blockIdx.x) * 12 + threadIdx.x] = x;
     }
   }
+  if constexpr (kWantK) {
+    __shared__ float s_kred[kTile / 32][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float x = kacc[i];
+#pragma unroll
+      for (int s = 16; s > 0; s >>= 1) x += __shfl_xor_sync(0xffffffffu, x, s);
+      kacc[i] = x;
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) s_kred[warp][i] = kacc[i];
+    __syncthreads();
+    if (threadIdx.x < 4) {
+      float x = 0.0f;
+      for (int wv = 0; wv < kTile / 32; ++wv) x += s_kred[wv][threadIdx.x];
+      k_partials[((int64_t)img * a.tiles + blockIdx.x) * 4 + threadIdx.x] = x;
+    }
+  }
 }
 
 __global__ void k_pose_grad_reduce(const float *partials, int tiles, float *g_poses, int n_img) {
@@ -300,6 +333,41 @@ __global__ void k_pose_grad_reduce(const float *partials, int tiles, float *g_po
   g_poses[(int64_t)img * 16 + i] = x;  // bottom row gets zeros
 }
 
+// g_K (B,4,4) of element b from its L frames' per-CTA K^-1 partials, mapped through kinv_chain; every entry load_kinv
+// does not read gets 0.  128 threads: warp e sums K^-1 entry e, lane j the tiles j, j+32, ... of frame 0, then of frame
+// 1, ..., and the lanes are combined by a fixed butterfly, so the order of every sum is fixed.
+__global__ void __launch_bounds__(128) k_intrinsics_grad_reduce(const float *k_partials, int L, int tiles,
+                                                                const float *K, int64_t K_bstride, float *g_K) {
+  __shared__ float s_g[4];
+  const int b = blockIdx.x, lane = threadIdx.x & 31, e = threadIdx.x >> 5;
+  float x = 0.0f;
+  for (int l = 0; l < L; ++l)
+    for (int t = lane; t < tiles; t += 32) x += k_partials[(((int64_t)b * L + l) * tiles + t) * 4 + e];
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) x += __shfl_xor_sync(0xffffffffu, x, s);
+  if (lane == 0) s_g[e] = x;
+  __syncthreads();
+  if (threadIdx.x < 16) {
+    const int i = threadIdx.x;
+    const KGrad g = kinv_chain(K + b * K_bstride, KInv{s_g[0], s_g[1], s_g[2], s_g[3]});
+    g_K[(int64_t)b * 16 + i] = i == 0 ? g.fx : i == 2 ? g.cx : i == 5 ? g.fy : i == 6 ? g.cy : 0.0f;
+  }
+}
+
+// scratch of the backward: the pose partials (B*L, tiles, 12), then the K^-1 partials (B*L, tiles, 4)
+struct FrameBwdScratch {
+  float *pose, *kinv;
+  int64_t bytes;
+};
+inline FrameBwdScratch frame_bwd_scratch(void *base, int B, int L, int64_t tiles) {
+  Carver c(base);
+  FrameBwdScratch s;
+  s.pose = c.take<float>((int64_t)B * L * tiles * 12);
+  s.kinv = c.take<float>((int64_t)B * L * tiles * 4);
+  s.bytes = c.bytes;
+  return s;
+}
+
 }  // namespace gsx
 
 extern "C" int64_t gsx_backproject_normals_bwd_scratch_bytes(int B, int L, int H, int W) {
@@ -308,26 +376,52 @@ extern "C" int64_t gsx_backproject_normals_bwd_scratch_bytes(int B, int L, int H
   return (int64_t)B * L * tiles * 12 * 4 + 256;
 }
 
-extern "C" int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const float *intrinsics,
-                                           int64_t K_bstride, const float *poses, int64_t pose_bstride, int B,
-                                           int L, int H, int W, const float *g_vertex, const float *g_normal,
-                                           const float *g_gvertex, const float *g_gnormal, float *g_depth,
-                                           float *g_poses, void *scratch, int64_t scratch_bytes, void *stream) {
+extern "C" int64_t gsx_backproject_normals_bwd_intrinsics_scratch_bytes(int B, int L, int H, int W) {
+  if (B < 0 || L < 0 || H < 2 || W < 2) return -1;
+  const int64_t tiles = ((int64_t)H * W + gsx::kTile - 1) / gsx::kTile;
+  return gsx::frame_bwd_scratch(nullptr, B, L, tiles).bytes;
+}
+
+extern "C" int gsx_backproject_normals_bwd_intrinsics(const float *depth, int64_t depth_bstride,
+                                                      const float *intrinsics, int64_t K_bstride, const float *poses,
+                                                      int64_t pose_bstride, int B, int L, int H, int W,
+                                                      const float *g_vertex, const float *g_normal,
+                                                      const float *g_gvertex, const float *g_gnormal, float *g_depth,
+                                                      float *g_poses, float *g_intrinsics, void *scratch,
+                                                      int64_t scratch_bytes, void *stream) {
   GSX_CHECK_ARG(depth && intrinsics && g_depth, "gsx_backproject_normals_bwd: null pointer");
   GSX_CHECK_ARG(B >= 0 && L >= 0 && H >= 2 && W >= 2, "gsx_backproject_normals_bwd: need H,W >= 2");
   GSX_CHECK_ARG((int64_t)B * L <= 65535, "gsx_backproject_normals_bwd: extents too large");
   if ((int64_t)B * L == 0) return 0;
   const int tiles = (int)(((int64_t)H * W + gsx::kTile - 1) / gsx::kTile);
-  const bool want_pose = g_poses && poses;
-  if (want_pose)
+  const bool want_pose = g_poses && poses, want_k = g_intrinsics != nullptr;
+  if (want_k)
+    GSX_CHECK_ARG(scratch && scratch_bytes >= gsx_backproject_normals_bwd_intrinsics_scratch_bytes(B, L, H, W),
+                  "gsx_backproject_normals_bwd: scratch too small");
+  else if (want_pose)
     GSX_CHECK_ARG(scratch && scratch_bytes >= gsx_backproject_normals_bwd_scratch_bytes(B, L, H, W),
                   "gsx_backproject_normals_bwd: scratch too small");
+  const gsx::FrameBwdScratch sc = gsx::frame_bwd_scratch(scratch, B, L, tiles);
   gsx::FrameBwdArgs a{depth, depth_bstride, intrinsics, K_bstride, poses, pose_bstride, B, L, H, W,
-                      {g_vertex, g_normal, g_gvertex, g_gnormal}, g_depth, want_pose ? (float *)scratch : nullptr,
-                      tiles};
+                      {g_vertex, g_normal, g_gvertex, g_gnormal}, g_depth, want_pose ? sc.pose : nullptr, tiles};
   cudaStream_t s = (cudaStream_t)stream;
-  gsx::k_backproject_normals_bwd<<<dim3((unsigned)tiles, (unsigned)(B * L)), gsx::kTile, 0, s>>>(a);
-  if (want_pose) gsx::k_pose_grad_reduce<<<B * L, 16, 0, s>>>((const float *)scratch, tiles, g_poses, B * L);
+  const dim3 grid((unsigned)tiles, (unsigned)(B * L));
+  if (want_k)
+    gsx::k_backproject_normals_bwd<true><<<grid, gsx::kTile, 0, s>>>(a, sc.kinv);
+  else
+    gsx::k_backproject_normals_bwd<false><<<grid, gsx::kTile, 0, s>>>(a, nullptr);
+  if (want_pose) gsx::k_pose_grad_reduce<<<B * L, 16, 0, s>>>(sc.pose, tiles, g_poses, B * L);
+  if (want_k) gsx::k_intrinsics_grad_reduce<<<B, 128, 0, s>>>(sc.kinv, L, tiles, intrinsics, K_bstride, g_intrinsics);
   GSX_CHECK_LAUNCH("gsx_backproject_normals_bwd");
   return 0;
+}
+
+extern "C" int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const float *intrinsics,
+                                           int64_t K_bstride, const float *poses, int64_t pose_bstride, int B,
+                                           int L, int H, int W, const float *g_vertex, const float *g_normal,
+                                           const float *g_gvertex, const float *g_gnormal, float *g_depth,
+                                           float *g_poses, void *scratch, int64_t scratch_bytes, void *stream) {
+  return gsx_backproject_normals_bwd_intrinsics(depth, depth_bstride, intrinsics, K_bstride, poses, pose_bstride, B, L,
+                                                H, W, g_vertex, g_normal, g_gvertex, g_gnormal, g_depth, g_poses,
+                                                nullptr, scratch, scratch_bytes, stream);
 }

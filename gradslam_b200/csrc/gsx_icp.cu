@@ -629,7 +629,7 @@ __device__ __forceinline__ bool model_gradient(const int64_t *idx, const float *
 // dv/dq_i = (k[4+i] - v k[8+i]) / den, c = R_prev (gu du/dq + gv dv/dq), R_prev = tinv^T.  -c is the derivative of the
 // residual I_s - I_m(pi(q(s))) with respect to s.
 // T = float, or Dual for the backward (one input direction per evaluation); r, t: T^-1 of the previous pose, k: the
-// first three rows of K (no derivative).
+// first three rows of K (TK = float: no derivative; TK = Dual when d/dK is wanted).
 struct Dual {  // value and one directional derivative; the value is computed with exactly the float operations
   float v, d;
 };
@@ -647,8 +647,8 @@ __device__ __forceinline__ Dual operator-(float a, Dual b) { return Dual{a - b.v
 __device__ __forceinline__ float value(float x) { return x; }
 __device__ __forceinline__ float value(Dual x) { return x.v; }
 
-template <class T>
-__device__ __forceinline__ void photometric_row_t(const T *r, const T *t, const float *k, T sx, T sy, T sz, T gu, T gv,
+template <class T, class TK = float>
+__device__ __forceinline__ void photometric_row_t(const T *r, const T *t, const TK *k, T sx, T sy, T sz, T gu, T gv,
                                                   T *A) {
   const T qx = ((r[0] * sx + r[1] * sy) + r[2] * sz) + t[0];
   const T qy = ((r[3] * sx + r[4] * sy) + r[5] * sz) + t[1];
@@ -945,10 +945,13 @@ __device__ __forceinline__ void row_adjoint(const float *g, const float *A, floa
 // Per source row: d/d(source point), d/d(source colour), d/d(target point and normal at the associated pixel), d/d(the
 // colours of the five stencil pixels j, j-1, j+1, j-W, j+W) (rows written per source row, the caller scatters them),
 // and the previous pose's gradient reduced per block in a fixed order (pose_partials (B, gridDim.x, 12), summed by
-// k_pose_grad_reduce).  No atomics.
+// k_pose_grad_reduce).  No atomics.  kWantK adds the 12 entries of K's first three rows, which only the photometric row
+// reads, to the dual-number inputs (29 directions) and reduces their gradient like the pose's into k_partials.
+template <bool kWantK>
 __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs a, const float *g, float *g_src,
                                                                       float *g_scol, float *g_tp, float *g_tn,
-                                                                      float *g_stencil, float *pose_partials) {
+                                                                      float *g_stencil, float *pose_partials,
+                                                                      float *k_partials) {
   __shared__ float s_g[kNumSums];
   __shared__ LiveCamera s_cam;
   __shared__ Rigid s_pose;
@@ -961,11 +964,15 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs
   const int64_t P = (int64_t)a.ib.H * a.ib.W;
   const int i = blockIdx.x * kIcpBlock + threadIdx.x;
   float gs[3] = {0.f, 0.f, 0.f}, gc[3] = {0.f, 0.f, 0.f}, gp[3] = {0.f, 0.f, 0.f}, gn[3] = {0.f, 0.f, 0.f};
-  float gst[15], gT[12];
+  float gst[15], gT[12], gK[12];
 #pragma unroll
   for (int k = 0; k < 15; ++k) gst[k] = 0.0f;
 #pragma unroll
   for (int k = 0; k < 12; ++k) gT[k] = 0.0f;
+  if constexpr (kWantK) {
+#pragma unroll
+    for (int k = 0; k < 12; ++k) gK[k] = 0.0f;
+  }
   const int64_t row = (int64_t)b * a.ns_stride + i;
   if (i < a.ns_stride && i < a.counts[b] && a.idx[row] >= 0) {
     const int64_t j = a.idx[row];
@@ -1011,6 +1018,26 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs
 #pragma unroll
         for (int p = 0; p < 6; ++p) v += ap[p] * Ad[p].d;
         gin[e] = v;
+      }
+      if constexpr (kWantK) {
+#pragma unroll 1
+        for (int e = 0; e < 12; ++e) {
+          Dual r9[9], t3[3], k12[12], in[5] = {{sx, 0.f}, {sy, 0.f}, {sz, 0.f}, {gu, 0.f}, {gv, 0.f}};
+#pragma unroll
+          for (int k = 0; k < 9; ++k) r9[k] = Dual{c.tinv.r[k], 0.0f};
+#pragma unroll
+          for (int k = 0; k < 3; ++k) t3[k] = Dual{c.tinv.t[k], 0.0f};
+#pragma unroll
+          for (int k = 0; k < 12; ++k) k12[k] = Dual{c.k[k], e == k ? 1.0f : 0.0f};
+          Dual Ad[6];
+          photometric_row_t<Dual, Dual>(r9, t3, k12, in[0], in[1], in[2], in[3], in[4], Ad);
+          float v = 0.0f;
+#pragma unroll
+          for (int p = 0; p < 6; ++p) v += ap[p] * Ad[p].d;
+#pragma unroll
+          for (int k = 0; k < 12; ++k)  // (a select, so that gK stays in registers)
+            if (k == e) gK[k] = v;
+        }
       }
       gs[0] += gin[0]; gs[1] += gin[1]; gs[2] += gin[2];
       // r_p = I_s - I_m[j]; g_u = (I_m[j+1] - I_m[j-1]) / 2, g_v = (I_m[j+W] - I_m[j-W]) / 2; I = 0.299 r + 0.587 g + 0.114 b
@@ -1061,6 +1088,25 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs
     float x = 0.0f;
     for (int w = 0; w < kIcpBlock / 32; ++w) x += s_red[w][threadIdx.x];
     pose_partials[((int64_t)b * gridDim.x + blockIdx.x) * 12 + threadIdx.x] = x;
+  }
+  if constexpr (kWantK) {
+    __shared__ float s_kred[kIcpBlock / 32][12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) {
+      float x = gK[k];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+      gK[k] = x;
+    }
+    if (lane == 0)
+#pragma unroll
+      for (int k = 0; k < 12; ++k) s_kred[warp][k] = gK[k];
+    __syncthreads();
+    if (threadIdx.x < 12) {
+      float x = 0.0f;
+      for (int w = 0; w < kIcpBlock / 32; ++w) x += s_kred[w][threadIdx.x];
+      k_partials[((int64_t)b * gridDim.x + blockIdx.x) * 12 + threadIdx.x] = x;
+    }
   }
 }
 
@@ -1873,6 +1919,25 @@ extern "C" int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, cons
                                                    float *g_tgt_normals_rows, float *g_stencil_colours_rows,
                                                    float *g_prev_poses, void *scratch, int64_t scratch_bytes,
                                                    void *stream) {
+  return gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
+      src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H, W, nn_idx,
+      prev_poses, intrinsics, photometric_weight, g_sums, g_src, g_src_colours, g_tgt_points_rows, g_tgt_normals_rows,
+      g_stencil_colours_rows, g_prev_poses, nullptr, scratch, scratch_bytes, stream);
+}
+
+extern "C" int64_t gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(int B, int ns_stride) {
+  if (B < 0 || ns_stride < 0) return -1;
+  const int64_t nblk = ((int64_t)ns_stride + kIcpBlock - 1) / kIcpBlock;
+  return (int64_t)B * nblk * 12 * 4 * 2;
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
+    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
+    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
+    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
+    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
+    void *stream) {
   JointArgs a;
   if (joint_args("gsx_icp_joint_normal_eq_batched_bwd", src_points, src_count, ns_stride, src_colours, tgt_points,
                  tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
@@ -1881,11 +1946,26 @@ extern "C" int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, cons
                     g_prev_poses && scratch,
                 "gsx_icp_joint_normal_eq_batched_bwd: null pointer");
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
-  GSX_CHECK_ARG(scratch_bytes >= (int64_t)B * nblk * 12 * 4, "gsx_icp_joint_normal_eq_batched_bwd: scratch too small");
+  const int64_t pose_bytes = (int64_t)B * nblk * 12 * 4;
+  if (g_intrinsics)
+    GSX_CHECK_ARG(scratch_bytes >= gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(B, ns_stride),
+                  "gsx_icp_joint_normal_eq_batched_bwd: scratch too small");
+  else
+    GSX_CHECK_ARG(scratch_bytes >= pose_bytes, "gsx_icp_joint_normal_eq_batched_bwd: scratch too small");
   cudaStream_t s = (cudaStream_t)stream;
-  k_icp_joint_linearize_bwd<<<dim3((unsigned)nblk, (unsigned)B), kIcpBlock, 0, s>>>(
-      a, g_sums, g_src, g_src_colours, g_tgt_points_rows, g_tgt_normals_rows, g_stencil_colours_rows, (float *)scratch);
-  k_pose_grad_reduce<<<B, 16, 0, s>>>((const float *)scratch, nblk, g_prev_poses, B);
+  const dim3 grid((unsigned)nblk, (unsigned)B);
+  float *pose_partials = (float *)scratch, *k_partials = pose_partials + (int64_t)B * nblk * 12;
+  if (g_intrinsics)
+    k_icp_joint_linearize_bwd<true><<<grid, kIcpBlock, 0, s>>>(a, g_sums, g_src, g_src_colours, g_tgt_points_rows,
+                                                                g_tgt_normals_rows, g_stencil_colours_rows,
+                                                                pose_partials, k_partials);
+  else
+    k_icp_joint_linearize_bwd<false><<<grid, kIcpBlock, 0, s>>>(a, g_sums, g_src, g_src_colours, g_tgt_points_rows,
+                                                                 g_tgt_normals_rows, g_stencil_colours_rows,
+                                                                 pose_partials, nullptr);
+  k_pose_grad_reduce<<<B, 16, 0, s>>>(pose_partials, nblk, g_prev_poses, B);
+  // the 12 entries of K's first three rows, summed over the blocks in order; the 4th row gets 0
+  if (g_intrinsics) k_pose_grad_reduce<<<B, 16, 0, s>>>(k_partials, nblk, g_intrinsics, B);
   GSX_CHECK_LAUNCH("gsx_icp_joint_normal_eq_batched_bwd");
   return 0;
 }

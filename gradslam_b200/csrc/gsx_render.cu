@@ -30,6 +30,9 @@ namespace gsx {
 
 // defined in gsx_frame.cu: partials (img, tile, 12) summed in tile order -> (img, 4, 4), bottom row zero
 __global__ void k_pose_grad_reduce(const float *partials, int tiles, float *g_poses, int n_img);
+// defined in gsx_frame.cu: K^-1 partials (b*L + l, tile, 4) summed per element in a fixed order -> g_K (B,4,4)
+__global__ void __launch_bounds__(128) k_intrinsics_grad_reduce(const float *k_partials, int L, int tiles,
+                                                                const float *K, int64_t K_bstride, float *g_K);
 
 constexpr int kRB = 256;        // threads per CTA of every render kernel
 constexpr int kViews = 32;      // cameras staged per CTA (blockIdx.z chunks beyond)
@@ -462,7 +465,11 @@ __global__ void __launch_bounds__(kRB) k_render_splat_bwd_rows(RenderBwdArgs a, 
 
 // Pose: per pixel, with gq = dL/dq and gm = dL/dm of the winning row (as in the rows kernel),
 //   dL/dR = (p - c) gq^T + n gm^T,  dL/dc = -R gq;  reduced per tile as k_render_bwd_pose does.
-__global__ void __launch_bounds__(kRB) k_render_splat_bwd_pose(RenderBwdArgs a) {
+// kWantK also reduces, per tile into k_partials (b*L + l, tile, 4), the K^-1 partials of a disk pixel's depth
+// t = (m.q)/(m.d) through its ray d = K^-1 (w, h, 1): dL/dd = -g t m / (m.d), so dL/dk00 = w dL/dd.x, dL/dk02 = dL/dd.x,
+// dL/dk11 = h dL/dd.y, dL/dk12 = dL/dd.y.  One-pixel rows do not depend on K.  Pose partials are then optional.
+template <bool kWantK>
+__global__ void __launch_bounds__(kRB) k_render_splat_bwd_pose(RenderBwdArgs a, float *k_partials) {
   __shared__ Rigid s_pose, s_tinv;
   __shared__ KInv s_kinv;
   __shared__ float s_red[kRB / 32][12];
@@ -479,6 +486,7 @@ __global__ void __launch_bounds__(kRB) k_render_splat_bwd_pose(RenderBwdArgs a) 
   float acc[12];
 #pragma unroll
   for (int j = 0; j < 12; ++j) acc[j] = 0.0f;
+  float kacc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
   const int64_t i = img * P + pix;
   const int64_t n = pix < P ? __ldg(a.index + i) : -1;
   if (n >= 0) {
@@ -500,6 +508,14 @@ __global__ void __launch_bounds__(kRB) k_render_splat_bwd_pose(RenderBwdArgs a) 
       const float s = gd / md;
       gq[0] = s * m.x; gq[1] = s * m.y; gq[2] = s * m.z;
       gm[0] += s * (q.x - t * ray.x); gm[1] += s * (q.y - t * ray.y); gm[2] += s * (q.z - t * ray.z);
+      if constexpr (kWantK) {
+        const float st = s * t;
+        const float grx = -(st * m.x), gry = -(st * m.y);
+        kacc[0] = grx * (float)w;
+        kacc[1] = grx;
+        kacc[2] = gry * (float)h;
+        kacc[3] = gry;
+      }
     }
     const Rigid &T = s_pose;
     const float pt[3] = {g0.x - T.t[0], g0.y - T.t[1], g0.z - T.t[2]};
@@ -523,11 +539,44 @@ __global__ void __launch_bounds__(kRB) k_render_splat_bwd_pose(RenderBwdArgs a) 
 #pragma unroll
     for (int j = 0; j < 12; ++j) s_red[warp][j] = acc[j];
   __syncthreads();
-  if (threadIdx.x < 12) {
+  if (threadIdx.x < 12 && (!kWantK || a.pose_partials)) {
     float x = 0.0f;
     for (int w = 0; w < kRB / 32; ++w) x += s_red[w][threadIdx.x];
     a.pose_partials[((int64_t)img * a.tiles + blockIdx.x) * 12 + threadIdx.x] = x;
   }
+  if constexpr (kWantK) {
+    __shared__ float s_kred[kRB / 32][4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float x = kacc[j];
+#pragma unroll
+      for (int s = 16; s > 0; s >>= 1) x += __shfl_xor_sync(0xffffffffu, x, s);
+      kacc[j] = x;
+    }
+    if (lane == 0)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s_kred[warp][j] = kacc[j];
+    __syncthreads();
+    if (threadIdx.x < 4) {
+      float x = 0.0f;
+      for (int w = 0; w < kRB / 32; ++w) x += s_kred[w][threadIdx.x];
+      k_partials[((int64_t)img * a.tiles + blockIdx.x) * 4 + threadIdx.x] = x;
+    }
+  }
+}
+
+// scratch of the render backward: the pose partials (B*L, tiles, 12), then the K^-1 partials (B*L, tiles, 4)
+struct RenderBwdScratch {
+  float *pose, *kinv;
+  int64_t bytes;
+};
+inline RenderBwdScratch render_bwd_scratch(void *base, int B, int L, int64_t tiles) {
+  Carver c(base);
+  RenderBwdScratch r;
+  r.pose = c.take<float>((int64_t)B * L * tiles * 12);
+  r.kinv = c.take<float>((int64_t)B * L * tiles * 4);
+  r.bytes = c.bytes;
+  return r;
 }
 
 }  // namespace gsx
@@ -662,31 +711,62 @@ extern "C" int gsx_render_splats_bwd(const float *map_geometry, const int32_t *c
                                      const float *g_depth, const float *g_rgb, const float *g_normals,
                                      const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses,
                                      void *scratch, int64_t scratch_bytes, int max_splat_px, void *stream) {
+  return gsx_render_splats_bwd_intrinsics(map_geometry, counts, capacity, intrinsics, K_bstride, poses, pose_bstride,
+                                          index, B, L, H, W, g_depth, g_rgb, g_normals, g_confidence, d_geometry,
+                                          d_colors, d_poses, nullptr, scratch, scratch_bytes, max_splat_px, stream);
+}
+
+extern "C" int64_t gsx_render_splats_bwd_intrinsics_scratch_bytes(int B, int L, int H, int W) {
+  if (B < 1 || L < 1 || H < 1 || W < 1) return -1;
+  return render_bwd_scratch(nullptr, B, L, pixel_tiles(H, W)).bytes;
+}
+
+extern "C" int gsx_render_splats_bwd_intrinsics(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                                const float *intrinsics, int64_t K_bstride, const float *poses,
+                                                int64_t pose_bstride, const int64_t *index, int B, int L, int H, int W,
+                                                const float *g_depth, const float *g_rgb, const float *g_normals,
+                                                const float *g_confidence, float *d_geometry, float *d_colors,
+                                                float *d_poses, float *g_intrinsics, void *scratch,
+                                                int64_t scratch_bytes, int max_splat_px, void *stream) {
   if (check_render_extents("gsx_render_views_bwd", B, L, H, W, capacity)) return 1;
   if (check_splat_px("gsx_render_splats_bwd", max_splat_px)) return 1;
   GSX_CHECK_ARG(intrinsics && poses && index, "gsx_render_views_bwd: null pointer");
   const bool want_rows = (d_geometry || d_colors) && capacity > 0;
-  if (capacity > 0 && (want_rows || d_poses))
+  const bool want_k = g_intrinsics != nullptr;
+  if (capacity > 0 && (want_rows || d_poses || want_k))
     GSX_CHECK_ARG(map_geometry && counts, "gsx_render_views_bwd: null map pointer");
   GSX_CHECK_ARG(aligned16(map_geometry) && aligned16(d_geometry) && aligned16(d_colors),
                 "gsx_render_views_bwd: map rows must be 16-byte aligned");
-  if (d_poses)
+  // one-pixel rows (max_splat_px = 0) do not depend on K: d/dK is zero and needs no scratch
+  const bool k_pass = want_k && max_splat_px > 0;
+  if (k_pass)
+    GSX_CHECK_ARG(scratch && scratch_bytes >= gsx_render_splats_bwd_intrinsics_scratch_bytes(B, L, H, W),
+                  "gsx_render_views_bwd: scratch too small");
+  else if (d_poses)
     GSX_CHECK_ARG(scratch && scratch_bytes >= gsx_render_views_bwd_scratch_bytes(B, L, H, W),
                   "gsx_render_views_bwd: scratch too small");
   cudaStream_t s = (cudaStream_t)stream;
   const unsigned tiles = pixel_tiles(H, W);
+  const RenderBwdScratch sc = render_bwd_scratch(scratch, B, L, tiles);
   RenderBwdArgs a{map_geometry, counts, capacity, intrinsics, K_bstride, poses, pose_bstride, index, L,
                   image_bounds(H, W), g_depth, g_rgb, g_normals, g_confidence, d_geometry, d_colors,
-                  (float *)scratch, (int)tiles};
+                  d_poses ? sc.pose : nullptr, (int)tiles};
   const dim3 row_grid((unsigned)((capacity + kRB - 1) / kRB), (unsigned)B);
+  const dim3 pix_grid(tiles, (unsigned)(B * L));
   if (want_rows && max_splat_px == 0) k_render_bwd_rows<<<row_grid, kRB, 0, s>>>(a);
   if (want_rows && max_splat_px > 0) k_render_splat_bwd_rows<<<row_grid, kRB, 0, s>>>(a, max_splat_px);
+  if (k_pass) {
+    k_render_splat_bwd_pose<true><<<pix_grid, kRB, 0, s>>>(a, sc.kinv);
+    k_intrinsics_grad_reduce<<<B, 128, 0, s>>>(sc.kinv, L, (int)tiles, intrinsics, K_bstride, g_intrinsics);
+  } else if (want_k) {
+    cudaMemsetAsync(g_intrinsics, 0, (size_t)B * 16 * sizeof(float), s);
+  }
   if (d_poses) {
     if (max_splat_px == 0)
-      k_render_bwd_pose<<<dim3(tiles, (unsigned)(B * L)), kRB, 0, s>>>(a);
-    else
-      k_render_splat_bwd_pose<<<dim3(tiles, (unsigned)(B * L)), kRB, 0, s>>>(a);
-    k_pose_grad_reduce<<<B * L, 16, 0, s>>>((const float *)scratch, (int)tiles, d_poses, B * L);
+      k_render_bwd_pose<<<pix_grid, kRB, 0, s>>>(a);
+    else if (!k_pass)
+      k_render_splat_bwd_pose<false><<<pix_grid, kRB, 0, s>>>(a, nullptr);
+    k_pose_grad_reduce<<<B * L, 16, 0, s>>>(sc.pose, (int)tiles, d_poses, B * L);
   }
   GSX_CHECK_LAUNCH("gsx_render_views_bwd");
   return 0;

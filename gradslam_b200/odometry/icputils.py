@@ -375,8 +375,9 @@ class _RigidTransformBatchedFn(torch.autograd.Function):
 class _JointNormalEqBatchedFn(torch.autograd.Function):
     """The joint geometric + photometric normal equations of the projective ICP at a given association (idx (B,Ns) pixel
     or -1): (src, src_col (B,Ns,3), tgt, tgt_n, model_col (B,H*W,3), prev (B,4,4)) -> (B,28).  forward =
-    gsx_icp_joint_normal_eq_batched_fwd, backward = gsx_icp_joint_normal_eq_batched_bwd; the gradients of the model
-    colours come per source row for the five stencil pixels and are scattered here."""
+    gsx_icp_joint_normal_eq_batched_fwd, backward = gsx_icp_joint_normal_eq_batched_bwd, or
+    gsx_icp_joint_normal_eq_batched_bwd_intrinsics when K requires grad (the photometric row reads K's first three rows);
+    the gradients of the model colours come per source row for the five stencil pixels and are scattered here."""
 
     @staticmethod
     def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W):
@@ -390,6 +391,7 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         _C.launch("gsx_icp_joint_normal_eq_batched_fwd", ins[0], src_counts, Ns, ins[1], ins[2], ins[3], ins[4], index_c,
                   Bn, int(H), int(W), idx_c, ins[5], K_c, float(w), sums, scratch, nbytes)
         ctx.saved = (ins, idx_c, index_c, src_counts, K_c, float(w), int(H), int(W), prev.shape)
+        ctx.K_shape = K.shape
         return sums
 
     @staticmethod
@@ -401,10 +403,20 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         g_src, g_col, rows_p, rows_n = (torch.empty_like(src) for _ in range(4))
         rows_st = torch.empty((Bn, Ns, 5, 3), dtype=torch.float32, device=dev)
         g_prev = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
-        nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
-        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _C.launch("gsx_icp_joint_normal_eq_batched_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col, index, Bn,
-                  H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, scratch, nbytes)
+        g_K = None
+        if ctx.needs_input_grad[9]:
+            g_K = torch.zeros((Bn, 4, 4), dtype=torch.float32, device=dev)
+            nbytes = _C.lib().gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(Bn, Ns)
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _C.launch("gsx_icp_joint_normal_eq_batched_bwd_intrinsics", src, src_counts, Ns, src_col, tgt, tgt_n,
+                      model_col, index, Bn, H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev,
+                      g_K, scratch, nbytes)
+            g_K = g_K.view(ctx.K_shape)
+        else:
+            nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _C.launch("gsx_icp_joint_normal_eq_batched_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col, index,
+                      Bn, H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, scratch, nbytes)
         base = torch.arange(Bn, device=dev).view(Bn, 1) * P
         flat = (idx.clamp(min=0) + base).view(-1)  # rows with idx < 0 carry zero gradients
         g_tgt = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_p.view(-1, 3))
@@ -413,7 +425,7 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         st = ((idx.clamp(min=0).unsqueeze(-1) + offs).clamp(0, P - 1) + base.unsqueeze(-1)).view(-1)
         g_model = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, st, rows_st.view(-1, 3))
         return (g_src, g_col, g_tgt.view(Bn, P, 3), g_tn.view(Bn, P, 3), g_model.view(Bn, P, 3),
-                g_prev.view(prev_shape), None, None, None, None, None, None, None)
+                g_prev.view(prev_shape), None, None, None, g_K, None, None, None)
 
 
 def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, target_cache=None, associate=None,
@@ -826,6 +838,9 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     photometric_weight w > 0 adds the photometric term through _JointNormalEqBatchedFn: the model colour image is the
     gather of the map's colours at the index image (the gradient reaches the colours of the winning rows), the source
     colours are the live rgb on the lattice, and the previous pose gets the gradient of q = T_prev^-1 s and R_prev too.
+    The gradient w.r.t. the intrinsics reaches the poses through the live points (K1), the disk depths of the splatted
+    targets and their surface points (R3d, K1) and the photometric row; the index image and the association use K only
+    to choose pixels and carry none.
     live_frame.poses must be the previous poses.  Returns (B,1,4,4)."""
     from ..slam.icpslam import _compose_canonical
     from ..structures.rgbdimages import RGBDImages
@@ -835,11 +850,12 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     live = live_frame.to_channels_last()
     B, _, H, W = live.shape
     dev = pointclouds.device
-    K = live.intrinsics.detach().contiguous()
+    Kg = live.intrinsics  # values: carries d/dK
+    K = Kg.detach().contiguous()  # pixel choices only
     prev = prev_frame.poses
     prev_d = prev.detach().contiguous()
     if target_splat_px:
-        splat = render_pointclouds(pointclouds, K, prev, H, W, max_splat_px=target_splat_px)
+        splat = render_pointclouds(pointclouds, Kg, prev, H, W, max_splat_px=target_splat_px)
         index = splat.index.view(B, H * W)
     else:
         index = torch.empty((B, H * W), dtype=torch.int64, device=dev)
@@ -859,7 +875,7 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
         radii = pointclouds.radii_padded.detach()[..., 0]
         radius = torch.gather(torch.cat([radii, radii.new_zeros(B, 1)], 1), 1, index.clamp(min=0))
         disk = covered[..., 0] & (radius > 0) & (tgt_n.detach() != 0).any(-1)
-        surface = RGBDImages(splat.depth.new_zeros(B, 1, H, W, 3), splat.depth, K, prev).global_vertex_map
+        surface = RGBDImages(splat.depth.new_zeros(B, 1, H, W, 3), splat.depth, Kg, prev).global_vertex_map
         tgt_p = torch.where(disk.unsqueeze(-1), surface.reshape(B, H * W, 3), tgt_p)
     src_counts = frames_pc._counts_dev[frames_pc._cur]
     dth = odomprov.dist_thresh
@@ -876,7 +892,7 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
             src_col = src_col.new_zeros(B, 1, 3)
         prev_v = prev.reshape(B, 4, 4)
         normal_eq = lambda cur, t_p, t_n, idx: _JointNormalEqBatchedFn.apply(
-            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, K, photometric_weight, H, W)
+            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, Kg, photometric_weight, H, W)
     T, _ = _taped_icp_batched(frames_pc.points_padded, src_counts, tgt_p, tgt_n, None, None, mode, odomprov.numiters,
                               odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc, normal_eq=normal_eq)
     return _compose_canonical(T, prev.squeeze(1)).unsqueeze(1)

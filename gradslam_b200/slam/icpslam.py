@@ -188,7 +188,8 @@ class ICPSLAM(nn.Module):
         from ..odometry.icputils import _wants_grad, downsample_pointclouds, downsample_rgbdimages, localize_against_map
 
         live_frame.poses = prev_frame.poses
-        wants_grad = _wants_grad(live_frame.depth_image, prev_frame.poses, *pointclouds._grad_tensors())
+        wants_grad = _wants_grad(live_frame.depth_image, prev_frame.poses, live_frame.intrinsics,
+                                 *pointclouds._grad_tensors())
         if self.photometric_weight > 0:
             wants_grad = wants_grad or _wants_grad(live_frame.rgb_image)
         if self.association == "projective":

@@ -34,7 +34,8 @@ def _frame_base(t: torch.Tensor, inner: int):
 
 class _BackprojectFn(torch.autograd.Function):
     """depth, intrinsics, poses -> (vertex, normal, gvertex, gnormal); all channels-last.
-    forward = gsx_backproject_normals_fwd, backward = gsx_backproject_normals_bwd (d/d depth, d/d poses)."""
+    forward = gsx_backproject_normals_fwd, backward = gsx_backproject_normals_bwd (d/d depth, d/d poses), or
+    gsx_backproject_normals_bwd_intrinsics when the intrinsics require grad (also d/d fx, cx, fy, cy)."""
 
     @staticmethod
     def forward(ctx, depth, intrinsics, poses, want):
@@ -51,6 +52,7 @@ class _BackprojectFn(torch.autograd.Function):
         _C.launch("gsx_backproject_normals_fwd", d, d_bs, K, 16, P, L * 16, B, L, H, W, *outs)
         ctx.saved = (d, d_bs, K, P, (B, L, H, W))
         ctx.need_pose = poses is not None and poses.requires_grad
+        ctx.K_shape = intrinsics.shape
         return tuple(outs)
 
     @staticmethod
@@ -60,6 +62,13 @@ class _BackprojectFn(torch.autograd.Function):
         gs = [None if g is None else g.contiguous() for g in (g_v, g_n, g_gv, g_gn)]
         g_depth = torch.empty((B, L, H, W, 1), dtype=torch.float32, device=dev)
         g_poses = torch.empty((B, L, 4, 4), dtype=torch.float32, device=dev) if ctx.need_pose else None
+        if ctx.needs_input_grad[1]:
+            g_K = torch.zeros((B, 4, 4), dtype=torch.float32, device=dev)  # (B*L == 0 launches nothing)
+            nbytes = _C.lib().gsx_backproject_normals_bwd_intrinsics_scratch_bytes(B, L, H, W)
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _C.launch("gsx_backproject_normals_bwd_intrinsics", d, d_bs, K, 16, P, L * 16, B, L, H, W, *gs, g_depth,
+                      g_poses, g_K, scratch, nbytes)
+            return g_depth, g_K.view(ctx.K_shape), g_poses, None
         nbytes = _C.lib().gsx_backproject_normals_bwd_scratch_bytes(B, L, H, W)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev) if ctx.need_pose else None
         _C.launch("gsx_backproject_normals_bwd", d, d_bs, K, 16, P, L * 16, B, L, H, W, *gs, g_depth, g_poses, scratch,

@@ -56,26 +56,28 @@ def _render(geo, col, counts, bound, K, poses, H, W, want_normals, want_conf, sp
 
 
 class _RenderFn(torch.autograd.Function):
-    """gsx_render_splats as one differentiable op over (geometry rows, colour rows, poses); backward =
-    gsx_render_splats_bwd at the forward's index (the association and the footprint carry no gradient, the radius
-    none either)."""
+    """gsx_render_splats as one differentiable op over (geometry rows, colour rows, poses, intrinsics); backward =
+    gsx_render_splats_bwd at the forward's index, or gsx_render_splats_bwd_intrinsics when the intrinsics require grad
+    (the association and the footprint carry no gradient, the radius none either)."""
 
     @staticmethod
-    def forward(ctx, pack, geo, col, poses):
-        counts, bound, K, H, W, want_normals, want_conf, splat = pack
+    def forward(ctx, pack, geo, col, poses, intrinsics):
+        counts, bound, H, W, want_normals, want_conf, splat = pack
+        K = intrinsics.detach().contiguous()
         outs = _render(geo.detach(), None if col is None else col.detach(), counts, bound, K, poses.detach(), H, W,
                        want_normals, want_conf, splat)
         ctx.mark_non_differentiable(outs[4])
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(geo, poses, outs[4])
         ctx.pack = (counts, K, H, W, splat)
+        ctx.K_shape = intrinsics.shape
         return outs
 
     @staticmethod
     def backward(ctx, g_depth, g_rgb, g_normals, g_conf, _g_index):
         geo, poses, index = ctx.saved_tensors
         counts, K, H, W, splat = ctx.pack
-        _, need_geo, need_col, need_pose = ctx.needs_input_grad
+        _, need_geo, need_col, need_pose, need_K = ctx.needs_input_grad
         B, L = poses.shape[:2]
         dev, cap = geo.device, geo.shape[1]
         d_geo = torch.empty_like(geo) if need_geo else None
@@ -86,9 +88,16 @@ class _RenderFn(torch.autograd.Function):
             scratch = torch.empty(_C.lib().gsx_render_views_bwd_scratch_bytes(B, L, H, W), dtype=torch.uint8,
                                   device=dev)
         gs = [None if g is None else g.contiguous() for g in (g_depth, g_rgb, g_normals, g_conf)]
+        if need_K:
+            g_K = torch.zeros((B, 4, 4), dtype=torch.float32, device=dev)
+            scratch = torch.empty(_C.lib().gsx_render_splats_bwd_intrinsics_scratch_bytes(B, L, H, W),
+                                  dtype=torch.uint8, device=dev)
+            _C.launch("gsx_render_splats_bwd_intrinsics", geo.detach(), counts, cap, K, 16, poses.detach(), L * 16,
+                      index, B, L, H, W, *gs, d_geo, d_col, d_poses, g_K, scratch, scratch.numel(), splat)
+            return None, d_geo, d_col, d_poses, g_K.view(ctx.K_shape)
         _C.launch("gsx_render_splats_bwd", geo.detach(), counts, cap, K, 16, poses.detach(), L * 16, index, B, L, H, W,
                   *gs, d_geo, d_col, d_poses, scratch, 0 if scratch is None else scratch.numel(), splat)
-        return None, d_geo, d_col, d_poses
+        return None, d_geo, d_col, d_poses, None
 
 
 def _camera(t, name, B):
@@ -111,8 +120,9 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
 
     intrinsics (B, 1, 4, 4) as in RGBDImages; poses (B, L, 4, 4) camera-to-world.  `RGBDImages(out.rgb, out.depth,
     intrinsics, poses)` turns the result into frames.  Differentiable w.r.t. the map rows (points, normals, colours,
-    confidence counts) and the poses, at the fixed pixel assignment; not w.r.t. the intrinsics.  No host
-    synchronisation.
+    confidence counts), the poses and the intrinsics, at the fixed pixel assignment.  Only a disk pixel's depth depends on
+    the intrinsics' values (through its ray, max_splat_px >= 1), so with max_splat_px = 0 their gradient is zero.  No
+    host synchronisation.
 
     max_splat_px (extension, 0 .. 16, default 0 = the one-pixel rule above for every row): a row with a surfel radius
     (`radii_padded` > 0, PointFusion(surfel_radii=True)) and a non-zero normal is drawn as an oriented disk: every pixel
@@ -160,9 +170,9 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
     poses_c = poses.contiguous()
     from ..odometry.icputils import _wants_grad
 
-    if _wants_grad(geo, col, poses_c):
-        outs = _RenderFn.apply((counts.clone(), pointclouds._bound, K, height, width) + want + (max_splat_px,), geo, col,
-                               poses_c)
+    if _wants_grad(geo, col, poses_c, intrinsics):
+        outs = _RenderFn.apply((counts.clone(), pointclouds._bound, height, width) + want + (max_splat_px,), geo, col,
+                               poses_c, intrinsics)
     else:
         outs = _render(geo.detach(), None if col is None else col.detach(), counts, pointclouds._bound, K,
                        poses_c.detach(), height, width, *want, max_splat_px)

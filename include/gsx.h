@@ -57,15 +57,32 @@ int gsx_backproject_normals_fwd(const float *depth, int64_t depth_bstride, const
 /* backward of K1: from the upstream gradients of any of the four maps (dense (B,L,H,W,3), NULL = zero)
  * computes d(loss)/d(depth) (B,L,H,W) and, if g_poses != NULL and poses != NULL, d(loss)/d(poses)
  * (B*L,4,4) (top 3x4 block; bottom row zero).  Autograd counterpart of the op chain above (the reference
- * obtains it from PyTorch's tape).  Gradients w.r.t. the intrinsics are not produced.  Deterministic: no
- * atomics; pose gradients are reduced per tile then summed in tile order.
- * scratch: gsx_backproject_normals_bwd_scratch_bytes(B,L,H,W) bytes (only needed for g_poses). */
+ * obtains it from PyTorch's tape).  No gradient w.r.t. the intrinsics: gsx_backproject_normals_bwd_intrinsics
+ * below adds it.  Deterministic: no atomics; pose gradients are reduced per tile then summed in tile order.
+ * scratch: gsx_backproject_normals_bwd_scratch_bytes(B,L,H,W) bytes (only needed for g_poses).  Same as
+ * gsx_backproject_normals_bwd_intrinsics with g_intrinsics = NULL. */
 int64_t gsx_backproject_normals_bwd_scratch_bytes(int B, int L, int H, int W);
 int gsx_backproject_normals_bwd(const float *depth, int64_t depth_bstride, const float *intrinsics,
                                 int64_t K_bstride, const float *poses, int64_t pose_bstride, int B, int L,
                                 int H, int W, const float *g_vertex, const float *g_normal,
                                 const float *g_gvertex, const float *g_gnormal, float *g_depth,
                                 float *g_poses, void *scratch, int64_t scratch_bytes, void *stream);
+
+/* backward of K1 that also computes, if g_intrinsics != NULL, d(loss)/d(intrinsics) into g_intrinsics (B,4,4) dense:
+ * the gradient of projutils.inverse_intrinsics' K^-1 (k00 = 1/(fx+1e-6), k02 = -cx/(fx+1e-6), and the same for y)
+ * through every vertex the four maps depend on, including the normal stencil's.  Only fx, cx, fy, cy (entries 0, 2, 5,
+ * 6) are read by K1; every other entry of g_intrinsics is 0.  The L frames of an element share its K: their
+ * contributions are summed per element.  Deterministic: per-pixel terms are reduced per tile, then summed over the
+ * element's frames and tiles in a fixed order.  g_depth and g_poses are bit-identical to gsx_backproject_normals_bwd's.
+ * scratch: gsx_backproject_normals_bwd_intrinsics_scratch_bytes(B,L,H,W) bytes when g_intrinsics != NULL, else as
+ * gsx_backproject_normals_bwd. */
+int64_t gsx_backproject_normals_bwd_intrinsics_scratch_bytes(int B, int L, int H, int W);
+int gsx_backproject_normals_bwd_intrinsics(const float *depth, int64_t depth_bstride, const float *intrinsics,
+                                           int64_t K_bstride, const float *poses, int64_t pose_bstride, int B, int L,
+                                           int H, int W, const float *g_vertex, const float *g_normal,
+                                           const float *g_gvertex, const float *g_gnormal, float *g_depth,
+                                           float *g_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
+                                           void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fused PointFusion map update, one live frame for all B elements: three kernels
@@ -581,8 +598,9 @@ int gsx_icp_projective_targets_rgb(const float *map_geometry, const float *map_c
  * The backward takes g_sums (B, 28) and writes per SOURCE row: g_src, g_src_colours, g_tgt_points_rows,
  * g_tgt_normals_rows (B, ns_stride, 3) and g_stencil_colours_rows (B, ns_stride, 5, 3), the gradients of the model
  * colours at pixels j, j-1, j+1, j-W, j+W (zeros where the row has none; the caller scatters them), and g_prev_poses
- * (B, 4, 4), reduced in a fixed order without atomics (bottom row zero).  No gradient w.r.t. the intrinsics.  A negative
- * or non-finite weight is refused before any launch. */
+ * (B, 4, 4), reduced in a fixed order without atomics (bottom row zero).  No gradient w.r.t. the intrinsics: that is
+ * gsx_icp_joint_normal_eq_batched_bwd_intrinsics, to which gsx_icp_joint_normal_eq_batched_bwd forwards with
+ * g_intrinsics = NULL.  A negative or non-finite weight is refused before any launch. */
 int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
                                         const float *src_colours, const float *tgt_points, const float *tgt_normals,
                                         const float *model_colours, const int64_t *index, int B, int H, int W,
@@ -597,6 +615,23 @@ int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, const int32_t *
                                         float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
                                         float *g_stencil_colours_rows, float *g_prev_poses, void *scratch,
                                         int64_t scratch_bytes, void *stream);
+/* gsx_icp_joint_normal_eq_batched_bwd that also writes, if g_intrinsics != NULL, d(loss)/d(intrinsics) (B, 4, 4): the
+ * photometric row reads all 12 entries of K's first three rows (its projection and du/dq, dv/dq), skew and the 4th column
+ * included, so each of them gets a gradient here (dual numbers over 29 inputs); the bottom row is 0.  Reduced per block
+ * and then over the blocks in a fixed order, like g_prev_poses.  scratch:
+ * gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(B, ns_stride) bytes when g_intrinsics != NULL, else as
+ * gsx_icp_joint_normal_eq_batched_bwd. */
+int64_t gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(int B, int ns_stride);
+int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(const float *src_points, const int32_t *src_count, int ns_stride,
+                                                   const float *src_colours, const float *tgt_points,
+                                                   const float *tgt_normals, const float *model_colours,
+                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                                                   const float *prev_poses, const float *intrinsics,
+                                                   float photometric_weight, const float *g_sums, float *g_src,
+                                                   float *g_src_colours, float *g_tgt_points_rows,
+                                                   float *g_tgt_normals_rows, float *g_stencil_colours_rows,
+                                                   float *g_prev_poses, float *g_intrinsics, void *scratch,
+                                                   int64_t scratch_bytes, void *stream);
 
 /* The association of gsx_icp_localize_projective alone (the index-only op of the differentiable mode): for the source
  * rows i < src_count[b] of src_points (B, ns_stride, 3), world frame, idx_out int64 (B, ns_stride) = the pixel
@@ -653,12 +688,27 @@ int gsx_render_views_bwd(const float *map_geometry, const int32_t *counts, int64
 /* Backward of gsx_render_splats at a fixed index (max_splat_px = 0 is gsx_render_views_bwd itself).  A disk row's
  * depth is t: dt/dq = m/(m.d), dt/dm = (q - t d)/(m.d) carry the gradient to its position, its normal and the pose; a
  * row sums, in (view, h, w) order, the gradients of the pixels of its footprint that it won.  No gradient w.r.t. the
- * radius (slot 7 of d_geometry is zero), the footprint or the intrinsics.  Deterministic, no atomics. */
+ * radius (slot 7 of d_geometry is zero), the footprint or the intrinsics (gsx_render_splats_bwd_intrinsics adds
+ * the latter).  Deterministic, no atomics.  Same as gsx_render_splats_bwd_intrinsics with g_intrinsics = NULL. */
 int gsx_render_splats_bwd(const float *map_geometry, const int32_t *counts, int64_t capacity, const float *intrinsics,
                           int64_t K_bstride, const float *poses, int64_t pose_bstride, const int64_t *index, int B,
                           int L, int H, int W, const float *g_depth, const float *g_rgb, const float *g_normals,
                           const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses, void *scratch,
                           int64_t scratch_bytes, int max_splat_px, void *stream);
+/* gsx_render_splats_bwd that also writes, if g_intrinsics != NULL, d(loss)/d(intrinsics) (B,4,4) dense: a disk pixel's
+ * depth t = (m.q)/(m.d) depends on its ray d = K^-1 (w, h, 1), dt/dd = -t m/(m.d), taken through load_kinv's K^-1
+ * (fx, cx, fy, cy; every other entry 0) and summed per element over its views and tiles in a fixed order.  One-pixel
+ * rows, colours, normals and confidences do not depend on K: with max_splat_px = 0 g_intrinsics is all zero.
+ * scratch: gsx_render_splats_bwd_intrinsics_scratch_bytes(B,L,H,W) bytes when g_intrinsics != NULL and
+ * max_splat_px >= 1, else as gsx_render_splats_bwd. */
+int64_t gsx_render_splats_bwd_intrinsics_scratch_bytes(int B, int L, int H, int W);
+int gsx_render_splats_bwd_intrinsics(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                     const float *intrinsics, int64_t K_bstride, const float *poses,
+                                     int64_t pose_bstride, const int64_t *index, int B, int L, int H, int W,
+                                     const float *g_depth, const float *g_rgb, const float *g_normals,
+                                     const float *g_confidence, float *d_geometry, float *d_colors, float *d_poses,
+                                     float *g_intrinsics, void *scratch, int64_t scratch_bytes, int max_splat_px,
+                                     void *stream);
 
 #ifdef __cplusplus
 }
