@@ -86,6 +86,9 @@ SIGNATURES = {
     "gsx_ingest_raw": (c_int, [c_vp, c_vp, c_i64, c_double, c_int, c_vp, c_vp, c_vp]),
     "gsx_ingest_calibration": (c_int, [c_vp, c_i64, c_int, c_double, c_double, c_vp, c_vp, c_int, c_int, c_vp, c_vp,
                                        c_vp]),
+    "gsx_depth_bilateral": (c_int, [c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_int, c_double, c_double, c_vp]),
+    "gsx_depth_bilateral_bwd": (
+        c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_int, c_double, c_double, c_vp]),
     "gsx_compact_scratch_bytes": (c_i64, [c_i64]),
     "gsx_compact_indices": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_u32, c_vp]),
     "gsx_active_eval": (c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp,

@@ -13,7 +13,7 @@ import torch
 import torch.nn as nn
 
 from ..structures.pointclouds import Pointclouds
-from ..structures.rgbdimages import RGBDImages
+from ..structures.rgbdimages import BilateralFilter, RGBDImages
 from ..structures.utils import MAX_SPLAT_PX
 from .fusionutils import update_map_aggregate
 
@@ -62,7 +62,8 @@ class ICPSLAM(nn.Module):
                  dist_thresh: Union[float, int, None] = None, lambda_max: Union[float, int] = 2.0,
                  B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0, nu: Union[float, int] = 200.0,
                  association: str = "nn", device: Union[torch.device, str, None] = None, target_splat_px: int = 0,
-                 photometric_weight: Union[float, int] = 0.0):
+                 photometric_weight: Union[float, int] = 0.0, depth_filter: Optional[BilateralFilter] = None,
+                 depth_filter_tracking_only: bool = False):
         """association (extension): how the ICP odometry pairs live points with the map.  'nn' (default, the
         reference's) = exact 1-NN between the lattice-thinned live cloud and the lattice-active map points; 'projective'
         = each live point with the map row visible at the pixel it projects to in the map rendered from the previous
@@ -80,8 +81,22 @@ class ICPSLAM(nn.Module):
         (0.299 r + 0.587 g) + 0.114 b with the intensity of the map's colour rendered there, linearised with the central
         differences of that model image; w absorbs the colours' scale.  Texture then pins the motions geometry cannot see
         (sliding along a wall).  0 (default) = depth alone, exactly as without the keyword.  In the differentiable mode the
-        gradient also reaches the live rgb and the map's colours.  No effect with odom='gt'."""
+        gradient also reaches the live rgb and the map's colours.  No effect with odom='gt'.
+
+        depth_filter (extension, a BilateralFilter or None): smooth each live frame's depth with an edge-preserving
+        bilateral filter before its vertex and normal maps are computed (KinectFusion; Keller et al. 2013), so sensor
+        noise does not ruin the normals the tracking and the fusion's normal test rely on.  Holes stay holes.  By default
+        the tracking and the map update both see the filtered depth, which is the same as filtering the input beforehand.
+        In the differentiable mode the filter is on the tape: gradients reach the raw depth.  None (default): no filter.
+
+        depth_filter_tracking_only (extension, default False): KinectFusion's split - the odometry tracks the filtered
+        frame and the map fuses the raw depth.  With odom='gt' there is no tracking, so nothing is filtered."""
         super().__init__()
+        if depth_filter is not None and not isinstance(depth_filter, BilateralFilter):
+            raise TypeError("Expected depth_filter to be a BilateralFilter or None. Got {0}.".format(type(depth_filter)))
+        if not isinstance(depth_filter_tracking_only, bool):
+            raise TypeError("Expected depth_filter_tracking_only to be of type bool. Got {0}.".format(
+                type(depth_filter_tracking_only)))
         if not isinstance(association, str):
             raise TypeError("Expected association to be of type str. Got {0}.".format(type(association)))
         if association not in ("nn", "projective"):
@@ -112,6 +127,8 @@ class ICPSLAM(nn.Module):
         self.association = association
         self.target_splat_px = target_splat_px
         self.photometric_weight = float(photometric_weight)
+        self.depth_filter = depth_filter
+        self.depth_filter_tracking_only = depth_filter_tracking_only
         self.device = _normalize_device(device if device is not None else "cuda")
 
     # ------------------------------------------------------------------ sequence driver
@@ -159,8 +176,16 @@ class ICPSLAM(nn.Module):
         """One SLAM step on `live_frame` (sequence length 1).  Returns (Pointclouds, poses (B,1,4,4))."""
         if not isinstance(live_frame, RGBDImages):
             raise TypeError("Expected live_frame to be of type gradslam.RGBDImages. Got {0}.".format(type(live_frame)))
-        live_frame.poses = self._localize(pointclouds, live_frame, prev_frame)
-        pointclouds = self._map(pointclouds, live_frame, inplace)
+        filtered = None
+        if self.depth_filter is not None and not (self.depth_filter_tracking_only and (
+                self.odom == "gt" or prev_frame is None)):  # (the tracking-only filter is for the odometry alone)
+            filtered = live_frame.bilateral_filtered(self.depth_filter)
+        live_frame.poses = self._localize(pointclouds, live_frame if filtered is None else filtered, prev_frame)
+        mapped = live_frame
+        if filtered is not None and not self.depth_filter_tracking_only:
+            filtered.poses = live_frame.poses
+            mapped = filtered
+        pointclouds = self._map(pointclouds, mapped, inplace)
         return pointclouds, live_frame.poses
 
     def _localize(self, pointclouds: Pointclouds, live_frame: RGBDImages, prev_frame: RGBDImages):

@@ -11,7 +11,7 @@ import torch
 
 from .. import _C
 from ..structures.pointclouds import Pointclouds
-from ..structures.rgbdimages import RGBDImages
+from ..structures.rgbdimages import BilateralFilter, RGBDImages
 from ..structures.pointclouds import _PruneHistory
 from .fusionutils import (_check_free_space_margin, _check_history, _check_merge_overlapping, _prune_scratch,
                           fuse_and_prune, prune_unstable, update_map_fusion)
@@ -47,7 +47,8 @@ class PointFusion(ICPSLAM):
                  device: Union[torch.device, str, None] = None, stable_confidence: Union[float, int, None] = None,
                  max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None,
                  surfel_radii: bool = False, merge_overlapping: bool = False, target_splat_px: int = 0,
-                 photometric_weight: Union[float, int] = 0.0):
+                 photometric_weight: Union[float, int] = 0.0, depth_filter: Optional[BilateralFilter] = None,
+                 depth_filter_tracking_only: bool = False):
         """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
         surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
         (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
@@ -77,7 +78,13 @@ class PointFusion(ICPSLAM):
         the map rendered with its surfels as oriented disks, see ICPSLAM.
 
         photometric_weight (extension, default 0; > 0 needs association='projective'): joint geometric and photometric
-        tracking against the map's colours, see ICPSLAM."""
+        tracking against the map's colours, see ICPSLAM.
+
+        depth_filter, depth_filter_tracking_only (extension; default None, False): bilateral filtering of the live depth
+        for the tracking and the fusion, or for the tracking alone, see ICPSLAM.  The whole-sequence call (odom='gt')
+        filters the frames on the device as they arrive - all at once when they are already there, else each uploaded
+        (and, for RawRGBD, converted) chunk - and fuses the filtered depth; with depth_filter_tracking_only it filters
+        nothing, since there is no tracking."""
         if not isinstance(surfel_radii, bool):
             raise TypeError("surfel_radii must be of type bool; but was of type {}.".format(type(surfel_radii)))
         _check_merge_overlapping(merge_overlapping, surfel_radii)
@@ -101,7 +108,8 @@ class PointFusion(ICPSLAM):
                              "the age rule a no-op)")
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
                          lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device,
-                         target_splat_px=target_splat_px, photometric_weight=photometric_weight)
+                         target_splat_px=target_splat_px, photometric_weight=photometric_weight,
+                         depth_filter=depth_filter, depth_filter_tracking_only=depth_filter_tracking_only)
         if target_splat_px > 0 and not surfel_radii:
             raise ValueError("target_splat_px > 0 needs surfel_radii=True (a map without radii has no disks)")
         if not isinstance(dist_th, (float, int)):
@@ -216,6 +224,9 @@ class PointFusion(ICPSLAM):
                 ms = torch.empty(_C.lib().gsx_fusion_merge_scratch_bytes(B, H, W, pc.capacity), dtype=torch.uint8,
                                  device=dev)
                 merge = (ms, ms.numel())
+        # the depth the driver fuses: the frames' own, or its bilateral filter in a second buffer
+        filt = self.depth_filter if not self.depth_filter_tracking_only else None
+        fused_depth = depth if filt is None else torch.empty_like(depth)
         main = torch.cuda.current_stream(dev)
         ready = []
         if not on_device:
@@ -238,8 +249,13 @@ class PointFusion(ICPSLAM):
                 for b in range(B):
                     _C.launch("gsx_ingest_raw", raw_rgb[b, s0:s1], raw_depth[b, s0:s1], (s1 - s0) * P,
                               frames.scaling_factor, 1 if frames.normalize_color else 0, rgb[b, s0:s1], depth[b, s0:s1])
+            if filt is not None:  # the whole (B, L) at once, or this chunk of every element
+                for src, dst, n in ([(depth, fused_depth, B * L)] if on_device else
+                                    [(depth[b, s0:s1], fused_depth[b, s0:s1], s1 - s0) for b in range(B)]):
+                    _C.launch("gsx_depth_bilateral", src, dst, None, n, H, W, filt.radius, filt.sigma_space,
+                              filt.sigma_range)
             _C.launch("gsx_pointfusion_sequence_gt_merge", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                      min(s0 * P, pc.capacity), depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                      min(s0 * P, pc.capacity), fused_depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
                       float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag(),
                       1 if self.surfel_radii else 0, *merge)
         if not on_device:

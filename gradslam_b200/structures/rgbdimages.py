@@ -6,13 +6,16 @@ kernel (gsx_backproject_normals_fwd) instead of the reference's einsum / slice /
 (rgbdimages.py:643-762).  Containers may hold tensors on any device, but computing a map requires CUDA
 tensors: there is no CPU compute path.
 """
+import math
+from dataclasses import dataclass
 from typing import Optional, Union
 
+import numpy as np
 import torch
 
 from .. import _C
 
-__all__ = ["RGBDImages"]
+__all__ = ["RGBDImages", "BilateralFilter", "bilateral_filter_depth"]
 
 
 def _frame_base(t: torch.Tensor, inner: int):
@@ -79,6 +82,89 @@ class _BackprojectFn(torch.autograd.Function):
 def backproject(depth, intrinsics, poses, want=(True, True, True, True)):
     """Runs K1.  depth (B,L,H,W,1) channels-last.  Returns a 4-tuple (entries not wanted are None)."""
     return _BackprojectFn.apply(depth, intrinsics, poses, tuple(bool(w) for w in want))
+
+
+_MAX_FILTER_RADIUS = 7
+
+
+@dataclass(frozen=True)
+class BilateralFilter:
+    """Edge-preserving bilateral filter of input depth (KinectFusion, Newcombe et al. 2011), as gsx_depth_bilateral
+    computes it: each valid pixel (0 < d < inf) becomes the mean of the valid depths in its (2 radius + 1)^2 window,
+    weighted by exp(-(du^2 + dv^2) / (2 sigma_space^2) - (d_q - d_p)^2 / (2 sigma_range^2)); invalid pixels (holes,
+    NaN, inf) stay as they are.  radius: pixels, 1 .. 7; sigma_space: pixels; sigma_range: metres (depth units).
+    A depth step much larger than sigma_range keeps both sides apart."""
+
+    radius: int
+    sigma_space: float
+    sigma_range: float
+
+    def __post_init__(self):
+        if isinstance(self.radius, bool) or not isinstance(self.radius, int):
+            raise TypeError("BilateralFilter.radius must be an int; got {}".format(type(self.radius)))
+        if not 1 <= self.radius <= _MAX_FILTER_RADIUS:
+            raise ValueError("BilateralFilter.radius must be in 1..{}; got {}".format(_MAX_FILTER_RADIUS, self.radius))
+        for name in ("sigma_space", "sigma_range"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (float, int)):
+                raise TypeError("BilateralFilter.{} must be a float; got {}".format(name, type(v)))
+            ok = math.isfinite(float(v)) and v > 0
+            if ok:  # the kernel takes c = 1/(2 sigma^2) rounded once to float32: finite and non-zero there too
+                two_var = 2.0 * float(v) * float(v)
+                with np.errstate(over="ignore", under="ignore"):
+                    c = np.float32(1.0 / two_var) if two_var > 0 else np.float32(np.inf)
+                ok = bool(np.isfinite(c) and c > 0)
+            if not ok:
+                raise ValueError("BilateralFilter.{} must be finite and > 0 with 1/(2 sigma^2) a finite positive "
+                                 "float32; got {}".format(name, v))
+            object.__setattr__(self, name, float(v))
+
+
+def _depth_layout(depth):
+    """(B,L,H,W,1) channels-last or (B,L,1,H,W) channels-first -> (n images, H, W); the two hold the same bytes."""
+    if depth.dim() != 5 or not (depth.shape[-1] == 1 or depth.shape[2] == 1):
+        raise ValueError("depth must be (B,L,H,W,1) or (B,L,1,H,W); got shape {}".format(tuple(depth.shape)))
+    B, L = depth.shape[:2]
+    H, W = (depth.shape[2], depth.shape[3]) if depth.shape[-1] == 1 else (depth.shape[3], depth.shape[4])
+    return B * L, H, W
+
+
+class _BilateralFn(torch.autograd.Function):
+    """depth -> filtered depth.  forward = gsx_depth_bilateral, backward = gsx_depth_bilateral_bwd (it needs the
+    forward's per-pixel weight sums, which are kept only when depth requires grad)."""
+
+    @staticmethod
+    def forward(ctx, depth, f):
+        _C.require_cuda(depth, "depth")
+        n, H, W = _depth_layout(depth)
+        d = depth.detach().contiguous()
+        out = torch.empty_like(d, memory_format=torch.contiguous_format)
+        den = torch.empty_like(d, memory_format=torch.contiguous_format) if ctx.needs_input_grad[0] else None
+        if n * H * W > 0:
+            _C.launch("gsx_depth_bilateral", d, out, den, n, H, W, f.radius, f.sigma_space, f.sigma_range)
+        if den is not None:
+            ctx.save_for_backward(d, out, den)
+        ctx.f, ctx.dims = f, (n, H, W)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_out):
+        d, out, den = ctx.saved_tensors
+        f, (n, H, W) = ctx.f, ctx.dims
+        g_depth = torch.empty_like(d)
+        if n * H * W > 0:
+                _C.launch("gsx_depth_bilateral_bwd", d, out, den, g_out.contiguous(), g_depth, n, H, W, f.radius,
+                      f.sigma_space, f.sigma_range)
+        return g_depth, None
+
+
+def bilateral_filter_depth(depth: torch.Tensor, f: BilateralFilter) -> torch.Tensor:
+    """Bilateral filter (`f`) of a CUDA float32 depth tensor, (B,L,H,W,1) channels-last or (B,L,1,H,W) channels-first;
+    returns a new tensor of the same shape.  Differentiable w.r.t. depth (exact, deterministic backward)."""
+    if not isinstance(f, BilateralFilter):
+        raise TypeError("Expected f to be of type BilateralFilter. Got {}.".format(type(f)))
+    return _BilateralFn.apply(depth, f)
 
 
 class RGBDImages(object):
@@ -262,6 +348,17 @@ class RGBDImages(object):
         if self._global_normal_map is None:
             self._compute_maps(False, True)
         return self._global_normal_map
+
+    # ------------------------------------------------------------------ depth filtering
+    def bilateral_filtered(self, f: BilateralFilter):
+        """A new RGBDImages whose depth is bilateral_filter_depth(depth_image, f), with the same rgb, intrinsics,
+        poses and pixel positions (not copies).  Differentiable w.r.t. the depth."""
+        if self.channels_first:  # (filtered as channels-last: a (B,L,1,H,1) shape alone does not say which it is)
+            depth = bilateral_filter_depth(self._depth_image.permute(0, 1, 3, 4, 2), f).permute(0, 1, 4, 2, 3)
+        else:
+            depth = bilateral_filter_depth(self._depth_image, f)
+        return RGBDImages(self._rgb_image, depth, self._intrinsics, self._poses, channels_first=self.channels_first,
+                          pixel_pos=self._pixel_pos)
 
     # ------------------------------------------------------------------ setters (cache invalidation as rgbdimages.py:399-463)
     @staticmethod

@@ -150,6 +150,19 @@ def make_dynamic_sequence(B, L, H, W, k0, k1, seed=0, hole_fraction=0.02, motion
     return rgb, depth, Kt, poses
 
 
+def add_depth_noise(depth, seed, a=0.0012, b=0.0019, z0=0.4):
+    """depth (any shape, float32, CPU) plus the axial noise of a Kinect v1 (Nguyen, Izadi and Lovell 2012): independent
+    zero-mean Gaussian noise of sigma(z) = a + b (z - z0)^2 metres per pixel, from a torch.Generator seeded with `seed`.
+    Holes (depth 0) stay 0, and a noisy depth is clamped to at least a tenth of the clean one, so no valid pixel becomes
+    a hole.  Real sensors' noise is spatially correlated and quantised: independent noise is the harsher case."""
+    gen = torch.Generator().manual_seed(int(seed))
+    noise = torch.randn(depth.shape, generator=gen, dtype=torch.float32)
+    d64 = depth.double()
+    sigma = a + b * (d64 - z0) ** 2
+    noisy = torch.maximum(d64 + sigma * noise.double(), 0.1 * d64)
+    return torch.where(depth > 0, noisy, d64).to(torch.float32)
+
+
 def punch_lattice_holes(depth, row_step=5, col_step=7):
     """Zeroes depth (..., H, W, 1) on a sparse lattice (rows 2, 2+row_step, ...; columns 3, 3+col_step, ...).  No two
     holes touch, not even diagonally, so no valid pixel has BOTH its right and its lower neighbour missing: at such

@@ -363,6 +363,29 @@ int gsx_ingest_calibration(const float *intrinsics, int64_t n_intrinsics, int in
                            int32_t *singular_flag, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Bilateral filter of input depth (KinectFusion, Newcombe et al. 2011: edge-preserving smoothing before the vertex and
+ * normal maps; gradslam has no such filter).  depth, out, den: n_images dense H x W float32 images (the depth of a
+ * (B,L,H,W,1) or (B,L,1,H,W) RGBDImages is n_images = B*L of them).  A pixel is valid iff 0 < d < +inf.  For a valid
+ * centre p, over the window offsets (du,dv) taken dv outer and du inner, each from -radius to radius, each in-image
+ * valid neighbour q gives x = -(float(du^2+dv^2) c_s + (d_q - d_p)^2 c_r) in float32; the pair is skipped if x < -17,
+ * else w = exp32(x) (a float32 exponential without FMA, gradslam_b200/csrc/gsx_exp32.cuh, within 1 ulp) adds w d_q to
+ * num and w to den in window order, and out_p = num / den.  An invalid centre passes through (out_p = d_p, den_p = 0).
+ * c_s = float32(1/(2 sigma_space^2)), c_r = float32(1/(2 sigma_range^2)), computed in float64 and rounded once.
+ * den may be NULL; the backward needs it.  Refused before any launch: null depth / out, n_images < 0, H or W < 1,
+ * radius outside 1..7, a sigma that is not finite and > 0 or whose c is not a finite positive float32, and out or den
+ * overlapping depth or each other. */
+int gsx_depth_bilateral(const float *depth, float *out, float *den, int64_t n_images, int H, int W, int radius,
+                        double sigma_space, double sigma_range, void *stream);
+
+/* Backward of gsx_depth_bilateral, from its depth, out and den and the upstream gradient g_out: g_depth (same shape) =
+ * the exact derivative with the skipped pairs held at zero; an invalid pixel passes its g_out through.  A gather
+ * (each pixel sums over its own window), no atomics: deterministic.  No gradient w.r.t. the sigmas or the radius.
+ * Refused as gsx_depth_bilateral, and when g_depth overlaps an input. */
+int gsx_depth_bilateral_bwd(const float *depth, const float *out, const float *den, const float *g_out, float *g_depth,
+                            int64_t n_images, int H, int W, int radius, double sigma_space, double sigma_range,
+                            void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Table-returning association steps (API parity with gradslam's module-level helpers; the fused path
  * above never materialises these tables).  Tables are int64 (rows,4) with rows [b, n, h, w].
  * replaces find_active_map_points gradslam/slam/fusionutils.py:198-287 (gsx_active_eval + compaction),
