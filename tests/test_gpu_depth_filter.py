@@ -49,8 +49,11 @@ def test_forward_matches_oracle_bit_for_bit_at_every_radius(radius):
     _assert_forward_exact(noisy, f)
 
 
-@pytest.mark.parametrize("B,L,H,W,radius", [(1, 1, 1, 1, 3), (2, 3, 5, 7, 7), (1, 2, 3, 40, 4), (3, 1, 33, 2, 2),
-                                            (1, 1, 9, 33, 1)])
+# images smaller than the 32 x 8 tile, one-pixel and two-pixel wide, a tile and one row or column
+SMALL_AND_ODD = [(1, 1, 1, 1, 3), (2, 3, 5, 7, 7), (1, 2, 3, 40, 4), (3, 1, 33, 2, 2), (1, 1, 9, 33, 1)]
+
+
+@pytest.mark.parametrize("B,L,H,W,radius", SMALL_AND_ODD)
 def test_forward_on_small_and_odd_images(B, L, H, W, radius):
     g = torch.Generator().manual_seed(H * 100 + W)
     depth = 2.0 + 0.05 * torch.randn((B, L, H, W, 1), generator=g)  # a different image per element
@@ -85,27 +88,75 @@ def test_channels_first_layout_and_rgbdimages():
 
 
 # ------------------------------------------------------------------------------------------------------------ backward
-@pytest.mark.parametrize("radius,H,W", [(1, 9, 11), (3, 37, 45), (6, 20, 70)])
+def _gpu_backward(depth, f, g_out):
+    """d(sum(g_out * filtered))/d(depth) on the GPU, twice: the two calls agree bit for bit.  depth, g_out (B,L,H,W,1)
+    CPU float32; returns the gradient as an (n, H, W) CPU tensor."""
+    B, L, H, W, _ = depth.shape
+    grads = []
+    for _ in range(2):
+        d = depth.to(DEV).requires_grad_(True)
+        gs.bilateral_filter_depth(d, f).backward(g_out.to(DEV))
+        grads.append(d.grad.cpu())
+    assert torch.equal(grads[0].view(torch.int32), grads[1].view(torch.int32))
+    return grads[0].view(B * L, H, W)
+
+
+def _assert_backward_close_to_autograd(depth, f, g_out):
+    B, L, H, W, _ = depth.shape
+    got = _gpu_backward(depth, f, g_out)
+    d2 = depth.numpy().reshape(B * L, H, W)
+    x = torch.from_numpy(d2.astype(np.float64)).requires_grad_(True)
+    keep = bo.keep_masks(d2, f.radius, f.sigma_space, f.sigma_range)
+    want, = torch.autograd.grad(bo.bilateral_f64(x, f.radius, f.sigma_space, f.sigma_range, keep)[0], x,
+                                g_out.double().view(B * L, H, W))
+    _, mag = bo.bilateral_bwd_formula(d2, g_out.numpy().reshape(B * L, H, W), f.radius, f.sigma_space, f.sigma_range)
+    err = np.abs(got.double().numpy() - want.numpy())
+    assert np.all(err <= 1e-4 * mag + 1e-30), float((err / mag).max())
+
+
+def _assert_backward_close_to_formula(depth, f, g_out):
+    """Against bilateral_bwd_formula (float64 numpy) where autograd of bilateral_f64 would not fit in memory."""
+    B, L, H, W, _ = depth.shape
+    got = _gpu_backward(depth, f, g_out)
+    want, mag = bo.bilateral_bwd_formula(depth.numpy().reshape(B * L, H, W), g_out.numpy().reshape(B * L, H, W),
+                                         f.radius, f.sigma_space, f.sigma_range)
+    err = np.abs(got.double().numpy() - want)
+    assert np.all(err <= 1e-4 * mag + 1e-30), float((err / mag).max())
+
+
+@pytest.mark.parametrize("radius,H,W", [(1, 9, 11), (2, 23, 35), (3, 37, 45), (4, 17, 66), (5, 30, 33), (6, 20, 70),
+                                        (7, 41, 39)])
 def test_backward_matches_float64_autograd_and_is_deterministic(radius, H, W):
+    """Every instantiation of k_depth_bilateral_bwd<R>, on images that are not a whole number of tiles."""
     _, depth, _, _ = make_sequence(2, 1, H, W, seed=radius, yaw0=0.6)
     depth = _with_bad_pixels(add_depth_noise(depth, seed=radius), radius + 1)
     f = gs.BilateralFilter(radius, 0.8 * radius, 0.05)
     g_out = torch.randn(depth.shape, generator=torch.Generator().manual_seed(2))
-    grads = []
-    for _ in range(2):
-        d = depth.to(DEV).requires_grad_(True)
-        out = gs.bilateral_filter_depth(d, f)
-        out.backward(g_out.to(DEV))
-        grads.append(d.grad.cpu())
-    assert torch.equal(grads[0].view(torch.int32), grads[1].view(torch.int32))
-    d2 = depth.numpy().reshape(2, H, W)
-    x = torch.from_numpy(d2.astype(np.float64)).requires_grad_(True)
-    keep = bo.keep_masks(d2, radius, f.sigma_space, f.sigma_range)
-    want, = torch.autograd.grad(bo.bilateral_f64(x, radius, f.sigma_space, f.sigma_range, keep)[0], x,
-                                g_out.double().view(2, H, W))
-    _, mag = bo.bilateral_bwd_formula(d2, g_out.numpy().reshape(2, H, W), radius, f.sigma_space, f.sigma_range)
-    err = np.abs(grads[0].double().numpy().reshape(2, H, W) - want.numpy())
-    assert np.all(err <= 1e-4 * mag + 1e-30), float((err / mag).max())
+    _assert_backward_close_to_autograd(depth, f, g_out)
+
+
+@pytest.mark.parametrize("B,L,H,W,radius", SMALL_AND_ODD)
+def test_backward_on_small_and_odd_images(B, L, H, W, radius):
+    g = torch.Generator().manual_seed(H * 100 + W + 1)
+    depth = 2.0 + 0.05 * torch.randn((B, L, H, W, 1), generator=g)
+    g_out = torch.randn(depth.shape, generator=g)
+    _assert_backward_close_to_autograd(_with_bad_pixels(depth, W), gs.BilateralFilter(radius, 1.5, 0.05), g_out)
+
+
+def test_backward_past_one_grid_dimension_of_images():
+    """70 000 images > 65 535: the images past gridDim.z come from the kernel's image-stride loop."""
+    n = 70_000
+    g = torch.Generator().manual_seed(10)
+    depth = (1.0 + 0.05 * torch.rand((n, 1, 2, 3, 1), generator=g)) * (torch.rand((n, 1, 2, 3, 1), generator=g) > 0.1)
+    g_out = torch.randn(depth.shape, generator=g)
+    _assert_backward_close_to_formula(depth, gs.BilateralFilter(1, 1.0, 0.1), g_out)
+
+
+def test_backward_at_full_size():
+    _, depth, _, _ = make_sequence(8, 2, 480, 640, seed=4, yaw0=0.6)
+    depth = _with_bad_pixels(add_depth_noise(depth, seed=4), 5)
+    g_out = torch.randn(depth.shape, generator=torch.Generator().manual_seed(3))
+    _assert_backward_close_to_formula(depth, gs.BilateralFilter(3, 2.0, 0.05), g_out)
 
 
 def test_no_grad_call_keeps_no_weight_sums():
