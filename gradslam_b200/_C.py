@@ -154,6 +154,27 @@ SIGNATURES = {
     "gsx_icp_joint_normal_eq_batched_bwd_intrinsics": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
                 c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "gsx_icp_align_robust": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_int, c_int, c_float, c_int, c_float,
+                c_float, c_float, c_float, c_float, c_vp, c_vp, c_vp, c_i64, c_float, c_vp]),
+    "gsx_icp_localize_robust": (
+        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int,
+                c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64,
+                c_vp, c_i64, c_u32, c_vp, c_float, c_vp]),
+    "gsx_icp_localize_projective_robust": (
+        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
+                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_int,
+                c_vp, c_vp, c_i64, c_float, c_float, c_float, c_vp]),
+    "gsx_icp_normal_eq_batched_robust_fwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_i64, c_float, c_vp]),
+    "gsx_icp_normal_eq_batched_robust_bwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_float, c_vp]),
+    "gsx_icp_joint_normal_eq_batched_robust_fwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
+                c_vp, c_i64, c_float, c_float, c_vp]),
+    "gsx_icp_joint_normal_eq_batched_robust_bwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
+                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_float, c_float, c_vp]),
     "gsx_icp_project_associate": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_float, c_vp, c_vp,
                 c_vp]),

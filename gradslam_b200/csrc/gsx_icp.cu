@@ -34,6 +34,9 @@
 //   k_icp_joint_linearize_idx / _bwd  the geometric + photometric sums at a given association and their backward
 //                        (gsx_icp_joint_normal_eq_batched_fwd / _bwd, the op of the differentiable mode; the same
 //                        photometric_row, the backward through dual numbers)
+// Huber weights (the *_robust entry points): kRobust = true instantiations of k_icp_knn_linearize, k_icp_proj_linearize
+// and the normal-equation ops weigh a row outside the scale delta in row_products<true> / add_weighted_products<true>,
+// shared by the fused and the taped kernels; huber_adjoint is their backward.
 #include "gsx_common.cuh"
 #include "../../include/gsx.h"
 
@@ -449,9 +452,19 @@ struct KnnArgs {
   TargetGrid grid;  // used by the kGrid variant
 };
 
-// point-to-plane row of one association and its 28 products (gauss_newton_solve, icputils.py:227-230)
+// Scales of the Huber-weighted kernels (kRobust = true): delta of the point-to-plane residual (metres), delta_p of the
+// photometric one (intensity).  +inf weighs every finite row 1, which is exactly the unweighted sums.
+struct Huber {
+  float delta, delta_p;
+};
+
+// point-to-plane row of one association and its 28 products (gauss_newton_solve, icputils.py:227-230).
+// kRobust: a row with |r| > delta (equality is inside) adds h (A_p A_q), h (A_p r) and rho = delta ((a + a) - delta)
+// instead, with a = |r| and h = delta / a, the IRLS weights of the Huber energy sum rho.
+template <bool kRobust = false>
 __device__ __forceinline__ void row_products(float sx, float sy, float sz, const float *__restrict__ tp,
-                                             const float *__restrict__ tn, int64_t bi, float *acc) {
+                                             const float *__restrict__ tn, int64_t bi, float *acc,
+                                             float delta = 0.0f) {
   const float dx = __ldg(tp + bi * 3), dy = __ldg(tp + bi * 3 + 1), dz = __ldg(tp + bi * 3 + 2);
   const float nx = __ldg(tn + bi * 3), ny = __ldg(tn + bi * 3 + 1), nz = __ldg(tn + bi * 3 + 2);
   float A[6];
@@ -460,6 +473,21 @@ __device__ __forceinline__ void row_products(float sx, float sy, float sz, const
   A[4] = nx * sz - nz * sx;
   A[5] = ny * sx - nx * sy;
   const float r = (nx * (dx - sx) + ny * (dy - sy)) + nz * (dz - sz);
+  if constexpr (kRobust) {
+    const float a = fabsf(r);
+    if (a > delta) {
+      const float h = delta / a;
+      int k = 0;
+#pragma unroll
+      for (int p = 0; p < 6; ++p)
+#pragma unroll
+        for (int q = p; q < 6; ++q) acc[k++] = h * (A[p] * A[q]);
+#pragma unroll
+      for (int p = 0; p < 6; ++p) acc[21 + p] = h * (A[p] * r);
+      acc[27] = delta * ((a + a) - delta);
+      return;
+    }
+  }
   int k = 0;
 #pragma unroll
   for (int p = 0; p < 6; ++p)
@@ -493,8 +521,8 @@ __device__ __forceinline__ void block_reduce_sums(float *acc, float (*s_red)[kNu
   }
 }
 
-template <bool kGrid>
-__global__ void __launch_bounds__(kIcpBlock) k_icp_knn_linearize(KnnArgs a) {
+template <bool kGrid, bool kRobust = false>
+__global__ void __launch_bounds__(kIcpBlock) k_icp_knn_linearize(KnnArgs a, float delta) {
   __shared__ float4 s_t[kGrid ? 1 : kTgtTile];
   __shared__ float s_red[kIcpBlock / 32][kNumSums];
   __shared__ Rigid s_pre;
@@ -559,7 +587,7 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_knn_linearize(KnnArgs a) {
   float acc[kNumSums];
 #pragma unroll
   for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0f;
-  if (use) row_products(sx, sy, sz, tp, tn, (int64_t)bi, acc);
+  if (use) row_products<kRobust>(sx, sy, sz, tp, tn, (int64_t)bi, acc, delta);
   block_reduce_sums(acc, s_red, a.partials + ((int64_t)b * gridDim.x + blockIdx.x) * kNumSums);
 }
 
@@ -676,8 +704,26 @@ __device__ __forceinline__ void photometric_row(const LiveCamera &c, float sx, f
   photometric_row_t<float>(c.tinv.r, c.tinv.t, c.k, sx, sy, sz, gu, gv, A);
 }
 
-// acc[k] += w (A_p A_q), w (A_p r), w (r r) in the order of row_products
-__device__ __forceinline__ void add_weighted_products(const float *A, float r, float w, float *acc) {
+// acc[k] += w (A_p A_q), w (A_p r), w (r r) in the order of row_products.  kRobust: a row with |r| > delta adds
+// (w h) (A_p A_q), (w h) (A_p r) and w rho instead (row_products' Huber weight h = delta / |r| and energy rho).
+template <bool kRobust = false>
+__device__ __forceinline__ void add_weighted_products(const float *A, float r, float w, float *acc,
+                                                      float delta = 0.0f) {
+  if constexpr (kRobust) {
+    const float a = fabsf(r);
+    if (a > delta) {
+      const float wh = w * (delta / a);
+      int k = 0;
+#pragma unroll
+      for (int p = 0; p < 6; ++p)
+#pragma unroll
+        for (int q = p; q < 6; ++q, ++k) acc[k] = acc[k] + wh * (A[p] * A[q]);
+#pragma unroll
+      for (int p = 0; p < 6; ++p) acc[21 + p] = acc[21 + p] + wh * (A[p] * r);
+      acc[27] = acc[27] + w * (delta * ((a + a) - delta));
+      return;
+    }
+  }
   int k = 0;
 #pragma unroll
   for (int p = 0; p < 6; ++p)
@@ -688,8 +734,8 @@ __device__ __forceinline__ void add_weighted_products(const float *A, float r, f
   acc[27] = acc[27] + w * (r * r);
 }
 
-template <bool kRgb>
-__global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a, ProjRgb pm) {
+template <bool kRgb, bool kRobust = false>
+__global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a, ProjRgb pm, Huber hb) {
   __shared__ float s_red[kIcpBlock / 32][kNumSums];
   __shared__ Rigid s_pre;
   __shared__ LiveCamera s_cam;
@@ -714,14 +760,15 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_proj_linearize(ProjLinArgs a,
     float d2;
     const int j = project_associate(s_cam, a.t, a.t.idx + b * P, tp, q.x, q.y, q.z, d2);
     if (j >= 0) {
-      row_products(q.x, q.y, q.z, tp, a.t.tgt_n + b * P * 3, (int64_t)j, acc);
+      row_products<kRobust>(q.x, q.y, q.z, tp, a.t.tgt_n + b * P * 3, (int64_t)j, acc, hb.delta);
       if constexpr (kRgb) {
         float gu, gv;
         const float *Im = pm.I_m + b * P;
         if (model_gradient(a.t.idx + b * P, Im, a.t.ib, j, gu, gv)) {
           float A[6];
           photometric_row(s_cam, q.x, q.y, q.z, gu, gv, A);
-          add_weighted_products(A, __ldg(pm.I_s + (int64_t)b * a.ns_stride + i) - __ldg(Im + j), pm.w, acc);
+          add_weighted_products<kRobust>(A, __ldg(pm.I_s + (int64_t)b * a.ns_stride + i) - __ldg(Im + j), pm.w, acc,
+                                         hb.delta_p);
         }
       }
     }
@@ -766,9 +813,10 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_model_intensity(const int64_t
 // normal equations for a GIVEN association (the differentiable op of the taped ICP): forward + backward
 // ---------------------------------------------------------------------------------------------------------
 // (batched: element b = blockIdx.y lives at b * ns_stride / b * nt_stride rows; counts may be null = ns_stride rows each)
+template <bool kRobust = false>
 __global__ void __launch_bounds__(kIcpBlock) k_icp_linearize_idx(const float *src, int ns_stride, const int32_t *counts,
                                                                  const float *tp, const float *tn, int nt_stride,
-                                                                 const int64_t *idx, float *partials) {
+                                                                 const int64_t *idx, float *partials, float delta) {
   __shared__ float s_red[kIcpBlock / 32][kNumSums];
   const int b = blockIdx.y;
   const int ns = counts ? counts[b] : ns_stride;
@@ -783,7 +831,9 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_linearize_idx(const float *sr
   for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0f;
   if (i < ns) {
     const int64_t j = idx[i];
-    if (j >= 0) row_products(src[(int64_t)i * 3], src[(int64_t)i * 3 + 1], src[(int64_t)i * 3 + 2], tp, tn, j, acc);
+    if (j >= 0)
+      row_products<kRobust>(src[(int64_t)i * 3], src[(int64_t)i * 3 + 1], src[(int64_t)i * 3 + 2], tp, tn, j, acc,
+                            delta);
   }
   block_reduce_sums(acc, s_red, partials + (int64_t)blockIdx.x * kNumSums);
 }
@@ -798,13 +848,45 @@ __global__ void k_icp_reduce_partials(const float *partials, int nblocks, float 
   }
 }
 
+// The adjoint of one row whose products row_products<true> / add_weighted_products<true> weighed, outside the Huber
+// scale (|r| > delta; returns false inside, where the caller takes the unweighted adjoint): with h = delta / |r| the
+// sums hold wt h (A_p A_q), wt h (A_p r) and wt rho, so dL/dA_p = wt h (sum_q G[p,q] A_q (x2 on the diagonal) + g_p r)
+// and, since h r = delta sgn(r) is constant, dh/dr = -h / r and drho/dr = 2 h r,
+// dL/dr = wt (-(h / r) sum_{p<=q} G[p,q] A_p A_q + 2 g_rr h r).
+__device__ __forceinline__ bool huber_adjoint(const float *g, const float *A, float r, float wt, float delta, float *a,
+                                              float &gr) {
+  const float ab = fabsf(r);
+  if (!(ab > delta)) return false;
+  const float h = delta / ab;
+  float Q = 0.0f;
+  int k = 0;
+#pragma unroll
+  for (int p = 0; p < 6; ++p)
+#pragma unroll
+    for (int q = p; q < 6; ++q) Q += g[k++] * (A[p] * A[q]);
+  gr = wt * (-(h / r) * Q + 2.0f * g[27] * (h * r));
+  const float wh = wt * h;
+#pragma unroll
+  for (int p = 0; p < 6; ++p) {
+    float v = g[21 + p] * r;
+#pragma unroll
+    for (int q = 0; q < 6; ++q) {
+      const int lo = p < q ? p : q, hi = p < q ? q : p;
+      v += g[lo * 6 - lo * (lo - 1) / 2 + (hi - lo)] * A[q] * ((p == q) ? 2.0f : 1.0f);
+    }
+    a[p] = wh * v;
+  }
+  return true;
+}
+
 // d(loss)/d(source point), d/d(associated target point), d/d(associated target normal) from d(loss)/d(28 sums).
 // One thread per source point; the target gradients are written per SOURCE row (the caller scatters them with the
-// association), so there are no atomics.
+// association), so there are no atomics.  kRobust: the sums of k_icp_linearize_idx<true> (huber_adjoint).
+template <bool kRobust = false>
 __global__ void __launch_bounds__(kIcpBlock) k_icp_linearize_bwd(const float *src, int ns_stride, const int32_t *counts,
                                                                  const float *tp, const float *tn, int nt_stride,
                                                                  const int64_t *idx, const float *g, float *g_src,
-                                                                 float *g_tp, float *g_tn) {
+                                                                 float *g_tp, float *g_tn, float delta) {
   __shared__ float s_g[kNumSums];
   const int b = blockIdx.y;
   const int ns = counts ? counts[b] : ns_stride;
@@ -835,18 +917,21 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_linearize_bwd(const float *sr
     const float r = (nx * (px - sx) + ny * (py - sy)) + nz * (pz - sz);
     // dL/dA_p = sum_{q>=p} G[p,q] A_q + sum_{q<=p} G[q,p] A_q + h_p r ;  dL/dr = sum_p h_p A_p + 2 g_rr r
     float a[6];
-    float gr = 2.0f * s_g[27] * r;
+    float gr;
+    if (!kRobust || !huber_adjoint(s_g, A, r, 1.0f, delta, a, gr)) {
+      gr = 2.0f * s_g[27] * r;
 #pragma unroll
-    for (int p = 0; p < 6; ++p) {
-      float v = s_g[21 + p] * r;
-      gr += s_g[21 + p] * A[p];
+      for (int p = 0; p < 6; ++p) {
+        float v = s_g[21 + p] * r;
+        gr += s_g[21 + p] * A[p];
 #pragma unroll
-      for (int q = 0; q < 6; ++q) {
-        const int lo = p < q ? p : q, hi = p < q ? q : p;
-        const int k = lo * 6 - lo * (lo - 1) / 2 + (hi - lo);  // index of (lo,hi) in the upper-triangular order
-        v += s_g[k] * A[q] * ((p == q) ? 2.0f : 1.0f);
+        for (int q = 0; q < 6; ++q) {
+          const int lo = p < q ? p : q, hi = p < q ? q : p;
+          const int k = lo * 6 - lo * (lo - 1) / 2 + (hi - lo);  // index of (lo,hi) in the upper-triangular order
+          v += s_g[k] * A[q] * ((p == q) ? 2.0f : 1.0f);
+        }
+        a[p] = v;
       }
-      a[p] = v;
     }
     // A3 = nz sy - ny sz, A4 = nx sz - nz sx, A5 = ny sx - nx sy ;  r = n . (p - s)
     gs[0] = (-nz * a[4] + ny * a[5]) - gr * nx;
@@ -896,7 +981,8 @@ __device__ __forceinline__ bool model_gradient_rgb(const int64_t *index, const f
   return true;
 }
 
-__global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_idx(JointArgs a, float *partials) {
+template <bool kRobust = false>
+__global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_idx(JointArgs a, float *partials, Huber hb) {
   __shared__ float s_red[kIcpBlock / 32][kNumSums];
   __shared__ LiveCamera s_cam;
   const int b = blockIdx.y;
@@ -912,21 +998,28 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_idx(JointArgs
     const int64_t j = a.idx[row];
     if (j >= 0) {
       const float sx = a.src[row * 3], sy = a.src[row * 3 + 1], sz = a.src[row * 3 + 2];
-      row_products(sx, sy, sz, a.tp + b * P * 3, a.tn + b * P * 3, j, acc);
+      row_products<kRobust>(sx, sy, sz, a.tp + b * P * 3, a.tn + b * P * 3, j, acc, hb.delta);
       const float *mcol = a.mcol + b * P * 3;
       float gu, gv;
       if (model_gradient_rgb(a.index + b * P, mcol, a.ib, (int)j, gu, gv)) {
         float A[6];
         photometric_row(s_cam, sx, sy, sz, gu, gv, A);
-        add_weighted_products(A, intensity3(a.src_col + row * 3) - intensity3(mcol + j * 3), a.w, acc);
+        add_weighted_products<kRobust>(A, intensity3(a.src_col + row * 3) - intensity3(mcol + j * 3), a.w, acc,
+                                       hb.delta_p);
       }
     }
   }
   block_reduce_sums(acc, s_red, partials + ((int64_t)b * gridDim.x + blockIdx.x) * kNumSums);
 }
 
-// dL/dA_p and dL/dr of one row A, r whose products enter the 28 sums with weight wt, from g = dL/d(sums)
-__device__ __forceinline__ void row_adjoint(const float *g, const float *A, float r, float wt, float *a, float &gr) {
+// dL/dA_p and dL/dr of one row A, r whose products enter the 28 sums with weight wt, from g = dL/d(sums).
+// kRobust: the row was weighed at the Huber scale delta (huber_adjoint outside it).
+template <bool kRobust = false>
+__device__ __forceinline__ void row_adjoint(const float *g, const float *A, float r, float wt, float *a, float &gr,
+                                            float delta = 0.0f) {
+  if constexpr (kRobust) {
+    if (huber_adjoint(g, A, r, wt, delta, a, gr)) return;
+  }
   gr = 2.0f * g[27] * r;
 #pragma unroll
   for (int p = 0; p < 6; ++p) {
@@ -947,11 +1040,13 @@ __device__ __forceinline__ void row_adjoint(const float *g, const float *A, floa
 // and the previous pose's gradient reduced per block in a fixed order (pose_partials (B, gridDim.x, 12), summed by
 // k_pose_grad_reduce).  No atomics.  kWantK adds the 12 entries of K's first three rows, which only the photometric row
 // reads, to the dual-number inputs (29 directions) and reduces their gradient like the pose's into k_partials.
-template <bool kWantK>
+// kRobust: the sums of k_icp_joint_linearize_idx<true>; only the two row adjoints change (r_p reads no K, so the d/dK
+// directions see the photometric adjoint scaled by its weight).
+template <bool kWantK, bool kRobust = false>
 __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs a, const float *g, float *g_src,
                                                                       float *g_scol, float *g_tp, float *g_tn,
                                                                       float *g_stencil, float *pose_partials,
-                                                                      float *k_partials) {
+                                                                      float *k_partials, Huber hb) {
   __shared__ float s_g[kNumSums];
   __shared__ LiveCamera s_cam;
   __shared__ Rigid s_pose;
@@ -983,7 +1078,7 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs
     const float A[6] = {nx, ny, nz, nz * sy - ny * sz, nx * sz - nz * sx, ny * sx - nx * sy};
     const float r = (nx * (px - sx) + ny * (py - sy)) + nz * (pz - sz);
     float ad[6], gr;
-    row_adjoint(s_g, A, r, 1.0f, ad, gr);
+    row_adjoint<kRobust>(s_g, A, r, 1.0f, ad, gr, hb.delta);
     gs[0] = (-nz * ad[4] + ny * ad[5]) - gr * nx;
     gs[1] = (nz * ad[3] - nx * ad[5]) - gr * ny;
     gs[2] = (-ny * ad[3] + nx * ad[4]) - gr * nz;
@@ -1000,7 +1095,7 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_joint_linearize_bwd(JointArgs
       photometric_row(c, sx, sy, sz, gu, gv, Ap);
       const float rp = intensity3(a.src_col + row * 3) - intensity3(mcol + j * 3);
       float ap[6], grp;
-      row_adjoint(s_g, Ap, rp, a.w, ap, grp);
+      row_adjoint<kRobust>(s_g, Ap, rp, a.w, ap, grp, hb.delta_p);
       // d(sum_p ap[p] A_p)/d(input) for the 17 inputs s (3), gu, gv, T^-1 rotation (9) and translation (3)
       float gin[17];
 #pragma unroll 1
@@ -1438,6 +1533,7 @@ struct KnnLinearize {
   KnnArgs ka;
   int64_t *nn_idx;  // written by the last iteration's first association (may be null)
   int B;
+  const Huber *hb;  // null: unweighted rows; else the Huber-weighted kernels at hb->delta
   void prepare(cudaStream_t s) {
     if (ka.grid.params) build_search_grid(ka.tgt_p, ka.tgt_count, ka.nt_stride, B, ka.grid, s);
   }
@@ -1445,22 +1541,35 @@ struct KnnLinearize {
     ka.pre = pre;
     ka.write_back = write_back;
     ka.nn_idx = last ? nn_idx : nullptr;
-    if (ka.grid.params) k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, s>>>(ka);
-    else k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, s>>>(ka);
+    if (hb) {
+      if (ka.grid.params) k_icp_knn_linearize<true, true><<<grid, kIcpBlock, 0, s>>>(ka, hb->delta);
+      else k_icp_knn_linearize<false, true><<<grid, kIcpBlock, 0, s>>>(ka, hb->delta);
+    } else if (ka.grid.params) {
+      k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, s>>>(ka, 0.0f);
+    } else {
+      k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, s>>>(ka, 0.0f);
+    }
   }
 };
 
 // projective association against target images rendered from the previous pose
-// (with the photometric term when pm.w > 0)
+// (with the photometric term when pm.w > 0, Huber-weighted when hb is set)
 struct ProjLinearize {
   ProjLinArgs pa;
   ProjRgb pm;
+  const Huber *hb;
   void prepare(cudaStream_t) {}
   void operator()(const float *pre, int write_back, bool, dim3 grid, cudaStream_t s) {
     pa.pre = pre;
     pa.write_back = write_back;
-    if (pm.w > 0.0f) k_icp_proj_linearize<true><<<grid, kIcpBlock, 0, s>>>(pa, pm);
-    else k_icp_proj_linearize<false><<<grid, kIcpBlock, 0, s>>>(pa, pm);
+    if (hb) {
+      if (pm.w > 0.0f) k_icp_proj_linearize<true, true><<<grid, kIcpBlock, 0, s>>>(pa, pm, *hb);
+      else k_icp_proj_linearize<false, true><<<grid, kIcpBlock, 0, s>>>(pa, pm, *hb);
+    } else if (pm.w > 0.0f) {
+      k_icp_proj_linearize<true><<<grid, kIcpBlock, 0, s>>>(pa, pm, Huber{});
+    } else {
+      k_icp_proj_linearize<false><<<grid, kIcpBlock, 0, s>>>(pa, pm, Huber{});
+    }
   }
 };
 
@@ -1468,10 +1577,11 @@ struct ProjLinearize {
 int run_icp_loop(float *src, const int32_t *src_count, int ns_stride, const float *tgt_p, const float *tgt_n,
                  const int32_t *tgt_count, int nt_stride, int B, const float *T0, int mode, int numiters, float damp,
                  int use_thresh, float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *partials,
-                 int nblk_cap, IcpState st, int64_t *nn_idx, const TargetGrid &tgt_grid, cudaStream_t stream) {
+                 int nblk_cap, IcpState st, int64_t *nn_idx, const TargetGrid &tgt_grid, const Huber *hb,
+                 cudaStream_t stream) {
   KnnLinearize lin{KnnArgs{src, src_count, ns_stride, tgt_p, tgt_n, tgt_count, nt_stride, nullptr, 0, dist_thresh,
                            use_thresh, partials, nullptr, nullptr, tgt_grid},
-                   nn_idx, B};
+                   nn_idx, B, hb};
   return icp_iterations(lin, ns_stride, B, T0, mode, numiters, damp, lambda_max, Bp, B2p, nu, partials, nblk_cap, st,
                         stream);
 }
@@ -1521,11 +1631,12 @@ extern "C" int64_t gsx_icp_workspace_bytes(int B, int H, int W, int ds, int64_t 
   return c.bytes;
 }
 
-extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
-                             const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
-                             const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
-                             float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
-                             int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, void *stream) {
+// gsx_icp_align (hb == nullptr) and gsx_icp_align_robust
+static int icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
+                     const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
+                     const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
+                     float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
+                     int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, const Huber *hb, void *stream) {
   GSX_CHECK_ARG(src_points && src_count && tgt_points && tgt_normals && tgt_count && transform_out && scratch,
                 "gsx_icp_align: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1 && numiters >= 0, "gsx_icp_align: bad extents");
@@ -1539,10 +1650,37 @@ extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, 
   cudaMemcpyAsync(sc.src, src_points, (size_t)B * ns_stride * 12, cudaMemcpyDeviceToDevice, s);
   const int rc = run_icp_loop(sc.src, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
                               initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp,
-                              B2p, nu, sc.partials, nblk, sc.st, nn_idx_out, sc.grid, s);
+                              B2p, nu, sc.partials, nblk, sc.st, nn_idx_out, sc.grid, hb, s);
   if (rc) return rc;
   cudaMemcpyAsync(transform_out, sc.st.T_total, (size_t)B * 64, cudaMemcpyDeviceToDevice, s);
   return 0;
+}
+
+extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
+                             const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
+                             const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
+                             float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
+                             int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, void *stream) {
+  return icp_align(src_points, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
+                   initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu,
+                   transform_out, nn_idx_out, scratch, scratch_bytes, nullptr, stream);
+}
+
+// refuses a Huber scale that is not > 0 (NaN included); +inf is allowed and weighs every finite row 1
+#define GSX_CHECK_HUBER(fn, name, d) \
+  GSX_CHECK_ARG((d) > 0.0f, fn ": " name " %g must be > 0 (+inf = unweighted)", (double)(d))
+
+extern "C" int gsx_icp_align_robust(const float *src_points, const int32_t *src_count, int ns_stride,
+                                    const float *tgt_points, const float *tgt_normals, const int32_t *tgt_count,
+                                    int nt_stride, int B, const float *initial_transform, int mode, int numiters,
+                                    float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                                    float B2p, float nu, float *transform_out, int64_t *nn_idx_out, void *scratch,
+                                    int64_t scratch_bytes, float huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_align_robust", "huber_delta", huber_delta);
+  const Huber hb{huber_delta, 0.0f};
+  return icp_align(src_points, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
+                   initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu,
+                   transform_out, nn_idx_out, scratch, scratch_bytes, &hb, stream);
 }
 
 extern "C" int64_t gsx_icp_align_scratch_bytes(int B, int ns_stride, int nt_stride) {
@@ -1559,14 +1697,14 @@ extern "C" int64_t gsx_icp_tgt_scratch_bytes(int B, int64_t tgt_capacity) {
   return c.bytes;
 }
 
-extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts,
-                                int64_t capacity, int64_t max_count, const float *depth, int64_t depth_bstride,
-                                const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
-                                float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
-                                int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity,
-                                uint32_t epoch, int32_t *overflow_flag, void *stream) {
+// gsx_icp_localize (hb == nullptr) and gsx_icp_localize_robust
+static int icp_localize(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                        const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
+                        const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
+                        int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                        float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
+                        int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity, uint32_t epoch,
+                        int32_t *overflow_flag, const Huber *hb, void *stream) {
   GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace && tgt_scratch,
                 "gsx_icp_localize: null pointer");
   GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_geometry) & 15) == 0,
@@ -1598,12 +1736,42 @@ extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts
   GSX_CHECK_LAUNCH("gsx_icp_localize(gather)");
   const int rc = run_icp_loop(w.src, w.src_count, w.ns_cap, tgt.p, tgt.n, w.tgt_count, (int)tgt_capacity, B, nullptr,
                               mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu, w.partials,
-                              w.nblk, w.st, nullptr, tgt.grid, s);
+                              w.nblk, w.st, nullptr, tgt.grid, hb, s);
   if (rc) return rc;
   k_pose_compose<<<(B + 63) / 64, 64, 0, s>>>(w.st.T_total, prev_poses, prev_pose_bstride, poses_out,
                                               poses_out_bstride, B);
   GSX_CHECK_LAUNCH("gsx_icp_localize(compose)");
   return 0;
+}
+
+extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts,
+                                int64_t capacity, int64_t max_count, const float *depth, int64_t depth_bstride,
+                                const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
+                                float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                                float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
+                                int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity,
+                                uint32_t epoch, int32_t *overflow_flag, void *stream) {
+  return icp_localize(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
+                      prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh, dist_thresh,
+                      lambda_max, Bp, B2p, nu, tgt_scratch, tgt_capacity, poses_out, poses_out_bstride, workspace,
+                      workspace_map_capacity, epoch, overflow_flag, nullptr, stream);
+}
+
+extern "C" int gsx_icp_localize_robust(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                       int64_t max_count, const float *depth, int64_t depth_bstride,
+                                       const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                       int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
+                                       float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                                       float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
+                                       int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity,
+                                       uint32_t epoch, int32_t *overflow_flag, float huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_localize_robust", "huber_delta", huber_delta);
+  const Huber hb{huber_delta, 0.0f};
+  return icp_localize(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
+                      prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh, dist_thresh,
+                      lambda_max, Bp, B2p, nu, tgt_scratch, tgt_capacity, poses_out, poses_out_bstride, workspace,
+                      workspace_map_capacity, epoch, overflow_flag, &hb, stream);
 }
 
 extern "C" int64_t gsx_knn1_scratch_bytes(int B, int ns_stride, int nt_stride) {
@@ -1629,9 +1797,9 @@ extern "C" int gsx_knn1(const float *src_points, const int32_t *src_count, int n
   if (sc.grid.params) {
     // (build_grid == 0: `scratch` still holds the grid a previous call built for this very target)
     if (build_grid) build_search_grid(tgt_points, tgt_count, nt_stride, B, sc.grid, s);
-    k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, s>>>(ka);
+    k_icp_knn_linearize<true><<<grid, kIcpBlock, 0, s>>>(ka, 0.0f);
   } else {
-    k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, s>>>(ka);
+    k_icp_knn_linearize<false><<<grid, kIcpBlock, 0, s>>>(ka, 0.0f);
   }
   GSX_CHECK_LAUNCH("gsx_knn1");
   return 0;
@@ -1642,10 +1810,11 @@ extern "C" int64_t gsx_icp_normal_eq_scratch_bytes(int ns) {
   return (int64_t)((ns + kIcpBlock - 1) / kIcpBlock) * kNumSums * 4;
 }
 
-extern "C" int gsx_icp_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                             const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                             const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
-                                             void *stream) {
+// gsx_icp_normal_eq_batched_fwd (hb == nullptr) and gsx_icp_normal_eq_batched_robust_fwd
+static int normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                 const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
+                                 const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
+                                 const Huber *hb, void *stream) {
   GSX_CHECK_ARG(src_points && tgt_points && tgt_normals && nn_idx && sums_out && scratch,
                 "gsx_icp_normal_eq_batched_fwd: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1 &&
@@ -1653,11 +1822,56 @@ extern "C" int gsx_icp_normal_eq_batched_fwd(const float *src_points, const int3
                 "gsx_icp_normal_eq_batched_fwd: bad sizes");
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   cudaStream_t s = (cudaStream_t)stream;
-  k_icp_linearize_idx<<<dim3((unsigned)nblk, (unsigned)B), kIcpBlock, 0, s>>>(src_points, ns_stride, src_count, tgt_points,
-                                                                            tgt_normals, nt_stride, nn_idx,
-                                                                            (float *)scratch);
+  const dim3 grid((unsigned)nblk, (unsigned)B);
+  if (hb)
+    k_icp_linearize_idx<true><<<grid, kIcpBlock, 0, s>>>(src_points, ns_stride, src_count, tgt_points, tgt_normals,
+                                                         nt_stride, nn_idx, (float *)scratch, hb->delta);
+  else
+    k_icp_linearize_idx<<<grid, kIcpBlock, 0, s>>>(src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride,
+                                                   nn_idx, (float *)scratch, 0.0f);
   k_icp_reduce_partials<<<B, 32, 0, s>>>((const float *)scratch, nblk, sums_out);
   GSX_CHECK_LAUNCH("gsx_icp_normal_eq_batched_fwd");
+  return 0;
+}
+
+extern "C" int gsx_icp_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                             const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
+                                             const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
+                                             void *stream) {
+  return normal_eq_batched_fwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx,
+                               sums_out, scratch, scratch_bytes, nullptr, stream);
+}
+
+extern "C" int gsx_icp_normal_eq_batched_robust_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                                    const float *tgt_points, const float *tgt_normals, int nt_stride,
+                                                    int B, const int64_t *nn_idx, float *sums_out, void *scratch,
+                                                    int64_t scratch_bytes, float huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_normal_eq_batched_robust_fwd", "huber_delta", huber_delta);
+  const Huber hb{huber_delta, 0.0f};
+  return normal_eq_batched_fwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx,
+                               sums_out, scratch, scratch_bytes, &hb, stream);
+}
+
+// gsx_icp_normal_eq_batched_bwd (hb == nullptr) and gsx_icp_normal_eq_batched_robust_bwd
+static int normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                 const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
+                                 const int64_t *nn_idx, const float *g_sums, float *g_src, float *g_tgt_points_rows,
+                                 float *g_tgt_normals_rows, const Huber *hb, void *stream) {
+  GSX_CHECK_ARG(src_points && tgt_points && tgt_normals && nn_idx && g_sums && g_src && g_tgt_points_rows &&
+                    g_tgt_normals_rows,
+                "gsx_icp_normal_eq_batched_bwd: null pointer");
+  GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1, "gsx_icp_normal_eq_batched_bwd: bad sizes");
+  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
+  const dim3 grid((unsigned)nblk, (unsigned)B);
+  if (hb)
+    k_icp_linearize_bwd<true><<<grid, kIcpBlock, 0, (cudaStream_t)stream>>>(
+        src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride, nn_idx, g_sums, g_src, g_tgt_points_rows,
+        g_tgt_normals_rows, hb->delta);
+  else
+    k_icp_linearize_bwd<<<grid, kIcpBlock, 0, (cudaStream_t)stream>>>(
+        src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride, nn_idx, g_sums, g_src, g_tgt_points_rows,
+        g_tgt_normals_rows, 0.0f);
+  GSX_CHECK_LAUNCH("gsx_icp_normal_eq_batched_bwd");
   return 0;
 }
 
@@ -1665,16 +1879,19 @@ extern "C" int gsx_icp_normal_eq_batched_bwd(const float *src_points, const int3
                                              const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
                                              const int64_t *nn_idx, const float *g_sums, float *g_src,
                                              float *g_tgt_points_rows, float *g_tgt_normals_rows, void *stream) {
-  GSX_CHECK_ARG(src_points && tgt_points && tgt_normals && nn_idx && g_sums && g_src && g_tgt_points_rows &&
-                    g_tgt_normals_rows,
-                "gsx_icp_normal_eq_batched_bwd: null pointer");
-  GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1, "gsx_icp_normal_eq_batched_bwd: bad sizes");
-  const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
-  k_icp_linearize_bwd<<<dim3((unsigned)nblk, (unsigned)B), kIcpBlock, 0, (cudaStream_t)stream>>>(
-      src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride, nn_idx, g_sums, g_src, g_tgt_points_rows,
-      g_tgt_normals_rows);
-  GSX_CHECK_LAUNCH("gsx_icp_normal_eq_batched_bwd");
-  return 0;
+  return normal_eq_batched_bwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx, g_sums,
+                               g_src, g_tgt_points_rows, g_tgt_normals_rows, nullptr, stream);
+}
+
+extern "C" int gsx_icp_normal_eq_batched_robust_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                                    const float *tgt_points, const float *tgt_normals, int nt_stride,
+                                                    int B, const int64_t *nn_idx, const float *g_sums, float *g_src,
+                                                    float *g_tgt_points_rows, float *g_tgt_normals_rows,
+                                                    float huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_normal_eq_batched_robust_bwd", "huber_delta", huber_delta);
+  const Huber hb{huber_delta, 0.0f};
+  return normal_eq_batched_bwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx, g_sums,
+                               g_src, g_tgt_points_rows, g_tgt_normals_rows, &hb, stream);
 }
 
 extern "C" int gsx_icp_normal_eq_fwd(const float *src_points, int ns, const float *tgt_points,
@@ -1686,7 +1903,7 @@ extern "C" int gsx_icp_normal_eq_fwd(const float *src_points, int ns, const floa
   const int nblk = (ns + kIcpBlock - 1) / kIcpBlock;
   cudaStream_t s = (cudaStream_t)stream;
   k_icp_linearize_idx<<<nblk, kIcpBlock, 0, s>>>(src_points, ns, nullptr, tgt_points, tgt_normals, 0, nn_idx,
-                                                 (float *)scratch);
+                                                 (float *)scratch, 0.0f);
   k_icp_reduce_partials<<<1, 32, 0, s>>>((const float *)scratch, nblk, sums_out);
   GSX_CHECK_LAUNCH("gsx_icp_normal_eq_fwd");
   return 0;
@@ -1703,7 +1920,7 @@ extern "C" int gsx_icp_normal_eq_bwd(const float *src_points, int ns, const floa
   const int nblk = (ns + kIcpBlock - 1) / kIcpBlock;
   k_icp_linearize_bwd<<<nblk, kIcpBlock, 0, (cudaStream_t)stream>>>(src_points, ns, nullptr, tgt_points, tgt_normals, 0,
                                                                     nn_idx, g_sums, g_src, g_tgt_points_rows,
-                                                                    g_tgt_normals_rows);
+                                                                    g_tgt_normals_rows, 0.0f);
   GSX_CHECK_LAUNCH("gsx_icp_normal_eq_bwd");
   return 0;
 }
@@ -1738,14 +1955,15 @@ struct PhotometricInputs {
   float w;
 };
 
-// gsx_icp_localize_projective_splats (pm == nullptr, the geometric workspace) and gsx_icp_localize_projective_rgb
+// gsx_icp_localize_projective_splats (pm == nullptr, the geometric workspace), gsx_icp_localize_projective_rgb and
+// gsx_icp_localize_projective_robust (hb != nullptr: the Huber-weighted kernels)
 static int localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                                const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
                                const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
                                int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max,
                                float Bp, float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
                                void *workspace, int64_t workspace_bytes, int max_splat_px, const PhotometricInputs *pm,
-                               void *stream) {
+                               const Huber *hb, void *stream) {
   GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX,
                 "gsx_icp_localize_projective: max_splat_px %d outside [0, %d]", max_splat_px, GSX_MAX_SPLAT_PX);
   GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace,
@@ -1773,7 +1991,7 @@ static int localize_projective(const float *map_geometry, const int32_t *counts,
                                 ProjTargets{prev_poses, prev_pose_bstride, intrinsics, K_bstride, image_bounds(H, W),
                                             w.index, w.tgt_p, w.tgt_n, dist_thresh, use_dist_thresh},
                                 w.partials},
-                    ProjRgb{w.I_s, w.I_m, rgb ? pm->w : 0.0f}};
+                    ProjRgb{w.I_s, w.I_m, rgb ? pm->w : 0.0f}, hb};
   const int rc = icp_iterations(lin, w.ns_cap, B, nullptr, mode, numiters, damp, lambda_max, Bp, B2p, nu, w.partials,
                                 w.nblk, w.st, s);
   if (rc) return rc;
@@ -1795,7 +2013,7 @@ extern "C" int gsx_icp_localize_projective_splats(const float *map_geometry, con
   return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
                              prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
                              dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
-                             workspace_bytes, max_splat_px, nullptr, stream);
+                             workspace_bytes, max_splat_px, nullptr, nullptr, stream);
 }
 
 extern "C" int64_t gsx_icp_projective_rgb_workspace_bytes(int B, int H, int W, int ds) {
@@ -1826,7 +2044,34 @@ extern "C" int gsx_icp_localize_projective_rgb(const float *map_geometry, const 
   return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
                              prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
                              dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
-                             workspace_bytes, max_splat_px, &pm, stream);
+                             workspace_bytes, max_splat_px, &pm, nullptr, stream);
+}
+
+extern "C" int gsx_icp_localize_projective_robust(
+    const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count, const float *depth,
+    int64_t depth_bstride, const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+    int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters, float damp, int use_dist_thresh,
+    float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
+    void *workspace, int64_t workspace_bytes, int max_splat_px, const float *map_colours, const float *rgb,
+    int64_t rgb_bstride, float photometric_weight, float huber_delta, float photometric_huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_localize_projective_robust", "huber_delta", huber_delta);
+  GSX_CHECK_HUBER("gsx_icp_localize_projective_robust", "photometric_huber_delta", photometric_huber_delta);
+  GSX_CHECK_ARG(photometric_weight >= 0.0f && photometric_weight <= 3.402823466e38f,
+                "gsx_icp_localize_projective_robust: photometric_weight %g must be finite and >= 0",
+                (double)photometric_weight);
+  GSX_CHECK_ARG(photometric_weight > 0.0f || photometric_huber_delta == INFINITY,
+                "gsx_icp_localize_projective_robust: a finite photometric_huber_delta needs photometric_weight > 0");
+  if (photometric_weight > 0.0f) {
+    GSX_CHECK_ARG(map_colours && rgb, "gsx_icp_localize_projective_robust: null colour pointer");
+    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
+                  "gsx_icp_localize_projective_robust: colour rows must be 16-byte aligned");
+  }
+  const PhotometricInputs pm{map_colours, rgb, rgb_bstride, photometric_weight};
+  const Huber hb{huber_delta, photometric_huber_delta};
+  return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
+                             prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
+                             dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
+                             workspace_bytes, max_splat_px, &pm, &hb, stream);
 }
 
 extern "C" int gsx_icp_projective_targets_rgb(const float *map_geometry, const float *map_colours,
@@ -1888,13 +2133,12 @@ static int joint_args(const char *fn, const float *src_points, const int32_t *sr
   return 0;
 }
 
-extern "C" int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                                   const float *src_colours, const float *tgt_points,
-                                                   const float *tgt_normals, const float *model_colours,
-                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
-                                                   const float *prev_poses, const float *intrinsics,
-                                                   float photometric_weight, float *sums_out, void *scratch,
-                                                   int64_t scratch_bytes, void *stream) {
+// gsx_icp_joint_normal_eq_batched_fwd (hb == nullptr) and gsx_icp_joint_normal_eq_batched_robust_fwd
+static int joint_fwd(const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+                     const float *tgt_points, const float *tgt_normals, const float *model_colours,
+                     const int64_t *index, int B, int H, int W, const int64_t *nn_idx, const float *prev_poses,
+                     const float *intrinsics, float photometric_weight, float *sums_out, void *scratch,
+                     int64_t scratch_bytes, const Huber *hb, void *stream) {
   JointArgs a;
   if (joint_args("gsx_icp_joint_normal_eq_batched_fwd", src_points, src_count, ns_stride, src_colours, tgt_points,
                  tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
@@ -1903,10 +2147,37 @@ extern "C" int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, cons
                 "gsx_icp_joint_normal_eq_batched_fwd: bad scratch");
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   cudaStream_t s = (cudaStream_t)stream;
-  k_icp_joint_linearize_idx<<<dim3((unsigned)nblk, (unsigned)B), kIcpBlock, 0, s>>>(a, (float *)scratch);
+  const dim3 grid((unsigned)nblk, (unsigned)B);
+  if (hb) k_icp_joint_linearize_idx<true><<<grid, kIcpBlock, 0, s>>>(a, (float *)scratch, *hb);
+  else k_icp_joint_linearize_idx<<<grid, kIcpBlock, 0, s>>>(a, (float *)scratch, Huber{});
   k_icp_reduce_partials<<<B, 32, 0, s>>>((const float *)scratch, nblk, sums_out);
   GSX_CHECK_LAUNCH("gsx_icp_joint_normal_eq_batched_fwd");
   return 0;
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                                   const float *src_colours, const float *tgt_points,
+                                                   const float *tgt_normals, const float *model_colours,
+                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                                                   const float *prev_poses, const float *intrinsics,
+                                                   float photometric_weight, float *sums_out, void *scratch,
+                                                   int64_t scratch_bytes, void *stream) {
+  return joint_fwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
+                   W, nn_idx, prev_poses, intrinsics, photometric_weight, sums_out, scratch, scratch_bytes, nullptr,
+                   stream);
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_robust_fwd(
+    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
+    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
+    float *sums_out, void *scratch, int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
+    void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_fwd", "huber_delta", huber_delta);
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_fwd", "photometric_huber_delta", photometric_huber_delta);
+  const Huber hb{huber_delta, photometric_huber_delta};
+  return joint_fwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
+                   W, nn_idx, prev_poses, intrinsics, photometric_weight, sums_out, scratch, scratch_bytes, &hb, stream);
 }
 
 extern "C" int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
@@ -1931,13 +2202,14 @@ extern "C" int64_t gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(
   return (int64_t)B * nblk * 12 * 4 * 2;
 }
 
-extern "C" int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
-    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
-    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
-    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
-    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
-    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
-    void *stream) {
+// gsx_icp_joint_normal_eq_batched_bwd_intrinsics (hb == nullptr) and gsx_icp_joint_normal_eq_batched_robust_bwd
+static int joint_bwd(const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+                     const float *tgt_points, const float *tgt_normals, const float *model_colours,
+                     const int64_t *index, int B, int H, int W, const int64_t *nn_idx, const float *prev_poses,
+                     const float *intrinsics, float photometric_weight, const float *g_sums, float *g_src,
+                     float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
+                     float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch,
+                     int64_t scratch_bytes, const Huber *hb, void *stream) {
   JointArgs a;
   if (joint_args("gsx_icp_joint_normal_eq_batched_bwd", src_points, src_count, ns_stride, src_colours, tgt_points,
                  tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
@@ -1955,17 +2227,56 @@ extern "C" int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 grid((unsigned)nblk, (unsigned)B);
   float *pose_partials = (float *)scratch, *k_partials = pose_partials + (int64_t)B * nblk * 12;
-  if (g_intrinsics)
+  if (hb && g_intrinsics)
+    k_icp_joint_linearize_bwd<true, true><<<grid, kIcpBlock, 0, s>>>(a, g_sums, g_src, g_src_colours,
+                                                                      g_tgt_points_rows, g_tgt_normals_rows,
+                                                                      g_stencil_colours_rows, pose_partials,
+                                                                      k_partials, *hb);
+  else if (hb)
+    k_icp_joint_linearize_bwd<false, true><<<grid, kIcpBlock, 0, s>>>(a, g_sums, g_src, g_src_colours,
+                                                                       g_tgt_points_rows, g_tgt_normals_rows,
+                                                                       g_stencil_colours_rows, pose_partials, nullptr,
+                                                                       *hb);
+  else if (g_intrinsics)
     k_icp_joint_linearize_bwd<true><<<grid, kIcpBlock, 0, s>>>(a, g_sums, g_src, g_src_colours, g_tgt_points_rows,
                                                                 g_tgt_normals_rows, g_stencil_colours_rows,
-                                                                pose_partials, k_partials);
+                                                                pose_partials, k_partials, Huber{});
   else
     k_icp_joint_linearize_bwd<false><<<grid, kIcpBlock, 0, s>>>(a, g_sums, g_src, g_src_colours, g_tgt_points_rows,
                                                                  g_tgt_normals_rows, g_stencil_colours_rows,
-                                                                 pose_partials, nullptr);
+                                                                 pose_partials, nullptr, Huber{});
   k_pose_grad_reduce<<<B, 16, 0, s>>>(pose_partials, nblk, g_prev_poses, B);
   // the 12 entries of K's first three rows, summed over the blocks in order; the 4th row gets 0
   if (g_intrinsics) k_pose_grad_reduce<<<B, 16, 0, s>>>(k_partials, nblk, g_intrinsics, B);
   GSX_CHECK_LAUNCH("gsx_icp_joint_normal_eq_batched_bwd");
   return 0;
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
+    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
+    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
+    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
+    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
+    void *stream) {
+  return joint_bwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
+                   W, nn_idx, prev_poses, intrinsics, photometric_weight, g_sums, g_src, g_src_colours,
+                   g_tgt_points_rows, g_tgt_normals_rows, g_stencil_colours_rows, g_prev_poses, g_intrinsics, scratch,
+                   scratch_bytes, nullptr, stream);
+}
+
+extern "C" int gsx_icp_joint_normal_eq_batched_robust_bwd(
+    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
+    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
+    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
+    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
+    float huber_delta, float photometric_huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_bwd", "huber_delta", huber_delta);
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_bwd", "photometric_huber_delta", photometric_huber_delta);
+  const Huber hb{huber_delta, photometric_huber_delta};
+  return joint_bwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
+                   W, nn_idx, prev_poses, intrinsics, photometric_weight, g_sums, g_src, g_src_colours,
+                   g_tgt_points_rows, g_tgt_normals_rows, g_stencil_colours_rows, g_prev_poses, g_intrinsics, scratch,
+                   scratch_bytes, &hb, stream);
 }

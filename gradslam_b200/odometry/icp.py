@@ -6,7 +6,7 @@ import torch
 
 from ..structures.pointclouds import Pointclouds
 from .base import OdometryProvider
-from .icputils import _taped_icp_batched, _wants_grad, icp_align
+from .icputils import _check_huber_delta, _taped_icp_batched, _wants_grad, icp_align
 
 __all__ = ["ICPOdometryProvider"]
 
@@ -27,7 +27,7 @@ def _check_provide_args(maps_pointclouds, frames_pointclouds, who):
 
 def _provide(prov, maps_pc, frames_pc, mode):
     kw = dict(lambda_max=getattr(prov, "lambda_max", 2.0), B=getattr(prov, "B", 1.0), B2=getattr(prov, "B2", 1.0),
-              nu=getattr(prov, "nu", 200.0))
+              nu=getattr(prov, "nu", 200.0), huber_delta=prov.huber_delta)
     if _wants_grad(*frames_pc._grad_tensors(), *maps_pc._grad_tensors()):
         # differentiable mode: ONE chain of batched autograd ops for all elements (the reference's providers loop over
         # the batch in Python, odometry/icp.py:84-97)
@@ -40,17 +40,22 @@ def _provide(prov, maps_pc, frames_pc, mode):
     tgt, tgt_n = maps_pc.points_padded.contiguous(), maps_pc.normals_padded.contiguous()
     src_c = frames_pc._counts_dev[frames_pc._cur]
     tgt_c = maps_pc._counts_dev[maps_pc._cur]
-    T, _ = icp_align(src, src_c, tgt, tgt_n, tgt_c, None, mode, prov.numiters, prov.damp, prov.dist_thresh,
-                     lambda_max=getattr(prov, "lambda_max", 2.0), B=getattr(prov, "B", 1.0),
-                     B2=getattr(prov, "B2", 1.0), nu=getattr(prov, "nu", 200.0))
+    T, _ = icp_align(src, src_c, tgt, tgt_n, tgt_c, None, mode, prov.numiters, prov.damp, prov.dist_thresh, **kw)
     return T.unsqueeze(1)
 
 
 class ICPOdometryProvider(OdometryProvider):
-    def __init__(self, numiters: int = 20, damp: float = 1e-8, dist_thresh: Union[float, int, None] = None):
+    def __init__(self, numiters: int = 20, damp: float = 1e-8, dist_thresh: Union[float, int, None] = None, *,
+                 huber_delta: Union[float, int, None] = None):
+        """huber_delta (extension, metres, None = off): weigh each point-to-plane residual r with Huber's M-estimator,
+        weight 1 for |r| <= huber_delta and huber_delta / |r| beyond, by iteratively reweighted least squares inside the
+        same LM loop, which then compares the Huber energy.  Unlike dist_thresh it has a gradient, and it composes
+        with it."""
+        _check_huber_delta(huber_delta)
         self.numiters = numiters
         self.damp = damp
         self.dist_thresh = dist_thresh
+        self.huber_delta = huber_delta
 
     def provide(self, maps_pointclouds: Pointclouds, frames_pointclouds: Pointclouds) -> torch.Tensor:
         """Transforms (B,1,4,4) aligning each frame cloud to its map cloud with point-to-plane ICP."""

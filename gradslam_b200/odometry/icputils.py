@@ -4,6 +4,8 @@ Host-side mirror of gradslam/odometry/icputils.py (same names, arguments, errors
 (`chamferdist.knn_points` in the reference), the row build, the normal-equation reduction, the damped solve,
 the SE(3) exponential and the LM / gradLM update all run in csrc/gsx_icp.cu; nothing here loops over points.
 """
+import ctypes
+import math
 from typing import Optional, Union
 
 import torch
@@ -61,6 +63,21 @@ def _check_clouds(src_pc, tgt_pc, tgt_normals, dist_thresh):
     for name, t in (("src_pc", src_pc), ("tgt_pc", tgt_pc), ("tgt_normals", tgt_normals)):
         if t.shape[2] != 3:
             raise ValueError("{}.shape[2] should be 3, but was {} instead".format(name, t.shape[2]))
+
+
+def _check_huber_delta(delta, name="huber_delta"):
+    """A Huber scale of the robust tracking energy: None (off) or a real number (not a bool), finite and > 0 that stays
+    > 0 and finite as the float32 the kernels take."""
+    if delta is None:
+        return
+    if isinstance(delta, bool) or not isinstance(delta, (float, int)):
+        raise TypeError("Expected {} to be None or of type float or int. Got {}.".format(name, type(delta)))
+    try:
+        d = float(delta)
+    except OverflowError:  # an int beyond float range
+        d = math.inf
+    if not (math.isfinite(d) and d > 0 and math.isfinite(ctypes.c_float(d).value) and ctypes.c_float(d).value > 0):
+        raise ValueError("Expected a finite float32 {} > 0 (or None). Got {}.".format(name, delta))
 
 
 def _counts(n, B, device):
@@ -132,8 +149,9 @@ def _check_icp_args(src_pc, tgt_pc, tgt_normals, initial_transform, numiters):
 
 
 def icp_align(src, src_counts, tgt, tgt_normals, tgt_counts, T0, mode, numiters, damp, dist_thresh, lambda_max=2.0,
-              B=1.0, B2=1.0, nu=200.0, want_idx=False):
-    """Batched ICP (mode 0) / gradICP (mode 1) on padded clouds (Bn, N, 3) with int32 sizes.  One C call."""
+              B=1.0, B2=1.0, nu=200.0, want_idx=False, huber_delta=None):
+    """Batched ICP (mode 0) / gradICP (mode 1) on padded clouds (Bn, N, 3) with int32 sizes.  One C call; with
+    huber_delta the Huber-weighted rows of gsx_icp_align_robust."""
     for name, t in (("src", src), ("tgt", tgt), ("tgt_normals", tgt_normals)):
         _C.require_cuda(t, name)
     Bn, Ns, _ = src.shape
@@ -144,10 +162,14 @@ def icp_align(src, src_counts, tgt, tgt_normals, tgt_counts, T0, mode, numiters,
     nbytes = _C.lib().gsx_icp_align_scratch_bytes(Bn, Ns, Nt)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     T0c = None if T0 is None else T0.to(dev).float().contiguous()
-    _C.launch("gsx_icp_align", src.contiguous(), src_counts, Ns, tgt.contiguous(), tgt_normals.contiguous(), tgt_counts,
-              Nt, Bn, T0c, int(mode), int(numiters), float(damp), 0 if dist_thresh is None else 1,
-              0.0 if dist_thresh is None else float(dist_thresh), float(lambda_max), float(B), float(B2), float(nu), out,
-              idx, scratch, nbytes)
+    args = (src.contiguous(), src_counts, Ns, tgt.contiguous(), tgt_normals.contiguous(), tgt_counts, Nt, Bn, T0c,
+            int(mode), int(numiters), float(damp), 0 if dist_thresh is None else 1,
+            0.0 if dist_thresh is None else float(dist_thresh), float(lambda_max), float(B), float(B2), float(nu), out,
+            idx, scratch, nbytes)
+    if huber_delta is None:
+        _C.launch("gsx_icp_align", *args)
+    else:
+        _C.launch("gsx_icp_align_robust", *args, float(huber_delta))
     return out, idx
 
 
@@ -271,8 +293,10 @@ class _RigidTransformFn(torch.autograd.Function):
 # kernel takes the batch index from blockIdx.y; values per element are bit-identical to the per-element ops (padding rows
 # contribute exact zeros to the fixed-order sums).
 class _NormalEqBatchedFn(torch.autograd.Function):
+    """huber_delta: None = gsx_icp_normal_eq_batched_fwd / _bwd; else their Huber-weighted variants at that scale."""
+
     @staticmethod
-    def forward(ctx, src, tgt, tgt_n, idx, src_counts):
+    def forward(ctx, src, tgt, tgt_n, idx, src_counts, huber_delta=None):
         src_c, tgt_c, tn_c = (t.detach().contiguous().float() for t in (src, tgt, tgt_n))
         idx_c = idx.contiguous()
         _C.require_cuda(src_c, "src")
@@ -281,9 +305,14 @@ class _NormalEqBatchedFn(torch.autograd.Function):
         sums = torch.empty((Bn, 28), dtype=torch.float32, device=dev)
         nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _C.launch("gsx_icp_normal_eq_batched_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums, scratch,
-                  nbytes)
+        if huber_delta is None:
+            _C.launch("gsx_icp_normal_eq_batched_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums, scratch,
+                      nbytes)
+        else:
+            _C.launch("gsx_icp_normal_eq_batched_robust_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums,
+                      scratch, nbytes, float(huber_delta))
         ctx.saved = (src_c, tgt_c, tn_c, idx_c, src_counts)
+        ctx.huber_delta = huber_delta
         return sums
 
     @staticmethod
@@ -294,13 +323,17 @@ class _NormalEqBatchedFn(torch.autograd.Function):
         g = g.contiguous().float()
         g_src = torch.empty_like(src_c)
         rows_p, rows_n = torch.empty_like(src_c), torch.empty_like(src_c)
-        _C.launch("gsx_icp_normal_eq_batched_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src, rows_p,
-                  rows_n)
+        if ctx.huber_delta is None:
+            _C.launch("gsx_icp_normal_eq_batched_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src,
+                      rows_p, rows_n)
+        else:
+            _C.launch("gsx_icp_normal_eq_batched_robust_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src,
+                      rows_p, rows_n, float(ctx.huber_delta))
         # rows with idx < 0 carry zero gradients; scatter the per-source-row target gradients with the association
         flat = (idx_c.clamp(min=0) + torch.arange(Bn, device=dev).view(Bn, 1) * Nt).view(-1)
         g_tgt = torch.zeros((Bn * Nt, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_p.view(-1, 3))
         g_tn = torch.zeros((Bn * Nt, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_n.view(-1, 3))
-        return g_src, g_tgt.view(Bn, Nt, 3), g_tn.view(Bn, Nt, 3), None, None
+        return g_src, g_tgt.view(Bn, Nt, 3), g_tn.view(Bn, Nt, 3), None, None, None
 
 
 class _SolveBatchedFn(torch.autograd.Function):
@@ -377,10 +410,12 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
     or -1): (src, src_col (B,Ns,3), tgt, tgt_n, model_col (B,H*W,3), prev (B,4,4)) -> (B,28).  forward =
     gsx_icp_joint_normal_eq_batched_fwd, backward = gsx_icp_joint_normal_eq_batched_bwd, or
     gsx_icp_joint_normal_eq_batched_bwd_intrinsics when K requires grad (the photometric row reads K's first three rows);
-    the gradients of the model colours come per source row for the five stencil pixels and are scattered here."""
+    the gradients of the model colours come per source row for the five stencil pixels and are scattered here.
+    huber: None, or (huber_delta, photometric_huber_delta) as float32 scales (+inf = that residual unweighted) for the
+    Huber-weighted gsx_icp_joint_normal_eq_batched_robust_fwd / _bwd."""
 
     @staticmethod
-    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W):
+    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W, huber=None):
         ins = [t.detach().contiguous().float() for t in (src, src_col, tgt, tgt_n, model_col, prev)]
         _C.require_cuda(ins[0], "src")
         Bn, Ns = ins[0].shape[:2]
@@ -388,9 +423,14 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         sums = torch.empty((Bn, 28), dtype=torch.float32, device=src.device)
         nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=src.device)
-        _C.launch("gsx_icp_joint_normal_eq_batched_fwd", ins[0], src_counts, Ns, ins[1], ins[2], ins[3], ins[4], index_c,
-                  Bn, int(H), int(W), idx_c, ins[5], K_c, float(w), sums, scratch, nbytes)
+        args = (ins[0], src_counts, Ns, ins[1], ins[2], ins[3], ins[4], index_c, Bn, int(H), int(W), idx_c, ins[5], K_c,
+                float(w), sums, scratch, nbytes)
+        if huber is None:
+            _C.launch("gsx_icp_joint_normal_eq_batched_fwd", *args)
+        else:
+            _C.launch("gsx_icp_joint_normal_eq_batched_robust_fwd", *args, *huber)
         ctx.saved = (ins, idx_c, index_c, src_counts, K_c, float(w), int(H), int(W), prev.shape)
+        ctx.huber = huber
         ctx.K_shape = K.shape
         return sums
 
@@ -404,7 +444,17 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         rows_st = torch.empty((Bn, Ns, 5, 3), dtype=torch.float32, device=dev)
         g_prev = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
         g_K = None
-        if ctx.needs_input_grad[9]:
+        if ctx.huber is not None:
+            want_K = ctx.needs_input_grad[9]
+            g_K = torch.zeros((Bn, 4, 4), dtype=torch.float32, device=dev) if want_K else None
+            nbytes = (_C.lib().gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(Bn, Ns) if want_K
+                      else Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns))
+            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            _C.launch("gsx_icp_joint_normal_eq_batched_robust_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col,
+                      index, Bn, H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, g_K, scratch,
+                      nbytes, *ctx.huber)
+            g_K = None if g_K is None else g_K.view(ctx.K_shape)
+        elif ctx.needs_input_grad[9]:
             g_K = torch.zeros((Bn, 4, 4), dtype=torch.float32, device=dev)
             nbytes = _C.lib().gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(Bn, Ns)
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
@@ -425,11 +475,11 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         st = ((idx.clamp(min=0).unsqueeze(-1) + offs).clamp(0, P - 1) + base.unsqueeze(-1)).view(-1)
         g_model = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, st, rows_st.view(-1, 3))
         return (g_src, g_col, g_tgt.view(Bn, P, 3), g_tn.view(Bn, P, 3), g_model.view(Bn, P, 3),
-                g_prev.view(prev_shape), None, None, None, g_K, None, None, None)
+                g_prev.view(prev_shape), None, None, None, g_K, None, None, None, None)
 
 
 def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, target_cache=None, associate=None,
-                              normal_eq=None):
+                              normal_eq=None, huber_delta=None):
     if normal_eq is not None:  # (the projective association with the photometric term)
         idx = associate(src.detach())
         return normal_eq(src, tgt, tgt_n, idx), idx
@@ -439,18 +489,22 @@ def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thre
             idx = torch.where(d2 < dist_thresh, idx, torch.full_like(idx, -1))
     else:
         idx = associate(src.detach())
+    if huber_delta is not None:
+        return _NormalEqBatchedFn.apply(src, tgt, tgt_n, idx, src_counts, huber_delta), idx
     return _NormalEqBatchedFn.apply(src, tgt, tgt_n, idx, src_counts), idx
 
 
 def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numiters, damp, dist_thresh, lambda_max=2.0,
-                       B=1.0, B2=1.0, nu=200.0, associate=None, normal_eq=None):
+                       B=1.0, B2=1.0, nu=200.0, associate=None, normal_eq=None, huber_delta=None):
     """The differentiable ICP / gradICP loop of `_taped_icp` for a padded batch: src (Bn,Ns,3), tgt / tgt_n (Bn,Nt,3),
     int32 sizes (Bn,).  One chain of batched ops for all elements; returns (T (Bn,4,4), last nn idx (Bn,Ns), -1 = none).
     Per element the values are bit-identical to the per-element chain and to the fused no-grad loop.
     associate: None = exact 1-NN in tgt (thresholded by dist_thresh); otherwise a function of the current source
     (Bn,Ns,3), detached, returning the int64 target row per source row (-1 = none) - the projective association.
     normal_eq: None = _NormalEqBatchedFn; otherwise a function (src, tgt, tgt_n, idx) -> (Bn,28) sums (the joint op of
-    the photometric term)."""
+    the photometric term, which then carries its own Huber scales).
+    huber_delta: None = unweighted rows; else the Huber-weighted normal-equation op at that scale (gsx_icp_align_robust's
+    rows), so the loop minimises the Huber energy as the fused robust loop does."""
     dev = src.device
     Bn, Ns = src.shape[0], src.shape[1]
     # No valid source (or target) point in any element gives a padded width of 0, which the kernels reject.  One zero
@@ -466,11 +520,11 @@ def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numite
     grid = {}  # the target's search grid: built by the first of the 2 * numiters associations
     for _ in range(numiters):
         sums, idx = _normal_equations_batched(cur, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid, associate,
-                                              normal_eq)
+                                              normal_eq, huber_delta)
         xi, dT = _SolveBatchedFn.apply(sums, dampt)
         one_step = _RigidTransformBatchedFn.apply(cur, dT, src_counts)
         sums_next, _ = _normal_equations_batched(one_step, src_counts, tgt, tgt_n, tgt_counts, dist_thresh, grid,
-                                                 associate, normal_eq)
+                                                 associate, normal_eq, huber_delta)
         dampt, dT_applied, T = _UpdateBatchedFn.apply(xi, sums[:, 27], sums_next[:, 27], dampt, T, mode, lambda_max, B,
                                                       B2, nu)
         cur = _RigidTransformBatchedFn.apply(cur, dT_applied, src_counts)
@@ -684,12 +738,17 @@ def localize_against_map(pointclouds, live_frame, prev_frame, dsratio, odomprov)
     out = torch.empty((B, 1, 4, 4), dtype=torch.float32, device=dev)
     mode = 1 if hasattr(odomprov, "lambda_max") else 0
     dth = odomprov.dist_thresh
-    _C.launch("gsx_icp_localize", geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity,
-              pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters),
-              float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth),
-              float(getattr(odomprov, "lambda_max", 2.0)), float(getattr(odomprov, "B", 1.0)),
-              float(getattr(odomprov, "B2", 1.0)), float(getattr(odomprov, "nu", 200.0)), tgt, bound, out, 16, ws.buf,
-              ws.capacity, ws.next_epoch(), pointclouds._overflow_flag())
+    args = (geo, pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, pointclouds._bound, depth, d_bs, K, 16,
+            prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters), float(odomprov.damp),
+            0 if dth is None else 1, 0.0 if dth is None else float(dth), float(getattr(odomprov, "lambda_max", 2.0)),
+            float(getattr(odomprov, "B", 1.0)), float(getattr(odomprov, "B2", 1.0)),
+            float(getattr(odomprov, "nu", 200.0)), tgt, bound, out, 16, ws.buf, ws.capacity, ws.next_epoch(),
+            pointclouds._overflow_flag())
+    huber = getattr(odomprov, "huber_delta", None)
+    if huber is None:
+        _C.launch("gsx_icp_localize", *args)
+    else:
+        _C.launch("gsx_icp_localize_robust", *args, float(huber))
     return out
 
 
@@ -791,13 +850,14 @@ class _ProjectiveRgbWorkspace:
 
 
 def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0,
-                        photometric_weight=0.0):
+                        photometric_weight=0.0, photometric_huber_delta=None):
     """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective_splats): the source
     is the live frame on the ds lattice at the previous pose, the target is the map rendered from the previous pose at
     full resolution (surfels with radii as disks when target_splat_px >= 1, see projective_targets), each source point
     is associated with the pixel it projects to.  Returns the new poses (B,1,4,4) = T_icp · prev pose.  No host
     synchronisation.  photometric_weight w > 0 adds the photometric term of gsx_icp_localize_projective_rgb (the live
-    frame's and the map's colours); w = 0 is the geometric call."""
+    frame's and the map's colours); w = 0 is the geometric call.  With odomprov.huber_delta or photometric_huber_delta
+    set, the residuals are Huber-weighted at those scales (gsx_icp_localize_projective_robust)."""
     live = live_frame.to_channels_last()
     B, _, H, W = live.shape
     dev = pointclouds.device
@@ -813,6 +873,19 @@ def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, 
             pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters),
             float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth), lambda_max, Bp, B2p, nu,
             out, 16)
+    huber = getattr(odomprov, "huber_delta", None)
+    if huber is not None or photometric_huber_delta is not None:
+        rgb, rgb_bs, col = None, 0, None
+        if photometric_weight:
+            if not pointclouds.has_colors or live.rgb_image is None:
+                raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
+            _C.require_cuda(live.rgb_image, "rgb_image")
+            rgb, rgb_bs = _frame_base(live.rgb_image, H * W * 3)
+            col = pointclouds._col.contiguous()
+        ws = _ProjectiveRgbWorkspace.get(dev, B, H, W, int(dsratio))
+        _C.launch("gsx_icp_localize_projective_robust", *args, ws, ws.numel(), int(target_splat_px), col, rgb, rgb_bs,
+                  float(photometric_weight), *_huber_scales(huber, photometric_huber_delta))
+        return out
     if photometric_weight == 0:
         ws = _ProjectiveWorkspace.get(dev, B, H, W, int(dsratio))
         _C.launch("gsx_icp_localize_projective_splats", *args, ws, ws.numel(), int(target_splat_px))
@@ -827,8 +900,14 @@ def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, 
     return out
 
 
+def _huber_scales(huber_delta, photometric_huber_delta):
+    """The two float32 scales of the robust projective entry points, +inf for a residual left unweighted."""
+    return (math.inf if huber_delta is None else float(huber_delta),
+            math.inf if photometric_huber_delta is None else float(photometric_huber_delta))
+
+
 def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0,
-                              photometric_weight=0.0):
+                              photometric_weight=0.0, photometric_huber_delta=None):
     """The differentiable counterpart of `localize_projective`, bit-identical poses: the index image comes from
     gsx_render_views, the target images are gathers of the map rows at that index (so the gradient reaches the rows that
     won a pixel, each at most one), and the batched ICP chain runs with the projective association.  With
@@ -840,7 +919,8 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     colours are the live rgb on the lattice, and the previous pose gets the gradient of q = T_prev^-1 s and R_prev too.
     The gradient w.r.t. the intrinsics reaches the poses through the live points (K1), the disk depths of the splatted
     targets and their surface points (R3d, K1) and the photometric row; the index image and the association use K only
-    to choose pixels and carry none.
+    to choose pixels and carry none.  odomprov.huber_delta and photometric_huber_delta weigh the residuals as
+    localize_projective does, through the Huber-weighted ops, so the poses stay the fused call's bit for bit.
     live_frame.poses must be the previous poses.  Returns (B,1,4,4)."""
     from ..slam.icpslam import _compose_canonical
     from ..structures.rgbdimages import RGBDImages
@@ -883,6 +963,8 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     assoc = lambda cur: project_associate(cur, src_counts, tgt_p_d, index, prev_d.view(B, 4, 4), K, H, W, dth)[1]
     mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
     normal_eq = None
+    huber = getattr(odomprov, "huber_delta", None)
+    scales = None if huber is None and photometric_huber_delta is None else _huber_scales(huber, photometric_huber_delta)
     if photometric_weight:
         if not pointclouds.has_colors or live.rgb_image is None:
             raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
@@ -892,7 +974,9 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
             src_col = src_col.new_zeros(B, 1, 3)
         prev_v = prev.reshape(B, 4, 4)
         normal_eq = lambda cur, t_p, t_n, idx: _JointNormalEqBatchedFn.apply(
-            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, Kg, photometric_weight, H, W)
+            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, Kg, photometric_weight, H, W,
+            *(() if scales is None else (scales,)))
     T, _ = _taped_icp_batched(frames_pc.points_padded, src_counts, tgt_p, tgt_n, None, None, mode, odomprov.numiters,
-                              odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc, normal_eq=normal_eq)
+                              odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc, normal_eq=normal_eq,
+                              huber_delta=huber)
     return _compose_canonical(T, prev.squeeze(1)).unsqueeze(1)

@@ -63,7 +63,8 @@ class ICPSLAM(nn.Module):
                  B: Union[float, int] = 1.0, B2: Union[float, int] = 1.0, nu: Union[float, int] = 200.0,
                  association: str = "nn", device: Union[torch.device, str, None] = None, target_splat_px: int = 0,
                  photometric_weight: Union[float, int] = 0.0, depth_filter: Optional[BilateralFilter] = None,
-                 depth_filter_tracking_only: bool = False):
+                 depth_filter_tracking_only: bool = False, huber_delta: Union[float, int, None] = None,
+                 photometric_huber_delta: Union[float, int, None] = None):
         """association (extension): how the ICP odometry pairs live points with the map.  'nn' (default, the
         reference's) = exact 1-NN between the lattice-thinned live cloud and the lattice-active map points; 'projective'
         = each live point with the map row visible at the pixel it projects to in the map rendered from the previous
@@ -90,7 +91,16 @@ class ICPSLAM(nn.Module):
         In the differentiable mode the filter is on the tape: gradients reach the raw depth.  None (default): no filter.
 
         depth_filter_tracking_only (extension, default False): KinectFusion's split - the odometry tracks the filtered
-        frame and the map fuses the raw depth.  With odom='gt' there is no tracking, so nothing is filtered."""
+        frame and the map fuses the raw depth.  With odom='gt' there is no tracking, so nothing is filtered.
+
+        huber_delta (extension, metres, None = off): robust tracking.  Each point-to-plane residual r gets Huber's weight,
+        1 for |r| <= huber_delta and huber_delta / |r| beyond, by iteratively reweighted least squares inside the LM /
+        gradLM loop, which then compares the Huber energy.  A part of the scene that does not match the map (an object
+        that appeared, a depth edge) then pulls the pose far less.  Unlike dist_thresh, a hard cut without a gradient,
+        the weight is differentiable, and the two compose.  Both associations.  No effect with odom='gt'.
+
+        photometric_huber_delta (extension, intensity units, None = off, needs photometric_weight > 0): the same weight
+        on the photometric residual, against specular patches and colour changes.  No effect with odom='gt'."""
         super().__init__()
         if depth_filter is not None and not isinstance(depth_filter, BilateralFilter):
             raise TypeError("Expected depth_filter to be a BilateralFilter or None. Got {0}.".format(type(depth_filter)))
@@ -108,6 +118,12 @@ class ICPSLAM(nn.Module):
         if target_splat_px > 0 and association != "projective":
             raise ValueError("target_splat_px > 0 needs association='projective'")
         _check_photometric_weight(photometric_weight, association)
+        from ..odometry.icputils import _check_huber_delta
+
+        _check_huber_delta(huber_delta)
+        _check_huber_delta(photometric_huber_delta, "photometric_huber_delta")
+        if photometric_huber_delta is not None and not photometric_weight > 0:
+            raise ValueError("photometric_huber_delta needs photometric_weight > 0")
         if odom not in ["gt", "icp", "gradicp"]:
             msg = "odometry method ({}) not supported for PointFusion. ".format(odom)
             msg += "Currently supported odometry modules for PointFusion are: 'gt', 'icp', 'gradicp'"
@@ -116,17 +132,19 @@ class ICPSLAM(nn.Module):
         if odom == "icp":
             from ..odometry.icp import ICPOdometryProvider
 
-            odomprov = ICPOdometryProvider(numiters, damp, dist_thresh)
+            odomprov = ICPOdometryProvider(numiters, damp, dist_thresh, huber_delta=huber_delta)
         elif odom == "gradicp":
             from ..odometry.gradicp import GradICPOdometryProvider
 
-            odomprov = GradICPOdometryProvider(numiters, damp, dist_thresh, lambda_max, B, B2, nu)
+            odomprov = GradICPOdometryProvider(numiters, damp, dist_thresh, lambda_max, B, B2, nu,
+                                               huber_delta=huber_delta)
         self.odom = odom
         self.odomprov = odomprov
         self.dsratio = dsratio
         self.association = association
         self.target_splat_px = target_splat_px
         self.photometric_weight = float(photometric_weight)
+        self.photometric_huber_delta = photometric_huber_delta
         self.depth_filter = depth_filter
         self.depth_filter_tracking_only = depth_filter_tracking_only
         self.device = _normalize_device(device if device is not None else "cuda")
@@ -223,6 +241,9 @@ class ICPSLAM(nn.Module):
             if not pointclouds.has_normals:
                 raise ValueError("projective ICP association needs a map with normals")
             fn = localize_projective_taped if wants_grad else localize_projective
+            if self.photometric_huber_delta is not None:
+                return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov, self.target_splat_px,
+                          self.photometric_weight, self.photometric_huber_delta)
             if self.photometric_weight > 0:
                 return fn(pointclouds, live_frame, prev_frame, self.dsratio, self.odomprov, self.target_splat_px,
                           self.photometric_weight)

@@ -48,8 +48,12 @@ class PointFusion(ICPSLAM):
                  max_unstable_age: Optional[int] = None, free_space_margin: Union[float, int, None] = None,
                  surfel_radii: bool = False, merge_overlapping: bool = False, target_splat_px: int = 0,
                  photometric_weight: Union[float, int] = 0.0, depth_filter: Optional[BilateralFilter] = None,
-                 depth_filter_tracking_only: bool = False):
-        """stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
+                 depth_filter_tracking_only: bool = False, huber_delta: Union[float, int, None] = None,
+                 photometric_huber_delta: Union[float, int, None] = None):
+        """huber_delta, photometric_huber_delta (extension, None = off): Huber-weighted tracking residuals, as in
+        ICPSLAM.
+
+        stable_confidence, max_unstable_age (extension, give both or neither): after every map update, remove the
         surfels whose confidence is still below `stable_confidence` `max_unstable_age` frames after they were created
         (Keller et al. 2013, section 4.3).  Confidence is the map's `features_padded` value - gradslam's alpha,
         clamp(exp(-|v|^2 / 2 sigma^2), 1e-7, 1.01) of the camera-frame vertex, summed over merges - so a good threshold
@@ -109,7 +113,8 @@ class PointFusion(ICPSLAM):
         super().__init__(odom=odom, dsratio=dsratio, numiters=numiters, damp=damp, dist_thresh=dist_thresh,
                          lambda_max=lambda_max, B=B, B2=B2, nu=nu, association=association, device=device,
                          target_splat_px=target_splat_px, photometric_weight=photometric_weight,
-                         depth_filter=depth_filter, depth_filter_tracking_only=depth_filter_tracking_only)
+                         depth_filter=depth_filter, depth_filter_tracking_only=depth_filter_tracking_only,
+                         huber_delta=huber_delta, photometric_huber_delta=photometric_huber_delta)
         if target_splat_px > 0 and not surfel_radii:
             raise ValueError("target_splat_px > 0 needs surfel_radii=True (a map without radii has no disks)")
         if not isinstance(dist_th, (float, int)):

@@ -485,6 +485,21 @@ int gsx_icp_normal_eq_batched_bwd(const float *src_points, const int32_t *src_co
                                   const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
                                   const int64_t *nn_idx, const float *g_sums, float *g_src, float *g_tgt_points_rows,
                                   float *g_tgt_normals_rows, void *stream);
+/* Huber-weighted gsx_icp_normal_eq_batched_fwd / _bwd (the op of the robust differentiable mode), same arguments plus
+ * huber_delta.  A row with residual r and a = |r| <= huber_delta adds what the counterpart adds; a row with a > delta
+ * adds h (A_p A_q) and h (A_p r) with h = delta / a, and rho = delta ((a + a) - delta) instead of r r, so sums[27] is
+ * the Huber energy.  These are the row products of gsx_icp_localize_robust / gsx_icp_align_robust, bit for bit.  The
+ * backward carries dh/dr = -h / r of the h (A_p A_q) products and drho/dr = 2 h r.  huber_delta = +inf gives the
+ * counterpart's outputs bit for bit; a delta <= 0 or NaN is refused before any launch. */
+int gsx_icp_normal_eq_batched_robust_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                         const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
+                                         const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
+                                         float huber_delta, void *stream);
+int gsx_icp_normal_eq_batched_robust_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                         const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
+                                         const int64_t *nn_idx, const float *g_sums, float *g_src,
+                                         float *g_tgt_points_rows, float *g_tgt_normals_rows, float huber_delta,
+                                         void *stream);
 int gsx_icp_solve_fwd(const float *sums, const float *damp, int n, float *xi_out, float *dT_out, void *stream);
 int gsx_icp_solve_bwd(const float *sums, const float *damp, int n, const float *g_xi, const float *g_dT,
                       float *g_sums, float *g_damp, void *stream);
@@ -518,6 +533,15 @@ int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stri
                   const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
                   float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
                   int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, void *stream);
+/* gsx_icp_align with Huber-weighted point-to-plane rows (iteratively reweighted least squares inside the same LM /
+ * gradLM loop): each row is weighed as by gsx_icp_normal_eq_batched_robust_fwd at huber_delta (metres), and the error
+ * the loop compares (err, new_err) is the Huber energy sum rho.  Same arguments and scratch plus huber_delta; +inf gives
+ * gsx_icp_align's outputs bit for bit; a delta <= 0 or NaN is refused before any launch. */
+int gsx_icp_align_robust(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
+                         const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
+                         const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
+                         float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
+                         int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, float huber_delta, void *stream);
 
 /* ICPSLAM._localize for odom in {icp, gradicp} (gradslam/slam/icpslam.py:238-247) as one call:
  * source cloud = live depth on the ds-lattice placed at the previous pose (downsample_rgbdimages,
@@ -537,6 +561,15 @@ int gsx_icp_localize(const float *map_geometry, const int32_t *counts, int64_t c
                      float lambda_max, float Bp, float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity,
                      float *poses_out, int64_t poses_out_bstride, void *workspace,
                      int64_t workspace_map_capacity, uint32_t epoch, int32_t *overflow_flag, void *stream);
+/* gsx_icp_localize with the Huber-weighted rows of gsx_icp_align_robust.  Same arguments, workspace and target scratch
+ * plus huber_delta; +inf gives gsx_icp_localize's poses bit for bit; a delta <= 0 or NaN is refused before any launch. */
+int gsx_icp_localize_robust(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                            const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
+                            const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
+                            int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max,
+                            float Bp, float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
+                            int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity, uint32_t epoch,
+                            int32_t *overflow_flag, float huber_delta, void *stream);
 
 /* Projective frame-to-model ICP / gradICP odometry (an extension: the reference associates by exact 1-NN).  One call
  * per frame step: source cloud as in gsx_icp_localize (live depth on the ds-lattice at the previous pose, valid pixels
@@ -602,6 +635,22 @@ int gsx_icp_localize_projective_rgb(const float *map_geometry, const int32_t *co
                                     float B2p, float nu, float *poses_out, int64_t poses_out_bstride, void *workspace,
                                     int64_t workspace_bytes, int max_splat_px, const float *map_colours,
                                     const float *rgb, int64_t rgb_bstride, float photometric_weight, void *stream);
+/* gsx_icp_localize_projective_rgb with Huber-weighted residuals: the point-to-plane row at huber_delta (metres) as in
+ * gsx_icp_localize_robust, and the photometric row at photometric_huber_delta (intensity): outside it, with
+ * h_p = delta_p / |r_p|, its products enter as acc + (w h_p) (A_p A_q), acc + (w h_p) (A_p r_p) and acc + w rho_p.
+ * Same arguments plus the two scales; w = 0 and null colours keep the counterpart's meaning, and the workspace is
+ * gsx_icp_projective_rgb_workspace_bytes(B,H,W,ds).  Both scales +inf give the counterpart's poses bit for bit.
+ * A scale <= 0 or NaN, and a finite photometric_huber_delta with w = 0, are refused before any launch. */
+int gsx_icp_localize_projective_robust(const float *map_geometry, const int32_t *counts, int64_t capacity,
+                                       int64_t max_count, const float *depth, int64_t depth_bstride,
+                                       const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+                                       int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
+                                       float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
+                                       float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
+                                       void *workspace, int64_t workspace_bytes, int max_splat_px,
+                                       const float *map_colours, const float *rgb, int64_t rgb_bstride,
+                                       float photometric_weight, float huber_delta, float photometric_huber_delta,
+                                       void *stream);
 
 /* gsx_icp_projective_targets plus the model image I_m (B, H*W) of gsx_icp_localize_projective_rgb, 0 where uncovered.
  * map_colours may be NULL when max_count is 0. */
@@ -655,6 +704,30 @@ int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(const float *src_points, cons
                                                    float *g_tgt_normals_rows, float *g_stencil_colours_rows,
                                                    float *g_prev_poses, float *g_intrinsics, void *scratch,
                                                    int64_t scratch_bytes, void *stream);
+/* Huber-weighted gsx_icp_joint_normal_eq_batched_fwd and gsx_icp_joint_normal_eq_batched_bwd_intrinsics (the op of the
+ * robust differentiable projective mode): same arguments plus huber_delta and photometric_huber_delta, the rows of
+ * gsx_icp_localize_projective_robust bit for bit.  The backward's g_intrinsics may be NULL, with the scratch sizes of
+ * gsx_icp_joint_normal_eq_batched_bwd_intrinsics.  Both scales +inf give the counterparts' outputs bit for bit; a scale
+ * <= 0 or NaN is refused before any launch. */
+int gsx_icp_joint_normal_eq_batched_robust_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                               const float *src_colours, const float *tgt_points,
+                                               const float *tgt_normals, const float *model_colours,
+                                               const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                                               const float *prev_poses, const float *intrinsics,
+                                               float photometric_weight, float *sums_out, void *scratch,
+                                               int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
+                                               void *stream);
+int gsx_icp_joint_normal_eq_batched_robust_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                               const float *src_colours, const float *tgt_points,
+                                               const float *tgt_normals, const float *model_colours,
+                                               const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
+                                               const float *prev_poses, const float *intrinsics,
+                                               float photometric_weight, const float *g_sums, float *g_src,
+                                               float *g_src_colours, float *g_tgt_points_rows,
+                                               float *g_tgt_normals_rows, float *g_stencil_colours_rows,
+                                               float *g_prev_poses, float *g_intrinsics, void *scratch,
+                                               int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
+                                               void *stream);
 
 /* The association of gsx_icp_localize_projective alone (the index-only op of the differentiable mode): for the source
  * rows i < src_count[b] of src_points (B, ns_stride, 3), world frame, idx_out int64 (B, ns_stride) = the pixel
