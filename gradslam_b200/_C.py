@@ -51,6 +51,19 @@ SIGNATURES = {
     "gsx_fusion_merge_append_bwd": (
         c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int,
                 c_double, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "gsx_fusion_merge_append_rec": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_int,
+                c_vp]),
+    "gsx_embed_merge_append": (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "gsx_embed_merge_bwd": (
+        c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                c_vp]),
+    "gsx_fusion_merge_append_bwd_emb": (
+        c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int,
+                c_double, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "gsx_pointfusion_sequence_gt_emb": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                c_float, c_float, c_double, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp]),
     "gsx_pointfusion_sequence_groups": (c_int, [c_int]),
     "gsx_pointfusion_sequence_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
     "gsx_pointfusion_sequence_gt": (

@@ -8,6 +8,7 @@
 #include <mutex>
 
 #include "gsx_common.cuh"
+#include "gsx_embed.cuh"
 #include "gsx_fusion_ws.cuh"
 #include "gsx_prune.cuh"
 #include "../../include/gsx.h"
@@ -35,7 +36,33 @@ int sequence_headers_group(const float *poses, const float *K, const float *dept
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
                         int64_t rgb_bs, int B_total, int b0, int nb, int s, int H, int W, float dist_th, float dot_th,
-                        void *workspace, int32_t *overflow, int32_t *assoc, bool radii, cudaStream_t st);
+                        void *workspace, int32_t *overflow, int32_t *assoc, float2 *rec, bool radii,
+                        cudaStream_t st);
+
+// Embeddings of the sequence driver: map rows E (B, cap, D), frames e (B, L, H, W, D) dense, both of `dtype` (0 float32,
+// 1 float16, 2 bfloat16); assoc int32 and rec float2, each (B, H, W): K4's record of every frame, read by KE.
+struct SequenceEmbed {
+  void *E;
+  const void *e;
+  int D, dtype;
+  int32_t *assoc;
+  float2 *rec;
+};
+
+// the group's K4 record zeroed, K4 done by the caller, then KE of frame s for elements [b0, b0 + nb)
+static int32_t *sequence_embed_assoc(const SequenceEmbed *emb, int b0, int nb, int64_t P, cudaStream_t st) {
+  if (!emb) return nullptr;
+  cudaMemsetAsync(emb->assoc + (int64_t)b0 * P, 0, (size_t)nb * P * sizeof(int32_t), st);
+  return emb->assoc;
+}
+static int sequence_embed_group(const SequenceEmbed *emb, int64_t cap, int L, int s, int b0, int nb, int64_t P,
+                                cudaStream_t st) {
+  const int64_t es = emb->dtype == 0 ? 4 : 2;
+  const EmbedArgs a{(char *)emb->E + (int64_t)b0 * cap * emb->D * es,
+                    (const char *)emb->e + ((int64_t)b0 * L + s) * P * emb->D * es, (int64_t)L * P * emb->D,
+                    emb->assoc + (int64_t)b0 * P, emb->rec + (int64_t)b0 * P, cap, nb, (int)P, emb->D};
+  return launch_embed_merge_append(a, emb->dtype, st);
+}
 
 // Pruning of the sequence driver (Keller et al. 2013): frame s of the call is pruned step s; null = pruning off.
 // fs_scratch non-null adds the free-space rule: K4 records where each pixel went (its group's slice of the scratch's
@@ -120,15 +147,13 @@ extern "C" void gsx_debug_fail_at_frame(int s) { g_fail_at_frame = s; }
 
 extern "C" int gsx_pointfusion_sequence_groups(int B) { return B <= 0 ? 0 : gsx::sequence_groups(B); }
 
-extern "C" int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map_colors, int32_t *counts,
-                                                 int64_t capacity, int64_t max_count0, const float *depth,
-                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
-                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
-                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
-                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
-                                                 float margin, void *fs_scratch, int64_t fs_scratch_bytes,
-                                                 int32_t *overflow_flag, int surfel_radii, void *merge_scratch,
-                                                 int64_t merge_scratch_bytes, void *stream) {
+static int sequence_driver(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                           int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
+                           const float *poses, int B, int L, int s_begin, int s_end, int H, int W, float dist_th,
+                           float dot_th, double sigma, void *workspace, int32_t *ring, int t_max, float c_stable,
+                           void *prune_scratch, int64_t prune_scratch_bytes, float margin, void *fs_scratch,
+                           int64_t fs_scratch_bytes, int32_t *overflow_flag, int surfel_radii, void *merge_scratch,
+                           int64_t merge_scratch_bytes, const gsx::SequenceEmbed *emb, void *stream) {
   GSX_CHECK_ARG(B >= 0 && L >= 0 && H >= 2 && W >= 2, "gsx_pointfusion_sequence_gt: bad extents");
   GSX_CHECK_ARG(surfel_radii == 0 || surfel_radii == 1,
                 "gsx_pointfusion_sequence_gt: surfel_radii must be 0 or 1, not %d", surfel_radii);
@@ -197,7 +222,10 @@ extern "C" int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map
                                       counts + (int64_t)((s + 1) & 1) * B, capacity, max_count, poses + (int64_t)s * 16,
                                       (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, 0, B,
                                       s, H, W, dist_th, dot_th, workspace, overflow_flag,
-                                      gsx::sequence_assoc(prune, B, 0, B, H, W, capacity, user), radii, user);
+                                      emb ? gsx::sequence_embed_assoc(emb, 0, B, P, user)
+                                          : gsx::sequence_assoc(prune, B, 0, B, H, W, capacity, user),
+                                      emb ? emb->rec : nullptr, radii, user);
+      if (rc == 0 && emb) rc = gsx::sequence_embed_group(emb, capacity, L, s, 0, B, P, user);
       if (rc == 0 && prune)
         rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, counts + (int64_t)((s + 1) & 1) * B, capacity,
                                        intrinsics, poses + (int64_t)s * 16, (int64_t)L * 16, B, 0, B, s, H, W,
@@ -228,8 +256,10 @@ extern "C" int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map
       rc = gsx::fusion_update_group(map_geometry, map_colors, cin, cout, capacity, max_count, poses + (int64_t)s * 16,
                                     (int64_t)L * 16, intrinsics, 16, rgb + (int64_t)s * P * 3, (int64_t)L * P * 3, B, b0,
                                     b1 - b0, s, H, W, dist_th, dot_th, workspace, overflow_flag,
-                                    gsx::sequence_assoc(prune, B, b0, b1 - b0, H, W, capacity, gs->stream[g]), radii,
-                                    gs->stream[g]);
+                                    emb ? gsx::sequence_embed_assoc(emb, b0, b1 - b0, P, gs->stream[g])
+                                        : gsx::sequence_assoc(prune, B, b0, b1 - b0, H, W, capacity, gs->stream[g]),
+                                    emb ? emb->rec : nullptr, radii, gs->stream[g]);
+      if (rc == 0 && emb) rc = gsx::sequence_embed_group(emb, capacity, L, s, b0, b1 - b0, P, gs->stream[g]);
       if (rc == 0 && prune)
         rc = gsx::sequence_prune_group(prune, map_geometry, map_colors, cout, capacity, intrinsics,
                                        poses + (int64_t)s * 16, (int64_t)L * 16, B, b0, b1 - b0, s, H, W,
@@ -243,6 +273,43 @@ extern "C" int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map
     cudaStreamWaitEvent(user, gs->join[g], 0);
   }
   return rc;
+}
+
+extern "C" int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map_colors, int32_t *counts,
+                                                 int64_t capacity, int64_t max_count0, const float *depth,
+                                                 const float *rgb, const float *intrinsics, const float *poses, int B,
+                                                 int L, int s_begin, int s_end, int H, int W, float dist_th,
+                                                 float dot_th, double sigma, void *workspace, int32_t *ring, int t_max,
+                                                 float c_stable, void *prune_scratch, int64_t prune_scratch_bytes,
+                                                 float margin, void *fs_scratch, int64_t fs_scratch_bytes,
+                                                 int32_t *overflow_flag, int surfel_radii, void *merge_scratch,
+                                                 int64_t merge_scratch_bytes, void *stream) {
+  return sequence_driver(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
+                         s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, ring, t_max, c_stable, prune_scratch,
+                         prune_scratch_bytes, margin, fs_scratch, fs_scratch_bytes, overflow_flag, surfel_radii,
+                         merge_scratch, merge_scratch_bytes, nullptr, stream);
+}
+
+extern "C" int gsx_pointfusion_sequence_gt_emb(float *map_geometry, float *map_colors, int32_t *counts,
+                                               int64_t capacity, int64_t max_count0, const float *depth,
+                                               const float *rgb, const float *intrinsics, const float *poses, int B,
+                                               int L, int s_begin, int s_end, int H, int W, float dist_th,
+                                               float dot_th, double sigma, void *workspace, int32_t *overflow_flag,
+                                               int surfel_radii, void *map_embeddings,
+                                               const void *frame_embeddings, int D, int dtype, int32_t *assoc,
+                                               float *merge_rec, void *stream) {
+  GSX_CHECK_ARG(D >= 1 && dtype >= 0 && dtype <= 2,
+                "gsx_pointfusion_sequence_gt_emb: need D >= 1 and dtype 0 (float32), 1 (float16) or 2 (bfloat16)");
+  GSX_CHECK_ARG(B == 0 || s_begin == s_end || (map_embeddings && frame_embeddings && assoc && merge_rec),
+                "gsx_pointfusion_sequence_gt_emb: null embedding pointer");
+  GSX_CHECK_ARG(((reinterpret_cast<uintptr_t>(map_embeddings) | reinterpret_cast<uintptr_t>(frame_embeddings)) &
+                 (dtype == 0 ? 3 : 1)) == 0 && (reinterpret_cast<uintptr_t>(merge_rec) & 7) == 0,
+                "gsx_pointfusion_sequence_gt_emb: misaligned embeddings or record");
+  const gsx::SequenceEmbed emb{map_embeddings, frame_embeddings, D, dtype, assoc,
+                               reinterpret_cast<float2 *>(merge_rec)};
+  return sequence_driver(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
+                         s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, nullptr, 0, 0.0f, nullptr, 0, 0.0f,
+                         nullptr, 0, overflow_flag, surfel_radii, nullptr, 0, &emb, stream);
 }
 
 extern "C" int gsx_pointfusion_sequence_gt_radii(float *map_geometry, float *map_colors, int32_t *counts,

@@ -1,0 +1,20 @@
+// The embedding merge KE (gsx_embed.cu), as the sequence driver (gsx_api.cu) launches it.
+#pragma once
+#include "gsx_common.cuh"
+
+namespace gsx {
+
+struct EmbedArgs {
+  void *E;          // (B, cap, D) map embeddings
+  const void *e;    // frame embeddings: pixel p of element b starts at b * e_bstride + p * D (elements)
+  int64_t e_bstride;
+  const int32_t *assoc;  // (B, P): -(n+1) merged into row n, n+1 appended as row n, 0 untouched
+  const float2 *rec;     // (B, P): (c0, alpha) of every merged pixel
+  int64_t cap;
+  int B, P, D;
+};
+
+// KE over the pixels of elements [0, a.B); dtype 0 float32, 1 float16, 2 bfloat16
+int launch_embed_merge_append(const EmbedArgs &a, int dtype, cudaStream_t st);
+
+}  // namespace gsx

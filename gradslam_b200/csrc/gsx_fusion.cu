@@ -321,6 +321,7 @@ struct MergeArgs {
   int32_t *overflow;
   int32_t *assoc;  // optional (B,P): +row+1 appended at `row`, -(row+1) merged into `row`, 0 untouched
   int bin_cap;     // records per candidate bin that K2 filled (set at launch)
+  float2 *rec;     // optional (B,P), needs assoc: (c0, alpha) of every merged pixel, for the embedding merge (KE)
 };
 
 #ifndef GSX_K4_MINB
@@ -336,7 +337,9 @@ __device__ __forceinline__ void prefetch_l2(const float *p) { asm volatile("pref
 // kRadii: slot 7 of every merged or appended row holds the surfel radius (surfel_radius of the pixel; a merge takes the
 // confidence-weighted mean of the row's radius and the pixel's, as for the position, and a row of radius 0 adopts the
 // pixel's).  Nothing else depends on it: slots 0-6 and the colour rows are those of kRadii = false, bit for bit.
-template <bool kAssoc, bool kRadii>
+// kEmbRec (needs kAssoc): every merged pixel also leaves its merge's c0 and alpha in a.rec, which KE
+// (k_embed_merge_append, gsx_embed.cu) reads to merge the surfel embeddings with the same weights.
+template <bool kAssoc, bool kRadii, bool kEmbRec = false>
 __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) {
   __shared__ unsigned int s_ticket, s_table;
   __shared__ int s_warp_sums[kPix][kMB / 32];
@@ -544,6 +547,7 @@ __global__ void __launch_bounds__(kMB, GSX_K4_MINB) k_merge_append(MergeArgs a) 
       *reinterpret_cast<float4 *>(geo + n * kGeoW + 4) = o1;
       *reinterpret_cast<float4 *>(col + n * kColW) = oc;
       if (kAssoc) a.assoc[(int64_t)b * P + pix[j]] = -(int32_t)(n + 1);
+      if (kEmbRec) a.rec[(int64_t)b * P + pix[j]] = make_float2(c0, alpha);
     }
   }
 
@@ -586,7 +590,12 @@ int launch_merge_append(const MergeArgs &args, bool radii, cudaStream_t stream) 
   MergeArgs a = args;
   a.bin_cap = bin_capacity();
   const dim3 grid((unsigned)(a.ws.tiles * a.B));
-  if (a.assoc) {  // differentiable forward, or the free-space step's record
+  if (a.rec) {  // the embedding merge's record (a.assoc is set as well)
+    if (radii)
+      k_merge_append<true, true, true><<<grid, kMB, 0, stream>>>(a);
+    else
+      k_merge_append<true, false, true><<<grid, kMB, 0, stream>>>(a);
+  } else if (a.assoc) {  // differentiable forward, or the free-space step's record
     if (radii)
       k_merge_append<true, true><<<grid, kMB, 0, stream>>>(a);
     else
@@ -626,6 +635,7 @@ struct MergeBwdArgs {
   float *d_gv, *d_gn, *d_rgb, *d_vloc;  // (B, P, 3)
   int B, P;
   float two_sigma_sq;
+  const float *emb_dc0, *emb_dalpha;  // (B,P) the embedding merge's terms of d c0 and d alpha (kEmb; gsx_embed.cu)
 };
 
 // rows the frame did not touch pass their gradient through; padding rows get zero
@@ -651,6 +661,9 @@ __global__ void __launch_bounds__(256) k_merge_bwd_rows(MergeBwdArgs a) {
   *reinterpret_cast<float4 *>(a.d_col + ri * kColW) = gc;
 }
 
+// kEmb: the embedding merge's per-pixel terms (k_embed_merge_bwd) join d c0 and d alpha of every merged pixel, so that
+// its gradient reaches the pre-merge confidence and, through alpha, the camera-frame vertex
+template <bool kEmb = false>
 __global__ void __launch_bounds__(256) k_merge_bwd_pixels(MergeBwdArgs a) {
   const int b = blockIdx.y;
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
@@ -705,6 +718,10 @@ __global__ void __launch_bounds__(256) k_merge_bwd_pixels(MergeBwdArgs a) {
         df[q] = g[q] * alpha * inv;
         d_c0 += g[q] * (m[q] * inv + num * dinv);
         d_alpha += g[q] * (f[q] * inv + num * dinv);
+      }
+      if (kEmb) {
+        d_c0 += a.emb_dc0[(int64_t)b * a.P + pix];
+        d_alpha += a.emb_dalpha[(int64_t)b * a.P + pix];
       }
 #pragma unroll
       for (int q = 0; q < 6; ++q) a.d_geo[ri * kGeoW + q] = dm[q];
@@ -791,7 +808,8 @@ static Workspace group_workspace(void *workspace, int B_total, int b0, int H, in
 int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cout, int64_t cap, int64_t max_count,
                         const float *poses, int64_t pose_bs, const float *K, int64_t K_bs, const float *rgb,
                         int64_t rgb_bs, int B_total, int b0, int nb, int s, int H, int W, float dist_th, float dot_th,
-                        void *workspace, int32_t *overflow, int32_t *assoc, bool radii, cudaStream_t st) {
+                        void *workspace, int32_t *overflow, int32_t *assoc, float2 *rec, bool radii,
+                        cudaStream_t st) {
   Workspace ws = group_workspace(workspace, B_total, b0, H, W);
   ws.hdr = seq_headers(workspace, B_total, H, W) + (int64_t)(s % kSeqFrames) * B_total + b0;
   float *ggeo = geo + (int64_t)b0 * cap * kGeoW, *gcol = col + (int64_t)b0 * cap * kColW;
@@ -802,9 +820,10 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
     const int rc = launch_project_select(pa, max_count, st);
     if (rc) return rc;
   }
-  // assoc (full-batch base, zeroed by the caller, or null): where each pixel went, for the free-space step
+  // assoc (full-batch base, zeroed by the caller, or null): where each pixel went, for the free-space step or the
+  // embedding merge; rec (full-batch base, or null; needs assoc): the embedding merge's weights
   MergeArgs ma{ggeo, gcol, 1, cin + b0, cout + b0, cap, rgb + (int64_t)b0 * rgb_bs, rgb_bs, nb, H, W, ws, overflow,
-               assoc ? assoc + (int64_t)b0 * H * W : nullptr, 0};
+               assoc ? assoc + (int64_t)b0 * H * W : nullptr, 0, rec ? rec + (int64_t)b0 * H * W : nullptr};
   return launch_merge_append(ma, radii, st);
 }
 
@@ -895,6 +914,30 @@ extern "C" int gsx_fusion_merge_append_radii(float *map_geometry, float *map_col
   return launch_merge_append(a, surfel_radii != 0, (cudaStream_t)stream);
 }
 
+extern "C" int gsx_fusion_merge_append_rec(float *map_geometry, float *map_colors, int with_ccounts,
+                                           const int32_t *counts_in, int32_t *counts_out, int64_t capacity,
+                                           const float *rgb, int64_t rgb_bstride, int B, int H, int W,
+                                           void *workspace, int32_t *overflow_flag, int32_t *assoc_out,
+                                           float *merge_rec, int surfel_radii, void *stream) {
+  GSX_CHECK_ARG(B == 0 || (assoc_out && merge_rec), "gsx_fusion_merge_append_rec: null assoc_out / merge_rec");
+  GSX_CHECK_ARG(B >= 0 && H >= 2 && W >= 2, "gsx_fusion_merge_append: bad extents B=%d H=%d W=%d", B, H, W);
+  GSX_CHECK_ARG(surfel_radii == 0 || surfel_radii == 1, "gsx_fusion_merge_append: surfel_radii must be 0 or 1, not %d",
+                surfel_radii);
+  if (B == 0) return 0;
+  GSX_CHECK_ARG(map_geometry && map_colors && counts_in && counts_out, "gsx_fusion_merge_append: null map pointer");
+  GSX_CHECK_ARG(counts_in != counts_out, "gsx_fusion_merge_append: counts_in and counts_out must not alias");
+  GSX_CHECK_ARG(rgb && workspace && overflow_flag, "gsx_fusion_merge_append: null frame pointer");
+  GSX_CHECK_ARG(aligned16(map_geometry) && aligned16(map_colors) && aligned16(workspace),
+                "gsx_fusion_merge_append: map rows and workspace must be 16-byte aligned");
+  GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(merge_rec) & 7) == 0, "gsx_fusion_merge_append_rec: merge_rec must be "
+                "8-byte aligned");
+  GSX_CHECK_ARG(capacity <= 0x7fffffffll, "gsx_fusion_merge_append: capacity must fit int32 (counts are int32)");
+  MergeArgs a{map_geometry, map_colors, with_ccounts ? 1 : 0, counts_in, counts_out, capacity, rgb, rgb_bstride, B, H,
+              W, fusion_workspace(workspace, B, H, W), overflow_flag, assoc_out, 0,
+              reinterpret_cast<float2 *>(merge_rec)};
+  return launch_merge_append(a, surfel_radii != 0, (cudaStream_t)stream);
+}
+
 extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, int with_ccounts,
                                        const int32_t *counts_in, int32_t *counts_out, int64_t capacity,
                                        const float *rgb, int64_t rgb_bstride, int B, int H, int W, void *workspace,
@@ -903,13 +946,13 @@ extern "C" int gsx_fusion_merge_append(float *map_geometry, float *map_colors, i
                                        rgb_bstride, B, H, W, workspace, overflow_flag, assoc_out, 0, stream);
 }
 
-extern "C" int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, const float *map_geometry,
-                                           const float *map_colors, int with_ccounts, int64_t capacity_in,
-                                           const float *g_geometry, const float *g_colors, int64_t capacity_out,
-                                           const float *gvertex, const float *gnormal, const float *rgb,
-                                           const float *vertex, int B, int H, int W, double sigma,
-                                           float *d_map_geometry, float *d_map_colors, float *d_gvertex,
-                                           float *d_gnormal, float *d_rgb, float *d_vertex, void *stream) {
+static int merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, const float *map_geometry,
+                            const float *map_colors, int with_ccounts, int64_t capacity_in, const float *g_geometry,
+                            const float *g_colors, int64_t capacity_out, const float *gvertex, const float *gnormal,
+                            const float *rgb, const float *vertex, int B, int H, int W, double sigma,
+                            float *d_map_geometry, float *d_map_colors, float *d_gvertex, float *d_gnormal,
+                            float *d_rgb, float *d_vertex, const float *emb_dc0, const float *emb_dalpha,
+                            void *stream) {
   GSX_CHECK_ARG(B >= 0 && H >= 2 && W >= 2, "gsx_fusion_merge_append_bwd: bad extents B=%d H=%d W=%d", B, H, W);
   if (B == 0) return 0;
   GSX_CHECK_ARG(assoc && counts_in && gvertex && gnormal && rgb && vertex, "gsx_fusion_merge_append_bwd: null input");
@@ -921,13 +964,43 @@ extern "C" int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *
                 "gsx_fusion_merge_append_bwd: map rows must be 16-byte aligned");
   MergeBwdArgs a{assoc, counts_in, map_geometry, map_colors, with_ccounts ? 1 : 0, capacity_in, g_geometry, g_colors,
                  capacity_out, gvertex, gnormal, rgb, vertex, d_map_geometry, d_map_colors, d_gvertex, d_gnormal, d_rgb,
-                 d_vertex, B, H * W, (float)(2.0 * (sigma * sigma))};
+                 d_vertex, B, H * W, (float)(2.0 * (sigma * sigma)), emb_dc0, emb_dalpha};
   cudaStream_t st = (cudaStream_t)stream;
   if (capacity_in > 0) {
     k_merge_bwd_rows<<<dim3((unsigned)((capacity_in + 255) / 256), (unsigned)B), 256, 0, st>>>(a);
     GSX_CHECK_LAUNCH("gsx_fusion_merge_append_bwd(rows)");
   }
-  k_merge_bwd_pixels<<<dim3((unsigned)((a.P + 255) / 256), (unsigned)B), 256, 0, st>>>(a);
+  const dim3 grid((unsigned)((a.P + 255) / 256), (unsigned)B);
+  if (emb_dc0)
+    k_merge_bwd_pixels<true><<<grid, 256, 0, st>>>(a);
+  else
+    k_merge_bwd_pixels<false><<<grid, 256, 0, st>>>(a);
   GSX_CHECK_LAUNCH("gsx_fusion_merge_append_bwd(pixels)");
   return 0;
+}
+
+extern "C" int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, const float *map_geometry,
+                                           const float *map_colors, int with_ccounts, int64_t capacity_in,
+                                           const float *g_geometry, const float *g_colors, int64_t capacity_out,
+                                           const float *gvertex, const float *gnormal, const float *rgb,
+                                           const float *vertex, int B, int H, int W, double sigma,
+                                           float *d_map_geometry, float *d_map_colors, float *d_gvertex,
+                                           float *d_gnormal, float *d_rgb, float *d_vertex, void *stream) {
+  return merge_append_bwd(assoc, counts_in, map_geometry, map_colors, with_ccounts, capacity_in, g_geometry, g_colors,
+                          capacity_out, gvertex, gnormal, rgb, vertex, B, H, W, sigma, d_map_geometry, d_map_colors,
+                          d_gvertex, d_gnormal, d_rgb, d_vertex, nullptr, nullptr, stream);
+}
+
+extern "C" int gsx_fusion_merge_append_bwd_emb(const int32_t *assoc, const int32_t *counts_in,
+                                               const float *map_geometry, const float *map_colors, int with_ccounts,
+                                               int64_t capacity_in, const float *g_geometry, const float *g_colors,
+                                               int64_t capacity_out, const float *gvertex, const float *gnormal,
+                                               const float *rgb, const float *vertex, int B, int H, int W,
+                                               double sigma, const float *emb_d_c0, const float *emb_d_alpha,
+                                               float *d_map_geometry, float *d_map_colors, float *d_gvertex,
+                                               float *d_gnormal, float *d_rgb, float *d_vertex, void *stream) {
+  GSX_CHECK_ARG(B == 0 || (emb_d_c0 && emb_d_alpha), "gsx_fusion_merge_append_bwd_emb: null embedding term");
+  return merge_append_bwd(assoc, counts_in, map_geometry, map_colors, with_ccounts, capacity_in, g_geometry, g_colors,
+                          capacity_out, gvertex, gnormal, rgb, vertex, B, H, W, sigma, d_map_geometry, d_map_colors,
+                          d_gvertex, d_gnormal, d_rgb, d_vertex, emb_d_c0, emb_d_alpha, stream);
 }

@@ -164,7 +164,10 @@ def gather_maps_begin(pointclouds: Pointclouds, group=None, into: Optional[Gathe
     """First half of the map all-gather: exchanges the per-sequence sizes on a side (communication) stream and
     starts their copy to pinned host memory.  Does NOT block the host, so the caller can enqueue the next batch of
     sequences before calling `gather_maps_end` — the exchange then overlaps that compute.
-    into: the GatheredMaps store whose `local` block `pointclouds` is (see there)."""
+    into: the GatheredMaps store whose `local` block `pointclouds` is (see there).  Maps with per-surfel embeddings
+    are refused: the exchange moves the geometry and colour rows only."""
+    if pointclouds.has_points and pointclouds.has_embeddings:
+        raise ValueError("gather_maps does not exchange per-surfel embeddings; gather maps without them")
     h = _GatherHandle()
     h.pc, h.group, h.world = pointclouds, group, dist.get_world_size(group)
     h.into = into

@@ -15,7 +15,7 @@ from typing import Union
 import torch
 
 from .. import _C
-from ..structures.pointclouds import Pointclouds, _PruneHistory
+from ..structures.pointclouds import EMBED_DTYPES, Pointclouds, _PruneHistory
 from ..structures.rgbdimages import RGBDImages, _frame_base
 
 __all__ = ["update_map_fusion", "update_map_aggregate", "prune_unstable", "fuse_and_prune"]
@@ -91,6 +91,7 @@ class _Workspace:
         self.buf = torch.zeros(nbytes, dtype=torch.uint8, device=device)
         self.shape = (B, H * W)
         self.assoc = None  # K4's per-pixel record for the free-space step (fuse_and_prune), allocated on first use
+        self.rec = None  # K4's (c0, alpha) of every merged pixel, for the embedding merge (KE), allocated on first use
 
     def zeroed_assoc(self):
         """int32 (B, H*W) buffer for K4's assoc_out, zeroed in stream order (K4 writes only merged / appended pixels)."""
@@ -99,6 +100,13 @@ class _Workspace:
         else:
             self.assoc.zero_()
         return self.assoc
+
+    def merge_rec(self):
+        """float32 (B, H*W, 2) buffer for K4's merge_rec: KE reads only the records of merged pixels, so it is never
+        cleared."""
+        if self.rec is None:
+            self.rec = torch.empty(self.shape + (2,), dtype=torch.float32, device=self.buf.device)
+        return self.rec
 
     @classmethod
     def get(cls, device, B, H, W):
@@ -167,8 +175,16 @@ def _dense_frame(t, name, device):
     return t
 
 
+def _embedding_frame(e, device):
+    """(B,1,H,W,D) channels-last embedding image -> (base tensor, element stride) for KE."""
+    if not e.is_cuda or e.device != device:
+        raise ValueError("gradslam_b200: `embeddings` is on {} but the map lives on {}".format(e.device, device))
+    return _frame_base(e.detach(), e.shape[2] * e.shape[3] * e.shape[4])
+
+
 def _launch_merge_append(pointclouds, frames, ws, assoc=None, radii=False):
-    """K4 on the current workspace state (frame records + per-pixel winners); radii: write surfel radii (slot 7)."""
+    """K4 on the current workspace state (frame records + per-pixel winners); radii: write surfel radii (slot 7).  A
+    frame with embeddings runs K4 with its merge record, then KE on the map's embedding store."""
     B, _, H, W = frames.shape
     P = H * W
     dev = pointclouds.device
@@ -176,8 +192,22 @@ def _launch_merge_append(pointclouds, frames, ws, assoc=None, radii=False):
     geo, col = _map_ptrs(pointclouds, dev)
     cin = pointclouds._counts_dev[pointclouds._cur]
     cout = pointclouds._counts_dev[pointclouds._cur ^ 1]
-    _C.launch("gsx_fusion_merge_append_radii", geo, col, 1 if pointclouds._has_cc else 0, cin, cout,
-              pointclouds.capacity, rgb, c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, 1 if radii else 0)
+    if frames.embeddings is None:
+        _C.launch("gsx_fusion_merge_append_radii", geo, col, 1 if pointclouds._has_cc else 0, cin, cout,
+                  pointclouds.capacity, rgb, c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc,
+                  1 if radii else 0)
+    else:
+        e, e_bs = _embedding_frame(frames.embeddings, dev)
+        if pointclouds._emb is None:  # (a map this update starts)
+            pointclouds._alloc_embeddings(e.shape[-1], e.dtype)
+        emb = pointclouds._emb = pointclouds._emb.contiguous()
+        assoc = ws.zeroed_assoc() if assoc is None else assoc
+        rec = ws.merge_rec()
+        _C.launch("gsx_fusion_merge_append_rec", geo, col, 1 if pointclouds._has_cc else 0, cin, cout,
+                  pointclouds.capacity, rgb, c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, rec,
+                  1 if radii else 0)
+        _C.launch("gsx_embed_merge_append", emb, pointclouds.capacity, e, e_bs, assoc, rec, B, H, W, e.shape[-1],
+                  EMBED_DTYPES[e.dtype])
     pointclouds._mark_device_updated(pointclouds._bound + P)
 
 
@@ -206,6 +236,7 @@ def _append_valid_pixels(pointclouds, frames, global_coordinates=True, sigma=0.6
     if had_points and pointclouds._feat is not None:
         raise ValueError("pointclouds to append and to be appended must have the same number of features")
     with_features = pointclouds.has_features if had_points else False
+    _check_embeddings(pointclouds, frames)
     _prepare_map(pointclouds, frames, with_features)
     B, _, H, W = frames.shape
     dev = pointclouds.device
@@ -213,6 +244,30 @@ def _append_valid_pixels(pointclouds, frames, global_coordinates=True, sigma=0.6
     _launch_frame_records(ws, frames, _sigma_value(sigma), dev, world=global_coordinates)
     _launch_merge_append(pointclouds, frames, ws)
     return pointclouds
+
+
+def _check_embeddings(pointclouds, rgbdimages):
+    """A map update carries embeddings when the map and the frame both have them, or the map is empty and the frame has
+    them; any other mismatch is refused, as is half precision in the differentiable mode.  Host-side only."""
+    e = rgbdimages.embeddings
+    if pointclouds.has_points:
+        if pointclouds.has_embeddings != (e is not None):
+            raise ValueError("the map {} embeddings but the frame {}: both or neither must carry them".format(
+                "has" if pointclouds.has_embeddings else "has no", "does not" if e is None else "does"))
+        if e is not None:
+            D = e.shape[rgbdimages.cdim]
+            if (pointclouds._emb.shape[2], pointclouds._emb.dtype) != (D, e.dtype):
+                raise ValueError("the map's embeddings (D={}, {}) and the frame's (D={}, {}) differ".format(
+                    pointclouds._emb.shape[2], pointclouds._emb.dtype, D, e.dtype))
+    if e is not None and e.dtype != torch.float32 and _wants_grad(pointclouds, rgbdimages):
+        raise TypeError("the differentiable map update supports float32 embeddings only; got {}".format(e.dtype))
+
+
+def _refuse_embeddings(pointclouds, what, rgbdimages=None):
+    if (pointclouds.has_points and pointclouds.has_embeddings) or (rgbdimages is not None and
+                                                                   rgbdimages.embeddings is not None):
+        raise ValueError("{} is not supported on maps with embeddings: its compaction would have to move the "
+                         "embedding rows too".format(what))
 
 
 def _check_fusion_inputs(pointclouds, rgbdimages):
@@ -408,6 +463,7 @@ def fuse_with_map(pointclouds: Pointclouds, rgbdimages: RGBDImages, pc2im_bnhw: 
         if not pointclouds.has_features:
             raise ValueError("Pointclouds must have features (ccounts) for map fusion, but did not.")
     _check_frame(rgbdimages)
+    _check_embeddings(pointclouds, rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
     return _fuse(pointclouds, rgbdimages, sigma, table=pc2im_bnhw, radii=surfel_radii)
@@ -437,7 +493,8 @@ def _launch_association(ws, pointclouds, frames, dist_th=None, dot_th=None, tabl
 def _wants_grad(pointclouds, frames):
     if not torch.is_grad_enabled():
         return False
-    ts = [frames.depth_image, frames.poses, frames.rgb_image, frames.intrinsics] + pointclouds._grad_tensors()
+    ts = [frames.depth_image, frames.poses, frames.rgb_image, frames.intrinsics, frames.embeddings,
+          pointclouds._emb] + pointclouds._grad_tensors()
     return any(torch.is_tensor(t) and t.requires_grad for t in ts)
 
 
@@ -448,10 +505,13 @@ class _MergeAppendFn(torch.autograd.Function):
     points / normals / colors / features / radii tensors are slices of the rows, so autograd carries the gradients in
     and out of the rows by itself).  The radii carry no gradient: the gradient w.r.t. `radii_padded` is identically
     zero.  The frame records and the per-pixel winners must already sit in the fusion workspace
-    (K1r; K2, or gsx_records_from_table); the winners are index-only, as in the reference (fusionutils.py:523)."""
+    (K1r; K2, or gsx_records_from_table); the winners are index-only, as in the reference (fusionutils.py:523).
+    With the map's embeddings `emb` (B, cap, D) and the frame's `e` (B, 1, H, W, D), float32, K4 also records each
+    merge's weights and KE (gsx_embed_merge_append) merges the embeddings, a third output; the backward runs
+    gsx_embed_merge_bwd first and hands its d c0 / d alpha terms to K4's (gsx_fusion_merge_append_bwd_emb)."""
 
     @staticmethod
-    def forward(ctx, pack, geo, col, gv, gn, rgb, vloc):
+    def forward(ctx, pack, geo, col, gv, gn, rgb, vloc, emb=None, e=None):
         pointclouds, frames, sigma, ws, _, radii = pack
         B, _, H, W = frames.shape
         P = H * W
@@ -468,8 +528,22 @@ class _MergeAppendFn(torch.autograd.Function):
         counts_out = pointclouds._counts_dev[pointclouds._cur ^ 1]
         assoc = torch.zeros((B, P), dtype=torch.int32, device=dev)
         with_cc = 1 if pointclouds._has_cc else 0
-        _C.launch("gsx_fusion_merge_append_radii", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c,
-                  P * 3, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, 1 if radii else 0)
+        ctx.emb = None
+        if e is None:
+            _C.launch("gsx_fusion_merge_append_radii", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c,
+                      P * 3, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, 1 if radii else 0)
+        else:
+            D = e.shape[-1]
+            emb_out = torch.zeros((B, cap_out, D), dtype=torch.float32, device=dev)
+            if bound > 0:
+                emb_out[:, :bound] = emb.detach()[:, :bound]
+            rec = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
+            e_c = e.detach().contiguous()
+            _C.launch("gsx_fusion_merge_append_rec", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c,
+                      P * 3, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, rec, 1 if radii else 0)
+            _C.launch("gsx_embed_merge_append", emb_out, cap_out, e_c, P * D, assoc, rec, B, H, W, D, 0)
+            outs.append(emb_out)
+            ctx.emb = (rec, emb.detach().contiguous(), e_c, e.shape)
         if pack[4] is not None:  # (fuse_and_prune's free-space step reads it)
             pack[4].append(assoc)
         ctx.saved = (assoc, counts_in, geo.detach(), col.detach(), gv_c, gn_c, rgb_c, vloc_c)
@@ -478,7 +552,7 @@ class _MergeAppendFn(torch.autograd.Function):
         return tuple(outs)
 
     @staticmethod
-    def backward(ctx, g_geo, g_col):
+    def backward(ctx, g_geo, g_col, g_emb=None):
         assoc, counts_in, geo, col, gv, gn, rgb, vloc = ctx.saved
         B, H, W, cap_in, cap_out, sigma, with_cc = ctx.dims
         dev = assoc.device
@@ -486,11 +560,23 @@ class _MergeAppendFn(torch.autograd.Function):
         geo_c, col_c = geo.contiguous(), col.contiguous()
         d_map = [torch.empty_like(geo_c), torch.empty_like(col_c)]
         d_frame = [torch.empty((B, 1, H, W, 3), dtype=torch.float32, device=dev) for _ in range(4)]
-        _C.launch("gsx_fusion_merge_append_bwd", assoc, counts_in, geo_c, col_c, with_cc, cap_in, *gs, cap_out, gv, gn,
-                  rgb, vloc, B, H, W, sigma, *d_map, *d_frame)
         gv_shape, rgb_shape = ctx.shapes
+        if ctx.emb is None:
+            _C.launch("gsx_fusion_merge_append_bwd", assoc, counts_in, geo_c, col_c, with_cc, cap_in, *gs, cap_out, gv,
+                      gn, rgb, vloc, B, H, W, sigma, *d_map, *d_frame)
+            return (None, d_map[0], d_map[1], d_frame[0].view(gv_shape), d_frame[1].view(gv_shape),
+                    d_frame[2].view(rgb_shape), d_frame[3].view(gv_shape))
+        rec, emb, e, e_shape = ctx.emb
+        D = e.shape[-1]
+        d_emb = torch.empty_like(emb)
+        d_e = torch.empty_like(e)
+        d_w = torch.empty((2, B, H * W), dtype=torch.float32, device=dev)  # d c0, d alpha per pixel
+        _C.launch("gsx_embed_merge_bwd", assoc, rec, counts_in, emb, cap_in, e,
+                  None if g_emb is None else g_emb.contiguous(), cap_out, B, H, W, D, d_emb, d_e, d_w[0], d_w[1])
+        _C.launch("gsx_fusion_merge_append_bwd_emb", assoc, counts_in, geo_c, col_c, with_cc, cap_in, *gs, cap_out, gv,
+                  gn, rgb, vloc, B, H, W, sigma, d_w[0], d_w[1], *d_map, *d_frame)
         return (None, d_map[0], d_map[1], d_frame[0].view(gv_shape), d_frame[1].view(gv_shape),
-                d_frame[2].view(rgb_shape), d_frame[3].view(gv_shape))
+                d_frame[2].view(rgb_shape), d_frame[3].view(gv_shape), d_emb, d_e.view(e_shape))
 
 
 def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=None, dot_th=None, table=None,
@@ -510,14 +596,23 @@ def _update_differentiable(pointclouds, frames, sigma, with_features, dist_th=No
         raise ValueError("Expected equal batch sizes for pointclouds and rgbdimages. Got {0} and {1} "
                          "respectively.".format(len(pointclouds), B))
     dev = pointclouds.device
+    e = frames.embeddings
+    emb_args = ()
+    if e is not None:
+        if pointclouds._emb is None:
+            pointclouds._alloc_embeddings(e.shape[-1], e.dtype)
+        _embedding_frame(e, dev)  # (device check)
+        emb_args = (pointclouds._emb, e)
     sig = _sigma_value(sigma)
     gv, gn, vloc = frames.global_vertex_map, frames.global_normal_map, frames.vertex_map  # K1, carries its backward
     ws = _Workspace.get(dev, B, H, W)
     _launch_frame_records(ws, frames, sig, dev)
     _launch_association(ws, pointclouds, frames, dist_th=dist_th, dot_th=dot_th, table=table)
-    geo_out, col_out = _MergeAppendFn.apply((pointclouds, frames, sig, ws, assoc_out, radii), pointclouds._geo,
-                                            pointclouds._col, gv, gn, frames.rgb_image, vloc)
-    pointclouds._geo, pointclouds._col = geo_out, col_out
+    outs = _MergeAppendFn.apply((pointclouds, frames, sig, ws, assoc_out, radii), pointclouds._geo, pointclouds._col,
+                                gv, gn, frames.rgb_image, vloc, *emb_args)
+    pointclouds._geo, pointclouds._col = outs[0], outs[1]
+    if e is not None:
+        pointclouds._emb = outs[2]
     pointclouds._uninit = False
     pointclouds._mark_device_updated(pointclouds._bound + P)
     return pointclouds
@@ -654,6 +749,7 @@ def prune_unstable(pointclouds: Pointclouds, stable_confidence: float, max_unsta
     gradslam keeps every surfel).  The rows created `max_unstable_age` pruned steps ago whose confidence (the
     `features_padded` value: gradslam's alpha summed over merges) is still below `stable_confidence` are removed; every
     other row keeps its order.  Run it after each fused update (PointFusion does, when configured)."""
+    _refuse_embeddings(pointclouds, "prune_unstable")
     if not pointclouds.has_points:
         return pointclouds
     if not pointclouds._has_cc or pointclouds._col is None:
@@ -705,6 +801,7 @@ def fuse_and_prune(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th: Un
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     _check_frame(rgbdimages)
+    _refuse_embeddings(pointclouds, "fuse_and_prune", rgbdimages)
     _check_surfel_radii(surfel_radii)
     _check_merge_overlapping(merge_overlapping, surfel_radii)
     _check_free_space_margin(free_space_margin)
@@ -738,6 +835,7 @@ def update_map_aggregate(pointclouds: Pointclouds, rgbdimages: RGBDImages, inpla
         # Pointclouds.append_points refuses the mismatch (pointclouds.py:1170-1177)
         raise ValueError("pointclouds to append and to be appended must either both have or not have features: "
                          "(False != True)")
+    _check_embeddings(pointclouds, rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
     if _wants_grad(pointclouds, rgbdimages):
@@ -761,6 +859,7 @@ def update_map_fusion(pointclouds: Pointclouds, rgbdimages: RGBDImages, dist_th:
     _check_frame(rgbdimages)
     _check_surfel_radii(surfel_radii)
     _check_fusion_inputs(pointclouds, rgbdimages)
+    _check_embeddings(pointclouds, rgbdimages)
     if not inplace:
         pointclouds = pointclouds.clone()
     return _fuse(pointclouds, rgbdimages, sigma, dist_th, dot_th, radii=surfel_radii)

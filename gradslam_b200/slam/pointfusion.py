@@ -10,7 +10,7 @@ from typing import Optional, Union
 import torch
 
 from .. import _C
-from ..structures.pointclouds import Pointclouds
+from ..structures.pointclouds import EMBED_DTYPES, Pointclouds
 from ..structures.rgbdimages import BilateralFilter, RGBDImages
 from ..structures.pointclouds import _PruneHistory
 from .fusionutils import (_check_free_space_margin, _check_history, _check_merge_overlapping, _prune_scratch,
@@ -84,6 +84,10 @@ class PointFusion(ICPSLAM):
         photometric_weight (extension, default 0; > 0 needs association='projective'): joint geometric and photometric
         tracking against the map's colours, see ICPSLAM.
 
+        Frames with embeddings (RGBDImages(embeddings=...)) give maps with per-surfel embeddings, merged with the
+        colours' weights, on every path; the pruning options (stable_confidence, free_space_margin, merge_overlapping)
+        refuse them with ValueError.
+
         depth_filter, depth_filter_tracking_only (extension; default None, False): bilateral filtering of the live depth
         for the tracking and the fusion, or for the tracking alone, see ICPSLAM.  The whole-sequence call (odom='gt')
         filters the frames on the device as they arrive - all at once when they are already there, else each uploaded
@@ -136,7 +140,13 @@ class PointFusion(ICPSLAM):
         self.surfel_radii = surfel_radii
         self.merge_overlapping = merge_overlapping
 
+    def _refuse_pruned_embeddings(self, frames):
+        if frames.embeddings is not None and self.stable_confidence is not None:
+            raise ValueError("PointFusion's pruning options (stable_confidence, free_space_margin, merge_overlapping) "
+                             "are not supported on frames with embeddings")
+
     def _map(self, pointclouds: Pointclouds, live_frame: RGBDImages, inplace: bool = False):
+        self._refuse_pruned_embeddings(live_frame)
         if self.stable_confidence is not None and isinstance(pointclouds, Pointclouds):
             _check_history(pointclouds, self.max_unstable_age)
         if self.free_space_margin is not None or self.merge_overlapping:
@@ -161,6 +171,8 @@ class PointFusion(ICPSLAM):
                                  "ingest.rgbdimages_from_raw for the other odometry modes")
             self._check_out(out, frames.shape[0])
             return self._forward_sequence(frames, raw=True, out=out)
+        if isinstance(frames, RGBDImages):
+            self._refuse_pruned_embeddings(frames)
         return super().forward(frames, out)
 
     def _forward_sequence(self, frames, chunk: int = 4, raw: bool = False, out=None):
@@ -182,22 +194,25 @@ class PointFusion(ICPSLAM):
             on_device = False
         else:
             if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (
-                    frames.depth_image, frames.rgb_image, frames.poses, frames.intrinsics)):
+                    frames.depth_image, frames.rgb_image, frames.poses, frames.intrinsics, frames.embeddings)):
                 return None  # differentiable mode goes through the per-frame step loop
             if frames.channels_first:
                 frames = frames.to_channels_last()
             B, L, H, W = frames.shape
             src_depth, src_rgb = frames.depth_image, frames.rgb_image
             on_device = src_depth.device == dev
+        src_emb = None if raw else frames.embeddings
         P = H * W
         K = frames.intrinsics.to(dev).contiguous()
         poses = frames.poses.to(dev).contiguous()
         if on_device:
             depth, rgb = src_depth.contiguous(), src_rgb.contiguous()
+            emb = None if src_emb is None else src_emb.contiguous()
             chunk = L
         else:
             depth = torch.empty((B, L, H, W, 1), dtype=torch.float32, device=dev)
             rgb = torch.empty((B, L, H, W, 3), dtype=torch.float32, device=dev)
+            emb = None if src_emb is None else torch.empty(src_emb.shape, dtype=src_emb.dtype, device=dev)
             copy_stream = torch.cuda.Stream(device=dev)
             if raw:  # staging buffers for the 5-byte pixels; converted chunk by chunk on the compute stream
                 raw_depth = torch.empty((B, L, H, W), dtype=src_depth.dtype, device=dev)
@@ -207,11 +222,17 @@ class PointFusion(ICPSLAM):
         if out is not None:  # caller-provided storage (validated by forward: empty, B maps, this device)
             if not (out.has_normals and out.has_colors and out._has_cc):
                 raise ValueError("out must have normals, colours and a confidence count per point for map fusion")
+            if out.has_embeddings != (emb is not None) or (emb is not None and (
+                    out._emb.shape[2], out._emb.dtype) != (emb.shape[-1], emb.dtype)):
+                raise ValueError("out must have embeddings of the frames' dimension and dtype exactly when the frames "
+                                 "have embeddings")
             pc = out
             pc._cur = 0
         else:
             pc = Pointclouds(device=dev)
             pc._allocate(B, L * P, 1, zero=False)
+            if emb is not None:  # L*H*W rows of D channels per element: see INTEGRATION.md for a smaller `out`
+                pc._alloc_embeddings(emb.shape[-1], emb.dtype)
         ws = _SequenceWorkspace.get(dev, B, H, W)
         prune = (None, 0, 0.0, None, 0)  # ring, t_max, c_stable, scratch, its bytes: pruning off
         free_space = (0.0, None, 0)  # margin, scratch, its bytes: the age rule alone
@@ -243,6 +264,8 @@ class PointFusion(ICPSLAM):
                     for b in range(B):  # per-element slices are contiguous: true async DMA from pinned memory
                         dst_d[b, s0:s1].copy_(src_depth[b, s0:s1], non_blocking=True)
                         dst_c[b, s0:s1].copy_(src_rgb[b, s0:s1], non_blocking=True)
+                        if emb is not None:
+                            emb[b, s0:s1].copy_(src_emb[b, s0:s1], non_blocking=True)
                     ev = torch.cuda.Event()
                     ev.record(copy_stream)
                     ready.append(ev)
@@ -259,13 +282,25 @@ class PointFusion(ICPSLAM):
                                     [(depth[b, s0:s1], fused_depth[b, s0:s1], s1 - s0) for b in range(B)]):
                     _C.launch("gsx_depth_bilateral", src, dst, None, n, H, W, filt.radius, filt.sigma_space,
                               filt.sigma_range)
-            _C.launch("gsx_pointfusion_sequence_gt_merge", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                      min(s0 * P, pc.capacity), fused_depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                      float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag(),
-                      1 if self.surfel_radii else 0, *merge)
+            if emb is None:
+                _C.launch("gsx_pointfusion_sequence_gt_merge", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                          min(s0 * P, pc.capacity), fused_depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                          float(self.dot_th), float(self.sigma), ws.buf, *prune, *free_space, pc._overflow_flag(),
+                          1 if self.surfel_radii else 0, *merge)
+            else:
+                if i == 0:
+                    assoc = torch.empty((B, P), dtype=torch.int32, device=dev)
+                    rec = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
+                _C.launch("gsx_pointfusion_sequence_gt_emb", pc._geo, pc._col, pc._counts_dev, pc.capacity,
+                          min(s0 * P, pc.capacity), fused_depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
+                          float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag(),
+                          1 if self.surfel_radii else 0, pc._emb, emb, emb.shape[-1], EMBED_DTYPES[emb.dtype], assoc,
+                          rec)
         if not on_device:
             for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
                 t.record_stream(copy_stream)
+            if emb is not None:
+                emb.record_stream(copy_stream)
         pc._cur = L & 1
         pc._counts_host = None
         pc._bound = pc.capacity

@@ -16,7 +16,9 @@ spread over four arrays.  gradslam's tensors are STRIDED VIEWS of these rows: `p
 `colors_padded = colours[:, :N, 0:3]`, `radii_padded = geometry[:, :N, 7:8]` (the surfel radius: 0 unless the map
 was fused with surfel_radii=True); `*_list[b]` are the same views cut at `counts[b]`.  (Features with more than
 one channel are not part of the fusion path; they live in a separate dense (B, capacity, C) tensor.)  Rows >=
-counts[b] are always zero inside the padded width.  The per-element sizes live on the device (the kernels bump them);
+counts[b] are always zero inside the padded width.  A map may also carry one embedding per surfel (ConceptFusion-style
+feature maps), a dense (B, capacity, D) store of float32, float16 or bfloat16 beside the rows: `embeddings_padded` /
+`embeddings_list`; the fused map update merges it with the colours' weights (fusionutils.update_map_fusion).  The per-element sizes live on the device (the kernels bump them);
 the host copy is refreshed lazily, only when a caller asks for a shape-dependent view.  Everything is float32: other
 floating inputs are cast on construction (the kernels read raw float32 rows).
 """
@@ -25,6 +27,9 @@ from typing import List, Optional, Union
 import torch
 
 __all__ = ["Pointclouds"]
+
+# storage types of per-surfel embeddings, and their dtype code in the C ABI (gsx_embed_merge_append)
+EMBED_DTYPES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
 _ATTRS = ("points", "normals", "colors", "features")
 GEO_W, COL_W = 8, 4  # floats per geometry / colour row (csrc/gsx_fusion.cu)
@@ -53,8 +58,13 @@ class _PruneHistory:
 
 class Pointclouds(object):
     def __init__(self, points=None, normals=None, colors=None, features=None,
-                 device: Union[torch.device, str, None] = None):
+                 device: Union[torch.device, str, None] = None, *, embeddings=None):
+        """embeddings (extension): per-surfel embeddings, of the same type as points - a list of (N_b, D) tensors or a
+        (B, N, D) tensor - in float32, float16 or bfloat16 (kept in that dtype), D >= 1."""
         super().__init__()
+        if not (embeddings is None or isinstance(embeddings, type(points))):
+            raise TypeError("Expected embeddings to be of same type as points (%r); got %r" % (type(points),
+                                                                                            type(embeddings)))
         if not (points is None or isinstance(points, list) or torch.is_tensor(points)):
             raise TypeError("Expected points to be of type list or tensor or None; got %r" % type(points))
         for name, val in (("normals", normals), ("colors", colors), ("features", features)):
@@ -78,6 +88,7 @@ class Pointclouds(object):
         self._uninit = False  # store was allocated without zero-fill: rows >= counts[b] may hold garbage
         self._tail_dirty = False  # the ragged tail [counts[b], max(counts)) must be zeroed before a padded view
         self._prune = None  # _PruneHistory once unstable surfels have been removed from this map (PointFusion)
+        self._emb = None  # (B, cap, D) per-surfel embeddings, or None
 
         if isinstance(points, list):
             shapes = [p.shape for p in points]
@@ -107,6 +118,16 @@ class Pointclouds(object):
                 for b, x in enumerate(lst):
                     if x.shape[0] > 0:
                         dst[b, : x.shape[0]] = _f32(x, self.device)
+            if embeddings is not None:
+                if len(embeddings) != len(points) or any(not torch.is_tensor(e) or e.ndim != 2 for e in embeddings):
+                    raise ValueError("embeddings should be a list of one 2-D tensor per pointcloud")
+                if [int(e.shape[0]) for e in embeddings] != counts:
+                    raise ValueError("number of embeddings per pointcloud has to be equal to number of points")
+                if len(set((e.shape[1], e.dtype) for e in embeddings)) != 1:
+                    raise ValueError("embeddings of every pointcloud must have the same dimension and dtype")
+                self._alloc_embeddings(embeddings[0].shape[1], embeddings[0].dtype, max(counts))
+                for b, e in enumerate(embeddings):
+                    self._emb[b, : e.shape[0]] = e.to(self.device)
             self._set_counts(counts)
         elif torch.is_tensor(points):
             self.device = torch.empty(0, device=device).device if device is not None else points.device
@@ -134,8 +155,16 @@ class Pointclouds(object):
             for key, t in zip(_ATTRS, (points, normals, colors, features)):
                 if t is not None and N > 0:
                     self._view(key)[:, :N] = _f32(t, self.device)
+            if embeddings is not None:
+                if embeddings.ndim != 3 or embeddings.shape[:2] != points.shape[:2]:
+                    raise ValueError("embeddings should be (B, N, D) with the points' B and N; got %r" % (
+                        tuple(embeddings.shape),))
+                self._alloc_embeddings(embeddings.shape[2], embeddings.dtype, N)
+                self._emb[:, :N] = embeddings.to(self.device)
             self._set_counts([N] * self._B)
         else:
+            if embeddings is not None:
+                raise ValueError("embeddings need points")
             self.device = torch.empty(0, device=device).device if device is not None else torch.device("cpu")
 
     # ------------------------------------------------------------------ packed storage
@@ -149,8 +178,17 @@ class Pointclouds(object):
         self._feat = (alloc((self._B, cap, int(features_dim)), dtype=torch.float32, device=self.device)
                       if features_dim > 1 else None)
 
+    def _alloc_embeddings(self, dim, dtype, capacity=None):
+        """A zeroed (B, capacity, dim) embedding store (capacity: the rows' by default)."""
+        if isinstance(dim, bool) or not isinstance(dim, int) or dim < 1:
+            raise ValueError("embedding dimension must be an int >= 1; got {}".format(dim))
+        if dtype not in EMBED_DTYPES:
+            raise TypeError("embeddings must be float32, float16 or bfloat16; got {}".format(dtype))
+        cap = self.capacity if capacity is None else max(int(capacity), 0)
+        self._emb = torch.zeros((self._B, cap, dim), dtype=dtype, device=self.device)
+
     def _buffers(self):
-        return [t for t in (self._geo, self._col, self._feat) if t is not None]
+        return [t for t in (self._geo, self._col, self._feat, self._emb) if t is not None]
 
     def _view(self, key):
         """Full-capacity strided view (B, capacity, C) of one attribute, or None."""
@@ -166,11 +204,14 @@ class Pointclouds(object):
             return self._geo[..., 6:7] if self._has_cc else self._feat
         if key == "radii":
             return self._geo[..., 7:8]
+        if key == "embeddings":
+            return self._emb
         raise KeyError(key)
 
     def _grad_tensors(self):
-        """Tensors whose requires_grad switches the fusion / ICP ops to their differentiable mode."""
-        return self._buffers()
+        """Tensors whose requires_grad switches the fusion / ICP ops to their differentiable mode (the embeddings only
+        switch the fusion's: tracking does not read them)."""
+        return [t for t in (self._geo, self._col, self._feat) if t is not None]
 
     # ------------------------------------------------------------------ size bookkeeping
     def _set_counts(self, counts: List[int]):
@@ -274,6 +315,7 @@ class Pointclouds(object):
             return grown
 
         self._geo, self._col, self._feat = grow(self._geo), grow(self._col), grow(self._feat)
+        self._emb = grow(self._emb)
         self._list_cache = {}
 
     # ------------------------------------------------------------------ protocol
@@ -295,6 +337,15 @@ class Pointclouds(object):
     @property
     def has_features(self):
         return self._geo is not None and (self._has_cc or self._feat is not None)
+
+    @property
+    def has_embeddings(self):
+        return self._geo is not None and self._emb is not None
+
+    @property
+    def embedding_dim(self):
+        """D of the per-surfel embeddings, 0 without."""
+        return int(self._emb.shape[2]) if self.has_embeddings else 0
 
     @property
     def num_features(self):
@@ -363,6 +414,9 @@ class Pointclouds(object):
     # no gradient through the fusion ops
     radii_padded = property(lambda self: self._padded("radii"))
     radii_list = property(lambda self: self._list("radii"))
+    # per-surfel embeddings (B, N, D) / [(N_b, D)] in their storage dtype, or None
+    embeddings_padded = property(lambda self: self._padded("embeddings"))
+    embeddings_list = property(lambda self: self._list("embeddings"))
 
     @property
     def nonpad_mask(self):
@@ -444,6 +498,28 @@ class Pointclouds(object):
     features_list = features_list.setter(lambda self, v: self._set_list("features", v, True))
     radii_padded = radii_padded.setter(lambda self, v: self._set_radii_padded(v))
     radii_list = radii_list.setter(lambda self, v: self._set_radii_list(v))
+    embeddings_padded = embeddings_padded.setter(lambda self, v: self._set_embeddings_padded(v))
+    embeddings_list = embeddings_list.setter(lambda self, v: self._set_embeddings_list(v))
+
+    def _fresh_embeddings(self, dim, dtype):
+        """A new (never a tensor a caller may hold) zeroed store for the setters."""
+        cap = max(self.capacity, self._N)
+        self._alloc_embeddings(dim, dtype, cap)
+        self._list_cache = {}
+        return self._emb
+
+    def _set_embeddings_padded(self, value):
+        self._assert_set_padded(value, True)
+        dst = self._fresh_embeddings(value.shape[-1], value.dtype)
+        dst[:, : self._N] = value
+
+    def _set_embeddings_list(self, value):
+        self._assert_set_list(value, True)
+        if len(set((v.shape[1], v.dtype) for v in value)) != 1:
+            raise ValueError("embeddings of every pointcloud must have the same dimension and dtype")
+        dst = self._fresh_embeddings(value[0].shape[1], value[0].dtype)
+        for b, v in enumerate(value):
+            dst[b, : v.shape[0]] = v
 
     def _set_radii_padded(self, value):
         self._assert_set_padded(value, True)
@@ -475,7 +551,8 @@ class Pointclouds(object):
             raise IndexError(index)
         pick = lambda lst: None if lst is None else [lst[i] for i in idx]
         return Pointclouds(points=pick(self.points_list), normals=pick(self.normals_list),
-                           colors=pick(self.colors_list), features=pick(self.features_list))
+                           colors=pick(self.colors_list), features=pick(self.features_list),
+                           embeddings=pick(self.embeddings_list))
 
     # ------------------------------------------------------------------ arithmetic helpers (pointclouds.py:303-614)
     def __add__(self, other):
@@ -604,6 +681,7 @@ class Pointclouds(object):
         keep = max(self._N, 1)  # copy the populated rows only (one sync beats cloning gigabytes of spare capacity)
         cp = lambda st: None if st is None else fn(st[:, :keep])
         other._geo, other._col, other._feat = cp(self._geo), cp(self._col), cp(self._feat)
+        other._emb = cp(self._emb)
         other._has_normals, other._has_cc = self._has_normals, self._has_cc
         other.device = other._geo.device
         other._counts_dev = self._counts_dev.clone().to(other.device)
@@ -645,10 +723,17 @@ class Pointclouds(object):
             pin = lambda st: None if st is None else torch.zeros((st.shape[0], cap, st.shape[2]), dtype=st.dtype,
                                                                  pin_memory=True)
             out._geo, out._col, out._feat = pin(self._geo), pin(self._col), pin(self._feat)
+        if self._emb is not None and (out._emb is None or out._emb.shape[1] < n or out._emb.shape[2] != self._emb.shape[2]
+                                      or out._emb.dtype != self._emb.dtype):
+            out._emb = torch.zeros((self._B, out._geo.shape[1], self._emb.shape[2]), dtype=self._emb.dtype,
+                                   pin_memory=True)
+        elif self._emb is None:
+            out._emb = None
         out._has_normals, out._has_cc = self._has_normals, self._has_cc
         ctx = torch.cuda.stream(stream) if stream is not None else torch.cuda.device(self.device)
         with ctx:
-            for dst, src in ((out._geo, self._geo), (out._col, self._col), (out._feat, self._feat)):
+            for dst, src in ((out._geo, self._geo), (out._col, self._col), (out._feat, self._feat),
+                             (out._emb, self._emb)):
                 if src is None:
                     continue
                 for b, c in enumerate(counts):
@@ -682,6 +767,7 @@ class Pointclouds(object):
     # ------------------------------------------------------------------ growth
     def _adopt(self, src: "Pointclouds"):
         self._geo, self._col, self._feat, self._B = src._geo, src._col, src._feat, src._B
+        self._emb = src._emb
         self._has_normals, self._has_cc = src._has_normals, src._has_cc
         self._counts_dev, self._cur = src._counts_dev, src._cur
         self._counts_host, self._bound, self._overflow = src._counts_host, src._bound, src._overflow
@@ -713,11 +799,18 @@ class Pointclouds(object):
         if self.has_features and self.num_features != pointclouds.num_features:
             raise ValueError("pointclouds to append and to be appended must have the same number of features: "
                              "({0} != {1})".format(pointclouds.num_features, self.num_features))
+        if self.has_embeddings != pointclouds.has_embeddings:
+            raise ValueError("pointclouds to append and to be appended must either both have or not have embeddings: "
+                             "({} != {})".format(pointclouds.has_embeddings, self.has_embeddings))
+        if self.has_embeddings and (self._emb.shape[2], self._emb.dtype) != (pointclouds._emb.shape[2],
+                                                                            pointclouds._emb.dtype):
+            raise ValueError("pointclouds to append and to be appended must have embeddings of the same dimension and "
+                             "dtype")
         mine, theirs = self._host_counts(), pointclouds._host_counts()
         total = [a + b for a, b in zip(mine, theirs)]
         self.reserve(max(total))
         for dst, src in ((self._geo, pointclouds._geo), (self._col, pointclouds._col),
-                         (self._feat, pointclouds._feat)):
+                         (self._feat, pointclouds._feat), (self._emb, pointclouds._emb)):
             if dst is None:
                 continue
             for b in range(self._B):

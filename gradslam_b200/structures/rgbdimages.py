@@ -167,15 +167,38 @@ def bilateral_filter_depth(depth: torch.Tensor, f: BilateralFilter) -> torch.Ten
     return _BilateralFn.apply(depth, f)
 
 
+_EMBED_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def _check_embedding_image(e, rgb_shape, cdim):
+    """(B, L, H, W, D) channels-last (cdim 4) or (B, L, D, H, W) channels-first (cdim 2) beside rgb of rgb_shape."""
+    if not torch.is_tensor(e):
+        raise TypeError("Expected embeddings to be of type tensor or None; got {}".format(type(e)))
+    if e.dtype not in _EMBED_DTYPES:
+        raise TypeError("embeddings must be float32, float16 or bfloat16; got {}".format(e.dtype))
+    if e.ndim != 5:
+        raise ValueError("embeddings should have ndim=5, but had ndim={}".format(e.ndim))
+    D = e.shape[cdim]
+    exp = tuple(v if i != cdim else D for i, v in enumerate(rgb_shape))
+    if D < 1 or tuple(e.shape) != exp:
+        raise ValueError("Expected embeddings to have shape {0} with D >= 1 ({1}). Got {2} instead".format(
+            tuple("D" if i == cdim else v for i, v in enumerate(exp)),
+            "(B, L, D, H, W)" if cdim == 2 else "(B, L, H, W, D)", tuple(e.shape)))
+
+
 class RGBDImages(object):
     _INTERNAL_TENSORS = [
         "_rgb_image", "_depth_image", "_intrinsics", "_poses", "_pixel_pos",
-        "_vertex_map", "_normal_map", "_global_vertex_map", "_global_normal_map",
+        "_vertex_map", "_normal_map", "_global_vertex_map", "_global_normal_map", "_embeddings",
     ]
 
     def __init__(self, rgb_image: torch.Tensor, depth_image: torch.Tensor, intrinsics: torch.Tensor,
                  poses: Optional[torch.Tensor] = None, channels_first: bool = False,
-                 device: Union[torch.device, str, None] = None, *, pixel_pos: Optional[torch.Tensor] = None):
+                 device: Union[torch.device, str, None] = None, *, pixel_pos: Optional[torch.Tensor] = None,
+                 embeddings: Optional[torch.Tensor] = None):
+        """embeddings (extension): a per-pixel embedding image at the depth's resolution, (B, L, H, W, D) or, with
+        channels_first, (B, L, D, H, W), D >= 1, in float32, float16 or bfloat16, on the frames' device.  The fused map
+        update keeps a confidence-weighted mean of it per surfel (Pointclouds.embeddings_padded)."""
         super().__init__()
         for name, val, opt in (("rgb_image", rgb_image, False), ("depth_image", depth_image, False),
                                ("intrinsics", intrinsics, False), ("poses", poses, True),
@@ -218,8 +241,11 @@ class RGBDImages(object):
         if pixel_pos is not None and pixel_pos.shape != self._pixel_pos_shape:
             raise ValueError("Expected pixel_pos to have shape {0}. Got {1} instead".format(
                 self._pixel_pos_shape, pixel_pos.shape))
+        if embeddings is not None:
+            _check_embedding_image(embeddings, rgb_image.shape, cdim)
 
-        devices = set(x.device for x in (rgb_image, depth_image, intrinsics, poses, pixel_pos) if x is not None)
+        devices = set(x.device for x in (rgb_image, depth_image, intrinsics, poses, pixel_pos, embeddings)
+                      if x is not None)
         if len(devices) != 1:
             raise ValueError("All inputs must be on same device, but got more than 1 device: {}".format(devices))
 
@@ -229,6 +255,7 @@ class RGBDImages(object):
         self._intrinsics = intrinsics.to(self.device)
         self._poses = poses.to(self.device) if poses is not None else None
         self._pixel_pos = pixel_pos.to(self.device) if pixel_pos is not None else None
+        self._embeddings = embeddings.to(self.device) if embeddings is not None else None
 
         self._vertex_map = None
         self._global_vertex_map = None
@@ -302,6 +329,11 @@ class RGBDImages(object):
         return self._pixel_pos
 
     @property
+    def embeddings(self):
+        """The per-pixel embedding image (B, L, H, W, D) ((B, L, D, H, W) channels-first), or None."""
+        return self._embeddings
+
+    @property
     def has_poses(self):
         return self._poses is not None
 
@@ -358,7 +390,7 @@ class RGBDImages(object):
         else:
             depth = bilateral_filter_depth(self._depth_image, f)
         return RGBDImages(self._rgb_image, depth, self._intrinsics, self._poses, channels_first=self.channels_first,
-                          pixel_pos=self._pixel_pos)
+                          pixel_pos=self._pixel_pos, embeddings=self._embeddings)
 
     # ------------------------------------------------------------------ setters (cache invalidation as rgbdimages.py:399-463)
     @staticmethod
@@ -455,7 +487,7 @@ class RGBDImages(object):
 
     def _permute_all(self, order):
         for k in ("_rgb_image", "_depth_image", "_vertex_map", "_global_vertex_map", "_normal_map",
-                  "_global_normal_map"):
+                  "_global_normal_map", "_embeddings"):
             v = getattr(self, k)
             if v is not None:
                 setattr(self, k, v.permute(*order).contiguous())

@@ -181,6 +181,48 @@ int gsx_fusion_merge_append_bwd(const int32_t *assoc, const int32_t *counts_in, 
                                 int B, int H, int W, double sigma, float *d_map_geometry, float *d_map_colors,
                                 float *d_gvertex, float *d_gnormal, float *d_rgb, float *d_vertex, void *stream);
 
+/* Per-surfel embeddings (ConceptFusion-style feature maps: one D-channel vector per surfel, fused beside the colour).
+ * gsx_fusion_merge_append_rec: gsx_fusion_merge_append_radii that also records, for every merged pixel, the merge's
+ * c0 (the row's confidence before the merge) and alpha (the pixel's confidence weight) in merge_rec, float32 (B,H,W,2),
+ * 8-byte aligned; assoc_out (int32 (B,H,W), zero-filled by the caller) is required.  Pixels that were not merged leave
+ * their record unwritten.  Every other output equals gsx_fusion_merge_append_radii's bit for bit.
+ * mirrors the merge weights of   gradslam/slam/fusionutils.py:678-699 */
+int gsx_fusion_merge_append_rec(float *map_geometry, float *map_colors, int with_ccounts, const int32_t *counts_in,
+                                int32_t *counts_out, int64_t capacity, const float *rgb, int64_t rgb_bstride, int B,
+                                int H, int W, void *workspace, int32_t *overflow_flag, int32_t *assoc_out,
+                                float *merge_rec, int surfel_radii, void *stream);
+/* KE: the embedding merge after gsx_fusion_merge_append_rec, with its assoc_out and merge_rec.  map_embeddings
+ * (B,capacity,D), frame_embeddings (B,H,W,D) with element stride frame_bstride (elements), both of dtype 0 float32,
+ * 1 float16 or 2 bfloat16.  Per pixel: merged into row n (assoc -(n+1)) with (c0, alpha), tot = c0 + alpha,
+ * inv = 1 / (tot == 0 ? 1 : tot):  E[n,d] = ((c0 * E[n,d]) + (alpha * e[pix,d])) * inv;  appended as row n (assoc n+1):
+ * E[n] = e[pix];  every other row is not written.  Arithmetic in float32, each separately rounded (no contraction); a
+ * half-precision value is read exactly and each result rounded once to the storage type (round to nearest even).
+ * mirrors the colour merge / append of   gradslam/slam/fusionutils.py:678-699 (merge), :702-720 (append) */
+int gsx_embed_merge_append(void *map_embeddings, int64_t capacity, const void *frame_embeddings, int64_t frame_bstride,
+                           const int32_t *assoc, const float *merge_rec, int B, int H, int W, int D, int dtype,
+                           void *stream);
+/* Backward of KE (float32): upstream g_embeddings (B,capacity_out,D) or NULL = zero -> d_map_embeddings
+ * (B,capacity_in,D): g * c0 * inv for merged rows, g for the other rows below counts_in, 0 beyond; d_frame_embeddings
+ * (B,H,W,D): g * alpha * inv merged, g appended, 0 otherwise; d_c0, d_alpha (B,H,W): per merged pixel
+ * sum_d g_d (E_d inv - num_d inv^2) and sum_d g_d (e_d inv - num_d inv^2), num = c0 E + alpha e, summed in a fixed
+ * order (0 for the other pixels).  gsx_fusion_merge_append_bwd_emb adds them to K4's own d c0 and d alpha.
+ * mirrors the tape of   gradslam/slam/fusionutils.py:678-699 (merge), :702-720 (append) */
+int gsx_embed_merge_bwd(const int32_t *assoc, const float *merge_rec, const int32_t *counts_in,
+                        const float *map_embeddings, int64_t capacity_in, const float *frame_embeddings,
+                        const float *g_embeddings, int64_t capacity_out, int B, int H, int W, int D,
+                        float *d_map_embeddings, float *d_frame_embeddings, float *d_c0, float *d_alpha, void *stream);
+/* gsx_fusion_merge_append_bwd whose d c0 (slot 6 of a merged row's d_map_geometry) and d alpha of every merged pixel
+ * also receive emb_d_c0 / emb_d_alpha (B,H,W) of gsx_embed_merge_bwd, so that the embeddings' gradient reaches the
+ * pre-merge confidence and, through alpha, the camera-frame vertex.
+ * replaces the tape PyTorch builds through   gradslam/slam/fusionutils.py:654-720, get_alpha :16-73 */
+int gsx_fusion_merge_append_bwd_emb(const int32_t *assoc, const int32_t *counts_in, const float *map_geometry,
+                                    const float *map_colors, int with_ccounts, int64_t capacity_in,
+                                    const float *g_geometry, const float *g_colors, int64_t capacity_out,
+                                    const float *gvertex, const float *gnormal, const float *rgb, const float *vertex,
+                                    int B, int H, int W, double sigma, const float *emb_d_c0, const float *emb_d_alpha,
+                                    float *d_map_geometry, float *d_map_colors, float *d_gvertex, float *d_gnormal,
+                                    float *d_rgb, float *d_vertex, void *stream);
+
 /* Whole-sequence driver with ground-truth poses: for s in [s_begin,s_end): K2/K3 -> K4, no host sync and no K1r.  The
  * workspace's re-arm state is zeroed once per call and then kept armed by K4 from frame to frame, so nothing survives
  * from one call to the next, also after a failed call.  Frame headers are written for blocks of 64 frames.
@@ -236,6 +278,18 @@ int gsx_pointfusion_sequence_gt_merge(float *map_geometry, float *map_colors, in
                                       float margin, void *fs_scratch, int64_t fs_scratch_bytes,
                                       int32_t *overflow_flag, int surfel_radii, void *merge_scratch,
                                       int64_t merge_scratch_bytes, void *stream);
+/* gsx_pointfusion_sequence_gt_radii (no pruning) with per-surfel embeddings: every frame's K4 runs as
+ * gsx_fusion_merge_append_rec, followed on the same group stream by gsx_embed_merge_append.  map_embeddings
+ * (B,capacity,D), frame_embeddings (B,L,H,W,D) dense, of dtype 0 float32, 1 float16 or 2 bfloat16; assoc int32 (B,H,W)
+ * and merge_rec float32 (B,H,W,2) are K4's per-frame record (zeroed here per frame and group, no initialisation
+ * needed).  Geometry, colours and counts equal gsx_pointfusion_sequence_gt_radii's bit for bit.
+ * mirrors   gradslam/slam/fusionutils.py:678-699 (merge), :702-720 (append) */
+int gsx_pointfusion_sequence_gt_emb(float *map_geometry, float *map_colors, int32_t *counts, int64_t capacity,
+                                    int64_t max_count0, const float *depth, const float *rgb, const float *intrinsics,
+                                    const float *poses, int B, int L, int s_begin, int s_end, int H, int W,
+                                    float dist_th, float dot_th, double sigma, void *workspace, int32_t *overflow_flag,
+                                    int surfel_radii, void *map_embeddings, const void *frame_embeddings, int D,
+                                    int dtype, int32_t *assoc, float *merge_rec, void *stream);
 /* ------------------------------------------------------------------------------------------------
  * Removal of unstable surfels (opt-in extension; gradslam has no such step, so no reference line is replaced).
  * Keller et al. 2013, "Real-time 3D reconstruction in dynamic scenes using point-based fusion", section 4.3: a surfel
