@@ -64,6 +64,15 @@ SIGNATURES = {
     "gsx_pointfusion_sequence_gt_emb": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                 c_float, c_float, c_double, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp]),
+    "gsx_embed_merge_append_upsampled": (
+        c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "gsx_embed_merge_bwd_upsampled": (
+        c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                c_vp, c_vp, c_vp]),
+    "gsx_pointfusion_sequence_gt_emb_upsampled": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                c_float, c_float, c_double, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                c_vp]),
     "gsx_pointfusion_sequence_groups": (c_int, [c_int]),
     "gsx_pointfusion_sequence_workspace_bytes": (c_i64, [c_int, c_int, c_int]),
     "gsx_pointfusion_sequence_gt": (

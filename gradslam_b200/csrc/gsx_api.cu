@@ -41,12 +41,15 @@ int fusion_update_group(float *geo, float *col, const int32_t *cin, int32_t *cou
 
 // Embeddings of the sequence driver: map rows E (B, cap, D), frames e (B, L, H, W, D) dense, both of `dtype` (0 float32,
 // 1 float16, 2 bfloat16); assoc int32 and rec float2, each (B, H, W): K4's record of every frame, read by KE.
+// upsampled: the frames are coarse (B, L, eh, ew, D) images, dense, that the upsampled KE samples at the (H, W) pixels.
 struct SequenceEmbed {
   void *E;
   const void *e;
   int D, dtype;
   int32_t *assoc;
   float2 *rec;
+  bool upsampled;
+  int H, W, eh, ew;
 };
 
 // the group's K4 record zeroed, K4 done by the caller, then KE of frame s for elements [b0, b0 + nb)
@@ -58,9 +61,16 @@ static int32_t *sequence_embed_assoc(const SequenceEmbed *emb, int b0, int nb, i
 static int sequence_embed_group(const SequenceEmbed *emb, int64_t cap, int L, int s, int b0, int nb, int64_t P,
                                 cudaStream_t st) {
   const int64_t es = emb->dtype == 0 ? 4 : 2;
-  const EmbedArgs a{(char *)emb->E + (int64_t)b0 * cap * emb->D * es,
-                    (const char *)emb->e + ((int64_t)b0 * L + s) * P * emb->D * es, (int64_t)L * P * emb->D,
-                    emb->assoc + (int64_t)b0 * P, emb->rec + (int64_t)b0 * P, cap, nb, (int)P, emb->D};
+  const int64_t EP = emb->upsampled ? (int64_t)emb->eh * emb->ew : P;  // embedding texels per frame
+  EmbedArgs a{(char *)emb->E + (int64_t)b0 * cap * emb->D * es,
+              (const char *)emb->e + ((int64_t)b0 * L + s) * EP * emb->D * es, (int64_t)L * EP * emb->D,
+              emb->assoc + (int64_t)b0 * P, emb->rec + (int64_t)b0 * P, cap, nb, (int)P, emb->D};
+  if (emb->upsampled) {
+    a.H = emb->H;
+    a.W = emb->W;
+    a.eh = emb->eh;
+    a.ew = emb->ew;
+  }
   return launch_embed_merge_append(a, emb->dtype, st);
 }
 
@@ -307,6 +317,33 @@ extern "C" int gsx_pointfusion_sequence_gt_emb(float *map_geometry, float *map_c
                 "gsx_pointfusion_sequence_gt_emb: misaligned embeddings or record");
   const gsx::SequenceEmbed emb{map_embeddings, frame_embeddings, D, dtype, assoc,
                                reinterpret_cast<float2 *>(merge_rec)};
+  return sequence_driver(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
+                         s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, nullptr, 0, 0.0f, nullptr, 0, 0.0f,
+                         nullptr, 0, overflow_flag, surfel_radii, nullptr, 0, &emb, stream);
+}
+
+extern "C" int gsx_pointfusion_sequence_gt_emb_upsampled(float *map_geometry, float *map_colors, int32_t *counts,
+                                                         int64_t capacity, int64_t max_count0, const float *depth,
+                                                         const float *rgb, const float *intrinsics, const float *poses,
+                                                         int B, int L, int s_begin, int s_end, int H, int W,
+                                                         float dist_th, float dot_th, double sigma, void *workspace,
+                                                         int32_t *overflow_flag, int surfel_radii,
+                                                         void *map_embeddings, const void *frame_embeddings, int eh,
+                                                         int ew, int D, int dtype, int32_t *assoc, float *merge_rec,
+                                                         void *stream) {
+  GSX_CHECK_ARG(D >= 1 && dtype >= 0 && dtype <= 2, "gsx_pointfusion_sequence_gt_emb_upsampled: need D >= 1 and "
+                "dtype 0 (float32), 1 (float16) or 2 (bfloat16)");
+  GSX_CHECK_ARG(eh >= 1 && eh <= H && ew >= 1 && ew <= W,
+                "gsx_pointfusion_sequence_gt_emb_upsampled: the embedding image (%d, %d) must be at most (H, W) = "
+                "(%d, %d) and at least (1, 1)", eh, ew, H, W);
+  GSX_CHECK_ARG(B == 0 || s_begin == s_end || (map_embeddings && frame_embeddings && assoc && merge_rec),
+                "gsx_pointfusion_sequence_gt_emb_upsampled: null embedding pointer");
+  GSX_CHECK_ARG(((reinterpret_cast<uintptr_t>(map_embeddings) | reinterpret_cast<uintptr_t>(frame_embeddings)) &
+                 (dtype == 0 ? 3 : 1)) == 0 && (reinterpret_cast<uintptr_t>(merge_rec) & 7) == 0 &&
+                (reinterpret_cast<uintptr_t>(assoc) & 3) == 0,
+                "gsx_pointfusion_sequence_gt_emb_upsampled: misaligned embeddings, assoc or record");
+  const gsx::SequenceEmbed emb{map_embeddings, frame_embeddings, D, dtype, assoc,
+                               reinterpret_cast<float2 *>(merge_rec), true, H, W, eh, ew};
   return sequence_driver(map_geometry, map_colors, counts, capacity, max_count0, depth, rgb, intrinsics, poses, B, L,
                          s_begin, s_end, H, W, dist_th, dot_th, sigma, workspace, nullptr, 0, 0.0f, nullptr, 0, 0.0f,
                          nullptr, 0, overflow_flag, surfel_radii, nullptr, 0, &emb, stream);

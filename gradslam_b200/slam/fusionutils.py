@@ -176,7 +176,8 @@ def _dense_frame(t, name, device):
 
 
 def _embedding_frame(e, device):
-    """(B,1,H,W,D) channels-last embedding image -> (base tensor, element stride) for KE."""
+    """(B,1,H,W,D) channels-last embedding image ((B,1,h,w,D) when upsampled) -> (base tensor, element stride) for
+    KE."""
     if not e.is_cuda or e.device != device:
         raise ValueError("gradslam_b200: `embeddings` is on {} but the map lives on {}".format(e.device, device))
     return _frame_base(e.detach(), e.shape[2] * e.shape[3] * e.shape[4])
@@ -184,7 +185,8 @@ def _embedding_frame(e, device):
 
 def _launch_merge_append(pointclouds, frames, ws, assoc=None, radii=False):
     """K4 on the current workspace state (frame records + per-pixel winners); radii: write surfel radii (slot 7).  A
-    frame with embeddings runs K4 with its merge record, then KE on the map's embedding store."""
+    frame with embeddings runs K4 with its merge record, then KE on the map's embedding store (the upsampled KE when
+    the frame's embedding image is coarser than the depth)."""
     B, _, H, W = frames.shape
     P = H * W
     dev = pointclouds.device
@@ -206,8 +208,13 @@ def _launch_merge_append(pointclouds, frames, ws, assoc=None, radii=False):
         _C.launch("gsx_fusion_merge_append_rec", geo, col, 1 if pointclouds._has_cc else 0, cin, cout,
                   pointclouds.capacity, rgb, c_bs, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, rec,
                   1 if radii else 0)
-        _C.launch("gsx_embed_merge_append", emb, pointclouds.capacity, e, e_bs, assoc, rec, B, H, W, e.shape[-1],
-                  EMBED_DTYPES[e.dtype])
+        if frames.upsample_embeddings:
+            eh, ew = frames.embeddings.shape[2], frames.embeddings.shape[3]
+            _C.launch("gsx_embed_merge_append_upsampled", emb, pointclouds.capacity, e, e_bs, assoc, rec, B, H, W, eh,
+                      ew, e.shape[-1], EMBED_DTYPES[e.dtype])
+        else:
+            _C.launch("gsx_embed_merge_append", emb, pointclouds.capacity, e, e_bs, assoc, rec, B, H, W, e.shape[-1],
+                      EMBED_DTYPES[e.dtype])
     pointclouds._mark_device_updated(pointclouds._bound + P)
 
 
@@ -508,7 +515,9 @@ class _MergeAppendFn(torch.autograd.Function):
     (K1r; K2, or gsx_records_from_table); the winners are index-only, as in the reference (fusionutils.py:523).
     With the map's embeddings `emb` (B, cap, D) and the frame's `e` (B, 1, H, W, D), float32, K4 also records each
     merge's weights and KE (gsx_embed_merge_append) merges the embeddings, a third output; the backward runs
-    gsx_embed_merge_bwd first and hands its d c0 / d alpha terms to K4's (gsx_fusion_merge_append_bwd_emb)."""
+    gsx_embed_merge_bwd first and hands its d c0 / d alpha terms to K4's (gsx_fusion_merge_append_bwd_emb).  A frame
+    with upsample_embeddings carries its coarse (B, 1, h, w, D) image instead, through the _upsampled entry points,
+    and gets its gradient in that shape."""
 
     @staticmethod
     def forward(ctx, pack, geo, col, gv, gn, rgb, vloc, emb=None, e=None):
@@ -541,9 +550,14 @@ class _MergeAppendFn(torch.autograd.Function):
             e_c = e.detach().contiguous()
             _C.launch("gsx_fusion_merge_append_rec", outs[0], outs[1], with_cc, counts_in, counts_out, cap_out, rgb_c,
                       P * 3, B, H, W, ws.buf, pointclouds._overflow_flag(), assoc, rec, 1 if radii else 0)
-            _C.launch("gsx_embed_merge_append", emb_out, cap_out, e_c, P * D, assoc, rec, B, H, W, D, 0)
+            up = (e.shape[2], e.shape[3]) if frames.upsample_embeddings else None  # the coarse image's (h, w)
+            if up is None:
+                _C.launch("gsx_embed_merge_append", emb_out, cap_out, e_c, P * D, assoc, rec, B, H, W, D, 0)
+            else:
+                _C.launch("gsx_embed_merge_append_upsampled", emb_out, cap_out, e_c, up[0] * up[1] * D, assoc, rec, B,
+                          H, W, up[0], up[1], D, 0)
             outs.append(emb_out)
-            ctx.emb = (rec, emb.detach().contiguous(), e_c, e.shape)
+            ctx.emb = (rec, emb.detach().contiguous(), e_c, e.shape, up)
         if pack[4] is not None:  # (fuse_and_prune's free-space step reads it)
             pack[4].append(assoc)
         ctx.saved = (assoc, counts_in, geo.detach(), col.detach(), gv_c, gn_c, rgb_c, vloc_c)
@@ -566,13 +580,18 @@ class _MergeAppendFn(torch.autograd.Function):
                       gn, rgb, vloc, B, H, W, sigma, *d_map, *d_frame)
             return (None, d_map[0], d_map[1], d_frame[0].view(gv_shape), d_frame[1].view(gv_shape),
                     d_frame[2].view(rgb_shape), d_frame[3].view(gv_shape))
-        rec, emb, e, e_shape = ctx.emb
+        rec, emb, e, e_shape, up = ctx.emb
         D = e.shape[-1]
         d_emb = torch.empty_like(emb)
         d_e = torch.empty_like(e)
         d_w = torch.empty((2, B, H * W), dtype=torch.float32, device=dev)  # d c0, d alpha per pixel
-        _C.launch("gsx_embed_merge_bwd", assoc, rec, counts_in, emb, cap_in, e,
-                  None if g_emb is None else g_emb.contiguous(), cap_out, B, H, W, D, d_emb, d_e, d_w[0], d_w[1])
+        g_emb = None if g_emb is None else g_emb.contiguous()
+        if up is None:
+            _C.launch("gsx_embed_merge_bwd", assoc, rec, counts_in, emb, cap_in, e, g_emb, cap_out, B, H, W, D, d_emb,
+                      d_e, d_w[0], d_w[1])
+        else:
+            _C.launch("gsx_embed_merge_bwd_upsampled", assoc, rec, counts_in, emb, cap_in, e, g_emb, cap_out, B, H, W,
+                      up[0], up[1], D, d_emb, d_e, d_w[0], d_w[1])
         _C.launch("gsx_fusion_merge_append_bwd_emb", assoc, counts_in, geo_c, col_c, with_cc, cap_in, *gs, cap_out, gv,
                   gn, rgb, vloc, B, H, W, sigma, d_w[0], d_w[1], *d_map, *d_frame)
         return (None, d_map[0], d_map[1], d_frame[0].view(gv_shape), d_frame[1].view(gv_shape),

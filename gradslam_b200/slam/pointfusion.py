@@ -86,7 +86,9 @@ class PointFusion(ICPSLAM):
 
         Frames with embeddings (RGBDImages(embeddings=...)) give maps with per-surfel embeddings, merged with the
         colours' weights, on every path; the pruning options (stable_confidence, free_space_margin, merge_overlapping)
-        refuse them with ValueError.
+        refuse them with ValueError.  With RGBDImages(..., upsample_embeddings=True) the embedding image may be coarser
+        than the depth and is upsampled bilinearly where it is fused; the whole-sequence call then uploads only the
+        coarse images.
 
         depth_filter, depth_filter_tracking_only (extension; default None, False): bilateral filtering of the live depth
         for the tracking and the fusion, or for the tracking alone, see ICPSLAM.  The whole-sequence call (odom='gt')
@@ -291,11 +293,15 @@ class PointFusion(ICPSLAM):
                 if i == 0:
                     assoc = torch.empty((B, P), dtype=torch.int32, device=dev)
                     rec = torch.empty((B, P, 2), dtype=torch.float32, device=dev)
-                _C.launch("gsx_pointfusion_sequence_gt_emb", pc._geo, pc._col, pc._counts_dev, pc.capacity,
-                          min(s0 * P, pc.capacity), fused_depth, rgb, K, poses, B, L, s0, s1, H, W, float(self.dist_th),
-                          float(self.dot_th), float(self.sigma), ws.buf, pc._overflow_flag(),
-                          1 if self.surfel_radii else 0, pc._emb, emb, emb.shape[-1], EMBED_DTYPES[emb.dtype], assoc,
-                          rec)
+                args = (pc._geo, pc._col, pc._counts_dev, pc.capacity, min(s0 * P, pc.capacity), fused_depth, rgb, K,
+                        poses, B, L, s0, s1, H, W, float(self.dist_th), float(self.dot_th), float(self.sigma), ws.buf,
+                        pc._overflow_flag(), 1 if self.surfel_radii else 0, pc._emb, emb)
+                if frames.upsample_embeddings:  # (B, L, h, w, D) coarse images, sampled by the upsampled KE
+                    _C.launch("gsx_pointfusion_sequence_gt_emb_upsampled", *args, emb.shape[2], emb.shape[3],
+                              emb.shape[-1], EMBED_DTYPES[emb.dtype], assoc, rec)
+                else:
+                    _C.launch("gsx_pointfusion_sequence_gt_emb", *args, emb.shape[-1], EMBED_DTYPES[emb.dtype], assoc,
+                              rec)
         if not on_device:
             for t in ((raw_depth, raw_rgb) if raw else (depth, rgb)):
                 t.record_stream(copy_stream)

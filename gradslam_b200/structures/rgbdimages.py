@@ -186,6 +186,24 @@ def _check_embedding_image(e, rgb_shape, cdim):
             "(B, L, D, H, W)" if cdim == 2 else "(B, L, H, W, D)", tuple(e.shape)))
 
 
+def _check_coarse_embedding_image(e, rgb_shape, cdim):
+    """(B, L, h, w, D) channels-last (cdim 4) or (B, L, D, h, w) channels-first (cdim 2), 1 <= h <= H, 1 <= w <= W, an
+    embedding image that the fused map update upsamples bilinearly to the (H, W) of rgb_shape."""
+    if not torch.is_tensor(e):
+        raise TypeError("Expected embeddings to be of type tensor or None; got {}".format(type(e)))
+    if e.dtype not in _EMBED_DTYPES:
+        raise TypeError("embeddings must be float32, float16 or bfloat16; got {}".format(e.dtype))
+    if e.ndim != 5:
+        raise ValueError("embeddings should have ndim=5, but had ndim={}".format(e.ndim))
+    sp = (2, 3) if cdim == 4 else (3, 4)  # (h, w) dimensions of e
+    D, (h, w) = e.shape[cdim], (e.shape[sp[0]], e.shape[sp[1]])
+    H, W = rgb_shape[sp[0]], rgb_shape[sp[1]]
+    if tuple(e.shape[:2]) != tuple(rgb_shape[:2]) or D < 1 or not (1 <= h <= H and 1 <= w <= W):
+        raise ValueError("Expected upsampled embeddings to have shape {0} with D >= 1, 1 <= h <= {1} and 1 <= w <= {2}. "
+                         "Got {3} instead".format("(B, L, D, h, w)" if cdim == 2 else "(B, L, h, w, D)", H, W,
+                                                  tuple(e.shape)))
+
+
 class RGBDImages(object):
     _INTERNAL_TENSORS = [
         "_rgb_image", "_depth_image", "_intrinsics", "_poses", "_pixel_pos",
@@ -195,10 +213,14 @@ class RGBDImages(object):
     def __init__(self, rgb_image: torch.Tensor, depth_image: torch.Tensor, intrinsics: torch.Tensor,
                  poses: Optional[torch.Tensor] = None, channels_first: bool = False,
                  device: Union[torch.device, str, None] = None, *, pixel_pos: Optional[torch.Tensor] = None,
-                 embeddings: Optional[torch.Tensor] = None):
+                 embeddings: Optional[torch.Tensor] = None, upsample_embeddings: bool = False):
         """embeddings (extension): a per-pixel embedding image at the depth's resolution, (B, L, H, W, D) or, with
         channels_first, (B, L, D, H, W), D >= 1, in float32, float16 or bfloat16, on the frames' device.  The fused map
-        update keeps a confidence-weighted mean of it per surfel (Pointclouds.embeddings_padded)."""
+        update keeps a confidence-weighted mean of it per surfel (Pointclouds.embeddings_padded).
+        upsample_embeddings (extension, default False): the embedding image is coarser than the depth, (B, L, h, w, D)
+        or (B, L, D, h, w) with 1 <= h <= H and 1 <= w <= W (a CLIP or DINO feature grid), and the map update samples
+        it bilinearly at each pixel it fuses, as F.interpolate(e, (H, W), mode='bilinear', align_corners=False) would,
+        without forming the full-resolution image."""
         super().__init__()
         for name, val, opt in (("rgb_image", rgb_image, False), ("depth_image", depth_image, False),
                                ("intrinsics", intrinsics, False), ("poses", poses, True),
@@ -241,7 +263,13 @@ class RGBDImages(object):
         if pixel_pos is not None and pixel_pos.shape != self._pixel_pos_shape:
             raise ValueError("Expected pixel_pos to have shape {0}. Got {1} instead".format(
                 self._pixel_pos_shape, pixel_pos.shape))
-        if embeddings is not None:
+        if not isinstance(upsample_embeddings, bool):
+            raise TypeError("Expected upsample_embeddings to be of type bool; got {}".format(type(upsample_embeddings)))
+        if upsample_embeddings:
+            if embeddings is None:
+                raise ValueError("upsample_embeddings=True needs an embedding image (embeddings=...)")
+            _check_coarse_embedding_image(embeddings, rgb_image.shape, cdim)
+        elif embeddings is not None:
             _check_embedding_image(embeddings, rgb_image.shape, cdim)
 
         devices = set(x.device for x in (rgb_image, depth_image, intrinsics, poses, pixel_pos, embeddings)
@@ -256,6 +284,7 @@ class RGBDImages(object):
         self._poses = poses.to(self.device) if poses is not None else None
         self._pixel_pos = pixel_pos.to(self.device) if pixel_pos is not None else None
         self._embeddings = embeddings.to(self.device) if embeddings is not None else None
+        self._upsample_embeddings = upsample_embeddings
 
         self._vertex_map = None
         self._global_vertex_map = None
@@ -288,6 +317,7 @@ class RGBDImages(object):
             raise IndexError("Incorrect indexing at dimension 1, make sure range is within 0 and {0}".format(self._L))
         other = RGBDImages(new_rgb, self._depth_image[sl[0], sl[1]], self._intrinsics[sl[0], :],
                            channels_first=self.channels_first)
+        other._upsample_embeddings = self._upsample_embeddings
         for k in self._INTERNAL_TENSORS:
             if k in ("_rgb_image", "_depth_image", "_intrinsics"):
                 continue
@@ -330,8 +360,14 @@ class RGBDImages(object):
 
     @property
     def embeddings(self):
-        """The per-pixel embedding image (B, L, H, W, D) ((B, L, D, H, W) channels-first), or None."""
+        """The per-pixel embedding image (B, L, H, W, D) ((B, L, D, H, W) channels-first), or None; with
+        upsample_embeddings, the coarse (B, L, h, w, D) image."""
         return self._embeddings
+
+    @property
+    def upsample_embeddings(self):
+        """True when the embedding image is coarser than the depth and is upsampled bilinearly where it is fused."""
+        return self._upsample_embeddings
 
     @property
     def has_poses(self):
@@ -390,7 +426,8 @@ class RGBDImages(object):
         else:
             depth = bilateral_filter_depth(self._depth_image, f)
         return RGBDImages(self._rgb_image, depth, self._intrinsics, self._poses, channels_first=self.channels_first,
-                          pixel_pos=self._pixel_pos, embeddings=self._embeddings)
+                          pixel_pos=self._pixel_pos, embeddings=self._embeddings,
+                          upsample_embeddings=self._upsample_embeddings)
 
     # ------------------------------------------------------------------ setters (cache invalidation as rgbdimages.py:399-463)
     @staticmethod
@@ -439,6 +476,7 @@ class RGBDImages(object):
     def clone(self):
         other = RGBDImages(self._rgb_image.clone(), self._depth_image.clone(), self._intrinsics.clone(),
                            channels_first=self.channels_first)
+        other._upsample_embeddings = self._upsample_embeddings
         for k in self._INTERNAL_TENSORS:
             if k in ("_rgb_image", "_depth_image", "_intrinsics"):
                 continue

@@ -211,6 +211,28 @@ int gsx_embed_merge_bwd(const int32_t *assoc, const float *merge_rec, const int3
                         const float *map_embeddings, int64_t capacity_in, const float *frame_embeddings,
                         const float *g_embeddings, int64_t capacity_out, int B, int H, int W, int D,
                         float *d_map_embeddings, float *d_frame_embeddings, float *d_c0, float *d_alpha, void *stream);
+/* KE with an embedding image coarser than the depth (the upsampled KE): frame_embeddings (B,eh,ew,D), 1 <= eh <= H,
+ * 1 <= ew <= W, with element stride frame_bstride >= eh*ew*D (elements).  Each merged or appended pixel (v,u) takes, in
+ * place of e[pix], the bilinear sample of F.interpolate(mode='bilinear', align_corners=False), per axis (y likewise
+ * with v, H, eh):  scale = (float)ew / (float)W,  sx = max(scale * (u + 0.5f) - 0.5f, 0),  x0 = (int)sx,
+ * x1 = x0 + (x0 < ew-1),  lx1 = sx - x0,  lx0 = 1 - lx1;
+ * f = ly0 * (lx0 * e[y0,x0] + lx1 * e[y0,x1]) + ly1 * (lx0 * e[y1,x0] + lx1 * e[y1,x1]) in float32, each operation
+ * rounded separately, half taps upcast exactly, f itself not rounded; then merged ((c0*E) + (alpha*f)) * inv or
+ * appended f, rounded once to the storage type, as gsx_embed_merge_append.  At eh = H, ew = W, f = e[pix] (finite e).
+ * Refused before any launch: eh, ew out of range, a short stride, null or misaligned pointers. */
+int gsx_embed_merge_append_upsampled(void *map_embeddings, int64_t capacity, const void *frame_embeddings,
+                                     int64_t frame_bstride, const int32_t *assoc, const float *merge_rec, int B, int H,
+                                     int W, int eh, int ew, int D, int dtype, void *stream);
+/* Backward of gsx_embed_merge_append_upsampled (float32): frame_embeddings and d_frame_embeddings are dense
+ * (B,eh,ew,D).  d_map_embeddings, d_c0 and d_alpha as gsx_embed_merge_bwd with f re-sampled from the taps; d e[t] is
+ * the sum over the merged and appended pixels p, in row-major order, of w_k(p) * d f(p) for every tap k of p (in the
+ * order 00, 01, 10, 11) on texel t, with w_00 = ly0*lx0 and so on and d f = g * alpha * inv (merged) or g
+ * (appended); a tap that lands on t twice at the clamped border counts twice.  No atomics: two runs give equal bits. */
+int gsx_embed_merge_bwd_upsampled(const int32_t *assoc, const float *merge_rec, const int32_t *counts_in,
+                                  const float *map_embeddings, int64_t capacity_in, const float *frame_embeddings,
+                                  const float *g_embeddings, int64_t capacity_out, int B, int H, int W, int eh, int ew,
+                                  int D, float *d_map_embeddings, float *d_frame_embeddings, float *d_c0,
+                                  float *d_alpha, void *stream);
 /* gsx_fusion_merge_append_bwd whose d c0 (slot 6 of a merged row's d_map_geometry) and d alpha of every merged pixel
  * also receive emb_d_c0 / emb_d_alpha (B,H,W) of gsx_embed_merge_bwd, so that the embeddings' gradient reaches the
  * pre-merge confidence and, through alpha, the camera-frame vertex.
@@ -290,6 +312,16 @@ int gsx_pointfusion_sequence_gt_emb(float *map_geometry, float *map_colors, int3
                                     float dist_th, float dot_th, double sigma, void *workspace, int32_t *overflow_flag,
                                     int surfel_radii, void *map_embeddings, const void *frame_embeddings, int D,
                                     int dtype, int32_t *assoc, float *merge_rec, void *stream);
+/* gsx_pointfusion_sequence_gt_emb with embedding images coarser than the depth: frame_embeddings (B,L,eh,ew,D)
+ * dense, 1 <= eh <= H, 1 <= ew <= W; every frame's KE is gsx_embed_merge_append_upsampled's.  Geometry, colours and
+ * counts equal gsx_pointfusion_sequence_gt_radii's bit for bit. */
+int gsx_pointfusion_sequence_gt_emb_upsampled(float *map_geometry, float *map_colors, int32_t *counts,
+                                              int64_t capacity, int64_t max_count0, const float *depth,
+                                              const float *rgb, const float *intrinsics, const float *poses, int B,
+                                              int L, int s_begin, int s_end, int H, int W, float dist_th, float dot_th,
+                                              double sigma, void *workspace, int32_t *overflow_flag, int surfel_radii,
+                                              void *map_embeddings, const void *frame_embeddings, int eh, int ew,
+                                              int D, int dtype, int32_t *assoc, float *merge_rec, void *stream);
 /* ------------------------------------------------------------------------------------------------
  * Removal of unstable surfels (opt-in extension; gradslam has no such step, so no reference line is replaced).
  * Keller et al. 2013, "Real-time 3D reconstruction in dynamic scenes using point-based fusion", section 4.3: a surfel
