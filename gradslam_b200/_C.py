@@ -125,9 +125,10 @@ SIGNATURES = {
     "gsx_icp_normal_eq_scratch_bytes": (c_i64, [c_int]),
     "gsx_icp_normal_eq_fwd": (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gsx_icp_normal_eq_bwd": (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "gsx_icp_normal_eq_batched_fwd": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_i64, c_vp]),
-    "gsx_icp_normal_eq_batched_bwd": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
-                                              c_vp]),
+    "gsx_icp_normal_eq_batched_fwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_i64, c_float, c_vp]),
+    "gsx_icp_normal_eq_batched_bwd": (
+        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_float, c_vp]),
     "gsx_icp_solve_fwd": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
     "gsx_icp_solve_bwd": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "gsx_icp_update_fwd": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_float, c_float, c_float, c_float,
@@ -142,59 +143,25 @@ SIGNATURES = {
     "gsx_icp_align_scratch_bytes": (c_i64, [c_int, c_int, c_int]),
     "gsx_icp_align": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_int, c_int, c_float, c_int, c_float,
-                c_float, c_float, c_float, c_float, c_vp, c_vp, c_vp, c_i64, c_vp]),
+                c_float, c_float, c_float, c_float, c_vp, c_vp, c_vp, c_i64, c_float, c_vp]),
     "gsx_icp_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int, c_i64]),
     "gsx_icp_localize": (
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int,
                 c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64,
-                c_vp, c_i64, c_u32, c_vp, c_vp]),
-    "gsx_icp_projective_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
+                c_vp, c_i64, c_u32, c_vp, c_float, c_vp]),
+    "gsx_icp_projective_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int, c_int]),
     "gsx_icp_localize_projective": (
         c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
-                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_vp]),
-    "gsx_icp_localize_projective_splats": (
-        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
                 c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_int,
-                c_vp]),
+                c_vp, c_vp, c_i64, c_float, c_float, c_float, c_vp]),
     "gsx_icp_projective_targets": (
-        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
-    "gsx_icp_projective_rgb_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
-    "gsx_icp_localize_projective_rgb": (
-        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
-                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_int,
-                c_vp, c_vp, c_i64, c_float, c_vp]),
-    "gsx_icp_projective_targets_rgb": (
         c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
                 c_vp, c_vp]),
     "gsx_icp_joint_normal_eq_batched_fwd": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
-                c_vp, c_i64, c_vp]),
-    "gsx_icp_joint_normal_eq_batched_bwd": (
-        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
-                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
-    "gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes": (c_i64, [c_int, c_int]),
-    "gsx_icp_joint_normal_eq_batched_bwd_intrinsics": (
-        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
-                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
-    "gsx_icp_align_robust": (
-        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_int, c_int, c_float, c_int, c_float,
-                c_float, c_float, c_float, c_float, c_vp, c_vp, c_vp, c_i64, c_float, c_vp]),
-    "gsx_icp_localize_robust": (
-        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int,
-                c_int, c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64,
-                c_vp, c_i64, c_u32, c_vp, c_float, c_vp]),
-    "gsx_icp_localize_projective_robust": (
-        c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int,
-                c_int, c_float, c_int, c_float, c_float, c_float, c_float, c_float, c_vp, c_i64, c_vp, c_i64, c_int,
-                c_vp, c_vp, c_i64, c_float, c_float, c_float, c_vp]),
-    "gsx_icp_normal_eq_batched_robust_fwd": (
-        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_i64, c_float, c_vp]),
-    "gsx_icp_normal_eq_batched_robust_bwd": (
-        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_float, c_vp]),
-    "gsx_icp_joint_normal_eq_batched_robust_fwd": (
-        c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
                 c_vp, c_i64, c_float, c_float, c_vp]),
-    "gsx_icp_joint_normal_eq_batched_robust_bwd": (
+    "gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes": (c_i64, [c_int, c_int]),
+    "gsx_icp_joint_normal_eq_batched_bwd": (
         c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_float, c_vp,
                 c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_float, c_float, c_vp]),
     "gsx_icp_project_associate": (

@@ -20,12 +20,11 @@
 //   render_icp_targets   (gsx_render.cu) the map seen from the previous pose through R1's z-buffer: index image and the
 //                        winning rows' world-frame points / normals at full resolution; with max_splat_px >= 1
 //                        through R1d's, a disk row's point being the surface point its pixel sees
-//                        (gsx_icp_localize_projective_splats)
 //   k_icp_proj_linearize a source point is associated with the pixel it projects to in the previous camera (the fusion
 //                        step's project()) if a row covers that pixel; the same rows, reduction and partials layout as
 //                        k_icp_knn_linearize, so k_icp_solve / k_icp_update run unchanged
 //   k_icp_project_associate  the association alone (index-only op of the differentiable mode)
-// Photometric term (gsx_icp_localize_projective_rgb, photometric_weight w > 0): E_icp + w E_rgb as in ElasticFusion.
+// Photometric term (gsx_icp_localize_projective at photometric_weight w > 0): E_icp + w E_rgb as in ElasticFusion.
 //   k_icp_gather_src<true>    also the intensity I_s of each source point's live colour
 //   k_icp_model_intensity     after the target build: I_m, the intensity of the colour of each pixel's winning row
 //   k_icp_proj_linearize<true> an associated point whose pixel is photometrically valid (off the border, it and its
@@ -34,9 +33,10 @@
 //   k_icp_joint_linearize_idx / _bwd  the geometric + photometric sums at a given association and their backward
 //                        (gsx_icp_joint_normal_eq_batched_fwd / _bwd, the op of the differentiable mode; the same
 //                        photometric_row, the backward through dual numbers)
-// Huber weights (the *_robust entry points): kRobust = true instantiations of k_icp_knn_linearize, k_icp_proj_linearize
-// and the normal-equation ops weigh a row outside the scale delta in row_products<true> / add_weighted_products<true>,
-// shared by the fused and the taped kernels; huber_adjoint is their backward.
+// Huber weights (a finite huber_delta or photometric_huber_delta; all +inf runs the unweighted kernels): kRobust = true
+// instantiations of k_icp_knn_linearize, k_icp_proj_linearize and the normal-equation ops weigh a row outside the
+// scale delta in row_products<true> / add_weighted_products<true>, shared by the fused and the taped kernels;
+// huber_adjoint is their backward.
 #include "gsx_common.cuh"
 #include "../../include/gsx.h"
 
@@ -1593,11 +1593,11 @@ struct ProjectiveWorkspace {  // of gsx_icp_localize_projective; nothing in it o
   IcpState st;
   int64_t *index;        // (B, H*W) z-buffer, then the index image
   float *tgt_p, *tgt_n;  // (B, H*W, 3)
-  float *I_s, *I_m;      // (B, ns_cap) source and (B, H*W) model intensities, with_rgb only
+  float *I_s, *I_m;      // (B, ns_cap) source and (B, H*W) model intensities, with_rgb only (else null)
   int ns_cap, nblk;
 };
 
-// with_rgb: the layout of gsx_icp_localize_projective_rgb, the geometric layout followed by the intensity arrays
+// with_rgb: the layout of the photometric term (w > 0), the geometric layout followed by the intensity arrays
 inline ProjectiveWorkspace projective_workspace_layout(Carver &c, int B, int H, int W, int ds, bool with_rgb = false) {
   ProjectiveWorkspace w;
   const int64_t P = (int64_t)H * W;
@@ -1631,12 +1631,24 @@ extern "C" int64_t gsx_icp_workspace_bytes(int B, int H, int W, int ds, int64_t 
   return c.bytes;
 }
 
-// gsx_icp_align (hb == nullptr) and gsx_icp_align_robust
-static int icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
-                     const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
-                     const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
-                     float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
-                     int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, const Huber *hb, void *stream) {
+// refuses a Huber scale that is not > 0 (NaN included); +inf is allowed and leaves that residual unweighted
+#define GSX_CHECK_HUBER(fn, name, d) \
+  GSX_CHECK_ARG((d) > 0.0f, fn ": " name " %g must be > 0 (+inf = unweighted)", (double)(d))
+
+// The Huber-weighted kernels (kRobust = true) run only when a scale is finite: with every scale +inf they would add
+// exactly the unweighted sums, which the unweighted instantiations compute faster.
+static inline const Huber *huber_weights(const Huber &hb) {
+  return hb.delta == INFINITY && hb.delta_p == INFINITY ? nullptr : &hb;
+}
+
+extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
+                             const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
+                             const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
+                             float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
+                             int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, float huber_delta,
+                             void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_align", "huber_delta", huber_delta);
+  const Huber scales{huber_delta, INFINITY};
   GSX_CHECK_ARG(src_points && src_count && tgt_points && tgt_normals && tgt_count && transform_out && scratch,
                 "gsx_icp_align: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1 && numiters >= 0, "gsx_icp_align: bad extents");
@@ -1650,37 +1662,10 @@ static int icp_align(const float *src_points, const int32_t *src_count, int ns_s
   cudaMemcpyAsync(sc.src, src_points, (size_t)B * ns_stride * 12, cudaMemcpyDeviceToDevice, s);
   const int rc = run_icp_loop(sc.src, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
                               initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp,
-                              B2p, nu, sc.partials, nblk, sc.st, nn_idx_out, sc.grid, hb, s);
+                              B2p, nu, sc.partials, nblk, sc.st, nn_idx_out, sc.grid, huber_weights(scales), s);
   if (rc) return rc;
   cudaMemcpyAsync(transform_out, sc.st.T_total, (size_t)B * 64, cudaMemcpyDeviceToDevice, s);
   return 0;
-}
-
-extern "C" int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
-                             const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
-                             const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
-                             float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
-                             int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, void *stream) {
-  return icp_align(src_points, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
-                   initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu,
-                   transform_out, nn_idx_out, scratch, scratch_bytes, nullptr, stream);
-}
-
-// refuses a Huber scale that is not > 0 (NaN included); +inf is allowed and weighs every finite row 1
-#define GSX_CHECK_HUBER(fn, name, d) \
-  GSX_CHECK_ARG((d) > 0.0f, fn ": " name " %g must be > 0 (+inf = unweighted)", (double)(d))
-
-extern "C" int gsx_icp_align_robust(const float *src_points, const int32_t *src_count, int ns_stride,
-                                    const float *tgt_points, const float *tgt_normals, const int32_t *tgt_count,
-                                    int nt_stride, int B, const float *initial_transform, int mode, int numiters,
-                                    float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                    float B2p, float nu, float *transform_out, int64_t *nn_idx_out, void *scratch,
-                                    int64_t scratch_bytes, float huber_delta, void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_align_robust", "huber_delta", huber_delta);
-  const Huber hb{huber_delta, 0.0f};
-  return icp_align(src_points, src_count, ns_stride, tgt_points, tgt_normals, tgt_count, nt_stride, B,
-                   initial_transform, mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu,
-                   transform_out, nn_idx_out, scratch, scratch_bytes, &hb, stream);
 }
 
 extern "C" int64_t gsx_icp_align_scratch_bytes(int B, int ns_stride, int nt_stride) {
@@ -1697,14 +1682,16 @@ extern "C" int64_t gsx_icp_tgt_scratch_bytes(int B, int64_t tgt_capacity) {
   return c.bytes;
 }
 
-// gsx_icp_localize (hb == nullptr) and gsx_icp_localize_robust
-static int icp_localize(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
-                        const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
-                        const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
-                        int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                        float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
-                        int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity, uint32_t epoch,
-                        int32_t *overflow_flag, const Huber *hb, void *stream) {
+extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
+                                const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
+                                const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds,
+                                int mode, int numiters, float damp, int use_dist_thresh, float dist_thresh,
+                                float lambda_max, float Bp, float B2p, float nu, void *tgt_scratch,
+                                int64_t tgt_capacity, float *poses_out, int64_t poses_out_bstride, void *workspace,
+                                int64_t workspace_map_capacity, uint32_t epoch, int32_t *overflow_flag,
+                                float huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_localize", "huber_delta", huber_delta);
+  const Huber scales{huber_delta, INFINITY};
   GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace && tgt_scratch,
                 "gsx_icp_localize: null pointer");
   GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_geometry) & 15) == 0,
@@ -1736,42 +1723,12 @@ static int icp_localize(const float *map_geometry, const int32_t *counts, int64_
   GSX_CHECK_LAUNCH("gsx_icp_localize(gather)");
   const int rc = run_icp_loop(w.src, w.src_count, w.ns_cap, tgt.p, tgt.n, w.tgt_count, (int)tgt_capacity, B, nullptr,
                               mode, numiters, damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu, w.partials,
-                              w.nblk, w.st, nullptr, tgt.grid, hb, s);
+                              w.nblk, w.st, nullptr, tgt.grid, huber_weights(scales), s);
   if (rc) return rc;
   k_pose_compose<<<(B + 63) / 64, 64, 0, s>>>(w.st.T_total, prev_poses, prev_pose_bstride, poses_out,
                                               poses_out_bstride, B);
   GSX_CHECK_LAUNCH("gsx_icp_localize(compose)");
   return 0;
-}
-
-extern "C" int gsx_icp_localize(const float *map_geometry, const int32_t *counts,
-                                int64_t capacity, int64_t max_count, const float *depth, int64_t depth_bstride,
-                                const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
-                                float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
-                                int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity,
-                                uint32_t epoch, int32_t *overflow_flag, void *stream) {
-  return icp_localize(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
-                      prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh, dist_thresh,
-                      lambda_max, Bp, B2p, nu, tgt_scratch, tgt_capacity, poses_out, poses_out_bstride, workspace,
-                      workspace_map_capacity, epoch, overflow_flag, nullptr, stream);
-}
-
-extern "C" int gsx_icp_localize_robust(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                       int64_t max_count, const float *depth, int64_t depth_bstride,
-                                       const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                       int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
-                                       float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                       float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
-                                       int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity,
-                                       uint32_t epoch, int32_t *overflow_flag, float huber_delta, void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_localize_robust", "huber_delta", huber_delta);
-  const Huber hb{huber_delta, 0.0f};
-  return icp_localize(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
-                      prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh, dist_thresh,
-                      lambda_max, Bp, B2p, nu, tgt_scratch, tgt_capacity, poses_out, poses_out_bstride, workspace,
-                      workspace_map_capacity, epoch, overflow_flag, &hb, stream);
 }
 
 extern "C" int64_t gsx_knn1_scratch_bytes(int B, int ns_stride, int nt_stride) {
@@ -1810,11 +1767,12 @@ extern "C" int64_t gsx_icp_normal_eq_scratch_bytes(int ns) {
   return (int64_t)((ns + kIcpBlock - 1) / kIcpBlock) * kNumSums * 4;
 }
 
-// gsx_icp_normal_eq_batched_fwd (hb == nullptr) and gsx_icp_normal_eq_batched_robust_fwd
-static int normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                 const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                 const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
-                                 const Huber *hb, void *stream) {
+extern "C" int gsx_icp_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+                                             const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
+                                             const int64_t *nn_idx, float *sums_out, void *scratch,
+                                             int64_t scratch_bytes, float huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_normal_eq_batched_fwd", "huber_delta", huber_delta);
+  const Huber scales{huber_delta, INFINITY};
   GSX_CHECK_ARG(src_points && tgt_points && tgt_normals && nn_idx && sums_out && scratch,
                 "gsx_icp_normal_eq_batched_fwd: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1 &&
@@ -1823,9 +1781,9 @@ static int normal_eq_batched_fwd(const float *src_points, const int32_t *src_cou
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 grid((unsigned)nblk, (unsigned)B);
-  if (hb)
+  if (huber_weights(scales))
     k_icp_linearize_idx<true><<<grid, kIcpBlock, 0, s>>>(src_points, ns_stride, src_count, tgt_points, tgt_normals,
-                                                         nt_stride, nn_idx, (float *)scratch, hb->delta);
+                                                         nt_stride, nn_idx, (float *)scratch, huber_delta);
   else
     k_icp_linearize_idx<<<grid, kIcpBlock, 0, s>>>(src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride,
                                                    nn_idx, (float *)scratch, 0.0f);
@@ -1834,64 +1792,29 @@ static int normal_eq_batched_fwd(const float *src_points, const int32_t *src_cou
   return 0;
 }
 
-extern "C" int gsx_icp_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
+extern "C" int gsx_icp_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
                                              const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                             const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
+                                             const int64_t *nn_idx, const float *g_sums, float *g_src,
+                                             float *g_tgt_points_rows, float *g_tgt_normals_rows, float huber_delta,
                                              void *stream) {
-  return normal_eq_batched_fwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx,
-                               sums_out, scratch, scratch_bytes, nullptr, stream);
-}
-
-extern "C" int gsx_icp_normal_eq_batched_robust_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                                    const float *tgt_points, const float *tgt_normals, int nt_stride,
-                                                    int B, const int64_t *nn_idx, float *sums_out, void *scratch,
-                                                    int64_t scratch_bytes, float huber_delta, void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_normal_eq_batched_robust_fwd", "huber_delta", huber_delta);
-  const Huber hb{huber_delta, 0.0f};
-  return normal_eq_batched_fwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx,
-                               sums_out, scratch, scratch_bytes, &hb, stream);
-}
-
-// gsx_icp_normal_eq_batched_bwd (hb == nullptr) and gsx_icp_normal_eq_batched_robust_bwd
-static int normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                 const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                 const int64_t *nn_idx, const float *g_sums, float *g_src, float *g_tgt_points_rows,
-                                 float *g_tgt_normals_rows, const Huber *hb, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_normal_eq_batched_bwd", "huber_delta", huber_delta);
+  const Huber scales{huber_delta, INFINITY};
   GSX_CHECK_ARG(src_points && tgt_points && tgt_normals && nn_idx && g_sums && g_src && g_tgt_points_rows &&
                     g_tgt_normals_rows,
                 "gsx_icp_normal_eq_batched_bwd: null pointer");
   GSX_CHECK_ARG(B >= 1 && ns_stride >= 1 && nt_stride >= 1, "gsx_icp_normal_eq_batched_bwd: bad sizes");
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   const dim3 grid((unsigned)nblk, (unsigned)B);
-  if (hb)
+  if (huber_weights(scales))
     k_icp_linearize_bwd<true><<<grid, kIcpBlock, 0, (cudaStream_t)stream>>>(
         src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride, nn_idx, g_sums, g_src, g_tgt_points_rows,
-        g_tgt_normals_rows, hb->delta);
+        g_tgt_normals_rows, huber_delta);
   else
     k_icp_linearize_bwd<<<grid, kIcpBlock, 0, (cudaStream_t)stream>>>(
         src_points, ns_stride, src_count, tgt_points, tgt_normals, nt_stride, nn_idx, g_sums, g_src, g_tgt_points_rows,
         g_tgt_normals_rows, 0.0f);
   GSX_CHECK_LAUNCH("gsx_icp_normal_eq_batched_bwd");
   return 0;
-}
-
-extern "C" int gsx_icp_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                             const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                             const int64_t *nn_idx, const float *g_sums, float *g_src,
-                                             float *g_tgt_points_rows, float *g_tgt_normals_rows, void *stream) {
-  return normal_eq_batched_bwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx, g_sums,
-                               g_src, g_tgt_points_rows, g_tgt_normals_rows, nullptr, stream);
-}
-
-extern "C" int gsx_icp_normal_eq_batched_robust_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                                    const float *tgt_points, const float *tgt_normals, int nt_stride,
-                                                    int B, const int64_t *nn_idx, const float *g_sums, float *g_src,
-                                                    float *g_tgt_points_rows, float *g_tgt_normals_rows,
-                                                    float huber_delta, void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_normal_eq_batched_robust_bwd", "huber_delta", huber_delta);
-  const Huber hb{huber_delta, 0.0f};
-  return normal_eq_batched_bwd(src_points, src_count, ns_stride, tgt_points, tgt_normals, nt_stride, B, nn_idx, g_sums,
-                               g_src, g_tgt_points_rows, g_tgt_normals_rows, &hb, stream);
 }
 
 extern "C" int gsx_icp_normal_eq_fwd(const float *src_points, int ns, const float *tgt_points,
@@ -1925,45 +1848,33 @@ extern "C" int gsx_icp_normal_eq_bwd(const float *src_points, int ns, const floa
   return 0;
 }
 
-extern "C" int64_t gsx_icp_projective_workspace_bytes(int B, int H, int W, int ds) {
+extern "C" int64_t gsx_icp_projective_workspace_bytes(int B, int H, int W, int ds, int photometric) {
   if (B < 1 || H < 1 || W < 1 || ds < 1) return -1;
   Carver c(nullptr);
-  projective_workspace_layout(c, B, H, W, ds);
+  projective_workspace_layout(c, B, H, W, ds, photometric != 0);
   return c.bytes;
 }
 
-extern "C" int gsx_icp_localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                           int64_t max_count, const float *depth, int64_t depth_bstride,
-                                           const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                           int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
-                                           int numiters, float damp, int use_dist_thresh, float dist_thresh,
-                                           float lambda_max, float Bp, float B2p, float nu, float *poses_out,
-                                           int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
-                                           void *stream) {
-  return gsx_icp_localize_projective_splats(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics,
-                                            K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters,
-                                            damp, use_dist_thresh, dist_thresh, lambda_max, Bp, B2p, nu, poses_out,
-                                            poses_out_bstride, workspace, workspace_bytes, 0, stream);
-}
-
-namespace gsx {
-// colours of the photometric term (gsx_icp_localize_projective_rgb); w == 0 runs the geometric kernels
-struct PhotometricInputs {
-  const float *map_colours;  // (B, capacity, 4)
-  const float *rgb;          // live colour, channels-last, element stride rgb_bstride
-  int64_t rgb_bstride;
-  float w;
-};
-
-// gsx_icp_localize_projective_splats (pm == nullptr, the geometric workspace), gsx_icp_localize_projective_rgb and
-// gsx_icp_localize_projective_robust (hb != nullptr: the Huber-weighted kernels)
-static int localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
-                               const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
-                               const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
-                               int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max,
-                               float Bp, float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
-                               void *workspace, int64_t workspace_bytes, int max_splat_px, const PhotometricInputs *pm,
-                               const Huber *hb, void *stream) {
+extern "C" int gsx_icp_localize_projective(
+    const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count, const float *depth,
+    int64_t depth_bstride, const float *intrinsics, int64_t K_bstride, const float *prev_poses,
+    int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters, float damp, int use_dist_thresh,
+    float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
+    void *workspace, int64_t workspace_bytes, int max_splat_px, const float *map_colours, const float *rgb,
+    int64_t rgb_bstride, float photometric_weight, float huber_delta, float photometric_huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_localize_projective", "huber_delta", huber_delta);
+  GSX_CHECK_HUBER("gsx_icp_localize_projective", "photometric_huber_delta", photometric_huber_delta);
+  GSX_CHECK_ARG(photometric_weight >= 0.0f && photometric_weight <= 3.402823466e38f,
+                "gsx_icp_localize_projective: photometric_weight %g must be finite and >= 0",
+                (double)photometric_weight);
+  GSX_CHECK_ARG(photometric_weight > 0.0f || photometric_huber_delta == INFINITY,
+                "gsx_icp_localize_projective: a finite photometric_huber_delta needs photometric_weight > 0");
+  const bool photometric = photometric_weight > 0.0f;
+  if (photometric) {
+    GSX_CHECK_ARG(map_colours && rgb, "gsx_icp_localize_projective: null colour pointer");
+    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
+                  "gsx_icp_localize_projective: colour rows must be 16-byte aligned");
+  }
   GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX,
                 "gsx_icp_localize_projective: max_splat_px %d outside [0, %d]", max_splat_px, GSX_MAX_SPLAT_PX);
   GSX_CHECK_ARG(map_geometry && counts && depth && intrinsics && prev_poses && poses_out && workspace,
@@ -1971,27 +1882,27 @@ static int localize_projective(const float *map_geometry, const int32_t *counts,
   GSX_CHECK_ARG(B >= 1 && H >= 2 && W >= 2 && ds >= 1 && numiters >= 0, "gsx_icp_localize_projective: bad extents");
   GSX_CHECK_ARG(mode == 0 || mode == 1, "gsx_icp_localize_projective: mode must be 0 (ICP) or 1 (gradICP)");
   Carver c(workspace);
-  const ProjectiveWorkspace w = projective_workspace_layout(c, B, H, W, ds, pm != nullptr);
+  const ProjectiveWorkspace w = projective_workspace_layout(c, B, H, W, ds, photometric);
   GSX_CHECK_ARG(workspace_bytes >= c.bytes, "gsx_icp_localize_projective: workspace too small (%lld < %lld)",
                 (long long)workspace_bytes, (long long)c.bytes);
-  const bool rgb = pm && pm->w > 0.0f;
+  const Huber scales{huber_delta, photometric_huber_delta};
   cudaStream_t s = (cudaStream_t)stream;
   GatherSrcArgs gs{depth, depth_bstride, intrinsics, K_bstride, prev_poses, prev_pose_bstride, B, H, W, ds,
                    w.src, w.src_count, w.ns_cap};
-  if (rgb) k_icp_gather_src<true><<<B, 1024, 0, s>>>(gs, GatherRgbArgs{pm->rgb, pm->rgb_bstride, w.I_s});
+  if (photometric) k_icp_gather_src<true><<<B, 1024, 0, s>>>(gs, GatherRgbArgs{rgb, rgb_bstride, w.I_s});
   else k_icp_gather_src<false><<<B, 1024, 0, s>>>(gs, GatherRgbArgs{});
   if (render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
                          prev_pose_bstride, B, H, W, max_splat_px, w.index, w.tgt_p, w.tgt_n, s))
     return 1;
   const int64_t P = (int64_t)H * W;
-  if (rgb)
+  if (photometric)
     k_icp_model_intensity<<<dim3((unsigned)((P + kIcpBlock - 1) / kIcpBlock), (unsigned)B), kIcpBlock, 0, s>>>(
-        w.index, pm->map_colours, capacity, P, w.I_m);
+        w.index, map_colours, capacity, P, w.I_m);
   ProjLinearize lin{ProjLinArgs{w.src, w.src_count, w.ns_cap, nullptr, 0,
                                 ProjTargets{prev_poses, prev_pose_bstride, intrinsics, K_bstride, image_bounds(H, W),
                                             w.index, w.tgt_p, w.tgt_n, dist_thresh, use_dist_thresh},
                                 w.partials},
-                    ProjRgb{w.I_s, w.I_m, rgb ? pm->w : 0.0f}, hb};
+                    ProjRgb{w.I_s, w.I_m, photometric ? photometric_weight : 0.0f}, huber_weights(scales)};
   const int rc = icp_iterations(lin, w.ns_cap, B, nullptr, mode, numiters, damp, lambda_max, Bp, B2p, nu, w.partials,
                                 w.nblk, w.st, s);
   if (rc) return rc;
@@ -2000,98 +1911,31 @@ static int localize_projective(const float *map_geometry, const int32_t *counts,
   GSX_CHECK_LAUNCH("gsx_icp_localize_projective");
   return 0;
 }
-}  // namespace gsx
 
-extern "C" int gsx_icp_localize_projective_splats(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                                  int64_t max_count, const float *depth, int64_t depth_bstride,
-                                                  const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                                  int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
-                                                  int numiters, float damp, int use_dist_thresh, float dist_thresh,
-                                                  float lambda_max, float Bp, float B2p, float nu, float *poses_out,
-                                                  int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
-                                                  int max_splat_px, void *stream) {
-  return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
-                             prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
-                             dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
-                             workspace_bytes, max_splat_px, nullptr, nullptr, stream);
-}
-
-extern "C" int64_t gsx_icp_projective_rgb_workspace_bytes(int B, int H, int W, int ds) {
-  if (B < 1 || H < 1 || W < 1 || ds < 1) return -1;
-  Carver c(nullptr);
-  projective_workspace_layout(c, B, H, W, ds, true);
-  return c.bytes;
-}
-
-extern "C" int gsx_icp_localize_projective_rgb(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                               int64_t max_count, const float *depth, int64_t depth_bstride,
-                                               const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                               int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
-                                               int numiters, float damp, int use_dist_thresh, float dist_thresh,
-                                               float lambda_max, float Bp, float B2p, float nu, float *poses_out,
-                                               int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes,
-                                               int max_splat_px, const float *map_colours, const float *rgb,
-                                               int64_t rgb_bstride, float photometric_weight, void *stream) {
-  GSX_CHECK_ARG(photometric_weight >= 0.0f && photometric_weight <= 3.402823466e38f,
-                "gsx_icp_localize_projective_rgb: photometric_weight %g must be finite and >= 0",
-                (double)photometric_weight);
-  if (photometric_weight > 0.0f) {
-    GSX_CHECK_ARG(map_colours && rgb, "gsx_icp_localize_projective_rgb: null colour pointer");
+extern "C" int gsx_icp_projective_targets(const float *map_geometry, const float *map_colours, const int32_t *counts,
+                                          int64_t capacity, int64_t max_count, const float *intrinsics,
+                                          int64_t K_bstride, const float *prev_poses, int64_t pose_bstride, int B,
+                                          int H, int W, int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n,
+                                          float *I_m, void *stream) {
+  GSX_CHECK_ARG(max_splat_px >= 0 && max_splat_px <= GSX_MAX_SPLAT_PX,
+                "gsx_icp_projective_targets: max_splat_px %d outside [0, %d]", max_splat_px, GSX_MAX_SPLAT_PX);
+  GSX_CHECK_ARG(intrinsics && prev_poses && index && tgt_p && tgt_n, "gsx_icp_projective_targets: null pointer");
+  if (max_count > 0) GSX_CHECK_ARG(map_geometry && counts, "gsx_icp_projective_targets: null map pointer");
+  if (I_m && max_count > 0) {
+    GSX_CHECK_ARG(map_colours, "gsx_icp_projective_targets: null colour pointer");
     GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
-                  "gsx_icp_localize_projective_rgb: colour rows must be 16-byte aligned");
+                  "gsx_icp_projective_targets: colour rows must be 16-byte aligned");
   }
-  const PhotometricInputs pm{map_colours, rgb, rgb_bstride, photometric_weight};
-  return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
-                             prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
-                             dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
-                             workspace_bytes, max_splat_px, &pm, nullptr, stream);
-}
-
-extern "C" int gsx_icp_localize_projective_robust(
-    const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count, const float *depth,
-    int64_t depth_bstride, const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-    int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters, float damp, int use_dist_thresh,
-    float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
-    void *workspace, int64_t workspace_bytes, int max_splat_px, const float *map_colours, const float *rgb,
-    int64_t rgb_bstride, float photometric_weight, float huber_delta, float photometric_huber_delta, void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_localize_projective_robust", "huber_delta", huber_delta);
-  GSX_CHECK_HUBER("gsx_icp_localize_projective_robust", "photometric_huber_delta", photometric_huber_delta);
-  GSX_CHECK_ARG(photometric_weight >= 0.0f && photometric_weight <= 3.402823466e38f,
-                "gsx_icp_localize_projective_robust: photometric_weight %g must be finite and >= 0",
-                (double)photometric_weight);
-  GSX_CHECK_ARG(photometric_weight > 0.0f || photometric_huber_delta == INFINITY,
-                "gsx_icp_localize_projective_robust: a finite photometric_huber_delta needs photometric_weight > 0");
-  if (photometric_weight > 0.0f) {
-    GSX_CHECK_ARG(map_colours && rgb, "gsx_icp_localize_projective_robust: null colour pointer");
-    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
-                  "gsx_icp_localize_projective_robust: colour rows must be 16-byte aligned");
-  }
-  const PhotometricInputs pm{map_colours, rgb, rgb_bstride, photometric_weight};
-  const Huber hb{huber_delta, photometric_huber_delta};
-  return localize_projective(map_geometry, counts, capacity, max_count, depth, depth_bstride, intrinsics, K_bstride,
-                             prev_poses, prev_pose_bstride, B, H, W, ds, mode, numiters, damp, use_dist_thresh,
-                             dist_thresh, lambda_max, Bp, B2p, nu, poses_out, poses_out_bstride, workspace,
-                             workspace_bytes, max_splat_px, &pm, &hb, stream);
-}
-
-extern "C" int gsx_icp_projective_targets_rgb(const float *map_geometry, const float *map_colours,
-                                              const int32_t *counts, int64_t capacity, int64_t max_count,
-                                              const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                              int64_t pose_bstride, int B, int H, int W, int max_splat_px,
-                                              int64_t *index, float *tgt_p, float *tgt_n, float *I_m, void *stream) {
-  GSX_CHECK_ARG(I_m, "gsx_icp_projective_targets_rgb: null pointer");
-  if (max_count > 0) {
-    GSX_CHECK_ARG(map_colours, "gsx_icp_projective_targets_rgb: null colour pointer");
-    GSX_CHECK_ARG((reinterpret_cast<uintptr_t>(map_colours) & 15) == 0,
-                  "gsx_icp_projective_targets_rgb: colour rows must be 16-byte aligned");
-  }
-  if (gsx_icp_projective_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses,
-                                 pose_bstride, B, H, W, max_splat_px, index, tgt_p, tgt_n, stream))
+  cudaStream_t s = (cudaStream_t)stream;
+  if (render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses, pose_bstride, B,
+                         H, W, max_splat_px, index, tgt_p, tgt_n, s))
     return 1;
-  const int64_t P = (int64_t)H * W;
-  k_icp_model_intensity<<<dim3((unsigned)((P + kIcpBlock - 1) / kIcpBlock), (unsigned)B), kIcpBlock, 0,
-                          (cudaStream_t)stream>>>(index, map_colours, capacity, P, I_m);
-  GSX_CHECK_LAUNCH("gsx_icp_projective_targets_rgb");
+  if (I_m) {
+    const int64_t P = (int64_t)H * W;
+    k_icp_model_intensity<<<dim3((unsigned)((P + kIcpBlock - 1) / kIcpBlock), (unsigned)B), kIcpBlock, 0, s>>>(
+        index, map_colours, capacity, P, I_m);
+    GSX_CHECK_LAUNCH("gsx_icp_projective_targets");
+  }
   return 0;
 }
 
@@ -2133,12 +1977,16 @@ static int joint_args(const char *fn, const float *src_points, const int32_t *sr
   return 0;
 }
 
-// gsx_icp_joint_normal_eq_batched_fwd (hb == nullptr) and gsx_icp_joint_normal_eq_batched_robust_fwd
-static int joint_fwd(const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
-                     const float *tgt_points, const float *tgt_normals, const float *model_colours,
-                     const int64_t *index, int B, int H, int W, const int64_t *nn_idx, const float *prev_poses,
-                     const float *intrinsics, float photometric_weight, float *sums_out, void *scratch,
-                     int64_t scratch_bytes, const Huber *hb, void *stream) {
+extern "C" int gsx_icp_joint_normal_eq_batched_fwd(
+    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
+    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
+    float *sums_out, void *scratch, int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
+    void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_fwd", "huber_delta", huber_delta);
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_fwd", "photometric_huber_delta", photometric_huber_delta);
+  const Huber scales{huber_delta, photometric_huber_delta};
+  const Huber *hb = huber_weights(scales);
   JointArgs a;
   if (joint_args("gsx_icp_joint_normal_eq_batched_fwd", src_points, src_count, ns_stride, src_colours, tgt_points,
                  tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
@@ -2155,61 +2003,23 @@ static int joint_fwd(const float *src_points, const int32_t *src_count, int ns_s
   return 0;
 }
 
-extern "C" int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                                   const float *src_colours, const float *tgt_points,
-                                                   const float *tgt_normals, const float *model_colours,
-                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
-                                                   const float *prev_poses, const float *intrinsics,
-                                                   float photometric_weight, float *sums_out, void *scratch,
-                                                   int64_t scratch_bytes, void *stream) {
-  return joint_fwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
-                   W, nn_idx, prev_poses, intrinsics, photometric_weight, sums_out, scratch, scratch_bytes, nullptr,
-                   stream);
-}
-
-extern "C" int gsx_icp_joint_normal_eq_batched_robust_fwd(
-    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
-    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
-    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
-    float *sums_out, void *scratch, int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
-    void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_fwd", "huber_delta", huber_delta);
-  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_fwd", "photometric_huber_delta", photometric_huber_delta);
-  const Huber hb{huber_delta, photometric_huber_delta};
-  return joint_fwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
-                   W, nn_idx, prev_poses, intrinsics, photometric_weight, sums_out, scratch, scratch_bytes, &hb, stream);
-}
-
-extern "C" int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                                   const float *src_colours, const float *tgt_points,
-                                                   const float *tgt_normals, const float *model_colours,
-                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
-                                                   const float *prev_poses, const float *intrinsics,
-                                                   float photometric_weight, const float *g_sums, float *g_src,
-                                                   float *g_src_colours, float *g_tgt_points_rows,
-                                                   float *g_tgt_normals_rows, float *g_stencil_colours_rows,
-                                                   float *g_prev_poses, void *scratch, int64_t scratch_bytes,
-                                                   void *stream) {
-  return gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
-      src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H, W, nn_idx,
-      prev_poses, intrinsics, photometric_weight, g_sums, g_src, g_src_colours, g_tgt_points_rows, g_tgt_normals_rows,
-      g_stencil_colours_rows, g_prev_poses, nullptr, scratch, scratch_bytes, stream);
-}
-
-extern "C" int64_t gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(int B, int ns_stride) {
+extern "C" int64_t gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(int B, int ns_stride) {
   if (B < 0 || ns_stride < 0) return -1;
   const int64_t nblk = ((int64_t)ns_stride + kIcpBlock - 1) / kIcpBlock;
   return (int64_t)B * nblk * 12 * 4 * 2;
 }
 
-// gsx_icp_joint_normal_eq_batched_bwd_intrinsics (hb == nullptr) and gsx_icp_joint_normal_eq_batched_robust_bwd
-static int joint_bwd(const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
-                     const float *tgt_points, const float *tgt_normals, const float *model_colours,
-                     const int64_t *index, int B, int H, int W, const int64_t *nn_idx, const float *prev_poses,
-                     const float *intrinsics, float photometric_weight, const float *g_sums, float *g_src,
-                     float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
-                     float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch,
-                     int64_t scratch_bytes, const Huber *hb, void *stream) {
+extern "C" int gsx_icp_joint_normal_eq_batched_bwd(
+    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
+    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
+    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
+    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
+    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
+    float huber_delta, float photometric_huber_delta, void *stream) {
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_bwd", "huber_delta", huber_delta);
+  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_bwd", "photometric_huber_delta", photometric_huber_delta);
+  const Huber scales{huber_delta, photometric_huber_delta};
+  const Huber *hb = huber_weights(scales);
   JointArgs a;
   if (joint_args("gsx_icp_joint_normal_eq_batched_bwd", src_points, src_count, ns_stride, src_colours, tgt_points,
                  tgt_normals, model_colours, index, B, H, W, nn_idx, prev_poses, intrinsics, photometric_weight, a))
@@ -2220,7 +2030,7 @@ static int joint_bwd(const float *src_points, const int32_t *src_count, int ns_s
   const int nblk = (ns_stride + kIcpBlock - 1) / kIcpBlock;
   const int64_t pose_bytes = (int64_t)B * nblk * 12 * 4;
   if (g_intrinsics)
-    GSX_CHECK_ARG(scratch_bytes >= gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(B, ns_stride),
+    GSX_CHECK_ARG(scratch_bytes >= gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(B, ns_stride),
                   "gsx_icp_joint_normal_eq_batched_bwd: scratch too small");
   else
     GSX_CHECK_ARG(scratch_bytes >= pose_bytes, "gsx_icp_joint_normal_eq_batched_bwd: scratch too small");
@@ -2250,33 +2060,4 @@ static int joint_bwd(const float *src_points, const int32_t *src_count, int ns_s
   if (g_intrinsics) k_pose_grad_reduce<<<B, 16, 0, s>>>(k_partials, nblk, g_intrinsics, B);
   GSX_CHECK_LAUNCH("gsx_icp_joint_normal_eq_batched_bwd");
   return 0;
-}
-
-extern "C" int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
-    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
-    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
-    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
-    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
-    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
-    void *stream) {
-  return joint_bwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
-                   W, nn_idx, prev_poses, intrinsics, photometric_weight, g_sums, g_src, g_src_colours,
-                   g_tgt_points_rows, g_tgt_normals_rows, g_stencil_colours_rows, g_prev_poses, g_intrinsics, scratch,
-                   scratch_bytes, nullptr, stream);
-}
-
-extern "C" int gsx_icp_joint_normal_eq_batched_robust_bwd(
-    const float *src_points, const int32_t *src_count, int ns_stride, const float *src_colours,
-    const float *tgt_points, const float *tgt_normals, const float *model_colours, const int64_t *index, int B, int H,
-    int W, const int64_t *nn_idx, const float *prev_poses, const float *intrinsics, float photometric_weight,
-    const float *g_sums, float *g_src, float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
-    float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics, void *scratch, int64_t scratch_bytes,
-    float huber_delta, float photometric_huber_delta, void *stream) {
-  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_bwd", "huber_delta", huber_delta);
-  GSX_CHECK_HUBER("gsx_icp_joint_normal_eq_batched_robust_bwd", "photometric_huber_delta", photometric_huber_delta);
-  const Huber hb{huber_delta, photometric_huber_delta};
-  return joint_bwd(src_points, src_count, ns_stride, src_colours, tgt_points, tgt_normals, model_colours, index, B, H,
-                   W, nn_idx, prev_poses, intrinsics, photometric_weight, g_sums, g_src, g_src_colours,
-                   g_tgt_points_rows, g_tgt_normals_rows, g_stencil_colours_rows, g_prev_poses, g_intrinsics, scratch,
-                   scratch_bytes, &hb, stream);
 }

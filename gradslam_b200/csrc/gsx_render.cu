@@ -677,18 +677,6 @@ int render_icp_targets(const float *map_geometry, const int32_t *counts, int64_t
 }
 }  // namespace gsx
 
-extern "C" int gsx_icp_projective_targets(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                          int64_t max_count, const float *intrinsics, int64_t K_bstride,
-                                          const float *prev_poses, int64_t pose_bstride, int B, int H, int W,
-                                          int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n,
-                                          void *stream) {
-  if (check_splat_px("gsx_icp_projective_targets", max_splat_px)) return 1;
-  GSX_CHECK_ARG(intrinsics && prev_poses && index && tgt_p && tgt_n, "gsx_icp_projective_targets: null pointer");
-  if (max_count > 0) GSX_CHECK_ARG(map_geometry && counts, "gsx_icp_projective_targets: null map pointer");
-  return render_icp_targets(map_geometry, counts, capacity, max_count, intrinsics, K_bstride, prev_poses, pose_bstride,
-                            B, H, W, max_splat_px, index, tgt_p, tgt_n, (cudaStream_t)stream);
-}
-
 extern "C" int64_t gsx_render_views_bwd_scratch_bytes(int B, int L, int H, int W) {
   if (B < 1 || L < 1 || H < 1 || W < 1) return -1;
   return (int64_t)B * L * pixel_tiles(H, W) * 12 * 4 + 256;

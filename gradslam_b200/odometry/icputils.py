@@ -151,7 +151,7 @@ def _check_icp_args(src_pc, tgt_pc, tgt_normals, initial_transform, numiters):
 def icp_align(src, src_counts, tgt, tgt_normals, tgt_counts, T0, mode, numiters, damp, dist_thresh, lambda_max=2.0,
               B=1.0, B2=1.0, nu=200.0, want_idx=False, huber_delta=None):
     """Batched ICP (mode 0) / gradICP (mode 1) on padded clouds (Bn, N, 3) with int32 sizes.  One C call; with
-    huber_delta the Huber-weighted rows of gsx_icp_align_robust."""
+    huber_delta the Huber-weighted rows of gsx_icp_align."""
     for name, t in (("src", src), ("tgt", tgt), ("tgt_normals", tgt_normals)):
         _C.require_cuda(t, name)
     Bn, Ns, _ = src.shape
@@ -165,11 +165,8 @@ def icp_align(src, src_counts, tgt, tgt_normals, tgt_counts, T0, mode, numiters,
     args = (src.contiguous(), src_counts, Ns, tgt.contiguous(), tgt_normals.contiguous(), tgt_counts, Nt, Bn, T0c,
             int(mode), int(numiters), float(damp), 0 if dist_thresh is None else 1,
             0.0 if dist_thresh is None else float(dist_thresh), float(lambda_max), float(B), float(B2), float(nu), out,
-            idx, scratch, nbytes)
-    if huber_delta is None:
-        _C.launch("gsx_icp_align", *args)
-    else:
-        _C.launch("gsx_icp_align_robust", *args, float(huber_delta))
+            idx, scratch, nbytes, _huber_scale(huber_delta))
+    _C.launch("gsx_icp_align", *args)
     return out, idx
 
 
@@ -293,10 +290,10 @@ class _RigidTransformFn(torch.autograd.Function):
 # kernel takes the batch index from blockIdx.y; values per element are bit-identical to the per-element ops (padding rows
 # contribute exact zeros to the fixed-order sums).
 class _NormalEqBatchedFn(torch.autograd.Function):
-    """huber_delta: None = gsx_icp_normal_eq_batched_fwd / _bwd; else their Huber-weighted variants at that scale."""
+    """gsx_icp_normal_eq_batched_fwd / _bwd; huber_delta: the float32 Huber scale of the rows (+inf = unweighted)."""
 
     @staticmethod
-    def forward(ctx, src, tgt, tgt_n, idx, src_counts, huber_delta=None):
+    def forward(ctx, src, tgt, tgt_n, idx, src_counts, huber_delta=math.inf):
         src_c, tgt_c, tn_c = (t.detach().contiguous().float() for t in (src, tgt, tgt_n))
         idx_c = idx.contiguous()
         _C.require_cuda(src_c, "src")
@@ -305,14 +302,10 @@ class _NormalEqBatchedFn(torch.autograd.Function):
         sums = torch.empty((Bn, 28), dtype=torch.float32, device=dev)
         nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        if huber_delta is None:
-            _C.launch("gsx_icp_normal_eq_batched_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums, scratch,
-                      nbytes)
-        else:
-            _C.launch("gsx_icp_normal_eq_batched_robust_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums,
-                      scratch, nbytes, float(huber_delta))
+        _C.launch("gsx_icp_normal_eq_batched_fwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, sums, scratch,
+                  nbytes, float(huber_delta))
         ctx.saved = (src_c, tgt_c, tn_c, idx_c, src_counts)
-        ctx.huber_delta = huber_delta
+        ctx.huber_delta = float(huber_delta)
         return sums
 
     @staticmethod
@@ -323,12 +316,8 @@ class _NormalEqBatchedFn(torch.autograd.Function):
         g = g.contiguous().float()
         g_src = torch.empty_like(src_c)
         rows_p, rows_n = torch.empty_like(src_c), torch.empty_like(src_c)
-        if ctx.huber_delta is None:
-            _C.launch("gsx_icp_normal_eq_batched_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src,
-                      rows_p, rows_n)
-        else:
-            _C.launch("gsx_icp_normal_eq_batched_robust_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src,
-                      rows_p, rows_n, float(ctx.huber_delta))
+        _C.launch("gsx_icp_normal_eq_batched_bwd", src_c, src_counts, Ns, tgt_c, tn_c, Nt, Bn, idx_c, g, g_src, rows_p,
+                  rows_n, ctx.huber_delta)
         # rows with idx < 0 carry zero gradients; scatter the per-source-row target gradients with the association
         flat = (idx_c.clamp(min=0) + torch.arange(Bn, device=dev).view(Bn, 1) * Nt).view(-1)
         g_tgt = torch.zeros((Bn * Nt, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_p.view(-1, 3))
@@ -408,14 +397,14 @@ class _RigidTransformBatchedFn(torch.autograd.Function):
 class _JointNormalEqBatchedFn(torch.autograd.Function):
     """The joint geometric + photometric normal equations of the projective ICP at a given association (idx (B,Ns) pixel
     or -1): (src, src_col (B,Ns,3), tgt, tgt_n, model_col (B,H*W,3), prev (B,4,4)) -> (B,28).  forward =
-    gsx_icp_joint_normal_eq_batched_fwd, backward = gsx_icp_joint_normal_eq_batched_bwd, or
-    gsx_icp_joint_normal_eq_batched_bwd_intrinsics when K requires grad (the photometric row reads K's first three rows);
-    the gradients of the model colours come per source row for the five stencil pixels and are scattered here.
-    huber: None, or (huber_delta, photometric_huber_delta) as float32 scales (+inf = that residual unweighted) for the
-    Huber-weighted gsx_icp_joint_normal_eq_batched_robust_fwd / _bwd."""
+    gsx_icp_joint_normal_eq_batched_fwd, backward = gsx_icp_joint_normal_eq_batched_bwd, with d/dK when K requires grad
+    (the photometric row reads K's first three rows); the gradients of the model colours come per source row for the
+    five stencil pixels and are scattered here.  huber: (huber_delta, photometric_huber_delta) as float32 scales
+    (+inf = that residual unweighted)."""
 
     @staticmethod
-    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W, huber=None):
+    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W,
+                huber=(math.inf, math.inf)):
         ins = [t.detach().contiguous().float() for t in (src, src_col, tgt, tgt_n, model_col, prev)]
         _C.require_cuda(ins[0], "src")
         Bn, Ns = ins[0].shape[:2]
@@ -423,12 +412,9 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         sums = torch.empty((Bn, 28), dtype=torch.float32, device=src.device)
         nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=src.device)
-        args = (ins[0], src_counts, Ns, ins[1], ins[2], ins[3], ins[4], index_c, Bn, int(H), int(W), idx_c, ins[5], K_c,
-                float(w), sums, scratch, nbytes)
-        if huber is None:
-            _C.launch("gsx_icp_joint_normal_eq_batched_fwd", *args)
-        else:
-            _C.launch("gsx_icp_joint_normal_eq_batched_robust_fwd", *args, *huber)
+        huber = tuple(float(d) for d in huber)
+        _C.launch("gsx_icp_joint_normal_eq_batched_fwd", ins[0], src_counts, Ns, ins[1], ins[2], ins[3], ins[4],
+                  index_c, Bn, int(H), int(W), idx_c, ins[5], K_c, float(w), sums, scratch, nbytes, *huber)
         ctx.saved = (ins, idx_c, index_c, src_counts, K_c, float(w), int(H), int(W), prev.shape)
         ctx.huber = huber
         ctx.K_shape = K.shape
@@ -443,30 +429,13 @@ class _JointNormalEqBatchedFn(torch.autograd.Function):
         g_src, g_col, rows_p, rows_n = (torch.empty_like(src) for _ in range(4))
         rows_st = torch.empty((Bn, Ns, 5, 3), dtype=torch.float32, device=dev)
         g_prev = torch.empty((Bn, 4, 4), dtype=torch.float32, device=dev)
-        g_K = None
-        if ctx.huber is not None:
-            want_K = ctx.needs_input_grad[9]
-            g_K = torch.zeros((Bn, 4, 4), dtype=torch.float32, device=dev) if want_K else None
-            nbytes = (_C.lib().gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(Bn, Ns) if want_K
-                      else Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns))
-            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _C.launch("gsx_icp_joint_normal_eq_batched_robust_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col,
-                      index, Bn, H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, g_K, scratch,
-                      nbytes, *ctx.huber)
-            g_K = None if g_K is None else g_K.view(ctx.K_shape)
-        elif ctx.needs_input_grad[9]:
-            g_K = torch.zeros((Bn, 4, 4), dtype=torch.float32, device=dev)
-            nbytes = _C.lib().gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(Bn, Ns)
-            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _C.launch("gsx_icp_joint_normal_eq_batched_bwd_intrinsics", src, src_counts, Ns, src_col, tgt, tgt_n,
-                      model_col, index, Bn, H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev,
-                      g_K, scratch, nbytes)
-            g_K = g_K.view(ctx.K_shape)
-        else:
-            nbytes = Bn * _C.lib().gsx_icp_normal_eq_scratch_bytes(Ns)
-            scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            _C.launch("gsx_icp_joint_normal_eq_batched_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col, index,
-                      Bn, H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, scratch, nbytes)
+        g_K = torch.zeros((Bn, 4, 4), dtype=torch.float32, device=dev) if ctx.needs_input_grad[9] else None
+        nbytes = _C.lib().gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(Bn, Ns)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _C.launch("gsx_icp_joint_normal_eq_batched_bwd", src, src_counts, Ns, src_col, tgt, tgt_n, model_col, index, Bn,
+                  H, W, idx, prev, K, w, g, g_src, g_col, rows_p, rows_n, rows_st, g_prev, g_K, scratch, nbytes,
+                  *ctx.huber)
+        g_K = None if g_K is None else g_K.view(ctx.K_shape)
         base = torch.arange(Bn, device=dev).view(Bn, 1) * P
         flat = (idx.clamp(min=0) + base).view(-1)  # rows with idx < 0 carry zero gradients
         g_tgt = torch.zeros((Bn * P, 3), dtype=torch.float32, device=dev).index_add_(0, flat, rows_p.view(-1, 3))
@@ -489,9 +458,7 @@ def _normal_equations_batched(src, src_counts, tgt, tgt_n, tgt_counts, dist_thre
             idx = torch.where(d2 < dist_thresh, idx, torch.full_like(idx, -1))
     else:
         idx = associate(src.detach())
-    if huber_delta is not None:
-        return _NormalEqBatchedFn.apply(src, tgt, tgt_n, idx, src_counts, huber_delta), idx
-    return _NormalEqBatchedFn.apply(src, tgt, tgt_n, idx, src_counts), idx
+    return _NormalEqBatchedFn.apply(src, tgt, tgt_n, idx, src_counts, _huber_scale(huber_delta)), idx
 
 
 def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numiters, damp, dist_thresh, lambda_max=2.0,
@@ -503,8 +470,8 @@ def _taped_icp_batched(src, src_counts, tgt, tgt_n, tgt_counts, T0, mode, numite
     (Bn,Ns,3), detached, returning the int64 target row per source row (-1 = none) - the projective association.
     normal_eq: None = _NormalEqBatchedFn; otherwise a function (src, tgt, tgt_n, idx) -> (Bn,28) sums (the joint op of
     the photometric term, which then carries its own Huber scales).
-    huber_delta: None = unweighted rows; else the Huber-weighted normal-equation op at that scale (gsx_icp_align_robust's
-    rows), so the loop minimises the Huber energy as the fused robust loop does."""
+    huber_delta: None = unweighted rows; else the Huber-weighted normal-equation op at that scale (the rows of
+    gsx_icp_align), so the loop minimises the Huber energy as the fused loop does."""
     dev = src.device
     Bn, Ns = src.shape[0], src.shape[1]
     # No valid source (or target) point in any element gives a padded width of 0, which the kernels reject.  One zero
@@ -743,12 +710,8 @@ def localize_against_map(pointclouds, live_frame, prev_frame, dsratio, odomprov)
             0 if dth is None else 1, 0.0 if dth is None else float(dth), float(getattr(odomprov, "lambda_max", 2.0)),
             float(getattr(odomprov, "B", 1.0)), float(getattr(odomprov, "B2", 1.0)),
             float(getattr(odomprov, "nu", 200.0)), tgt, bound, out, 16, ws.buf, ws.capacity, ws.next_epoch(),
-            pointclouds._overflow_flag())
-    huber = getattr(odomprov, "huber_delta", None)
-    if huber is None:
-        _C.launch("gsx_icp_localize", *args)
-    else:
-        _C.launch("gsx_icp_localize_robust", *args, float(huber))
+            pointclouds._overflow_flag(), _huber_scale(getattr(odomprov, "huber_delta", None)))
+    _C.launch("gsx_icp_localize", *args)
     return out
 
 
@@ -770,16 +733,17 @@ def project_associate(src, src_counts, tgt_points, tgt_index, prev_poses, K, H, 
 
 
 class _ProjectiveWorkspace:
-    """Workspace of gsx_icp_localize_projective per (device, B, H, W, ds): nothing in it outlives a call, so one
-    buffer serves every stream-ordered call with that shape."""
+    """Workspace of gsx_icp_localize_projective per (device, B, H, W, ds, photometric): nothing in it outlives a call,
+    so one buffer serves every stream-ordered call with that shape."""
     _cache = {}
 
     @classmethod
-    def get(cls, device, B, H, W, ds):
-        key = (str(device), B, H, W, ds)
+    def get(cls, device, B, H, W, ds, photometric):
+        key = (str(device), B, H, W, ds, bool(photometric))
         buf = cls._cache.get(key)
         if buf is None:
-            buf = torch.empty(_C.lib().gsx_icp_projective_workspace_bytes(B, H, W, ds), dtype=torch.uint8, device=device)
+            buf = torch.empty(_C.lib().gsx_icp_projective_workspace_bytes(B, H, W, ds, int(bool(photometric))),
+                              dtype=torch.uint8, device=device)
             cls._cache[key] = buf
         return buf
 
@@ -806,15 +770,15 @@ def projective_targets(pointclouds, K, prev_poses, H, W, target_splat_px=0):
         _C.require_cuda(pointclouds._geo, "pointclouds (geometry rows)")
         geo, counts = pointclouds._geo.detach().contiguous(), pointclouds._counts_dev[pointclouds._cur]
         cap, bound = pointclouds.capacity, pointclouds._bound
-    _C.launch("gsx_icp_projective_targets", geo, counts, cap, bound, K.detach().contiguous(), 16,
-              prev_poses.detach().contiguous(), 16, B, int(H), int(W), int(target_splat_px), index, tgt_p, tgt_n)
+    _C.launch("gsx_icp_projective_targets", geo, None, counts, cap, bound, K.detach().contiguous(), 16,
+              prev_poses.detach().contiguous(), 16, B, int(H), int(W), int(target_splat_px), index, tgt_p, tgt_n, None)
     return index, tgt_p, tgt_n
 
 
 def projective_intensity(pointclouds, K, prev_poses, H, W, target_splat_px=0):
     """The model image of the photometric term: (index (B,H*W) int64 as projective_targets gives it, I_m (B,H*W) the
     intensity (0.299 r + 0.587 g) + 0.114 b of the colour of each pixel's winning row, 0 where uncovered).  Forward only
-    (gsx_icp_projective_targets_rgb)."""
+    (gsx_icp_projective_targets)."""
     _C.require_cuda(K, "K")
     _C.require_cuda(prev_poses, "prev_poses")
     B = prev_poses.numel() // 16
@@ -829,35 +793,20 @@ def projective_intensity(pointclouds, K, prev_poses, H, W, target_splat_px=0):
         _C.require_cuda(pointclouds._geo, "pointclouds (geometry rows)")
         geo, col = pointclouds._geo.detach().contiguous(), pointclouds._col.detach().contiguous()
         counts, cap, bound = pointclouds._counts_dev[pointclouds._cur], pointclouds.capacity, pointclouds._bound
-    _C.launch("gsx_icp_projective_targets_rgb", geo, col, counts, cap, bound, K.detach().contiguous(), 16,
+    _C.launch("gsx_icp_projective_targets", geo, col, counts, cap, bound, K.detach().contiguous(), 16,
               prev_poses.detach().contiguous(), 16, B, int(H), int(W), int(target_splat_px), index, tgt_p, tgt_n, I_m)
     return index, I_m
 
 
-class _ProjectiveRgbWorkspace:
-    """Workspace of gsx_icp_localize_projective_rgb per (device, B, H, W, ds), as _ProjectiveWorkspace."""
-    _cache = {}
-
-    @classmethod
-    def get(cls, device, B, H, W, ds):
-        key = (str(device), B, H, W, ds)
-        buf = cls._cache.get(key)
-        if buf is None:
-            buf = torch.empty(_C.lib().gsx_icp_projective_rgb_workspace_bytes(B, H, W, ds), dtype=torch.uint8,
-                              device=device)
-            cls._cache[key] = buf
-        return buf
-
-
 def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0,
                         photometric_weight=0.0, photometric_huber_delta=None):
-    """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective_splats): the source
+    """ICPSLAM._localize with association='projective' as ONE C call (gsx_icp_localize_projective): the source
     is the live frame on the ds lattice at the previous pose, the target is the map rendered from the previous pose at
     full resolution (surfels with radii as disks when target_splat_px >= 1, see projective_targets), each source point
     is associated with the pixel it projects to.  Returns the new poses (B,1,4,4) = T_icp · prev pose.  No host
-    synchronisation.  photometric_weight w > 0 adds the photometric term of gsx_icp_localize_projective_rgb (the live
-    frame's and the map's colours); w = 0 is the geometric call.  With odomprov.huber_delta or photometric_huber_delta
-    set, the residuals are Huber-weighted at those scales (gsx_icp_localize_projective_robust)."""
+    synchronisation.  photometric_weight w > 0 adds the photometric term (the live frame's and the map's colours);
+    w = 0 is the geometric call.  With odomprov.huber_delta or photometric_huber_delta set, the residuals are
+    Huber-weighted at those scales."""
     live = live_frame.to_channels_last()
     B, _, H, W = live.shape
     dev = pointclouds.device
@@ -873,37 +822,23 @@ def localize_projective(pointclouds, live_frame, prev_frame, dsratio, odomprov, 
             pointclouds._bound, depth, d_bs, K, 16, prev, 16, B, H, W, int(dsratio), mode, int(odomprov.numiters),
             float(odomprov.damp), 0 if dth is None else 1, 0.0 if dth is None else float(dth), lambda_max, Bp, B2p, nu,
             out, 16)
-    huber = getattr(odomprov, "huber_delta", None)
-    if huber is not None or photometric_huber_delta is not None:
-        rgb, rgb_bs, col = None, 0, None
-        if photometric_weight:
-            if not pointclouds.has_colors or live.rgb_image is None:
-                raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
-            _C.require_cuda(live.rgb_image, "rgb_image")
-            rgb, rgb_bs = _frame_base(live.rgb_image, H * W * 3)
-            col = pointclouds._col.contiguous()
-        ws = _ProjectiveRgbWorkspace.get(dev, B, H, W, int(dsratio))
-        _C.launch("gsx_icp_localize_projective_robust", *args, ws, ws.numel(), int(target_splat_px), col, rgb, rgb_bs,
-                  float(photometric_weight), *_huber_scales(huber, photometric_huber_delta))
-        return out
-    if photometric_weight == 0:
-        ws = _ProjectiveWorkspace.get(dev, B, H, W, int(dsratio))
-        _C.launch("gsx_icp_localize_projective_splats", *args, ws, ws.numel(), int(target_splat_px))
-        return out
-    if not pointclouds.has_colors or live.rgb_image is None:
-        raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
-    _C.require_cuda(live.rgb_image, "rgb_image")
-    rgb, rgb_bs = _frame_base(live.rgb_image, H * W * 3)
-    ws = _ProjectiveRgbWorkspace.get(dev, B, H, W, int(dsratio))
-    _C.launch("gsx_icp_localize_projective_rgb", *args, ws, ws.numel(), int(target_splat_px),
-              pointclouds._col.contiguous(), rgb, rgb_bs, float(photometric_weight))
+    rgb, rgb_bs, col = None, 0, None
+    if photometric_weight:
+        if not pointclouds.has_colors or live.rgb_image is None:
+            raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
+        _C.require_cuda(live.rgb_image, "rgb_image")
+        rgb, rgb_bs = _frame_base(live.rgb_image, H * W * 3)
+        col = pointclouds._col.contiguous()
+    ws = _ProjectiveWorkspace.get(dev, B, H, W, int(dsratio), photometric_weight > 0)
+    _C.launch("gsx_icp_localize_projective", *args, ws, ws.numel(), int(target_splat_px), col, rgb, rgb_bs,
+              float(photometric_weight), _huber_scale(getattr(odomprov, "huber_delta", None)),
+              _huber_scale(photometric_huber_delta))
     return out
 
 
-def _huber_scales(huber_delta, photometric_huber_delta):
-    """The two float32 scales of the robust projective entry points, +inf for a residual left unweighted."""
-    return (math.inf if huber_delta is None else float(huber_delta),
-            math.inf if photometric_huber_delta is None else float(photometric_huber_delta))
+def _huber_scale(delta):
+    """The float32 Huber scale the C entry points take: +inf (None) leaves the residual unweighted."""
+    return math.inf if delta is None else float(delta)
 
 
 def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odomprov, target_splat_px=0,
@@ -964,7 +899,7 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
     mode, lambda_max, Bp, B2p, nu = _solver_params(odomprov)
     normal_eq = None
     huber = getattr(odomprov, "huber_delta", None)
-    scales = None if huber is None and photometric_huber_delta is None else _huber_scales(huber, photometric_huber_delta)
+    scales = (_huber_scale(huber), _huber_scale(photometric_huber_delta))
     if photometric_weight:
         if not pointclouds.has_colors or live.rgb_image is None:
             raise ValueError("photometric_weight > 0 needs a map with colours and a live frame with rgb_image")
@@ -974,8 +909,7 @@ def localize_projective_taped(pointclouds, live_frame, prev_frame, dsratio, odom
             src_col = src_col.new_zeros(B, 1, 3)
         prev_v = prev.reshape(B, 4, 4)
         normal_eq = lambda cur, t_p, t_n, idx: _JointNormalEqBatchedFn.apply(
-            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, Kg, photometric_weight, H, W,
-            *(() if scales is None else (scales,)))
+            cur, src_col, t_p, t_n, model_col, prev_v, idx, index, src_counts, Kg, photometric_weight, H, W, scales)
     T, _ = _taped_icp_batched(frames_pc.points_padded, src_counts, tgt_p, tgt_n, None, None, mode, odomprov.numiters,
                               odomprov.damp, dth, lambda_max, Bp, B2p, nu, associate=assoc, normal_eq=normal_eq,
                               huber_delta=huber)

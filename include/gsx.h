@@ -562,30 +562,21 @@ int gsx_icp_normal_eq_bwd(const float *src_points, int ns, const float *tgt_poin
 /* the same two ops for a padded batch (B, stride, 3) with int32 sizes (NULL = all rows): one launch for all elements
  * (the differentiable mode's op chain is recorded ONCE for the batch instead of once per element, which is what the
  * reference's providers do, odometry/icp.py:84-97).  sums (B,28); nn_idx (B, ns_stride), -1 = no neighbour; the target
- * gradients come back per SOURCE row (B, ns_stride, 3).  Padding rows get zero outputs / zero gradients. */
+ * gradients come back per SOURCE row (B, ns_stride, 3).  Padding rows get zero outputs / zero gradients.
+ * huber_delta (metres) weighs the rows by Huber's M-estimator (the op of the robust differentiable mode): a row with
+ * residual r and a = |r| <= huber_delta adds the unweighted products; a row with a > delta adds h (A_p A_q) and
+ * h (A_p r) with h = delta / a, and rho = delta ((a + a) - delta) instead of r r, so sums[27] is the Huber energy.
+ * These are the row products of gsx_icp_localize / gsx_icp_align at the same scale, bit for bit.  The backward carries
+ * dh/dr = -h / r of the h (A_p A_q) products and drho/dr = 2 h r.  +inf runs the unweighted kernels; a delta <= 0 or
+ * NaN is refused before any launch. */
 int gsx_icp_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
                                   const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
                                   const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
-                                  void *stream);
+                                  float huber_delta, void *stream);
 int gsx_icp_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
                                   const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
                                   const int64_t *nn_idx, const float *g_sums, float *g_src, float *g_tgt_points_rows,
-                                  float *g_tgt_normals_rows, void *stream);
-/* Huber-weighted gsx_icp_normal_eq_batched_fwd / _bwd (the op of the robust differentiable mode), same arguments plus
- * huber_delta.  A row with residual r and a = |r| <= huber_delta adds what the counterpart adds; a row with a > delta
- * adds h (A_p A_q) and h (A_p r) with h = delta / a, and rho = delta ((a + a) - delta) instead of r r, so sums[27] is
- * the Huber energy.  These are the row products of gsx_icp_localize_robust / gsx_icp_align_robust, bit for bit.  The
- * backward carries dh/dr = -h / r of the h (A_p A_q) products and drho/dr = 2 h r.  huber_delta = +inf gives the
- * counterpart's outputs bit for bit; a delta <= 0 or NaN is refused before any launch. */
-int gsx_icp_normal_eq_batched_robust_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                         const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                         const int64_t *nn_idx, float *sums_out, void *scratch, int64_t scratch_bytes,
-                                         float huber_delta, void *stream);
-int gsx_icp_normal_eq_batched_robust_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                         const float *tgt_points, const float *tgt_normals, int nt_stride, int B,
-                                         const int64_t *nn_idx, const float *g_sums, float *g_src,
-                                         float *g_tgt_points_rows, float *g_tgt_normals_rows, float huber_delta,
-                                         void *stream);
+                                  float *g_tgt_normals_rows, float huber_delta, void *stream);
 int gsx_icp_solve_fwd(const float *sums, const float *damp, int n, float *xi_out, float *dT_out, void *stream);
 int gsx_icp_solve_bwd(const float *sums, const float *damp, int n, const float *g_xi, const float *g_dT,
                       float *g_sums, float *g_damp, void *stream);
@@ -612,22 +603,16 @@ int gsx_rigid_transform_bwd(const float *points, int64_t n, const float *T, cons
 
 /* full ICP / gradICP on given clouds.  initial_transform (B,16) or NULL (identity).  transform_out (B,16).
  * nn_idx_out optional int64 (B, ns_stride): association of the last iteration (-1 = filtered out).
- * scratch: gsx_icp_align_scratch_bytes(B, ns_stride, nt_stride) bytes. */
+ * scratch: gsx_icp_align_scratch_bytes(B, ns_stride, nt_stride) bytes.  huber_delta (metres): a finite scale weighs the
+ * point-to-plane rows as gsx_icp_normal_eq_batched_fwd does (iteratively reweighted least squares inside the same LM /
+ * gradLM loop), and the error the loop compares (err, new_err) is the Huber energy sum rho; +inf runs the unweighted
+ * rows; a delta <= 0 or NaN is refused before any launch. */
 int64_t gsx_icp_align_scratch_bytes(int B, int ns_stride, int nt_stride);
 int gsx_icp_align(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
                   const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
                   const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
                   float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
-                  int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, void *stream);
-/* gsx_icp_align with Huber-weighted point-to-plane rows (iteratively reweighted least squares inside the same LM /
- * gradLM loop): each row is weighed as by gsx_icp_normal_eq_batched_robust_fwd at huber_delta (metres), and the error
- * the loop compares (err, new_err) is the Huber energy sum rho.  Same arguments and scratch plus huber_delta; +inf gives
- * gsx_icp_align's outputs bit for bit; a delta <= 0 or NaN is refused before any launch. */
-int gsx_icp_align_robust(const float *src_points, const int32_t *src_count, int ns_stride, const float *tgt_points,
-                         const float *tgt_normals, const int32_t *tgt_count, int nt_stride, int B,
-                         const float *initial_transform, int mode, int numiters, float damp, int use_dist_thresh,
-                         float dist_thresh, float lambda_max, float Bp, float B2p, float nu, float *transform_out,
-                         int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, float huber_delta, void *stream);
+                  int64_t *nn_idx_out, void *scratch, int64_t scratch_bytes, float huber_delta, void *stream);
 
 /* ICPSLAM._localize for odom in {icp, gradicp} (gradslam/slam/icpslam.py:238-247) as one call:
  * source cloud = live depth on the ds-lattice placed at the previous pose (downsample_rgbdimages,
@@ -638,7 +623,7 @@ int gsx_icp_align_robust(const float *src_points, const int32_t *src_count, int 
  * *overflow_flag is set to 1 if a target cloud did not fit tgt_capacity (surplus dropped).  workspace:
  * gsx_icp_workspace_bytes(B,H,W,ds,workspace_map_capacity) bytes zero-filled once (pass the same
  * workspace_map_capacity >= max_count on every call: it fixes the layout); `epoch` increases by one per
- * call on the same workspace, starting at 1. */
+ * call on the same workspace, starting at 1.  huber_delta weighs the rows as in gsx_icp_align (+inf = unweighted). */
 int64_t gsx_icp_workspace_bytes(int B, int H, int W, int ds, int64_t map_capacity);
 int64_t gsx_icp_tgt_scratch_bytes(int B, int64_t tgt_capacity);
 int gsx_icp_localize(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count, const float *depth, int64_t depth_bstride, const float *intrinsics,
@@ -646,16 +631,8 @@ int gsx_icp_localize(const float *map_geometry, const int32_t *counts, int64_t c
                      int ds, int mode, int numiters, float damp, int use_dist_thresh, float dist_thresh,
                      float lambda_max, float Bp, float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity,
                      float *poses_out, int64_t poses_out_bstride, void *workspace,
-                     int64_t workspace_map_capacity, uint32_t epoch, int32_t *overflow_flag, void *stream);
-/* gsx_icp_localize with the Huber-weighted rows of gsx_icp_align_robust.  Same arguments, workspace and target scratch
- * plus huber_delta; +inf gives gsx_icp_localize's poses bit for bit; a delta <= 0 or NaN is refused before any launch. */
-int gsx_icp_localize_robust(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
-                            const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
-                            const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode,
-                            int numiters, float damp, int use_dist_thresh, float dist_thresh, float lambda_max,
-                            float Bp, float B2p, float nu, void *tgt_scratch, int64_t tgt_capacity, float *poses_out,
-                            int64_t poses_out_bstride, void *workspace, int64_t workspace_map_capacity, uint32_t epoch,
-                            int32_t *overflow_flag, float huber_delta, void *stream);
+                     int64_t workspace_map_capacity, uint32_t epoch, int32_t *overflow_flag, float huber_delta,
+                     void *stream);
 
 /* Projective frame-to-model ICP / gradICP odometry (an extension: the reference associates by exact 1-NN).  One call
  * per frame step: source cloud as in gsx_icp_localize (live depth on the ds-lattice at the previous pose, valid pixels
@@ -665,155 +642,90 @@ int gsx_icp_localize_robust(const float *map_geometry, const int32_t *counts, in
  * (the projection of gsx_render_views: frustum (-1e-3, W - 0.999) x (-1e-3, H - 0.999), z > 0, round half to even,
  * clamp) iff a map row covers j and, with use_dist_thresh, |s - p_j|^2 < dist_thresh; poses_out[b] = T_icp[b] *
  * prev_poses[b].  intrinsics / prev_poses: B 4x4 matrices (the previous frame's camera) with the given element strides.
- * workspace: gsx_icp_projective_workspace_bytes(B,H,W,ds) bytes, any content (nothing in it outlives a call).
  * max_count = host upper bound on counts[b] <= capacity <= INT32_MAX.  An element with an empty map, or with no valid
- * live depth, keeps its previous pose exactly.  No host synchronisation. */
-int64_t gsx_icp_projective_workspace_bytes(int B, int H, int W, int ds);
+ * live depth, keeps its previous pose exactly.  No host synchronisation.
+ *
+ * Disk splats: max_splat_px = 0 renders one pixel per row; 1 .. GSX_MAX_SPLAT_PX renders the map as disks, others are
+ * refused before any launch.  The target images are then rendered with the z-buffer, keys, ties and fill of
+ * gsx_render_splats at max_splat_px; at a pixel j = h*W + w won by a disk row (radius > 0 and a non-zero normal) the
+ * target point is the surface point the pixel sees, (R v + t) with v = t_j K^-1 (w,h,1) (the K^-1 and arithmetic of
+ * gsx_backproject_normals_fwd) for the plane depth t_j and the previous pose [R | t], and the target normal the row's;
+ * other rows and uncovered pixels as at max_splat_px = 0.  The source, the association (the distance test measures
+ * against the surface point) and the loop are unchanged.  A map without radii gives the max_splat_px = 0 poses.
+ *
+ * Photometric term (ElasticFusion's E_icp + w E_rgb), photometric_weight = w > 0.  I(r, g, b) = (0.299 r + 0.587 g) +
+ * 0.114 b; the model image I_m is the intensity of map_colours (B, capacity, 4) of each pixel's winning row in the
+ * target index image, and a source point's I_s the intensity of the live colour at its lattice pixel (rgb:
+ * channels-last (H, W, 3) per element, element stride rgb_bstride floats).  A source point associated (geometrically,
+ * dist_thresh included) with a pixel j that is off the image border, with j and its four neighbours covered, also has
+ * the row A_p = [c, s x c], r_p = I_s - I_m[j], c = R_prev (g_u du/dq + g_v dv/dq) with the central differences g_u,
+ * g_v of I_m at j and the derivatives of the projection at q = T_prev^-1 s; its 28 sums become geo + w (A_p A_p),
+ * geo + w (A_p r_p), geo + w (r_p r_p).  w = 0 runs the geometric kernels, and map_colours / rgb may be NULL.  A
+ * negative or non-finite w, and null or unaligned colours with w > 0, are refused before any launch.
+ *
+ * Huber weights: the point-to-plane row at huber_delta (metres) as in gsx_icp_localize, and the photometric row at
+ * photometric_huber_delta (intensity): outside it, with h_p = delta_p / |r_p|, its products enter as
+ * acc + (w h_p) (A_p A_q), acc + (w h_p) (A_p r_p) and acc + w rho_p.  Both scales +inf run the unweighted kernels.
+ * A scale <= 0 or NaN, and a finite photometric_huber_delta with w = 0, are refused before any launch.
+ *
+ * workspace: gsx_icp_projective_workspace_bytes(B, H, W, ds, w > 0) bytes, any content (nothing in it outlives a call);
+ * the photometric layout also serves w = 0. */
+int64_t gsx_icp_projective_workspace_bytes(int B, int H, int W, int ds, int photometric);
 int gsx_icp_localize_projective(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
                                 const float *depth, int64_t depth_bstride, const float *intrinsics, int64_t K_bstride,
                                 const float *prev_poses, int64_t prev_pose_bstride, int B, int H, int W, int ds,
                                 int mode, int numiters, float damp, int use_dist_thresh, float dist_thresh,
                                 float lambda_max, float Bp, float B2p, float nu, float *poses_out,
-                                int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes, void *stream);
+                                int64_t poses_out_bstride, void *workspace, int64_t workspace_bytes, int max_splat_px,
+                                const float *map_colours, const float *rgb, int64_t rgb_bstride,
+                                float photometric_weight, float huber_delta, float photometric_huber_delta,
+                                void *stream);
 
-/* gsx_icp_localize_projective against the disk-splat render of the map (max_splat_px = 0 is gsx_icp_localize_projective
- * itself; 1 .. GSX_MAX_SPLAT_PX, others are refused before any launch).  The target images are rendered with the
- * z-buffer, keys, ties and fill of gsx_render_splats at max_splat_px; at a pixel j = h*W + w won by a disk row (radius
- * > 0 and a non-zero normal) the target point is the surface point the pixel sees, (R v + t) with v = t_j K^-1 (w,h,1)
- * (the K^-1 and arithmetic of gsx_backproject_normals_fwd) for the plane depth t_j and the previous pose [R | t], and
- * the target normal the row's; other rows and uncovered pixels as in gsx_icp_localize_projective.  The source, the
- * association (the distance test measures against the surface point) and the loop are unchanged; so is the workspace.
- * A map without radii gives the max_splat_px = 0 poses. */
-int gsx_icp_localize_projective_splats(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                       int64_t max_count, const float *depth, int64_t depth_bstride,
-                                       const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                       int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
-                                       float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                       float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
-                                       void *workspace, int64_t workspace_bytes, int max_splat_px, void *stream);
-
-/* The target images of gsx_icp_localize_projective_splats alone, the model's predicted vertex and normal maps seen from
+/* The target images of gsx_icp_localize_projective alone, the model's predicted vertex and normal maps seen from
  * prev_poses: index int64 (B, H*W) = the winning row or -1, tgt_p / tgt_n (B, H*W, 3) = the world-frame target point
- * and normal, zeros where uncovered.  index is the z-buffer while the call runs.  The map pointers may be NULL when
- * max_count is 0.  No host synchronisation. */
-int gsx_icp_projective_targets(const float *map_geometry, const int32_t *counts, int64_t capacity, int64_t max_count,
-                               const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                               int64_t pose_bstride, int B, int H, int W, int max_splat_px, int64_t *index,
-                               float *tgt_p, float *tgt_n, void *stream);
+ * and normal, zeros where uncovered.  index is the z-buffer while the call runs.  With I_m != NULL the call also writes
+ * the model image I_m (B, H*W) of the photometric term, 0 where uncovered, and then needs map_colours.  The map
+ * pointers may be NULL when max_count is 0.  No host synchronisation. */
+int gsx_icp_projective_targets(const float *map_geometry, const float *map_colours, const int32_t *counts,
+                               int64_t capacity, int64_t max_count, const float *intrinsics, int64_t K_bstride,
+                               const float *prev_poses, int64_t pose_bstride, int B, int H, int W, int max_splat_px,
+                               int64_t *index, float *tgt_p, float *tgt_n, float *I_m, void *stream);
 
-/* Joint geometric and photometric projective ICP (ElasticFusion's E_icp + w E_rgb): gsx_icp_localize_projective_splats
- * plus a photometric term of weight photometric_weight = w.  I(r, g, b) = (0.299 r + 0.587 g) + 0.114 b; the model image
- * I_m is the intensity of map_colours (B, capacity, 4) of each pixel's winning row in the target index image, and a
- * source point's I_s the intensity of the live colour at its lattice pixel (rgb: channels-last (H, W, 3) per element,
- * element stride rgb_bstride floats).  A source point associated (geometrically, dist_thresh included) with a pixel j
- * that is off the image border, with j and its four neighbours covered, also has the row A_p = [c, s x c],
- * r_p = I_s - I_m[j], c = R_prev (g_u du/dq + g_v dv/dq) with the central differences g_u, g_v of I_m at j and the
- * derivatives of the projection at q = T_prev^-1 s; its 28 sums become geo + w (A_p A_p), geo + w (A_p r_p),
- * geo + w (r_p r_p).  w = 0 computes exactly what gsx_icp_localize_projective_splats computes.  A negative or non-finite
- * w, and null colour pointers with w > 0, are refused before any launch.  workspace:
- * gsx_icp_projective_rgb_workspace_bytes(B,H,W,ds) bytes (it also serves gsx_icp_localize_projective_splats). */
-int64_t gsx_icp_projective_rgb_workspace_bytes(int B, int H, int W, int ds);
-int gsx_icp_localize_projective_rgb(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                    int64_t max_count, const float *depth, int64_t depth_bstride,
-                                    const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                    int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
-                                    float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                    float B2p, float nu, float *poses_out, int64_t poses_out_bstride, void *workspace,
-                                    int64_t workspace_bytes, int max_splat_px, const float *map_colours,
-                                    const float *rgb, int64_t rgb_bstride, float photometric_weight, void *stream);
-/* gsx_icp_localize_projective_rgb with Huber-weighted residuals: the point-to-plane row at huber_delta (metres) as in
- * gsx_icp_localize_robust, and the photometric row at photometric_huber_delta (intensity): outside it, with
- * h_p = delta_p / |r_p|, its products enter as acc + (w h_p) (A_p A_q), acc + (w h_p) (A_p r_p) and acc + w rho_p.
- * Same arguments plus the two scales; w = 0 and null colours keep the counterpart's meaning, and the workspace is
- * gsx_icp_projective_rgb_workspace_bytes(B,H,W,ds).  Both scales +inf give the counterpart's poses bit for bit.
- * A scale <= 0 or NaN, and a finite photometric_huber_delta with w = 0, are refused before any launch. */
-int gsx_icp_localize_projective_robust(const float *map_geometry, const int32_t *counts, int64_t capacity,
-                                       int64_t max_count, const float *depth, int64_t depth_bstride,
-                                       const float *intrinsics, int64_t K_bstride, const float *prev_poses,
-                                       int64_t prev_pose_bstride, int B, int H, int W, int ds, int mode, int numiters,
-                                       float damp, int use_dist_thresh, float dist_thresh, float lambda_max, float Bp,
-                                       float B2p, float nu, float *poses_out, int64_t poses_out_bstride,
-                                       void *workspace, int64_t workspace_bytes, int max_splat_px,
-                                       const float *map_colours, const float *rgb, int64_t rgb_bstride,
-                                       float photometric_weight, float huber_delta, float photometric_huber_delta,
-                                       void *stream);
-
-/* gsx_icp_projective_targets plus the model image I_m (B, H*W) of gsx_icp_localize_projective_rgb, 0 where uncovered.
- * map_colours may be NULL when max_count is 0. */
-int gsx_icp_projective_targets_rgb(const float *map_geometry, const float *map_colours, const int32_t *counts,
-                                   int64_t capacity, int64_t max_count, const float *intrinsics, int64_t K_bstride,
-                                   const float *prev_poses, int64_t pose_bstride, int B, int H, int W,
-                                   int max_splat_px, int64_t *index, float *tgt_p, float *tgt_n, float *I_m,
-                                   void *stream);
-
-/* The joint normal equations of gsx_icp_localize_projective_rgb at a GIVEN association (the op of the differentiable
- * mode; its rows are computed by the fused call's device functions, so the sums are the fused call's bit for bit).
- * Source rows i < src_count[b] of src_points / src_colours (B, ns_stride, 3), world frame and live colour; nn_idx
- * (B, ns_stride) the associated pixel or -1; tgt_points / tgt_normals / model_colours (B, H*W, 3) the target images and
- * the colour of each pixel's winning row (zeros where uncovered); index (B, H*W) the index image (-1 = uncovered);
- * prev_poses / intrinsics (B, 4, 4).  sums_out (B, 28): the geometric sums plus photometric_weight times the
- * photometric products.  scratch: B * gsx_icp_normal_eq_scratch_bytes(ns_stride) bytes.
+/* The joint normal equations of gsx_icp_localize_projective's photometric term at a GIVEN association (the op of the
+ * differentiable mode; its rows are computed by the fused call's device functions, so the sums are the fused call's bit
+ * for bit).  Source rows i < src_count[b] of src_points / src_colours (B, ns_stride, 3), world frame and live colour;
+ * nn_idx (B, ns_stride) the associated pixel or -1; tgt_points / tgt_normals / model_colours (B, H*W, 3) the target
+ * images and the colour of each pixel's winning row (zeros where uncovered); index (B, H*W) the index image (-1 =
+ * uncovered); prev_poses / intrinsics (B, 4, 4).  sums_out (B, 28): the geometric sums plus photometric_weight times
+ * the photometric products.  scratch: B * gsx_icp_normal_eq_scratch_bytes(ns_stride) bytes.
  * The backward takes g_sums (B, 28) and writes per SOURCE row: g_src, g_src_colours, g_tgt_points_rows,
  * g_tgt_normals_rows (B, ns_stride, 3) and g_stencil_colours_rows (B, ns_stride, 5, 3), the gradients of the model
  * colours at pixels j, j-1, j+1, j-W, j+W (zeros where the row has none; the caller scatters them), and g_prev_poses
- * (B, 4, 4), reduced in a fixed order without atomics (bottom row zero).  No gradient w.r.t. the intrinsics: that is
- * gsx_icp_joint_normal_eq_batched_bwd_intrinsics, to which gsx_icp_joint_normal_eq_batched_bwd forwards with
- * g_intrinsics = NULL.  A negative or non-finite weight is refused before any launch. */
+ * (B, 4, 4), reduced in a fixed order without atomics (bottom row zero).  If g_intrinsics != NULL it also writes
+ * d(loss)/d(intrinsics) (B, 4, 4): the photometric row reads all 12 entries of K's first three rows (its projection and
+ * du/dq, dv/dq), skew and the 4th column included, so each of them gets a gradient (dual numbers over 29 inputs); the
+ * bottom row is 0, reduced like g_prev_poses.  Backward scratch: gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(B,
+ * ns_stride) bytes; B * gsx_icp_normal_eq_scratch_bytes(ns_stride) suffice when g_intrinsics is NULL.
+ * huber_delta and photometric_huber_delta weigh the rows as gsx_icp_localize_projective does, bit for bit; both +inf
+ * run the unweighted kernels.  A negative or non-finite weight, and a scale <= 0 or NaN, are refused before any
+ * launch. */
 int gsx_icp_joint_normal_eq_batched_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
                                         const float *src_colours, const float *tgt_points, const float *tgt_normals,
                                         const float *model_colours, const int64_t *index, int B, int H, int W,
                                         const int64_t *nn_idx, const float *prev_poses, const float *intrinsics,
                                         float photometric_weight, float *sums_out, void *scratch,
-                                        int64_t scratch_bytes, void *stream);
+                                        int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
+                                        void *stream);
+int64_t gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(int B, int ns_stride);
 int gsx_icp_joint_normal_eq_batched_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
                                         const float *src_colours, const float *tgt_points, const float *tgt_normals,
                                         const float *model_colours, const int64_t *index, int B, int H, int W,
                                         const int64_t *nn_idx, const float *prev_poses, const float *intrinsics,
                                         float photometric_weight, const float *g_sums, float *g_src,
                                         float *g_src_colours, float *g_tgt_points_rows, float *g_tgt_normals_rows,
-                                        float *g_stencil_colours_rows, float *g_prev_poses, void *scratch,
-                                        int64_t scratch_bytes, void *stream);
-/* gsx_icp_joint_normal_eq_batched_bwd that also writes, if g_intrinsics != NULL, d(loss)/d(intrinsics) (B, 4, 4): the
- * photometric row reads all 12 entries of K's first three rows (its projection and du/dq, dv/dq), skew and the 4th column
- * included, so each of them gets a gradient here (dual numbers over 29 inputs); the bottom row is 0.  Reduced per block
- * and then over the blocks in a fixed order, like g_prev_poses.  scratch:
- * gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(B, ns_stride) bytes when g_intrinsics != NULL, else as
- * gsx_icp_joint_normal_eq_batched_bwd. */
-int64_t gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(int B, int ns_stride);
-int gsx_icp_joint_normal_eq_batched_bwd_intrinsics(const float *src_points, const int32_t *src_count, int ns_stride,
-                                                   const float *src_colours, const float *tgt_points,
-                                                   const float *tgt_normals, const float *model_colours,
-                                                   const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
-                                                   const float *prev_poses, const float *intrinsics,
-                                                   float photometric_weight, const float *g_sums, float *g_src,
-                                                   float *g_src_colours, float *g_tgt_points_rows,
-                                                   float *g_tgt_normals_rows, float *g_stencil_colours_rows,
-                                                   float *g_prev_poses, float *g_intrinsics, void *scratch,
-                                                   int64_t scratch_bytes, void *stream);
-/* Huber-weighted gsx_icp_joint_normal_eq_batched_fwd and gsx_icp_joint_normal_eq_batched_bwd_intrinsics (the op of the
- * robust differentiable projective mode): same arguments plus huber_delta and photometric_huber_delta, the rows of
- * gsx_icp_localize_projective_robust bit for bit.  The backward's g_intrinsics may be NULL, with the scratch sizes of
- * gsx_icp_joint_normal_eq_batched_bwd_intrinsics.  Both scales +inf give the counterparts' outputs bit for bit; a scale
- * <= 0 or NaN is refused before any launch. */
-int gsx_icp_joint_normal_eq_batched_robust_fwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                               const float *src_colours, const float *tgt_points,
-                                               const float *tgt_normals, const float *model_colours,
-                                               const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
-                                               const float *prev_poses, const float *intrinsics,
-                                               float photometric_weight, float *sums_out, void *scratch,
-                                               int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
-                                               void *stream);
-int gsx_icp_joint_normal_eq_batched_robust_bwd(const float *src_points, const int32_t *src_count, int ns_stride,
-                                               const float *src_colours, const float *tgt_points,
-                                               const float *tgt_normals, const float *model_colours,
-                                               const int64_t *index, int B, int H, int W, const int64_t *nn_idx,
-                                               const float *prev_poses, const float *intrinsics,
-                                               float photometric_weight, const float *g_sums, float *g_src,
-                                               float *g_src_colours, float *g_tgt_points_rows,
-                                               float *g_tgt_normals_rows, float *g_stencil_colours_rows,
-                                               float *g_prev_poses, float *g_intrinsics, void *scratch,
-                                               int64_t scratch_bytes, float huber_delta, float photometric_huber_delta,
-                                               void *stream);
+                                        float *g_stencil_colours_rows, float *g_prev_poses, float *g_intrinsics,
+                                        void *scratch, int64_t scratch_bytes, float huber_delta,
+                                        float photometric_huber_delta, void *stream);
 
 /* The association of gsx_icp_localize_projective alone (the index-only op of the differentiable mode): for the source
  * rows i < src_count[b] of src_points (B, ns_stride, 3), world frame, idx_out int64 (B, ns_stride) = the pixel

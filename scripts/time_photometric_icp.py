@@ -1,4 +1,4 @@
-"""What the photometric term (ICPSLAM / PointFusion(photometric_weight=w), gsx_icp_localize_projective_rgb) costs and
+"""What the photometric term (ICPSLAM / PointFusion(photometric_weight=w), gsx_icp_localize_projective) costs and
 gains, at 640x480, B=8, gradICP with 20 iterations at dsratio 4, M = 0 (one pixel per surfel) and 3 (disk splats):
 
   1. the fused localisation of frame 31 against the radii map of frames 0..30 of the bench's inputs

@@ -1,4 +1,4 @@
-"""What splatted ICP targets (ICPSLAM / PointFusion(target_splat_px=M), gsx_icp_localize_projective_splats) cost and
+"""What splatted ICP targets (ICPSLAM / PointFusion(target_splat_px=M), gsx_icp_localize_projective) cost and
 gain, at 640x480, B=8, gradICP with 20 iterations at dsratio 4, on the bench's inputs (make_sequence(8, 32, 480, 640,
 seed=0)), with M = 0 (one pixel per surfel), 1 and 3:
 

@@ -1,12 +1,12 @@
-"""What the Huber weights (ICPSLAM / PointFusion(huber_delta=, photometric_huber_delta=), the *_robust entry points)
-cost, at 640x480, B=8, gradICP with 20 iterations at dsratio 4, on the bench's inputs (make_sequence(8, 32, 480, 640,
-seed=0)): the localisation of frame 31 against the map of frames 0..30.
+"""What the Huber weights (ICPSLAM / PointFusion(huber_delta=, photometric_huber_delta=), finite scales of the ICP
+entry points) cost, at 640x480, B=8, gradICP with 20 iterations at dsratio 4, on the bench's inputs
+(make_sequence(8, 32, 480, 640, seed=0)): the localisation of frame 31 against the map of frames 0..30.
 
   1. the fused step per call, with the scales unset and set, the two alternated within each repetition (CUDA events
      over 5 calls, the median over repetitions):
-       1-NN association (gsx_icp_localize vs gsx_icp_localize_robust, delta = 0.02 m);
-       projective association at M = 0 and M = 3, w = 0 and w = 0.1 (gsx_icp_localize_projective_splats / _rgb vs
-       gsx_icp_localize_projective_robust, delta = 0.02 m and, with w, delta_p = 0.05);
+       1-NN association (gsx_icp_localize at delta = +inf vs 0.02 m);
+       projective association at M = 0 and M = 3, w = 0 and w = 0.1 (gsx_icp_localize_projective at +inf vs
+       delta = 0.02 m and, with w, delta_p = 0.05);
   2. config 3 (ICPSLAM(odom='gradicp', numiters=10) at B=8, two frames, the depth requiring grad): forward and backward
      of the taped run with and without delta.
 

@@ -1,5 +1,5 @@
 """Float64 reference of the joint geometric and photometric normal-equation op (_JointNormalEqBatchedFn,
-gsx_icp_joint_normal_eq_batched_fwd / _bwd / _bwd_intrinsics, include/gsx.h) for one batch element, with error bounds
+gsx_icp_joint_normal_eq_batched_fwd / _bwd, d/dK included, include/gsx.h) for one batch element, with error bounds
 for the float32 kernels.  Test infrastructure only.
 
 The statement is photometric_oracle's (tests/photometric_oracle.py) at a GIVEN association: the geometric row of every

@@ -1,5 +1,5 @@
 """CPU oracle of the joint geometric and photometric projective ICP (ICPSLAM / PointFusion(photometric_weight=w),
-gsx_icp_localize_projective_rgb, gsx_icp_projective_targets_rgb).  Test infrastructure only; built on projective_oracle
+gsx_icp_localize_projective, gsx_icp_projective_targets at w > 0).  Test infrastructure only; built on projective_oracle
 (association and loop) and projective_splat_oracle (target images at M >= 1), with the oracle's canonical arithmetic.
 
     intensity       I(r, g, b) = (0.299 r + 0.587 g) + 0.114 b, float32, every product and sum rounded on its own

@@ -1,7 +1,7 @@
 """CPU oracle of the projective ICP against the disk-splat render of the map (ICPSLAM / PointFusion(target_splat_px=M),
-gsx_icp_localize_projective_splats, gsx_icp_projective_targets).  Test infrastructure only; built on projective_oracle
-(association and loop), splat_oracle (the disk render) and radii_oracle (fusion with radii), with the oracle's canonical
-arithmetic.
+gsx_icp_localize_projective, gsx_icp_projective_targets at M >= 1).  Test infrastructure only; built on
+projective_oracle (association and loop), splat_oracle (the disk render) and radii_oracle (fusion with radii), with the
+oracle's canonical arithmetic.
 
 For M >= 1 and element b with prev = the previous camera-to-world pose:
     index       splat_oracle.splat_index of the map seen from prev at M (R1d's z-buffer, keys, ties and fill)

@@ -3,6 +3,8 @@ k_icp_joint_linearize_bwd<kWantK>, the fixed-order block reductions) called dire
 tests/joint_normal_eq_reference.py within its derived float32 bounds: hundreds of blocks, a ragged batch with a camera
 per element, the image border and holes, the identities of w = 0 and of images without an interior pixel, and the
 benchmark's size.  Each bound check prints its largest error-to-bound ratio."""
+import math
+
 import pytest
 import torch
 
@@ -193,7 +195,7 @@ def test_intrinsics_instantiation_leaves_the_other_gradients_unchanged():
     assert bool((with_k["K"][:, 0, 1] != 0).all()) and bool((with_k["K"][:, :3, 3] != 0).all())
 
 
-def test_backward_kernels_are_deterministic():
+def test_joint_backward_is_deterministic():
     """Two launches of the backward give every per-row output and the reduced pose and intrinsics gradients bit for
     bit (the fixed-order reductions: no atomics)."""
     from gradslam_b200 import _C
@@ -211,14 +213,14 @@ def test_backward_kernels_are_deterministic():
     args = (d(src), torch.tensor([70001, 3000], dtype=torch.int32, device=DEV), Ns, d(col), stack("tgt"),
             stack("tgt_n"), stack("model_col"), d(torch.stack([e[2] for e in els])), B, H, W, d(idx), stack("prev"),
             stack("K"), W_TRACK, d(torch.randn(B, 28, generator=torch.Generator().manual_seed(6))))
-    nbytes = _C.lib().gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(B, Ns)
+    nbytes = _C.lib().gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(B, Ns)
     outs = []
     for _ in range(2):
         o = [torch.full((B, Ns, 3), float("nan"), device=DEV) for _ in range(4)]
         o += [torch.full((B, Ns, 5, 3), float("nan"), device=DEV), torch.full((B, 4, 4), float("nan"), device=DEV),
               torch.full((B, 4, 4), float("nan"), device=DEV)]
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=DEV)
-        _C.launch("gsx_icp_joint_normal_eq_batched_bwd_intrinsics", *args, *o, scratch, nbytes)
+        _C.launch("gsx_icp_joint_normal_eq_batched_bwd", *args, *o, scratch, nbytes, math.inf, math.inf)
         outs.append([t.cpu() for t in o])
     for a, b in zip(*outs):
         assert bool(torch.isfinite(a).all())
@@ -234,20 +236,21 @@ def joint_calls(monkeypatch):
     last = {}
     orig = icputils._JointNormalEqBatchedFn.forward
 
-    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W):
+    def forward(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W,
+                huber=(math.inf, math.inf)):
         last.clear()
         last.update(src=src.detach().clone(), src_col=src_col.detach().clone(), tgt=tgt.detach().clone(),
                     tgt_n=tgt_n.detach().clone(), model_col=model_col.detach().clone(), prev=prev.detach().clone(),
                     idx=idx.clone(), index=index.clone(), counts=src_counts.clone(), K=K.detach().clone(), w=w, H=H,
                     W=W)
-        return orig(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W)
+        return orig(ctx, src, src_col, tgt, tgt_n, model_col, prev, idx, index, src_counts, K, w, H, W, huber)
 
     monkeypatch.setattr(icputils._JointNormalEqBatchedFn, "forward", staticmethod(forward))
     return last
 
 
 @pytest.mark.parametrize("M", [0, 3])
-def test_benchmark_size_taped_equals_fused_and_the_op_matches_the_reference(M, joint_calls):
+def test_benchmark_size_taped_poses_equal_fused_and_the_op_matches_the_reference(M, joint_calls):
     """B = 8, 640 x 480, ds = 1 (about 1,200 blocks per element), the textured scene at W_TRACK: the differentiable
     mode's poses equal the fused call's bit for bit, and the last joint op it ran, re-run on its recorded inputs,
     matches the reference for elements 0 and 7."""

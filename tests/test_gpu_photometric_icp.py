@@ -1,7 +1,9 @@
 """GPU parity of the joint geometric and photometric projective ICP (ICPSLAM / PointFusion(photometric_weight=w),
-gsx_icp_localize_projective_rgb, gsx_icp_projective_targets_rgb) with tests/photometric_oracle.py: the model image and
+gsx_icp_localize_projective, gsx_icp_projective_targets at w > 0) with tests/photometric_oracle.py: the model image and
 the association bit for bit, poses at the ICP tests' 1e-4, w = 0 and a black scene bit for bit against the geometric
 call; the differentiable mode's poses equal the fused call's and its gradients match autograd of the oracle."""
+import math
+
 import pytest
 import torch
 
@@ -74,9 +76,9 @@ def test_localize_matches_oracle(odom, dist_thresh, ds):
         assert not torch.equal(got, geo[:, 0].cpu())
 
 
-def test_zero_weight_and_a_black_scene_give_the_geometric_poses():
-    """gsx_icp_localize_projective_rgb at w = 0 is gsx_icp_localize_projective_splats bit for bit; so is w > 0 on a scene
-    whose colours are all 0 (every photometric row and residual is 0)."""
+def test_colours_at_zero_weight_and_a_black_scene_give_the_geometric_poses():
+    """gsx_icp_localize_projective with colours at w = 0 is its geometric call bit for bit; so is w > 0 on a scene whose
+    colours are all 0 (every photometric row and residual is 0)."""
     import gradslam_b200 as gs
     from gradslam_b200.odometry.icputils import localize_projective
 
@@ -91,14 +93,15 @@ def test_zero_weight_and_a_black_scene_give_the_geometric_poses():
             base = localize_projective(pc, live, frames[:, 1], 2, odom, M)
             for w in ((0.0, 0.5) if colours is not rgb else (0.0,)):
                 from gradslam_b200 import _C
-                from gradslam_b200.odometry.icputils import _ProjectiveRgbWorkspace
+                from gradslam_b200.odometry.icputils import _ProjectiveWorkspace
 
                 out = torch.empty_like(base)
-                ws = _ProjectiveRgbWorkspace.get(DEV, B, H, W, 2)
-                _C.launch("gsx_icp_localize_projective_rgb", pc._geo, pc._counts_dev[pc._cur], pc.capacity, pc._bound,
+                ws = _ProjectiveWorkspace.get(DEV, B, H, W, 2, True)
+                _C.launch("gsx_icp_localize_projective", pc._geo, pc._counts_dev[pc._cur], pc.capacity, pc._bound,
                           live.depth_image.contiguous(), H * W, K.to(DEV).contiguous(), 16,
                           poses[:, 1:2].to(DEV).contiguous(), 16, B, H, W, 2, 1, 10, 1e-8, 0, 0.0, 2.0, 1.0, 1.0, 200.0,
-                          out, 16, ws, ws.numel(), M, pc._col, live.rgb_image.contiguous(), H * W * 3, w)
+                          out, 16, ws, ws.numel(), M, pc._col, live.rgb_image.contiguous(), H * W * 3, w,
+                          math.inf, math.inf)
                 assert torch.equal(out, base), (M, w)
 
 
@@ -256,15 +259,15 @@ def test_differentiable_mode_gradients_match_oracle_autograd(M):
         torch.testing.assert_close(got, want, rtol=5e-2, atol=5e-3 * scale, msg=name)
 
 
-def test_c_entry_points_refuse_bad_weights_and_null_colours_without_a_launch():
+def test_projective_entry_points_refuse_bad_weights_and_null_colours_without_a_launch():
     from gradslam_b200 import _C
 
     bufs = [torch.full((256,), -7.25, device=DEV) for _ in range(8)]
     geo, counts, depth, K, prev, out, ws, col = bufs
     index = torch.full((64,), -7, dtype=torch.int64, device=DEV)
-    call = lambda w, c, r: _C.launch("gsx_icp_localize_projective_rgb", geo, counts, 4, 4, depth, 16, K, 16, prev, 16,
-                                     1, 4, 4, 1, 1, 1, 1e-8, 0, 0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, 1024, 0, c, r,
-                                     48, w)
+    call = lambda w, c, r: _C.launch("gsx_icp_localize_projective", geo, counts, 4, 4, depth, 16, K, 16, prev, 16, 1,
+                                     4, 4, 1, 1, 1, 1e-8, 0, 0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, 1024, 0, c, r, 48,
+                                     w, math.inf, math.inf)
     for bad in (-0.5, float("nan"), float("inf")):
         with pytest.raises(RuntimeError, match="photometric_weight"):
             call(bad, col, col)
@@ -272,8 +275,8 @@ def test_c_entry_points_refuse_bad_weights_and_null_colours_without_a_launch():
         with pytest.raises(RuntimeError, match="colour"):
             call(0.5, c, r)
     with pytest.raises(RuntimeError, match="null"):
-        _C.launch("gsx_icp_projective_targets_rgb", geo, None, counts, 4, 4, K, 16, prev, 16, 1, 4, 4, 0, index, col,
-                  col, col)
+        _C.launch("gsx_icp_projective_targets", geo, None, counts, 4, 4, K, 16, prev, 16, 1, 4, 4, 0, index, col, col,
+                  col)
     torch.cuda.synchronize()
     for t in bufs:
         assert torch.equal(t, torch.full((256,), -7.25, device=DEV))

@@ -1,6 +1,9 @@
 """GPU parity of the projective ICP against the disk-splat render (ICPSLAM / PointFusion(target_splat_px=M),
-gsx_icp_localize_projective_splats, gsx_icp_projective_targets) with tests/projective_splat_oracle.py: the target images
-bit for bit, poses at the ICP tests' 1e-4, maps at 1e-3, gradients at the tolerances of test_gpu_projective_icp.py."""
+gsx_icp_localize_projective and gsx_icp_projective_targets at max_splat_px = M) with tests/projective_splat_oracle.py:
+the target images bit for bit, poses at the ICP tests' 1e-4, maps at 1e-3, gradients at the tolerances of
+test_gpu_projective_icp.py."""
+import math
+
 import pytest
 import torch
 
@@ -158,12 +161,9 @@ def test_empty_map_no_depth_and_camera_turned_away_keep_the_previous_pose(odom):
     assert torch.equal(taped, got)
 
 
-def test_maps_without_radii_and_the_old_entry_point_give_the_point_poses():
-    """M > 0 on a map without radii gives the M = 0 poses bit for bit, fused and taped; gsx_icp_localize_projective is
-    gsx_icp_localize_projective_splats at M = 0."""
+def test_maps_without_radii_give_the_point_poses():
+    """M > 0 on a map without radii gives the M = 0 poses bit for bit, fused and taped."""
     import gradslam_b200 as gs
-    from gradslam_b200 import _C
-    from gradslam_b200.odometry.icputils import _ProjectiveWorkspace
 
     B, L, H, W = 3, 3, 45, 62
     rgb, depth, K, poses = camera_inputs(B, L, H, W, 65, skew=0.75)
@@ -178,14 +178,6 @@ def test_maps_without_radii_and_the_old_entry_point_give_the_point_poses():
     taped = gs.ICPSLAM(odom="gradicp", association="projective", numiters=10, dsratio=2, target_splat_px=3,
                        device=DEV)._localize(pc, live, frames[:, 1])
     assert torch.equal(taped.detach(), base)
-    # the old entry point
-    out = torch.empty((B, 1, 4, 4), device=DEV)
-    ws = _ProjectiveWorkspace.get(DEV, B, H, W, 2)
-    d = frames[:, 2].depth_image.contiguous()
-    _C.launch("gsx_icp_localize_projective", pc._geo.contiguous(), pc._counts_dev[pc._cur], pc.capacity, pc._bound, d,
-              H * W, K.to(DEV).contiguous(), 16, poses[:, 1:2].to(DEV).contiguous(), 16, B, H, W, 2, 1, 10, 1e-8, 0,
-              0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, ws.numel())
-    assert torch.equal(out, base)
 
 
 def test_icpslam_run_with_splat_targets_matches_oracle():
@@ -310,7 +302,7 @@ def test_differentiable_mode_gradients_match_oracle_autograd():
         torch.testing.assert_close(got, want, rtol=5e-2, atol=5e-3 * scale)
 
 
-def test_c_entry_points_refuse_a_bad_max_splat_px_without_a_launch():
+def test_projective_entry_points_refuse_a_bad_max_splat_px_without_a_launch():
     from gradslam_b200 import _C
 
     bufs = [torch.full((256,), -7.25, device=DEV) for _ in range(8)]
@@ -318,10 +310,12 @@ def test_c_entry_points_refuse_a_bad_max_splat_px_without_a_launch():
     index = torch.full((64,), -7, dtype=torch.int64, device=DEV)
     for bad in (-1, 17):
         with pytest.raises(RuntimeError, match="max_splat_px"):
-            _C.launch("gsx_icp_localize_projective_splats", geo, counts, 4, 4, depth, 16, K, 16, prev, 16, 1, 4, 4, 1,
-                      1, 1, 1e-8, 0, 0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, 1024, bad)
+            _C.launch("gsx_icp_localize_projective", geo, counts, 4, 4, depth, 16, K, 16, prev, 16, 1, 4, 4, 1, 1, 1,
+                      1e-8, 0, 0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, 1024, bad, None, None, 0, 0.0, math.inf,
+                      math.inf)
         with pytest.raises(RuntimeError, match="max_splat_px"):
-            _C.launch("gsx_icp_projective_targets", geo, counts, 4, 4, K, 16, prev, 16, 1, 4, 4, bad, index, tgt, tgt)
+            _C.launch("gsx_icp_projective_targets", geo, None, counts, 4, 4, K, 16, prev, 16, 1, 4, 4, bad, index, tgt,
+                      tgt, None)
     torch.cuda.synchronize()
     for t in bufs:
         assert torch.equal(t, torch.full((256,), -7.25, device=DEV))

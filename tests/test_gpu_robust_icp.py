@@ -1,7 +1,8 @@
-"""GPU checks of the Huber-weighted tracking (huber_delta / photometric_huber_delta, the *_robust entry points) against
-tests/robust_oracle.py: fused poses at the ICP tests' tolerances for both associations, +inf equal to the unweighted
-entry points bit for bit, taped poses equal to fused ones, the ops' gradients against float64 autograd on both sides of
-delta, the differentiable mode against autograd of the oracle, and the gain on a scene with an object that appears."""
+"""GPU checks of the Huber-weighted tracking (huber_delta / photometric_huber_delta of the ICP entry points) against
+tests/robust_oracle.py: fused poses at the ICP tests' tolerances for both associations, the Huber kernels at a scale no
+residual reaches equal to the unweighted ones bit for bit, taped poses equal to fused ones, the ops' gradients against
+float64 autograd on both sides of delta, the differentiable mode against autograd of the oracle, and the gain on a
+scene with an object that appears."""
 import math
 
 import pytest
@@ -18,6 +19,7 @@ from test_photometric_oracle import W_TRACK
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 INF = math.inf
+FLT_MAX = 3.4028234663852886e38  # the largest finite float32: a scale no residual reaches, so the Huber kernels run
 
 
 def _inputs(textured):
@@ -80,6 +82,8 @@ def test_fused_projective_poses_match_oracle(odom, w, ds):
 
 
 def test_every_robust_entry_point_at_infinity_is_its_counterpart_bit_for_bit():
+    """A finite scale runs the Huber-weighted kernels (+inf runs the unweighted ones); at FLT_MAX every row is inside
+    it, so they must give the unweighted outputs bit for bit."""
     from gradslam_b200.odometry import GradICPOdometryProvider
     from gradslam_b200.odometry.icputils import (_JointNormalEqBatchedFn, _NormalEqBatchedFn, downsample_rgbdimages,
                                                  icp_align, localize_against_map, localize_projective,
@@ -90,7 +94,7 @@ def test_every_robust_entry_point_at_infinity_is_its_counterpart_bit_for_bit():
     pc = _map(frames[:, :2])
     prov = GradICPOdometryProvider(10, 1e-8, None)
     robust = GradICPOdometryProvider(10, 1e-8, None)
-    robust.huber_delta = INF  # (the keyword refuses +inf: it is the C entry points' "off")
+    robust.huber_delta = FLT_MAX
     for ds in (1, 4):
         assert torch.equal(localize_against_map(pc, frames[:, 2], frames[:, 1], ds, robust),
                            localize_against_map(pc, frames[:, 2], frames[:, 1], ds, prov))
@@ -98,7 +102,7 @@ def test_every_robust_entry_point_at_infinity_is_its_counterpart_bit_for_bit():
             for w in (0.0, W_TRACK):
                 want = localize_projective(pc, frames[:, 2], frames[:, 1], ds, prov, M, w)
                 got = localize_projective(pc, frames[:, 2], frames[:, 1], ds, robust, M, w,
-                                          INF if w else None)
+                                          FLT_MAX if w else None)
                 assert torch.equal(got, want), (ds, M, w)
     # icp_align on ragged clouds
     g = torch.Generator().manual_seed(5)
@@ -108,7 +112,7 @@ def test_every_robust_entry_point_at_infinity_is_its_counterpart_bit_for_bit():
     cs, ct = (torch.tensor(c, dtype=torch.int32, device=DEV) for c in ([700, 0, 350], [500, 700, 1]))
     for mode in (0, 1):
         a = icp_align(src, cs, tgt, tn, ct, None, mode, 8, 1e-8, None, want_idx=True)
-        b = icp_align(src, cs, tgt, tn, ct, None, mode, 8, 1e-8, None, want_idx=True, huber_delta=INF)
+        b = icp_align(src, cs, tgt, tn, ct, None, mode, 8, 1e-8, None, want_idx=True, huber_delta=FLT_MAX)
         rows = torch.arange(700, device=DEV) < cs.unsqueeze(1)  # (rows beyond a source size are not written)
         assert torch.equal(a[0], b[0]) and torch.equal(a[1][rows], b[1][rows])
     # the two ops, forward and backward (d/dK included)
@@ -116,7 +120,7 @@ def test_every_robust_entry_point_at_infinity_is_its_counterpart_bit_for_bit():
                       torch.randint(0, 700, (3, 700), generator=g).to(DEV), torch.full((3, 700), -1, device=DEV))
     gs_ = torch.randn(3, 28, generator=g).to(DEV)
     outs = []
-    for h in ((), (INF,)):
+    for h in ((), (FLT_MAX,)):
         x = [t.clone().requires_grad_(True) for t in (src, tgt, tn)]
         s = _NormalEqBatchedFn.apply(*x, idx, cs, *h)
         (s * gs_).sum().backward()
@@ -133,7 +137,7 @@ def test_every_robust_entry_point_at_infinity_is_its_counterpart_bit_for_bit():
                         index.clamp(min=0).unsqueeze(-1).expand(3, H * W, 3)) * (index >= 0).unsqueeze(-1)
     gj = torch.randn(3, 28, generator=g).to(DEV)
     outs = []
-    for h in ((), ((INF, INF),)):
+    for h in ((), ((FLT_MAX, FLT_MAX),)):
         x = [t.clone().requires_grad_(True) for t in (s_pts, s_col, tp, tnn, mcol, prev, K4)]
         s = _JointNormalEqBatchedFn.apply(*x[:6], jdx, index, counts, x[6], W_TRACK, H, W, *h)
         (s * gj).sum().backward()

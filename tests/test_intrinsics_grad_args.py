@@ -1,6 +1,7 @@
 """Argument checks of gsx_backproject_normals_bwd_intrinsics and its scratch size: they run before any launch, so they
 are testable without a GPU."""
 import ctypes
+import math
 
 import pytest
 
@@ -49,7 +50,7 @@ def test_refuses_bad_extents():
     assert _call(B=70000, L=1) != 0
 
 
-def test_render_and_joint_intrinsics_entry_points_refuse_bad_arguments():
+def test_render_and_joint_backward_entry_points_refuse_bad_intrinsics_arguments():
     lib = _C.lib()
     n = lib.gsx_render_splats_bwd_intrinsics_scratch_bytes(2, 3, 8, 8)
     assert n >= lib.gsx_render_views_bwd_scratch_bytes(2, 3, 8, 8) + 2 * 3 * 1 * 4 * 4
@@ -61,10 +62,10 @@ def test_render_and_joint_intrinsics_entry_points_refuse_bad_arguments():
     for scratch, nbytes in ((None, n), (FAKE, n - 1)):
         assert call(FAKE, scratch, nbytes, 2) != 0 and b"scratch too small" in lib.gsx_last_error()
     assert call(FAKE, FAKE, n, 17) != 0 and b"max_splat_px" in lib.gsx_last_error()
-    m = lib.gsx_icp_joint_normal_eq_batched_bwd_intrinsics_scratch_bytes(2, 300)
+    m = lib.gsx_icp_joint_normal_eq_batched_bwd_scratch_bytes(2, 300)
     assert m >= 2 * 2 * 12 * 4 * 2
-    jcall = lambda g_prev, nbytes: lib.gsx_icp_joint_normal_eq_batched_bwd_intrinsics(
+    jcall = lambda g_prev, nbytes: lib.gsx_icp_joint_normal_eq_batched_bwd(
         FAKE, FAKE, 300, FAKE, FAKE, FAKE, FAKE, FAKE, 2, 8, 8, FAKE, FAKE, FAKE, ctypes.c_float(0.1), FAKE, FAKE, FAKE,
-        FAKE, FAKE, FAKE, g_prev, FAKE, FAKE, nbytes, None)
+        FAKE, FAKE, FAKE, g_prev, FAKE, FAKE, nbytes, math.inf, math.inf, None)
     assert jcall(None, m) != 0 and b"null pointer" in lib.gsx_last_error()
     assert jcall(FAKE, m - 1) != 0 and b"scratch too small" in lib.gsx_last_error()

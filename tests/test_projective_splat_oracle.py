@@ -112,17 +112,19 @@ def test_pointfusion_refuses_splat_targets_without_radii():
     assert gs.PointFusion(odom="gradicp", association="projective", target_splat_px=0).target_splat_px == 0
 
 
-def test_localize_entry_points_refuse_a_bad_max_splat_px_before_any_cuda_call():
+def test_projective_entry_points_refuse_a_bad_max_splat_px_before_any_cuda_call():
     from gradslam_b200 import _C
 
     lib = _C.lib()
     bufs = [torch.full((256,), -7.25) for _ in range(9)]
     geo, counts, depth, K, prev, out, ws, index, tgt = (t.data_ptr() for t in bufs)
     for bad in (-1, 17):
-        rc = lib.gsx_icp_localize_projective_splats(geo, counts, 4, 4, depth, 16, K, 16, prev, 16, 1, 4, 4, 1, 1, 1,
-                                                    1e-8, 0, 0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, 1 << 20, bad, None)
+        rc = lib.gsx_icp_localize_projective(geo, counts, 4, 4, depth, 16, K, 16, prev, 16, 1, 4, 4, 1, 1, 1, 1e-8, 0,
+                                             0.0, 2.0, 1.0, 1.0, 200.0, out, 16, ws, 1 << 20, bad, None, None, 0, 0.0,
+                                             math.inf, math.inf, None)
         assert rc != 0 and b"max_splat_px" in lib.gsx_last_error()
-        rc = lib.gsx_icp_projective_targets(geo, counts, 4, 4, K, 16, prev, 16, 1, 4, 4, bad, index, tgt, tgt, None)
+        rc = lib.gsx_icp_projective_targets(geo, None, counts, 4, 4, K, 16, prev, 16, 1, 4, 4, bad, index, tgt, tgt,
+                                            None, None)
         assert rc != 0 and b"max_splat_px" in lib.gsx_last_error()
     for t in bufs:
         assert torch.equal(t, torch.full((256,), -7.25))
