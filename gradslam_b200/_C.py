@@ -180,6 +180,14 @@ SIGNATURES = {
     "gsx_render_splats_bwd_intrinsics": (
         c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
                 c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
+    "gsx_render_blend_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int, c_i64, c_int]),
+    "gsx_render_blend": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int, c_double,
+                c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "gsx_render_blend_bwd_scratch_bytes": (c_i64, [c_int, c_int, c_i64]),
+    "gsx_render_blend_bwd": (
+        c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_int, c_int, c_int, c_int, c_int, c_double,
+                c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "gsx_render_views_bwd_scratch_bytes": (c_i64, [c_int, c_int, c_int, c_int]),
     "gsx_render_views_bwd": (
         c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,

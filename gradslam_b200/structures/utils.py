@@ -1,4 +1,5 @@
 """Frame -> cloud conversion (mirror of gradslam/structures/utils.py:7-57) and its inverse, cloud -> frames."""
+import math
 from typing import NamedTuple, Optional
 
 import torch
@@ -100,6 +101,72 @@ class _RenderFn(torch.autograd.Function):
         return None, d_geo, d_col, d_poses, None
 
 
+def _render_blend(geo, col, counts, bound, K, poses, H, W, want_normals, use_conf, band, splat):
+    """gsx_render_blend on dense CUDA tensors -> (depth, rgb, normals, weight, index, front depth)."""
+    B, L = poses.shape[:2]
+    dev = poses.device
+    cap = geo.shape[1]
+    img = lambda c: torch.empty((B, L, H, W, c), dtype=torch.float32, device=dev)
+    index = torch.empty((B, L, H, W), dtype=torch.int64, device=dev)
+    front, weight, depth = torch.empty((B, L, H, W), dtype=torch.float32, device=dev), img(1), img(1)
+    rgb, normals = None if col is None else img(3), img(3) if want_normals else None
+    scratch = torch.empty(_C.lib().gsx_render_blend_scratch_bytes(B, L, H, W, bound, splat), dtype=torch.uint8,
+                          device=dev)
+    _C.launch("gsx_render_blend", geo, col, counts, cap, bound, K, 16, poses, L * 16, B, L, H, W, int(use_conf), band,
+              splat, index, front, weight, depth, rgb, normals, scratch, scratch.numel())
+    return depth, rgb, normals, weight, index, front
+
+
+class _RenderBlendFn(torch.autograd.Function):
+    """gsx_render_blend as one differentiable op over (geometry rows, colour rows, poses); backward =
+    gsx_render_blend_bwd: through the blend weights to the rows' positions, normals, radii and confidence counts, to
+    their colours and to the poses.  Which rows cover a pixel, and the front depth, carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, pack, geo, col, poses):
+        counts, bound, H, W, want_normals, use_conf, band, splat, K = pack
+        depth, rgb, normals, weight, index, front = _render_blend(
+            geo.detach(), None if col is None else col.detach(), counts, bound, K, poses.detach(), H, W, want_normals,
+            use_conf, band, splat)
+        ctx.mark_non_differentiable(index)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(geo, col, poses, front, weight, depth, rgb, normals)
+        ctx.pack = pack
+        return depth, rgb, normals, weight, index
+
+    @staticmethod
+    def backward(ctx, g_depth, g_rgb, g_normals, g_weight, _g_index):
+        geo, col, poses, front, weight, depth, rgb, normals = ctx.saved_tensors
+        counts, bound, H, W, _, use_conf, band, splat, K = ctx.pack
+        _, need_geo, need_col, need_pose = ctx.needs_input_grad
+        B, L = poses.shape[:2]
+        dev, cap = geo.device, geo.shape[1]
+        d_geo = torch.empty_like(geo) if need_geo else None
+        d_col = torch.empty((B, cap, 4), dtype=torch.float32, device=dev) if need_col else None
+        d_poses = torch.empty((B, L, 4, 4), dtype=torch.float32, device=dev) if need_pose else None
+        scratch = None
+        if need_pose:
+            scratch = torch.empty(_C.lib().gsx_render_blend_bwd_scratch_bytes(B, L, bound), dtype=torch.uint8,
+                                  device=dev)
+        gs = [None if g is None else g.contiguous() for g in (g_depth, g_rgb, g_normals, g_weight)]
+        _C.launch("gsx_render_blend_bwd", geo.detach(), None if col is None else col.detach(), counts, cap, bound, K,
+                  16, poses.detach(), L * 16, B, L, H, W, int(use_conf), band, splat, front, weight, depth, rgb,
+                  normals, *gs, d_geo, d_col, d_poses, scratch, 0 if scratch is None else scratch.numel())
+        return None, d_geo, d_col, d_poses
+
+
+def _blend_band(blend_band):
+    """None, or blend_band as a float >= 0 (+inf allowed)."""
+    if blend_band is None:
+        return None
+    if isinstance(blend_band, bool) or not isinstance(blend_band, (int, float)):
+        raise TypeError("Expected blend_band to be None or a number. Got {}.".format(type(blend_band)))
+    band = float(blend_band)
+    if math.isnan(band) or band < 0:
+        raise ValueError("Expected blend_band >= 0 (metres, inf allowed). Got {}.".format(blend_band))
+    return band
+
+
 def _camera(t, name, B):
     if not torch.is_tensor(t):
         raise TypeError("Expected {} to be of type torch.Tensor. Got {}.".format(name, type(t)))
@@ -113,7 +180,7 @@ MAX_SPLAT_PX = 16  # GSX_MAX_SPLAT_PX (include/gsx.h)
 
 
 def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses: torch.Tensor, height: int,
-                       width: int, max_splat_px: int = 0) -> RenderedViews:
+                       width: int, max_splat_px: int = 0, blend_band: Optional[float] = None) -> RenderedViews:
     """Renders every map of the batch from L cameras: a map row covers the one pixel it projects to (the projection of
     find_active_map_points) and each pixel shows the covering row with the smallest camera-frame depth, ties to the
     lowest row index.
@@ -128,7 +195,16 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
     (`radii_padded` > 0, PointFusion(surfel_radii=True)) and a non-zero normal is drawn as an oriented disk: every pixel
     within max_splat_px pixels of its projected centre whose ray meets the disk shows it, at the depth where the ray
     meets the disk's plane.  Rows without a radius keep the one-pixel rule.  The footprint carries no gradient, and
-    the radius none either.  Cost grows with (2 max_splat_px + 1)^2 per disk row and view."""
+    the radius none either.  Cost grows with (2 max_splat_px + 1)^2 per disk row and view.
+
+    blend_band (extension, default None = the z-buffer above): a float >= 0 in metres (inf allowed) blends.  Each pixel
+    then shows the normalised, weighted mean of the rows that cover it (the coverage above, at max_splat_px) at a depth
+    no more than blend_band behind the front surface, the depth the z-buffer shows.  A disk row weighs
+    c (1 - s^2 / r^2), with s its in-plane distance from the ray's hit to its centre and r its radius; any other row
+    weighs c; c is the confidence count, or 1 for a map without one.  depth, rgb and normals (camera frame, not
+    renormalised) are the weighted means, confidence is the sum of the weights, and index is the z-buffer's.  Gradients
+    reach every contributing row's position, normal, radius, confidence count and colour, and the poses, through the
+    weights as well as the values.  Intrinsics that require grad are refused (no d/dK through the blend)."""
     if not isinstance(pointclouds, Pointclouds):
         raise TypeError("Expected pointclouds to be of type gradslam.Pointclouds. Got {0}.".format(type(pointclouds)))
     for name, v in (("height", height), ("width", width)):
@@ -140,11 +216,14 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
         raise TypeError("Expected max_splat_px to be of type int. Got {}.".format(type(max_splat_px)))
     if not 0 <= max_splat_px <= MAX_SPLAT_PX:
         raise ValueError("Expected 0 <= max_splat_px <= {}. Got {}.".format(MAX_SPLAT_PX, max_splat_px))
+    band = _blend_band(blend_band)
     _camera(poses, "poses", None)
     B = poses.shape[0]
     _camera(intrinsics, "intrinsics", B)
     if intrinsics.shape[1] != 1:
         raise ValueError("Expected intrinsics to have shape (B, 1, 4, 4). Got {}.".format(tuple(intrinsics.shape)))
+    if band is not None and torch.is_grad_enabled() and intrinsics.requires_grad:
+        raise ValueError("render_pointclouds: blend_band has no gradient w.r.t. the intrinsics; detach them")
     if pointclouds.has_points and len(pointclouds) != B:
         raise ValueError("Expected equal batch sizes for pointclouds and poses. Got {0} and {1}.".format(
             len(pointclouds), B))
@@ -170,6 +249,16 @@ def render_pointclouds(pointclouds: Pointclouds, intrinsics: torch.Tensor, poses
     poses_c = poses.contiguous()
     from ..odometry.icputils import _wants_grad
 
+    if band is not None:
+        pack = (counts.clone(), pointclouds._bound, height, width, pointclouds.has_normals, pointclouds._has_cc, band,
+                max_splat_px, K)
+        if _wants_grad(geo, col, poses_c):
+            depth, rgb, normals, weight, index = _RenderBlendFn.apply(pack, geo, col, poses_c)
+        else:
+            depth, rgb, normals, weight, index, _ = _render_blend(
+                geo.detach(), None if col is None else col.detach(), counts, pointclouds._bound, K, poses_c.detach(),
+                height, width, *pack[4:8])
+        return RenderedViews(depth, rgb, normals, weight if pointclouds._has_cc else None, index)
     if _wants_grad(geo, col, poses_c, intrinsics):
         outs = _RenderFn.apply((counts.clone(), pointclouds._bound, height, width) + want + (max_splat_px,), geo, col,
                                poses_c, intrinsics)

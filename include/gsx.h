@@ -804,6 +804,46 @@ int gsx_render_splats_bwd_intrinsics(const float *map_geometry, const int32_t *c
                                      float *g_intrinsics, void *scratch, int64_t scratch_bytes, int max_splat_px,
                                      void *stream);
 
+/* Blended splats: every pixel shows the normalised, weighted mean of the rows that cover it near the front surface.
+ * Coverage, the footprint and the plane depth are gsx_render_splats' at max_splat_px = M (0 .. GSX_MAX_SPLAT_PX; M = 0:
+ * one pixel per row): a disk row n covers pixel p when p is in its box and its ray meets the disk, at depth t_n(p),
+ * with s2_n(p) = |t d - q|^2 the squared in-plane distance the disk test compares with r^2; any other row covers the one
+ * pixel it projects to, at its camera z, with s2 = 0.  index and front_depth (B,L,H,W) are written exactly as
+ * gsx_render_splats writes its index and depth images: z_f(p), the depth of the row the z-buffer keeps.  Row n
+ * contributes to p when it covers p and t_n(p) <= fp32(z_f(p) + blend_band) (the sum taken in double, rounded once;
+ * blend_band in metres, >= 0, +inf allowed), with weight w_n = c_n (1 - s2_n / r_n^2) for a disk row and c_n for any
+ * other row; c_n = the row's confidence count (slot 6) if use_confidence, else 1.  Outputs (B,L,H,W[,C]) dense:
+ * weight (,1) = W = sum w_n, depth (,1) = sum w_n t_n / W, rgb (,3) = sum w_n colour_n / W, normals (,3) =
+ * sum w_n R^T n_n / W (not renormalised); all zero where W = 0.  The sums run per pixel over the buckets of the
+ * projected centres within +-M pixels in (dy, dx, row) order: deterministic, no float atomics, no host
+ * synchronisation.  rgb and normals may be NULL (rgb needs map_colors); index, front_depth, weight and depth may not.
+ * scratch: gsx_render_blend_scratch_bytes(B,L,H,W,max_count,max_splat_px) bytes (bucket counts and one key, slot and
+ * row index per (row, view) pair below max_count).  Refused before any launch: bad extents, max_splat_px, a negative or
+ * NaN blend_band, null or misaligned pointers, short scratch, and more than 2^31 - 1 buckets, (B L (H + 2M)(W + 2M)),
+ * or (row, view) pairs (B L max_count). */
+int64_t gsx_render_blend_scratch_bytes(int B, int L, int H, int W, int64_t max_count, int max_splat_px);
+int gsx_render_blend(const float *map_geometry, const float *map_colors, const int32_t *counts, int64_t capacity,
+                     int64_t max_count, const float *intrinsics, int64_t K_bstride, const float *poses,
+                     int64_t pose_bstride, int B, int L, int H, int W, int use_confidence, double blend_band,
+                     int max_splat_px, int64_t *index, float *front_depth, float *weight, float *depth, float *rgb,
+                     float *normals, void *scratch, int64_t scratch_bytes, void *stream);
+/* Backward of gsx_render_blend, from the forward's front_depth, weight and outputs and the upstream gradients of
+ * depth, rgb, normals and weight (NULL = zero; each needs its forward output).  Per pixel where row n contributed,
+ * d out/d w_n = (v_n - out)/W and d out/d v_n = w_n/W, chained to the row's position and normal (through t and s2),
+ * radius (slot 7, through r^2), confidence (slot 6, zero unless use_confidence) and colour, and to the pose.  A row
+ * re-enumerates its footprint per view in (view, h, w) order; d_geometry (B,cap,8) and d_colors (B,cap,4) have every
+ * row written (padding zero); d_poses (B*L,4,4) is reduced per CTA and view and summed in CTA order (bottom row zero).
+ * Any of the three may be NULL.  Deterministic, no atomics; no gradient w.r.t. the intrinsics.  scratch (d_poses only):
+ * gsx_render_blend_bwd_scratch_bytes(B,L,max_count) bytes.  Refused before any launch as gsx_render_blend. */
+int64_t gsx_render_blend_bwd_scratch_bytes(int B, int L, int64_t max_count);
+int gsx_render_blend_bwd(const float *map_geometry, const float *map_colors, const int32_t *counts, int64_t capacity,
+                         int64_t max_count, const float *intrinsics, int64_t K_bstride, const float *poses,
+                         int64_t pose_bstride, int B, int L, int H, int W, int use_confidence, double blend_band,
+                         int max_splat_px, const float *front_depth, const float *weight, const float *depth,
+                         const float *rgb, const float *normals, const float *g_depth, const float *g_rgb,
+                         const float *g_normals, const float *g_weight, float *d_geometry, float *d_colors,
+                         float *d_poses, void *scratch, int64_t scratch_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
