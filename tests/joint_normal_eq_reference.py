@@ -38,19 +38,37 @@ adds at most 3: every per-row gradient term has depth <= R_B = 132 + 48 + 9 = 18
 The per-row outputs (g_src, g_src_col) err by at most R_B u m', the scattered ones (g_tgt, g_tgt_n, g_model_col, summed
 by index_add_ in any order over at most c rows per pixel) by (R_B + c) u m', and g_prev, g_K (each row's term reduced
 like the sums, depth 13 + blocks) by (13 + blocks) u sum_rows |term| + R_B u m', where the per-row terms come from
-per-row leaf copies of prev and K (as tests/test_gpu_intrinsics_grad.py's _term_scale does for K1)."""
+per-row leaf copies of prev and K (as tests/test_gpu_intrinsics_grad.py's _term_scale does for K1).
+
+Huber scales (delta, delta_p: the op's huber=(huber_delta, photometric_huber_delta), robust_oracle's weights).  The
+kernels get the scales as float32 (`scales` rounds them the same way) and decide each row's branch on its float32
+residual, r or r_p, evaluated in their operation order: `float32_residuals` restates it bit for bit (the library builds
+with -fmad=false).  A row inside its scale (|r| <= delta, equality inside) adds the unweighted products; outside, with
+a = |r| and h = delta / a, the geometric row adds h (A_p A_q), h (A_p r), delta ((a + a) - delta) and the photometric
+row (w h_p) (A_p A_q), (w h_p) (A_p r_p), w (delta_p ((a_p + a_p) - delta_p)) with w h_p = w (delta_p / a_p).  The
+float64 values and autograd are evaluated on the float32 branch, so at a tie the inside branch's derivative applies.
+The pair arithmetic adds |.| (exact: e and m unchanged) and states those expressions in the same order; the sum bound
+follows as above.  The backward of an outside row (huber_adjoint) adds depth: r_p has depth 4 (the intensities 3, the
+difference 1), h_p = delta_p / a_p 5 (delta_p exact), w h_p 6.  The A_p adjoint (w h_p) v, v = g r_p + sum_q g A_q
+of depth R_A + 8, gets depth R_A + 8 + 6 + 1 = R_A + 15 instead of R_A + 9: every A_p path gains 6 levels,
+R_B_ROBUST = R_B + 6.  The r_p adjoint w (-(h_p / r_p) Q + 2 g_27 (h_p r_p)), Q the sum of 21 products g (A_p A_q)
+(depth 2 R_A + 2 + 21), has depth 2 R_A + 36, and the colours' chain adds 2: 2 R_A + 38 = 116 < R_B.  The geometric
+row's A and r have depth <= 4, so its adjoints stay far below.  R_B_ROBUST applies only when a scale is finite."""
 import math
 
 import torch
 
 import photometric_oracle as ph
 import projective_oracle as po
+import robust_oracle as ro
 
 U32 = 2.0 ** -24
 BLOCK = 256  # rows per block of the kernels (kIcpBlock)
 R_F = 80  # the products of the sums
 R_A, D = 39, 8  # the photometric row A_p, the projection's denominator
 R_B = (2 * R_A + 3 * (2 * D + 2)) + (R_A + 9) + 9
+R_H = 6  # w h_p = w (delta_p / |r_p|) of an outside photometric row
+R_B_ROBUST = (2 * R_A + 3 * (2 * D + 2)) + (R_A + 8 + R_H + 1) + 9
 NAMES = ("src", "src_col", "tgt", "tgt_n", "model_col", "prev", "K")
 _IU = torch.triu_indices(6, 6)
 
@@ -60,16 +78,42 @@ def blocks_of(ns_stride):
     return max(1, math.ceil(ns_stride / BLOCK))
 
 
-def joint_sums(src, src_col, tgt, tgt_n, model_col, prev, K, idx, index, H, W, w):
+def scales(delta, delta_p):
+    """The Huber scales as the kernels get them: float32 (+inf stays +inf)."""
+    return tuple(float(torch.tensor(float(d), dtype=torch.float32)) for d in (delta, delta_p))
+
+
+def float32_residuals(src, src_col, tgt, tgt_n, model_col, idx, index, H, W):
+    """The residuals the kernels decide the Huber branches on, in float32 with their operation order: r (rows with
+    idx >= 0, source order), r_p (those of them with a photometric row) and vj (which rows have one)."""
+    f = lambda t: t.detach().float()
+    _, b = po._rows(f(src), f(tgt), f(tgt_n), idx)
+    I_m = ph.intensity(f(model_col))
+    valid = ph.stencil(I_m.unsqueeze(0), index.unsqueeze(0), H, W)[0][0]
+    keep = idx >= 0
+    j = idx[keep]
+    vj = valid[j]
+    return b[:, 0], ph.intensity(f(src_col)[keep][vj]) - I_m[j[vj]], vj
+
+
+def joint_sums(src, src_col, tgt, tgt_n, model_col, prev, K, idx, index, H, W, w, delta=math.inf, delta_p=math.inf):
     """One element: src, src_col (n, 3) its rows (i < count); tgt, tgt_n, model_col (H*W, 3); prev, K (4, 4);
     idx (n,) int64 associated pixel or -1, only covered pixels; index (H*W,) int64, -1 = uncovered.  -> (28,) in the
-    inputs' dtype: the upper triangle of A^T A + w A_p^T A_p row by row, A^T b + w A_p^T r_p, b^T b + w r_p^T r_p."""
+    inputs' dtype: the upper triangle of A^T A + w A_p^T A_p row by row, A^T b + w A_p^T r_p, b^T b + w r_p^T r_p;
+    with a finite Huber scale delta / delta_p, the rows' Huber-weighted products summed (module docstring)."""
     A, b = po._rows(src, tgt, tgt_n, idx)
     I_m = ph.intensity(model_col)
     valid, gu, gv = ph.stencil(I_m.unsqueeze(0), index.unsqueeze(0), H, W)
     Ap, rp = ph.photometric_rows(src, ph.intensity(src_col), idx, valid[0], gu[0], gv[0], I_m, prev, K)
-    AtA, Atb, bb = ph._normal_equations(A, b, Ap, rp, w)
-    return torch.cat([AtA[_IU[0], _IU[1]], Atb[:, 0], bb.view(1)])
+    delta, delta_p = scales(delta, delta_p)
+    if math.isinf(delta) and math.isinf(delta_p):
+        AtA, Atb, bb = ph._normal_equations(A, b, Ap, rp, w)
+        return torch.cat([AtA[_IU[0], _IU[1]], Atb[:, 0], bb.view(1)])
+    r32, rp32, _ = float32_residuals(src, src_col, tgt, tgt_n, model_col, idx, index, H, W)
+    geo = ro.row_products(A, b[:, 0], delta, inside=r32.abs() <= delta)
+    pho = ro.row_products(Ap, rp[:, 0], delta_p, w=torch.tensor(w, dtype=torch.float32).to(A.dtype),
+                          inside=rp32.abs() <= delta_p)
+    return geo.sum(0) + pho.sum(0)
 
 
 class _P:
@@ -101,6 +145,33 @@ class _P:
     def __neg__(a):
         return _P(-a.v, a.m, a.e)
 
+    def __abs__(a):
+        return _P(a.v.abs(), a.m, a.e)
+
+
+def _where(mask, a, b):
+    """Row by row: pair a where mask, else pair b."""
+    return _P(torch.where(mask, a.v, b.v), torch.where(mask, a.m, b.m), torch.where(mask, a.e, b.e))
+
+
+def _huber_pairs(prods, r, wt, delta, inside):
+    """The 28 products of rows with residual pair r, as pairs: inside rows keep prods (their unweighted products, times
+    wt for the photometric row when wt is given); outside ones get h (A_p A_q), h (A_p r), delta ((a + a) - delta), h =
+    delta / a, or with wt (wt h) (..) and wt (delta ((a + a) - delta)), wt h = wt (delta / a).  prods: (products A_p A_q
+    and A_p r (27 pairs, unweighted), the 28 inside pairs)."""
+    raw, kept = prods
+    if math.isinf(delta):
+        return kept
+    a = abs(r)
+    one = _const(1.0, r.v)
+    a_out = _where(inside, one, a)  # (inside rows never divide)
+    d = _const(delta, r.v)
+    h = d / a_out
+    rho = d * ((a_out + a_out) - d)
+    if wt is not None:
+        h, rho = wt * h, wt * rho
+    return [_where(inside, k, o) for k, o in zip(kept, [h * p for p in raw] + [rho])]
+
 
 def _const(x, like):
     c = torch.tensor(x, dtype=torch.float32).to(like.dtype)  # the kernels' float32 constant
@@ -113,11 +184,13 @@ def _intensity(c):
     return (wr * c[0] + wg * c[1]) + wb * c[2]
 
 
-def _pair_rows(x, mx, idx, index, H, W, w, prev_rows=None, K_rows=None):
+def _pair_rows(x, mx, idx, index, H, W, w, prev_rows=None, K_rows=None, delta=math.inf, delta_p=math.inf):
     """The 28 per-row products in pair arithmetic, (28, n_rows) values and magnitudes, for the rows with idx >= 0.
     x: dict NAMES -> float tensors (values); mx: the same -> magnitudes (leaves of the backward's magnitude);
     prev_rows / K_rows: optional (n_rows, 12) per-row copies of the first three rows of prev and K used for the values
-    (leaves of the per-row terms).  Values are bit-identical to po._rows / ph.photometric_rows in the same dtype."""
+    (leaves of the per-row terms).  Values are bit-identical to po._rows / ph.photometric_rows in the same dtype.
+    delta, delta_p: Huber scales (the branches are the float32 residuals')."""
+    delta, delta_p = scales(delta, delta_p)
     keep = idx >= 0
     j = idx[keep]
     n = int(j.numel())
@@ -130,7 +203,12 @@ def _pair_rows(x, mx, idx, index, H, W, w, prev_rows=None, K_rows=None):
     px, py, pz = (comp(tp, c) for c in range(3))
     A = [nx, ny, nz, nz * sy - ny * sz, nx * sz - nz * sx, ny * sx - nx * sy]
     r = (nx * (px - sx) + ny * (py - sy)) + nz * (pz - sz)
-    geo = [A[p] * A[q] for p in range(6) for q in range(p, 6)] + [A[p] * r for p in range(6)] + [r * r]
+    raw = [A[p] * A[q] for p in range(6) for q in range(p, 6)] + [A[p] * r for p in range(6)]
+    geo = raw + [r * r]
+    if not (math.isinf(delta) and math.isinf(delta_p)):
+        r32, rp32, _ = float32_residuals(*(x[k] for k in ("src", "src_col", "tgt", "tgt_n", "model_col")), idx, index,
+                                         H, W)
+        geo = _huber_pairs((raw, geo), r, None, delta, r32.abs() <= delta)
 
     # photometric rows: the stencil's validity and g_u, g_v at j (values of the model colours, any dtype)
     I_m = ph.intensity(x["model_col"])
@@ -167,8 +245,10 @@ def _pair_rows(x, mx, idx, index, H, W, w, prev_rows=None, K_rows=None):
     cx, cy, cz = (((R[3 * a] * cc[0] + R[3 * a + 1] * cc[1]) + R[3 * a + 2] * cc[2]) for a in range(3))
     Ap = [cx, cy, cz, cz * sy - cy * sz, cx * sz - cz * sx, cy * sx - cx * sy]
     wt = _const(w, x["src"])
-    pho = [wt * (Ap[p] * Ap[q]) for p in range(6) for q in range(p, 6)] + [wt * (Ap[p] * rp) for p in range(6)]
-    pho.append(wt * (rp * rp))
+    raw = [Ap[p] * Ap[q] for p in range(6) for q in range(p, 6)] + [Ap[p] * rp for p in range(6)]
+    pho = [wt * p for p in raw] + [wt * (rp * rp)]
+    if not math.isinf(delta_p):
+        pho = _huber_pairs((raw, pho), rp, wt, delta_p, rp32.abs() <= delta_p)
 
     def scatter(p):  # the photometric products at the rows that have them, 0 elsewhere
         z = lambda t: torch.zeros(n, dtype=t.dtype).masked_scatter(vj, t)
@@ -179,20 +259,23 @@ def _pair_rows(x, mx, idx, index, H, W, w, prev_rows=None, K_rows=None):
     return stack(lambda o: o.v), stack(lambda o: o.m), stack(lambda o: o.e), (A, r), (Ap, rp), vj
 
 
-def reference(inputs, idx, index, H, W, w, blocks, g=None):
+def reference(inputs, idx, index, H, W, w, blocks, g=None, delta=math.inf, delta_p=math.inf):
     """inputs: dict NAMES -> one element's float32 tensors (CPU; src, src_col cut at the element's count);
     idx (n,), index (H*W,) int64; blocks: reduction blocks of the call (blocks_of(ns_stride)); g: optional (28,)
-    upstream gradient.  -> dict: "sums" (28,) float64, "sum_bound" (28,); with g also "grad" and "grad_bound", dicts
-    NAMES -> float64 tensors of the inputs' shapes (the bottom rows of prev and K get 0 and bound 0)."""
+    upstream gradient; delta, delta_p: the Huber scales of the call.  -> dict: "sums" (28,) float64, "sum_bound" (28,);
+    with g also "grad" and "grad_bound", dicts NAMES -> float64 tensors of the inputs' shapes (the bottom rows of prev
+    and K get 0 and bound 0)."""
+    delta, delta_p = scales(delta, delta_p)
+    R = R_B if math.isinf(delta) and math.isinf(delta_p) else R_B_ROBUST
     x = {k: v.detach().double().clone().requires_grad_(True) for k, v in inputs.items()}
-    sums = joint_sums(*(x[k] for k in NAMES), idx, index, H, W, w)
+    sums = joint_sums(*(x[k] for k in NAMES), idx, index, H, W, w, delta, delta_p)
     out = {"sums": sums.detach()}
     mx = {k: v.detach().abs().requires_grad_(True) for k, v in x.items()}
     rows = int((idx >= 0).sum())
     xd = {k: v.detach() for k, v in x.items()}
     prev_rows = x["prev"].detach()[:3].reshape(1, 12).expand(rows, 12).clone().requires_grad_(True)
     K_rows = x["K"].detach()[:3].reshape(1, 12).expand(rows, 12).clone().requires_grad_(True)
-    vals, mags, errs, *_ = _pair_rows(xd, mx, idx, index, H, W, w, prev_rows, K_rows)
+    vals, mags, errs, *_ = _pair_rows(xd, mx, idx, index, H, W, w, prev_rows, K_rows, delta, delta_p)
     out["row_err"], out["row_abs"] = errs.sum(1).detach(), vals.detach().abs().sum(1)
     out["sum_bound"] = U32 * (out["row_err"] + (13 + blocks) * out["row_abs"])
     if g is None:
@@ -213,13 +296,13 @@ def reference(inputs, idx, index, H, W, w, blocks, g=None):
     per_pixel = torch.bincount(j, minlength=P).max().item() if j.numel() else 0
     st = (j.unsqueeze(1) + torch.tensor([0, -1, 1, -W, W])).clamp(0, P - 1).reshape(-1)
     per_stencil = torch.bincount(st, minlength=P).max().item() if st.numel() else 0
-    bound = {"src": R_B * U32 * gm["src"], "src_col": R_B * U32 * gm["src_col"],
-             "tgt": (R_B + per_pixel) * U32 * gm["tgt"], "tgt_n": (R_B + per_pixel) * U32 * gm["tgt_n"],
-             "model_col": (R_B + per_stencil) * U32 * gm["model_col"]}
+    bound = {"src": R * U32 * gm["src"], "src_col": R * U32 * gm["src_col"],
+             "tgt": (R + per_pixel) * U32 * gm["tgt"], "tgt_n": (R + per_pixel) * U32 * gm["tgt_n"],
+             "model_col": (R + per_stencil) * U32 * gm["model_col"]}
     for name, term in (("prev", terms[0]), ("K", terms[1])):
         b = torch.zeros(4, 4, dtype=torch.float64)
         b[:3] = ((13 + blocks) * U32 * term.detach().abs().sum(0)).view(3, 4)
-        bound[name] = b + R_B * U32 * gm[name]
+        bound[name] = b + R * U32 * gm[name]
         bound[name][3] = 0.0
     out["grad_bound"] = {k: v.detach() for k, v in bound.items()}
     out["row_terms"] = {"prev": terms[0].detach(), "K": terms[1].detach()}

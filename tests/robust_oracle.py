@@ -25,12 +25,14 @@ import radii_oracle as ro
 F32 = torch.float32
 
 
-def weights(r, delta):
+def weights(r, delta, inside=None):
     """r (n,) residuals -> (inside (n,) bool, h (n,): 1 inside, delta / |r| outside, rho (n,): r r inside, delta ((a + a)
-    - delta) outside).  Safe for autograd: the branch a row does not take gets no gradient and no NaN."""
+    - delta) outside).  Safe for autograd: the branch a row does not take gets no gradient and no NaN.  inside: the
+    rows' branch decisions when they are given (a float64 evaluation on the float32 kernels' branches), else a <= delta."""
     d = torch.as_tensor(delta, dtype=r.dtype)
     a = r.abs()
-    inside = a <= d
+    if inside is None:
+        inside = a <= d
     one = torch.ones_like(a)
     a_out = torch.where(inside, one, a)  # (inside rows never divide)
     h = torch.where(inside, one, d / a_out)
@@ -38,10 +40,11 @@ def weights(r, delta):
     return inside, h, rho
 
 
-def row_products(A, r, delta, w=None):
+def row_products(A, r, delta, w=None, inside=None):
     """The 28 products every row adds, as the kernels write them (row_products<true>, and add_weighted_products<true>
-    when w is given): A (n,6), r (n,) -> (n,28) in the kernels' order (21 upper-triangular A_p A_q, 6 A_p r, slot 27)."""
-    inside, h, rho = weights(r, delta)
+    when w is given): A (n,6), r (n,) -> (n,28) in the kernels' order (21 upper-triangular A_p A_q, 6 A_p r, slot 27).
+    inside: optional branch decisions (weights)."""
+    inside, h, rho = weights(r, delta, inside)
     iu = torch.triu_indices(6, 6)
     pq = A[:, iu[0]] * A[:, iu[1]]
     pr = A * r.unsqueeze(1)

@@ -38,9 +38,10 @@ def _elements(sizes, H, W, seed, all_filtered=()):
     return els
 
 
-def _run(els, H, W, w, g, k_grad=True, ns=None, pad_value=0.0):
-    """The op on a padded batch of elements (x, idx, index) with upstream gradient g (B, 28).  Padding rows hold
-    pad_value and idx -1.  -> dict of CPU tensors: "sums" (B, 28) and the gradient of every input."""
+def _run(els, H, W, w, g, k_grad=True, ns=None, pad_value=0.0, huber=(math.inf, math.inf)):
+    """The op on a padded batch of elements (x, idx, index) with upstream gradient g (B, 28) at the Huber scales
+    huber = (huber_delta, photometric_huber_delta).  Padding rows hold pad_value and idx -1.  -> dict of CPU tensors:
+    "sums" (B, 28) and the gradient of every input."""
     from gradslam_b200.odometry.icputils import _JointNormalEqBatchedFn
 
     B = len(els)
@@ -59,7 +60,7 @@ def _run(els, H, W, w, g, k_grad=True, ns=None, pad_value=0.0):
     counts = torch.tensor(sizes, dtype=torch.int32, device=DEV)
     sums = _JointNormalEqBatchedFn.apply(leaves["src"], leaves["src_col"], leaves["tgt"], leaves["tgt_n"],
                                          leaves["model_col"], leaves["prev"], idx.to(DEV), index, counts, leaves["K"],
-                                         w, H, W)
+                                         w, H, W, huber)
     (sums * g.to(DEV)).sum().backward()
     out = {"sums": sums.detach().cpu()}
     for k, v in leaves.items():
